@@ -14,7 +14,7 @@
 //   H3        final decode pass writing quantised coefficients (natural order, DC still differential)
 //   D1        DC prediction (prefix sum per component, reset at restart intervals)
 //   I1        dequantisation + islow IDCT -> planar component samples
-//   C1        chroma upsampling (fancy / box) + colour conversion -> interleaved HWC u8
+//   C1        chroma upsampling (fancy / box) + colour conversion (YCbCr, RGB, CMYK, YCCK) -> interleaved HWC u8
 //   I1 + C1   fused, without the planes, for 4:2:0 YCbCr with fancy upsampling to RGB / BGR (idct_color_420)
 // The parallel entropy decode follows the self-synchronising scheme of Weissenberger & Schmidt
 // ("Accelerating JPEG decompression on GPUs", 2021): a decoder started at a wrong bit position
@@ -61,15 +61,25 @@ __host__ __device__ inline int LutOffset(int t) { return t < 2 ? t * kDcLutSize 
 
 struct QuantSet { uint16_t q[4][64]; };       // natural order
 
+// Colour space of the decoded components (libjpeg default_decompress_parms).  Decided once per image by the plan; the kernels read
+// nothing else to pick the conversion.
+enum JpegColor : int32_t {
+  kColorGray = 0,     // 1 component
+  kColorYCbCr = 1,    // 3 components
+  kColorRGB = 2,      // 3 components: Adobe transform 0, or R/G/B component ids without JFIF / Adobe markers
+  kColorCMYK = 3,     // 4 components: Adobe transform 0, or no Adobe marker
+  kColorYCCK = 4,     // 4 components: any other Adobe transform (components 0..2 are the YCbCr of 255 - C, 255 - M, 255 - Y)
+};
+
 struct JpegImage {
   uint8_t *out;               // HWC u8
   int32_t width, height, ncomp;
-  int32_t hs[3], vs[3], hmax, vmax;
+  int32_t hs[4], vs[4], hmax, vmax;
   int32_t mcux, mcuy, bpm;    // MCUs per row / column, blocks per MCU
   int32_t blk_comp[kMaxBlocksPerMcu];      // component of each block in the MCU
   int32_t blk_dc[kMaxBlocksPerMcu], blk_ac[kMaxBlocksPerMcu];   // table index (0..3) into TableSet
   int32_t blk_x[kMaxBlocksPerMcu], blk_y[kMaxBlocksPerMcu];     // block offset inside the MCU (in blocks)
-  int32_t tq[3];
+  int32_t tq[4];
   int32_t restart_interval;
   int32_t table_set, quant_set;
   int32_t unit_begin, unit_end;            // segments (restart intervals or the whole scan)
@@ -78,10 +88,10 @@ struct JpegImage {
   int32_t block_begin;                     // first sync block
   int32_t wblock_begin;                    // first block of the write pass (kWriteThreads subsequences each)
   int64_t coef_off;                        // int16 offset into the coefficient arena
-  int64_t plane_off[3];                    // byte offsets into the plane arena
-  int32_t plane_w[3], plane_h[3];          // padded plane sizes (multiples of the MCU)
+  int64_t plane_off[4];                    // byte offsets into the plane arena
+  int32_t plane_w[4], plane_h[4];          // padded plane sizes (multiples of the MCU)
   int32_t out_type, fancy;
-  int32_t is_rgb;                          // Adobe transform 0 / RGB ids: no YCbCr conversion
+  int32_t color;                           // JpegColor
   int32_t fast_color;                      // 1: color_fast_kernel, 2: idct_color_420 (4:2:0 fancy -> RGB / BGR), 0: color_kernel
   // decode window: the pixels [win_x0, win_x0 + win_w) x [win_y0, win_y0 + win_h) of the (un-oriented) image are produced, `out`
   // is a tight win_h x win_w x C buffer (the caller's sample, or plan scratch when a post pass follows).  win_x0 % 8 == 0.
@@ -1154,15 +1164,16 @@ __global__ void __launch_bounds__(256) color_kernel(const JpegImage *__restrict_
     const int nx = min(4, im.win_x0 + im.win_w - x0);
     for (int k = 0; k < nx; k++) {
       const int x = x0 + k;
-      int v[3];
+      int v[4];
       for (int c = 0; c < im.ncomp; c++) {
         const int hexp = im.hmax / im.hs[c], vexp = im.vmax / im.vs[c];
         const int dw = (W * im.hs[c] + im.hmax - 1) / im.hmax, dh = (H * im.vs[c] + im.vmax - 1) / im.vmax;
         v[c] = up_sample(planes + im.plane_off[c], im.plane_w[c], dw, dh, hexp, vexp, im.fancy, x, y);
       }
+      const int cm = im.color;
       int r, g, b, yy, cb, cr;
-      if (im.ncomp == 1) { r = g = b = yy = v[0]; cb = cr = 128; }
-      else if (im.is_rgb) { r = v[0]; g = v[1]; b = v[2]; yy = cb = cr = 0; }
+      if (cm == kColorGray) { r = g = b = yy = v[0]; cb = cr = 128; }
+      else if (cm == kColorRGB || cm == kColorCMYK) { r = v[0]; g = v[1]; b = v[2]; yy = cb = cr = 0; }
       else {
         yy = v[0]; cb = v[1]; cr = v[2];
         const int cbm = cb - 128, crm = cr - 128;                   // jdcolor.c, SCALEBITS = 16
@@ -1170,10 +1181,19 @@ __global__ void __launch_bounds__(256) color_kernel(const JpegImage *__restrict_
         g = clamp255(yy + ((-22554 * cbm + 32768 - 46802 * crm) >> 16));
         b = clamp255(yy + ((116130 * cbm + 32768) >> 16));
       }
+      if (cm >= kColorCMYK) {
+        // C, M, Y: the samples (CMYK) or 255 - the YCbCr->RGB above (YCCK, jdcolor.c ycck_cmyk_convert); then OpenCV's
+        // icvCvt_CMYK2BGR on these (inverted, Adobe-style) samples: R = K - ((255 - C) * K >> 8), and so on
+        const int kk = v[3];
+        const int ic = cm == kColorCMYK ? 255 - r : r, imy = cm == kColorCMYK ? 255 - g : g, iy = cm == kColorCMYK ? 255 - b : b;
+        r = kk - ((ic * kk) >> 8); g = kk - ((imy * kk) >> 8); b = kk - ((iy * kk) >> 8);
+      }
       if (im.out_type == DALIB200_RGB) { px[3 * k] = r; px[3 * k + 1] = g; px[3 * k + 2] = b; }
       else if (im.out_type == DALIB200_BGR) { px[3 * k] = b; px[3 * k + 1] = g; px[3 * k + 2] = r; }
       else if (im.out_type == DALIB200_YCbCr) { px[3 * k] = yy; px[3 * k + 1] = cb; px[3 * k + 2] = cr; }
-      else px[k] = (im.ncomp == 1 || !im.is_rgb) ? yy : ((r * 19595 + g * 38470 + b * 7471 + 32768) >> 16);
+      else if (cm == kColorRGB) px[k] = (r * 19595 + g * 38470 + b * 7471 + 32768) >> 16;
+      else if (cm >= kColorCMYK) px[k] = (b * 1868 + g * 9617 + r * 4899 + 8192) >> 14;      // OpenCV icvCvt_CMYK2Gray
+      else px[k] = yy;
     }
     uint8_t *o = im.out + ((int64_t)(y - im.win_y0) * im.win_w + (x0 - im.win_x0)) * nout;
     const int nb = nx * nout;
@@ -1887,7 +1907,7 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
-    im.fast_color = j.ncomp == 3 && !im.is_rgb && (im.out_type == DALIB200_RGB || im.out_type == DALIB200_BGR) &&
+    im.fast_color = j.ncomp == 3 && im.color == kColorYCbCr && (im.out_type == DALIB200_RGB || im.out_type == DALIB200_BGR) &&
                     ((j.hmax == 2 && j.vmax <= 2) || (j.hmax == 1 && j.vmax <= 2));
     if (im.fast_color && p->fancy && j.hmax == 2 && j.vmax == 2 && (j.width + 1) / 2 > 2) im.fast_color = 2;    // idct_color_420
     if (planes_only) im.fast_color = 1;                                   // IDCT into the planes, no colour work items
@@ -2054,10 +2074,14 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     }
     if ((int64_t)j.width * j.height >= (1ll << 31)) return unsupported("images of 2^31 pixels or more are not supported");
     if (j.precision != 8) return unsupported("only 8-bit baseline JPEG is supported");
-    if (j.ncomp != 1 && j.ncomp != 3) return unsupported("only 1- or 3-component JPEG is supported");
+    if (j.ncomp != 1 && j.ncomp != 3 && j.ncomp != 4) return unsupported("only 1-, 3- or 4-component JPEG is supported");
     if (j.scan_ncomp != j.ncomp) return unsupported("multi-scan (non-interleaved) baseline JPEG is not supported yet");
-    for (int c = 1; c < j.ncomp; c++)
-      if (j.hs[c] != 1 || j.vs[c] != 1) return unsupported("chroma sampling factors other than 1x1 are not supported");
+    if (j.ncomp == 3)
+      for (int c = 1; c < j.ncomp; c++)
+        if (j.hs[c] != 1 || j.vs[c] != 1) return unsupported("chroma sampling factors other than 1x1 are not supported");
+    if (j.ncomp == 4)              // every component is upsampled by whole factors (CMYK / YCCK: each component may have its own)
+      for (int c = 0; c < j.ncomp; c++)
+        if (j.hmax % j.hs[c] || j.vmax % j.vs[c]) return unsupported("non-integral component sampling ratios are not supported");
     if (j.ncomp == 1) { j.hs[0] = j.vs[0] = 1; j.hmax = j.vmax = 1; }     // a single-component scan is never interleaved
     if (!(j.hmax == 1 || j.hmax == 2 || j.hmax == 4) || !(j.vmax == 1 || j.vmax == 2)) return unsupported("unsupported luma sampling factor");
     JpegImage &im = p->images[i];
@@ -2068,8 +2092,10 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     im.mcuy = (j.height + 8 * j.vmax - 1) / (8 * j.vmax);
     im.restart_interval = prog ? 0 : j.restart_interval;      // progressive: the DC values arrive as one run of differences (jpeg_prog_core.h)
     im.out_type = output_type; im.fancy = p->fancy;
-    im.is_rgb = j.ncomp == 3 && (j.adobe_transform == 0 ||
-                (j.adobe_transform < 0 && !j.jfif && j.cid[0] == 'R' && j.cid[1] == 'G' && j.cid[2] == 'B'));
+    if (j.ncomp == 1) im.color = kColorGray;
+    else if (j.ncomp == 4) im.color = j.adobe_transform > 0 ? kColorYCCK : kColorCMYK;
+    else im.color = j.adobe_transform == 0 || (j.adobe_transform < 0 && !j.jfif && j.cid[0] == 'R' && j.cid[1] == 'G' && j.cid[2] == 'B')
+                    ? kColorRGB : kColorYCbCr;
     int bpm = 0;
     for (int si = 0; si < j.scan_ncomp; si++) {
       const int c = j.scan_comp[si];
@@ -2245,7 +2271,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
     ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
     // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
-    ge.planar_ok = j.ncomp == 3 && !im.is_rgb && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
+    ge.planar_ok = j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
                    output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
     const bool planes_only = rois && rois[i].planes_only;
     if (planes_only && !ge.planar_ok) {

@@ -114,7 +114,7 @@ inline int PlanProgressive(const uint8_t *d, size_t n, size_t base, int image, P
       if (sl < 6) return bad("JPEG: bad SOF");
       height = Rd16(s + 1); width = Rd16(s + 3); ncomp = s[5];
       if (s[0] != 8) return unsup("only 8-bit JPEG is supported");
-      if ((ncomp != 1 && ncomp != 3) || sl < 6 + 3 * ncomp) return unsup("only 1- or 3-component JPEG is supported");
+      if ((ncomp != 1 && ncomp != 3 && ncomp != 4) || sl < 6 + 3 * ncomp) return unsup("only 1-, 3- or 4-component JPEG is supported");
       for (int c = 0; c < ncomp; c++) {
         cid[c] = s[6 + 3 * c]; hs[c] = s[7 + 3 * c] >> 4; vs[c] = s[7 + 3 * c] & 15;
         if (hs[c] < 1 || hs[c] > 4 || vs[c] < 1 || vs[c] > 4) return bad("JPEG: bad sampling factors");

@@ -16,6 +16,9 @@ seeds = [synth(33, 47), synth(64, 64, sub=cv2.IMWRITE_JPEG_SAMPLING_FACTOR_444),
 seeds += [bytearray(po.with_exif_orientation(bytes(seeds[0]), o)) for o in (3, 6, 8)]
 seeds += [synth(33, 47, prog=True), synth(40, 24, rst=2, prog=True), synth(17, 19, gray=True, prog=True),
           synth(48, 40, sub=cv2.IMWRITE_JPEG_SAMPLING_FACTOR_444, prog=True)]
+# 4-component streams (CMYK, YCCK, no Adobe marker; baseline and progressive; 4:4:4 and subsampled), written by Pillow
+cmyk = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "tests", "golden", "jpeg_cmyk.npz"))
+seeds += [bytearray(cmyk[f"enc_{k}"].tobytes()) for k in range(len(cmyk.files) // 4) if str(cmyk[f"name_{k}"]).endswith("61x77")]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()

@@ -3,7 +3,7 @@
 # ROI and descriptor build of dalib200JpegGetInfo / dalib200JpegPlanSetupEx) under AddressSanitizer, without a GPU: jpeg.cu + common.cu
 # are built with -fsanitize=address and the handful of CUDA runtime calls the host side makes are replaced by a preloaded stub
 # (cuda_stub.c: events = no-ops, pinned / device allocations = malloc, so that ASAN's red zones surround them).
-# Inputs: valid baseline and progressive streams (4:2:0 / 4:4:4 / 4:2:2 / gray, restart intervals, EXIF orientations) with byte flips, truncation,
+# Inputs: valid baseline and progressive streams (4:2:0 / 4:4:4 / 4:2:2 / gray / CMYK / YCCK, restart intervals, EXIF orientations) with byte flips, truncation,
 # corrupted segment lengths, wrapping EXIF offsets, inserted / deleted bytes, markers sprinkled into the entropy data.
 # A finding is an ASAN report on stderr (non-zero exit).
 set -e
