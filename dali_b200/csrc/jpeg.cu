@@ -35,6 +35,7 @@ constexpr int kDcLutSize = 1 << kDcLutBits, kAcLutSize = 1 << kAcLutBits;
 constexpr int kLutWords = 2 * kDcLutSize + 2 * kAcLutSize;          // DC0 DC1 AC0 AC1 back to back: 20 KB
 constexpr int kSyncThreads = 256;            // subsequences per synchronisation block
 constexpr int kChunkBytes = 4096;            // un-stuffing chunk
+constexpr uint32_t kCleanPad = 32;           // zero bytes behind the clean stream of every unit (at least: units are 16-byte aligned)
 constexpr int kMaxBlocksPerMcu = 10;
 constexpr int kMaxLog2Sub = 10;              // largest subsequence: 2^10 bits = 128 bytes
 
@@ -302,7 +303,7 @@ __global__ void __launch_bounds__(256) unstuff_scatter_kernel(const uint8_t *__r
     if (c0 + kChunkBytes >= u.raw_len) {
       // last chunk of the unit: zero the pad behind the clean bytes (the bit reader peeks a few bytes past the end); the
       // clean buffer itself is never memset
-      const uint32_t e0 = out_base + total, e1 = u.clean_off + ((u.raw_len + 32u + 15u) & ~15u);
+      const uint32_t e0 = out_base + total, e1 = u.clean_off + ((u.raw_len + kCleanPad + 15u) & ~15u);
       for (uint32_t q = e0 + threadIdx.x; q < e1; q += blockDim.x) clean[(q & ~3u) | (3u - (q & 3u))] = 0;
     }
     __syncthreads();
@@ -312,9 +313,11 @@ __global__ void __launch_bounds__(256) unstuff_scatter_kernel(const uint8_t *__r
 // ============================================================================================
 // Huffman decoding
 //
-// Bit source: the clean (un-stuffed, word-swapped) stream of a unit.  The sync-block kernels stage the CTA's 128
-// subsequences (+ one look-ahead column) into shared memory with coalesced 16-byte loads; word g of the staged run sits at
-// g ^ ((g >> lsw) & 31) so that the 32 lanes of a warp, each inside its own subsequence, always hit 32 different banks.
+// Bit source: the clean (un-stuffed, word-swapped) stream of a unit.  The sync-intra pass stages the CTA's subsequences
+// (+ look-ahead columns) into shared memory with coalesced 16-byte loads; word g of the staged run sits at
+// g ^ ((g >> lsw) & 31) so that the 32 lanes of a warp, each inside its own subsequence, always hit 32 different banks.  The write
+// pass reads the stream straight from global memory through a register window (StreamWindow below); the chain walk copies a
+// subsequence into a private shared-memory column (ColSrc) or reads words from global (GlobalSrc).
 struct SmemSrc {
   uint32_t base; int lsw;                  // shared-window address of the staged run
   __device__ __forceinline__ uint32_t load(uint32_t g) const { return lds_u32(base + ((g ^ ((g >> lsw) & 31u)) << 2)); }
@@ -332,16 +335,18 @@ struct GlobalSrc {
 // the 32 lanes of a warp sit at unrelated bit positions, so a branch here would be divergent on almost every symbol.
 template <class Src>
 struct BitWindow {
+  Src s;
   uint32_t hi, lo, g;
   int avail;
-  __device__ __forceinline__ void init(const Src &s, uint32_t word, uint32_t sh) {
+  __device__ __forceinline__ void init(const Src &src, uint32_t word, uint32_t sh) {
+    s = src;
     const uint32_t w0 = s.load(word), w1 = s.load(word + 1);
     hi = __funnelshift_l(w1, w0, sh);
     lo = w1 << sh;
     avail = 64 - (int)sh;
     g = word + 2;
   }
-  __device__ __forceinline__ void consume(const Src &s, uint32_t e) {      // e & 31 = bits to drop, 1..31
+  __device__ __forceinline__ void consume(uint32_t e) {      // e & 31 = bits to drop, 0..31
     hi = __funnelshift_l(lo, hi, e);
     lo = __funnelshift_l(0u, lo, e);
     avail -= (int)(e & 31u);
@@ -352,6 +357,75 @@ struct BitWindow {
     lo = need ? (w << ((32u - a) & 31u)) : lo;
     avail += need ? 32 : 0;
     g += need ? 1u : 0u;
+  }
+};
+
+// The same window fed from global memory without shared memory.  The unit's stream is read in 16-byte chunks (ld.global.nc, always
+// aligned: units start 16-byte aligned in the clean buffer) into registers: a queue c0..c4 of up to 5 words (c0 = the word the
+// next refill takes; a refill moves the others up by one with selects, no branch) and the next chunk `nxt`, in flight.
+// A load's destination registers carry a scoreboard for the whole warp, so `nxt` is only ever read at warp-uniform points: every
+// second iteration of a warp-uniform symbol loop (top_up), where the lanes with at most one word left append `nxt` to their queue
+// and request the chunk behind it.  A refill takes at most one word per symbol, so a lane never runs dry between two top-ups, and
+// every load has had two loop iterations to arrive before its registers are read (huff_write's loop is warp-uniform).
+//
+// Read bound.  Window invariant: 32 * T = pos + avail, T = words taken by the window, 32 <= avail <= 64 after every consume, pos =
+// the unit bit position of `hi`'s MSB.  The decode loops only start a symbol at pos < clean_bits (= 8 * L, L = the unit's clean
+// length) and a symbol takes at most 31 bits, so pos <= 8L + 30 and T <= (8L + 94) / 32: every word the window takes lies within
+// L + 12 bytes, inside the unit's zero pad (>= kCleanPad bytes) -- the window never sees a byte of the next unit.  The queue ends
+// at word T + 4 at most, and the chunk loaded last is the one behind it: every load lies below 16 * ((T + 4) / 4 + 2) <= 4T + 48
+// <= L + 60 bytes behind the start of the unit.
+constexpr uint32_t kStreamReadBehind = 60;     // StreamWindow loads stay below clean_off + L + kStreamReadBehind (see above)
+// Predicated 16-byte load of the next chunk into `v` itself, read-only path, the L2 fetches the whole 128-byte line.  The
+// destination is tied to the registers that hold `v` across the loop: with a plain load the compiler picked other registers and
+// copied the result over right behind the load, which waits for it.
+__device__ __forceinline__ void ldg_stream(bool pred, uint4 &v, const uint4 *p) {
+  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %5, 0;\n\t@q ld.global.nc.L2::128B.v4.u32 {%0, %1, %2, %3}, [%4];\n\t}"
+               : "+r"(v.x), "+r"(v.y), "+r"(v.z), "+r"(v.w) : "l"(p), "r"((uint32_t)pred));
+}
+struct StreamWindow {
+  uint32_t hi, lo;
+  int avail;
+  uint32_t left;                   // valid words in the queue c0..c4
+  uint32_t c0, c1, c2, c3, c4;
+  uint4 nxt;
+  const uint4 *p;                  // the chunk behind `nxt`
+  __device__ __forceinline__ void clear() { left = 5; }            // a lane without a stream: top_up never loads
+  // window at unit bit position `pos`; `unit` = the unit's clean stream
+  __device__ __forceinline__ void init(const uint8_t *unit, uint32_t pos) {
+    const uint4 *q = reinterpret_cast<const uint4 *>(unit) + (pos >> 7);
+    const uint4 a = __ldg(q);
+    nxt = __ldg(q + 1);
+    p = q + 2;
+    hi = a.x; lo = a.y; avail = 64;
+    c0 = a.z; c1 = a.w; c2 = c3 = c4 = 0; left = 2;
+    for (uint32_t d = pos & 127u; d;) {            // skip to pos inside the chunk: at most 5 steps, once per window
+      const uint32_t e = min(d, 31u);
+      consume(e);
+      top_up();
+      d -= e;
+    }
+  }
+  __device__ __forceinline__ void consume(uint32_t e) {      // e & 31 = bits to drop, 0..31
+    hi = __funnelshift_l(lo, hi, e);
+    lo = __funnelshift_l(0u, lo, e);
+    avail -= (int)(e & 31u);
+    const bool need = avail < 32;                  // then 1 <= avail <= 31 and lo == 0
+    const uint32_t a = (uint32_t)avail & 31u;
+    hi |= (need ? c0 : 0u) >> a;
+    lo = need ? (c0 << ((32u - a) & 31u)) : lo;
+    avail += need ? 32 : 0;
+    c0 = need ? c1 : c0; c1 = need ? c2 : c1; c2 = need ? c3 : c2; c3 = need ? c4 : c3;
+    left -= need ? 1u : 0u;
+  }
+  __device__ __forceinline__ void top_up() {
+    const bool take = left <= 1;
+    if (take) {
+      const bool one = left != 0;
+      c0 = one ? c0 : nxt.x; c1 = one ? nxt.x : nxt.y; c2 = one ? nxt.y : nxt.z; c3 = one ? nxt.z : nxt.w; c4 = nxt.w;
+      left += 4;
+    }
+    ldg_stream(take, nxt, p);
+    p += take ? 1 : 0;
   }
 };
 
@@ -414,8 +488,8 @@ __device__ __forceinline__ uint32_t slow_symbol16(const HuffSlow *__restrict__ s
 // Decodes the symbols that START before `end` (absolute bit positions inside the unit) without producing coefficients: the
 // synchronisation only needs the state (pos, c, z) and `nb`, the number of completed blocks.  Branch-free apart from the loop
 // and the rare long-code path.
-template <class Src, class Lut, class Tbl>
-__device__ __forceinline__ void decode_span(const Src &src, BitWindow<Src> &win, const Lut &lut, const HuffSlow *__restrict__ slow,
+template <class Win, class Lut, class Tbl>
+__device__ __forceinline__ void decode_span(Win &win, const Lut &lut, const HuffSlow *__restrict__ slow,
                                             const Tbl &tbl, int bpm, uint32_t &pos, uint32_t end, int &c, int &z, uint32_t &nb) {
   uint32_t tb12 = tbl.load(c);                                // dc table offset | ac table offset << 16 (in LUT words)
   while (pos < end) {
@@ -427,7 +501,7 @@ __device__ __forceinline__ void decode_span(const Src &src, BitWindow<Src> &win,
     if (is_dc) e = lut.load((tb12 & 0xFFFFu) + (win.hi >> (32 - kDcLutBits)));
     if (__builtin_expect(e == 0, 0)) e = slow_symbol(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
     const uint32_t tb = e & 31u, adv = e >> 20;
-    win.consume(src, e);
+    win.consume(e);
     pos += tb;
     z += (int)adv;
     const bool endb = z >= 64;                                // block finished (EOB, 64th coefficient, or garbage overrun)
@@ -583,7 +657,7 @@ __global__ void __launch_bounds__(kSyncThreads) huff_sync_intra_kernel(HuffCtx c
   // ---- round 0
   if (sg.valid) {
     win.init(src, (uint32_t)threadIdx.x << lsw, 0);
-    decode_span(src, win, lut, slow, tbl, im.bpm, pos, sm.col_end[threadIdx.x], c, z, nb);
+    decode_span(win, lut, slow, tbl, im.bpm, pos, sm.col_end[threadIdx.x], c, z, nb);
     sm.exitst[threadIdx.x] = pack_state(pos, c, z);
     sm.cnt[threadIdx.x] = nb;
   }
@@ -595,7 +669,7 @@ __global__ void __launch_bounds__(kSyncThreads) huff_sync_intra_kernel(HuffCtx c
     } else {
       const uint32_t x = threadIdx.x + 1;
       nb = 0;
-      decode_span(src, win, lut, slow, tbl, im.bpm, pos, sm.col_end[x], c, z, nb);
+      decode_span(win, lut, slow, tbl, im.bpm, pos, sm.col_end[x], c, z, nb);
       const uint64_t ns = pack_state(pos, c, z);
       // The record is ALWAYS rewritten: a chain that merely converged inside this subsequence entered it in a different
       // state than the previous visitor; the chain that started further left is the better informed one.
@@ -627,6 +701,14 @@ __global__ void __launch_bounds__(kSyncThreads) huff_sync_intra_kernel(HuffCtx c
 // ([word][thread]: bank = thread, conflict free); the tables are shared by the CTA.
 constexpr int kTailThreads = 256;
 constexpr int kTailColWords = 36;          // 128-byte subsequence + 16 bytes of look-ahead
+// Bytes behind clean_off + L (L = a unit's clean length) that the Huffman passes may load: the sync-intra staging reads the
+// look-ahead columns (256 bytes) behind a subsequence that starts below L; a column of the walk spans the subsequence + 16
+// bytes; StreamWindow stays below kStreamReadBehind.  The clean buffer is allocated with this much minus kCleanPad of slack behind
+// the last unit (every unit has at least kCleanPad bytes of pad of its own).
+__host__ __device__ inline uint32_t clean_read_behind(int log2_sub) {
+  const uint32_t sub = 1u << (log2_sub - 3), staged = sub + (uint32_t)look_ahead_cols(log2_sub) * sub;
+  return staged > kStreamReadBehind ? staged : kStreamReadBehind;
+}
 struct ColSrc {
   uint32_t base;                           // shared-window address of column[0][threadIdx.x]
   __device__ __forceinline__ uint32_t load(uint32_t g) const { return lds_u32(base + g * (kTailThreads * 4u)); }
@@ -664,13 +746,13 @@ __device__ __forceinline__ void walk_chain(const HuffCtx &cx, const uint4 rec, i
       const uint32_t rel = pos - (jl << cx.log2_sub);
       BitWindow<ColSrc> win;
       win.init(src, rel >> 5, rel & 31u);
-      decode_span(src, win, SmemLut{smem_u32(s_lut)}, s_slow, SmemTbl<kTailThreads>{smem_u32(tblcol)}, im.bpm, pos, end, c, z, nb);
+      decode_span(win, SmemLut{smem_u32(s_lut)}, s_slow, SmemTbl<kTailThreads>{smem_u32(tblcol)}, im.bpm, pos, end, c, z, nb);
     } else {
       // another table set than the one this CTA keeps in shared memory (mixed batches), or an oversized subsequence: global path
       const GlobalSrc src{reinterpret_cast<const uint32_t *>(cx.clean + u.clean_off)};
       BitWindow<GlobalSrc> win;
       win.init(src, pos >> 5, pos & 31u);
-      decode_span(src, win, GlobalLut{cx.tables[im.table_set].lut}, cx.tables[im.table_set].slow, SmemTbl<kTailThreads>{smem_u32(tblcol)},
+      decode_span(win, GlobalLut{cx.tables[im.table_set].lut}, cx.tables[im.table_set].slow, SmemTbl<kTailThreads>{smem_u32(tblcol)},
                   im.bpm, pos, end, c, z, nb);
     }
     const uint64_t ns = pack_state(pos, c, z, nb, t);
@@ -744,42 +826,36 @@ __global__ void __launch_bounds__(1024) huff_scan_kernel(HuffCtx cx) {
 // H3: final pass -- every subsequence is decoded from its now-correct entry state and writes coefficients.
 //
 // A block belongs to the thread in whose subsequence it STARTS: a thread skips the tail of the block that is open at its
-// entry and runs past its own end until its last block is complete (the stream of the following subsequences is staged
-// too).  Every block therefore has exactly one writer, which assembles it in a private 128-byte shared-memory buffer
+// entry and runs past its own end until its last block is complete (its window simply reads on into the following
+// subsequences).  Every block therefore has exactly one writer, which assembles it in a private 128-byte shared-memory buffer
 // (word j of lane l at l * 32 + (j ^ l): conflict free for the per-symbol 16-bit scatter of all lanes to the same j and for the
 // flush) and the warp writes each finished block to HBM as ONE coalesced 128-byte line: no memset of the coefficient arena,
 // no 2-byte read-modify-write traffic, ~12x fewer store wavefronts than a per-symbol scatter.
 //
 // The loop is a chain of dependent fixed-latency instructions (its stalls are fixed-latency waits and short scoreboards):
-// throughput scales with resident warps.  The pass therefore runs its own block
-// shape -- kWriteThreads = 384 subsequences per CTA, 16-bit LUT entries (10 KB instead of 20), prologue scratch aliased with
-// the block buffers: 108 KB per CTA -> 2 CTAs = 24 warps per SM (was 2 x 8).
+// throughput scales with resident warps.  The pass therefore runs its own block shape -- kWriteThreads subsequences per CTA,
+// 16-bit LUT entries (10 KB instead of 20) and the stream read from global memory (StreamWindow), so that shared memory holds
+// only the tables and the block buffers: 10.1 KB + 128 B per thread.
 constexpr int kWriteThreads = 384;
+constexpr int kWriteCtasPerSm = 3;       // 3 x (58.1 KB + 1 KB reserved) of the 228 KB per SM
 struct WriteSmem {
-  uint16_t *lut; uint32_t *sw, *tbl, *blkbuf; uint8_t *zig; HuffSlow *slow; const uint8_t **colptr;
+  uint16_t *lut; uint32_t *tbl, *blkbuf; uint8_t *zig;
 };
-__host__ __device__ inline size_t write_sw_words(int log2_sub) { return (size_t)(kWriteThreads + look_ahead_cols(log2_sub)) << (log2_sub - 5); }
-__host__ __device__ inline size_t write_smem_bytes(int log2_sub) {
-  return kLutWords * 2 + write_sw_words(log2_sub) * 4 + 16 * 4 /*tbl*/ + 64 /*zig*/ + (size_t)kWriteThreads * 128;
-}
-__device__ __forceinline__ WriteSmem carve_write_smem(uint32_t *base, int log2_sub) {
+__host__ __device__ inline size_t write_smem_bytes() { return kLutWords * 2 + 16 * 4 /*tbl*/ + 64 /*zig*/ + (size_t)kWriteThreads * 128; }
+__device__ __forceinline__ WriteSmem carve_write_smem(uint32_t *base) {
   WriteSmem s;
   s.lut = reinterpret_cast<uint16_t *>(base);
-  s.sw = base + kLutWords / 2;
-  s.tbl = s.sw + write_sw_words(log2_sub);
+  s.tbl = base + kLutWords / 2;
   s.zig = reinterpret_cast<uint8_t *>(s.tbl + 16);
-  s.slow = nullptr;                                                          // the long-code tables stay in global memory (see below)
   s.blkbuf = reinterpret_cast<uint32_t *>(s.zig + 64);                       // 16-byte aligned: every size above is a multiple of 16
-  s.colptr = reinterpret_cast<const uint8_t **>(s.blkbuf);                  // prologue only, (kWriteThreads + 8) * 8 bytes
   return s;
 }
 
-__global__ void __launch_bounds__(kWriteThreads) huff_write_kernel(HuffCtx cx) {
+__global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_kernel(HuffCtx cx) {
   extern __shared__ __align__(16) uint32_t hsm[];
-  const WriteSmem sm = carve_write_smem(hsm, cx.log2_sub);
+  const WriteSmem sm = carve_write_smem(hsm);
   const JpegImage &im = cx.images[cx.wblock_image[blockIdx.x]];
-  const int lsw = cx.log2_sub - 5;
-  // ---- prologue: tables, per-thread subsequence geometry, cooperative staging of the stream
+  // ---- prologue: tables, per-thread subsequence geometry
   {
     const uint4 *src = reinterpret_cast<const uint4 *>(cx.tables[im.table_set].lut16);
     uint4 *dst = reinterpret_cast<uint4 *>(sm.lut);
@@ -793,7 +869,6 @@ __global__ void __launch_bounds__(kWriteThreads) huff_write_kernel(HuffCtx cx) {
     sg.valid = j < im.nsub;
     sg.ui = 0; sg.jl = 0; sg.nsub_eff = 0; sg.clean_bits = 0;
     sg.g = (int64_t)im.subseq_begin + j;
-    const uint8_t *ptr = nullptr;
     if (sg.valid) {
       sg.ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : find_unit_by_subseq(cx.units, im.unit_begin, im.unit_end, j);
       const JpegUnit &u = cx.units[sg.ui];
@@ -801,29 +876,11 @@ __global__ void __launch_bounds__(kWriteThreads) huff_write_kernel(HuffCtx cx) {
       sg.nsub_eff = (sg.clean_bits + (1u << cx.log2_sub) - 1) >> cx.log2_sub;
       sg.jl = (uint32_t)(j - u.first_subseq);
       sg.valid = sg.jl < sg.nsub_eff;
-      if (sg.valid) ptr = cx.clean + u.clean_off + ((size_t)sg.jl << (cx.log2_sub - 3));
     }
-    sm.colptr[threadIdx.x] = ptr;
-    const int la_cols = look_ahead_cols(cx.log2_sub);
-    if (threadIdx.x == kWriteThreads - 1)
-      for (int q = 1; q <= la_cols; q++) sm.colptr[kWriteThreads - 1 + q] = ptr ? ptr + ((size_t)q << (cx.log2_sub - 3)) : nullptr;
-    __syncthreads();
-    const int cpc = 1 << (cx.log2_sub - 7);                    // 16-byte chunks per column
-    for (int ch = threadIdx.x; ch < (kWriteThreads + la_cols) * cpc; ch += blockDim.x) {
-      const int col = ch / cpc, o = ch - col * cpc;
-      const uint8_t *p = sm.colptr[col];
-      if (p) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p) + o);
-        const uint32_t g = ((uint32_t)col << lsw) + 4u * o, x = (uint32_t)col & 31u;
-        sm.sw[(g + 0) ^ x] = v.x; sm.sw[(g + 1) ^ x] = v.y; sm.sw[(g + 2) ^ x] = v.z; sm.sw[(g + 3) ^ x] = v.w;
-      }
-    }
-    __syncthreads();                                           // colptr (aliased with the block buffers) is dead from here on
   }
   // long codes (~1 % of the symbols) are looked up in global memory (L1-resident, one load with the direct table): a shared-memory
   // copy cost 5.7 KB per CTA and made the compiler rebuild the generic address of the copy inside the symbol loop
   const HuffSlow *slow = cx.tables[im.table_set].slow;
-  const SmemSrc src{smem_u32(sm.sw), lsw};
   const uint32_t lane = threadIdx.x & 31u;
   // shared-window addresses (plain integers inside the loop, see lds_u32)
   const uint32_t a_lut = smem_u32(sm.lut), a_tbl = smem_u32(sm.tbl), a_zig = smem_u32(sm.zig);
@@ -849,18 +906,18 @@ __global__ void __launch_bounds__(kWriteThreads) huff_write_kernel(HuffCtx cx) {
     active = pos < end && blk0 < blk_limit;                  // pad bits behind the last block of a unit are not symbols
   }
   bool own = z == 0;                                          // a block starts exactly at the entry: it is ours
-  BitWindow<SmemSrc> win;
-  {
-    const uint32_t rel = active ? pos - (sg.jl << cx.log2_sub) : 0u;     // 0..31 bits into this thread's column
-    win.init(src, ((uint32_t)threadIdx.x << lsw) + (rel >> 5), rel & 31u);
-  }
+  StreamWindow win;
+  win.clear();
+  if (active) win.init(cx.clean + cx.units[sg.ui].clean_off, pos);
+  __syncthreads();                                            // the tables; the window's first loads are in flight meanwhile
   int16_t *coef = cx.coef + im.coef_off;
   int16_t *dcv = cx.dc + im.coef_off / 64;
   const int bpm = im.bpm;
   uint32_t tb12 = lds_u32(a_tbl + 4u * c);
-  while (__any_sync(0xffffffffu, active)) {
+  for (uint32_t it = 1; __any_sync(0xffffffffu, active); it++) {
     bool flush = false;
     const uint32_t blk = blk0 + nb;
+    if (it & 1u) win.top_up();                                // warp-uniform, see StreamWindow
     if (active) {
       const uint32_t e_ac = lds_u16(a_lut + 2u * ((tb12 >> 16) + (win.hi >> (32 - kAcLutBits))));
       const bool is_dc = z == 0;
@@ -883,7 +940,7 @@ __global__ void __launch_bounds__(kWriteThreads) huff_write_kernel(HuffCtx cx) {
           }
         }
       }
-      win.consume(src, e);
+      win.consume(e);
       pos += tb;
       z += (int)adv;
       const bool endb = z >= 64;                              // block finished (EOB, 64th coefficient, or garbage overrun)
@@ -1823,7 +1880,7 @@ struct dalib200JpegPlan {
   bool source_stable = false;               // JpegPlanSetSourceStable: page-locked sources are copied by the DMA engine directly
   int last_upload_direct = 0;
   std::vector<size_t> stage_off;            // offset of each sample's scan bytes inside the raw staging area
-  size_t raw_bytes = 0, clean_bytes = 0;
+  size_t raw_bytes = 0, clean_bytes = 0, clean_alloc = 0;   // clean_alloc = clean_bytes + the read slack (clean_read_behind)
   uint32_t nchunks = 0;
   int64_t total_subseq = 0, total_coefs = 0, total_plane_bytes = 0, total_quads = 0, total_items = 0;
   int total_blocks_sync = 0, total_blocks_write = 0;
@@ -2052,9 +2109,14 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   // subsequences per batch (a full H100 holds 132 x 2048 = 270k threads), between 32 and 256 bytes
   size_t total_len = 0;
   for (int i = 0; i < n; i++) total_len += lengths[i];
+  // DALIB200_JPEG_SUBSEQ_BYTES = 32 / 64 / 128 pins the size (rounded down to one of these), e.g. to test each size on small batches
   int log2_bytes = kMaxLog2Sub - 3;
-  if (const char *ev = getenv("DALIB200_JPEG_SUBSEQ_BYTES")) { int v = atoi(ev); log2_bytes = v >= 256 ? 8 : v >= 128 ? 7 : v >= 64 ? 6 : 5; }
-  while (log2_bytes > 5 && (total_len >> log2_bytes) < 200000) log2_bytes--;
+  if (const char *ev = getenv("DALIB200_JPEG_SUBSEQ_BYTES")) {
+    const int v = atoi(ev);
+    log2_bytes = v >= 128 ? 7 : v >= 64 ? 6 : 5;
+  } else {
+    while (log2_bytes > 5 && (total_len >> log2_bytes) < 200000) log2_bytes--;
+  }
   p->log2_sub = log2_bytes + 3;
   const size_t sub_bytes = (size_t)1 << log2_bytes;
   for (int i = 0; i < n; i++) {
@@ -2165,7 +2227,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       u.nsub_max = (int32_t)((u.raw_len + sub_bytes - 1) / sub_bytes);
       u.slot_base = mcu0 * bpm * 64;
       u.nslots = mcus * bpm * 64;
-      clean += Align(u.raw_len + 32, 16);
+      clean += Align(u.raw_len + kCleanPad, 16);
       chunks += (u.raw_len + kChunkBytes - 1) / kChunkBytes;
       local_sub += u.nsub_max;
       p->units.push_back(u);
@@ -2297,6 +2359,11 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   }
   DB_CHECK_ARG(raw < (1ull << 32) && clean < (1ull << 32), "decoders.image: batch of encoded data exceeds 4 GiB");
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
+  p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
+  for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
+    if ((size_t)u.clean_off + u.raw_len + clean_read_behind(p->log2_sub) > p->clean_alloc) {
+      SetLastError("decoders.image: internal error (clean stream read bound)"); return DALIB200_ERROR_INTERNAL;
+    }
   p->total_subseq = subseq; p->total_coefs = coefs; p->total_plane_bytes = planes;
   p->total_blocks_sync = sync_blocks; p->total_blocks_write = write_blocks;
   // ---- pack descriptors + raw scan bytes into pinned staging
@@ -2509,7 +2576,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   if (p->n == 0) return DALIB200_SUCCESS;
   DB_CHECK_ARG(p->d_stage && p->d_stage_cap >= p->desc_bytes + p->raw_bytes, "JpegLaunch: JpegUpload has not been called for this batch");
   int rc;
-  if ((rc = GrowDevice(p->d_clean, p->d_clean_cap, p->clean_bytes + 1024))) return rc;   // slack: the staging reads one column ahead
+  if ((rc = GrowDevice(p->d_clean, p->d_clean_cap, p->clean_alloc))) return rc;
   if ((rc = GrowDevice(p->d_chunk, p->d_chunk_cap, (size_t)p->nchunks + 1))) return rc;
   if ((rc = GrowDevice(p->d_unit_len, p->d_unit_cap, p->units.size() + 1))) return rc;
   {
@@ -2619,11 +2686,11 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   cx.clean = p->d_clean; cx.s_state = p->d_state; cx.s_n = p->d_n; cx.coef = p->d_coef; cx.dc = p->d_dc; cx.log2_sub = p->log2_sub;
   cx.status = p->d_status; cx.unit_nblk = p->d_unit_nblk;
   cx.chains[0] = p->d_chain1; cx.chains[1] = p->d_chain2; cx.chains[2] = p->d_chain3; cx.chain_count = p->d_chain_count;
-  const size_t hsmem = sync_smem_bytes(p->log2_sub, false), wsmem = write_smem_bytes(p->log2_sub);
+  const size_t hsmem = sync_smem_bytes(p->log2_sub, false), wsmem = write_smem_bytes();
   const size_t walk_smem = kLutWords * 4 + 4 * sizeof(HuffSlow) + (size_t)(kTailColWords + kMaxBlocksPerMcu) * kTailThreads * 4;
   if (!p->smem_opted) {
     DB_CUDA(cudaFuncSetAttribute(huff_sync_intra_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sync_smem_bytes(kMaxLog2Sub, false)));
-    DB_CUDA(cudaFuncSetAttribute(huff_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)write_smem_bytes(kMaxLog2Sub)));
+    DB_CUDA(cudaFuncSetAttribute(huff_write_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem));
     DB_CUDA(cudaFuncSetAttribute(huff_sync_walk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk_smem));
     int per_sm = 0;
     DB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, huff_sync_walk_kernel, kTailThreads, walk_smem));
