@@ -22,6 +22,10 @@
 // decoded speculatively and the exit states are then chained until they agree.
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): J (encoded bytes) + H*W*3 (decoded image).
+//
+// The plan also takes PNG streams (detected by their signature): png_plan.h walks their chunks at set-up, png.cu decodes them into
+// the same decode windows on a stream of its own, and the post pass below serves both formats.  A PNG sample has no units,
+// subsequences or MCUs, so every kernel of this file skips it.
 #include "common.cuh"
 #include <algorithm>
 #include <cstring>
@@ -1656,6 +1660,10 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 // progressive streams: planner + launch interface of jpeg_prog.cu (included here, behind the kernels, so that their line tables stay put)
 #include "jpeg_prog.h"
 #include "jpeg_prog_plan.h"
+// EXIF orientation (shared with the PNG planner); PNG streams: planner + launch interface of png.cu
+#include "exif.h"
+#include "png.h"
+#include "png_plan.h"
 namespace {
 
 struct ParsedJpeg {
@@ -1663,6 +1671,7 @@ struct ParsedJpeg {
   int cid[4] = {0}, hs[4] = {0}, vs[4] = {0}, tq[4] = {0};
   int hmax = 0, vmax = 0;
   bool progressive = false, jfif = false;
+  bool png = false;           // a PNG stream (png_plan.h): width / height / ncomp / orientation / scan range only
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
   HostHuff dc[4], ac[4];
@@ -1677,26 +1686,6 @@ const uint8_t kZigzag[64] = {
   58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
 
 inline int rd16(const uint8_t *p) { return (p[0] << 8) | p[1]; }
-
-int ParseExifOrientation(const uint8_t *p, int len) {
-  if (len < 8) return 1;
-  bool le;
-  if (p[0] == 'I' && p[1] == 'I') le = true; else if (p[0] == 'M' && p[1] == 'M') le = false; else return 1;
-  auto r16 = [&](unsigned o) { return le ? (p[o] | (p[o + 1] << 8)) : ((p[o] << 8) | p[o + 1]); };
-  auto r32 = [&](unsigned o) { return le ? (unsigned)(p[o] | (p[o + 1] << 8) | (p[o + 2] << 16) | ((unsigned)p[o + 3] << 24))
-                                         : (((unsigned)p[o] << 24) | (p[o + 1] << 16) | (p[o + 2] << 8) | p[o + 3]); };
-  const uint64_t ulen = (uint64_t)len;                      // 64-bit offsets: a crafted IFD offset must not wrap the bound checks
-  const uint64_t ifd = r32(4);
-  if (ifd + 2 > ulen) return 1;
-  int n = r16((unsigned)ifd);
-  for (int i = 0; i < n; i++) {
-    const uint64_t e64 = ifd + 2 + 12ull * (uint64_t)i;
-    if (e64 + 12 > ulen) return 1;
-    const unsigned e = (unsigned)e64;
-    if (r16(e) == 0x0112) { int v = r16(e + 8); return (v >= 1 && v <= 8) ? v : 1; }
-  }
-  return 1;
-}
 
 // T.81 Annex B marker walk up to and including SOS.  Returns a DALIB200 status.
 int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
@@ -1781,6 +1770,22 @@ int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
   if (!got_sof) { SetLastError("JPEG: no frame header found"); return DALIB200_ERROR_BAD_DATA; }
   if (j.width == 0 || j.height == 0) { SetLastError("JPEG: zero image size"); return DALIB200_ERROR_BAD_DATA; }
   if (need_scan && !j.scan_begin) { SetLastError("JPEG: no scan found"); return DALIB200_ERROR_BAD_DATA; }
+  return DALIB200_SUCCESS;
+}
+
+// PNG stream (png_plan.h): fills the fields of `j` the plan reads for every sample (size, components, orientation, staged byte
+// range); `im` / `chunks`, when given, receive the device descriptors of batch image `image`.  Returns a DALIB200 status.
+int ParsePng(const uint8_t *p, size_t n, ParsedJpeg &j, PngImage *im, std::vector<PngChunk> *chunks, int image) {
+  PngImage tmp;
+  std::vector<PngChunk> tmpc;
+  PngInfo info;
+  std::string err;
+  const int rc = PlanPng(p, n, image, im ? im : &tmp, chunks ? *chunks : tmpc, &info, &err);
+  if (rc) { SetLastError("%s", err.c_str()); return rc; }
+  j.png = true;
+  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
+  j.hs[0] = j.vs[0] = 1;
+  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
   return DALIB200_SUCCESS;
 }
 
@@ -1917,6 +1922,15 @@ struct dalib200JpegPlan {
   cudaEvent_t prog_uploaded = nullptr, prog_fork = nullptr, prog_join = nullptr;
   cudaStream_t prog_stream = nullptr;      // the scans are serial chains on one warp each: they run beside the baseline entropy stage
   bool prog_pending = false;
+  // PNG samples: decoded by png.cu on a stream of their own into the same decode windows; the post pass is shared
+  std::vector<dalib200::PngImage> png_images;
+  std::vector<dalib200::PngChunk> png_chunks;
+  int64_t png_scan_bytes = 0;
+  uint8_t *d_png_scan = nullptr; size_t d_png_scan_cap = 0;   // filtered scanlines (grow only)
+  dalib200::DescArena png_arena;
+  cudaEvent_t png_uploaded = nullptr, png_fork = nullptr, png_join = nullptr;
+  cudaStream_t png_stream = nullptr;
+  bool png_pending = false;
 };
 
 namespace {
@@ -1964,6 +1978,10 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
+    if (j.png) {                   // decoded by png.cu: no IDCT / colour work
+      p->first_work[i] = work; p->first_fused[i] = fused; p->first_quad[i] = quads; p->first_item[i] = items;
+      continue;
+    }
     im.fast_color = j.ncomp == 3 && im.color == kColorYCbCr && (im.out_type == DALIB200_RGB || im.out_type == DALIB200_BGR) &&
                     ((j.hmax == 2 && j.vmax <= 2) || (j.hmax == 1 && j.vmax <= 2));
     if (im.fast_color && p->fancy && j.hmax == 2 && j.vmax == 2 && (j.width + 1) / 2 > 2) im.fast_color = 2;    // idct_color_420
@@ -1985,6 +2003,63 @@ void BuildWorkLists(dalib200JpegPlan *p) {
   p->total_work = work; p->total_fused = fused; p->total_post_px = post_px; p->post_bytes = post_bytes; p->total_quads = quads;
   p->total_items = items;
 }
+
+// Output geometry of sample i: orientation, region of interest, decode window, post pass.  Returns a DALIB200 status.
+int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const ParsedJpeg &j, JpegImage &im) {
+  const int orient = p->adjust_orientation ? j.orientation : 1;
+  const int W = j.width, H = j.height;
+  const int OW = orient >= 5 ? H : W, OH = orient >= 5 ? W : H;          // oriented image size
+  int rx0 = 0, ry0 = 0, rx1 = OW, ry1 = OH;                              // region of interest, oriented coordinates
+  if (rois && rois[i].use_roi) {
+    rx0 = rois[i].x0; ry0 = rois[i].y0; rx1 = rois[i].x1; ry1 = rois[i].y1;
+    if (!(0 <= rx0 && rx0 < rx1 && rx1 <= OW && 0 <= ry0 && ry0 < ry1 && ry1 <= OH)) {
+      SetLastError("decoders.image: sample %d: ROI [%d, %d) x [%d, %d) must be non-empty and fit within the image bounds (%d x %d)",
+                   i, rx0, rx1, ry0, ry1, OW, OH);
+      return DALIB200_ERROR_INVALID_ARGUMENT;
+    }
+  }
+  // source rectangle of the region (the EXIF transforms map rectangles to rectangles)
+  int sx0, sx1, sy0, sy1;
+  {
+    auto src_of = [&](int fy, int fx, int &sy, int &sx) {
+      switch (orient) {
+        case 2: sy = fy; sx = W - 1 - fx; break;
+        case 3: sy = H - 1 - fy; sx = W - 1 - fx; break;
+        case 4: sy = H - 1 - fy; sx = fx; break;
+        case 5: sy = fx; sx = fy; break;
+        case 6: sy = H - 1 - fx; sx = fy; break;
+        case 7: sy = H - 1 - fx; sx = W - 1 - fy; break;
+        case 8: sy = fx; sx = W - 1 - fy; break;
+        default: sy = fy; sx = fx; break;
+      }
+    };
+    int ay, ax, by_, bx_;
+    src_of(ry0, rx0, ay, ax); src_of(ry1 - 1, rx1 - 1, by_, bx_);
+    sy0 = std::min(ay, by_); sy1 = std::max(ay, by_) + 1; sx0 = std::min(ax, bx_); sx1 = std::max(ax, bx_) + 1;
+  }
+  const int output_type = p->output_type;
+  const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
+  p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
+  if (j.png) {                   // any window: png_color produces pixels one by one
+    im.win_x0 = sx0; im.win_w = sx1 - sx0;
+  } else {
+    im.win_x0 = sx0 & ~7; im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0;
+  }
+  im.win_y0 = sy0; im.win_h = sy1 - sy0;
+  JpegGeo &ge = p->geo[i];
+  ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
+  ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
+  // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
+  ge.planar_ok = !j.png && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
+                 output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
+  const bool planes_only = rois && rois[i].planes_only;
+  if (planes_only && !ge.planar_ok) {
+    SetLastError("decoders.image: sample %d: planes_only needs a 3-component 4:2:0 YCbCr stream without orientation, RGB u8 output", i);
+    return DALIB200_ERROR_UNSUPPORTED;
+  }
+  p->planes_only[i] = planes_only;
+  return DALIB200_SUCCESS;
+}
 }  // namespace
 
 extern "C" {
@@ -1992,7 +2067,7 @@ extern "C" {
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info) try {
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
-  int rc = ParseHeaders(data, len, j, false);
+  int rc = IsPngStream(data, len) ? ParsePng(data, len, j, nullptr, nullptr, 0) : ParseHeaders(data, len, j, false);
   if (rc) return rc;
   FillInfo(j, info);
   return DALIB200_SUCCESS;
@@ -2006,7 +2081,10 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
       cudaEventCreateWithFlags(&p->img_uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->prog_uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->prog_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->prog_join, cudaEventDisableTiming) != cudaSuccess) {
+      cudaEventCreateWithFlags(&p->prog_join, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->png_uploaded, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->png_fork, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->png_join, cudaEventDisableTiming) != cudaSuccess) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2022,6 +2100,12 @@ int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (p->prog_fork) cudaEventDestroy(p->prog_fork);
   if (p->prog_join) cudaEventDestroy(p->prog_join);
   p->prog_arena.Free();
+  if (p->png_stream) { cudaStreamSynchronize(p->png_stream); cudaStreamDestroy(p->png_stream); }
+  if (p->png_uploaded) { cudaEventSynchronize(p->png_uploaded); cudaEventDestroy(p->png_uploaded); }
+  if (p->png_fork) cudaEventDestroy(p->png_fork);
+  if (p->png_join) cudaEventDestroy(p->png_join);
+  p->png_arena.Free();
+  if (p->d_png_scan) cudaFree(p->d_png_scan);
   if (p->h_stage) cudaFreeHost(p->h_stage);
   if (p->h_images) cudaFreeHost(p->h_images);
   if (p->h_status) cudaFreeHost(p->h_status);
@@ -2100,6 +2184,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->first_item.assign(n, 0);
   p->prog_images.clear(); p->prog_scans.clear(); p->prog_huff.clear(); p->prog_wave_begin.clear(); p->prog_first_blk.clear();
   p->prog_total_blocks = 0;
+  p->png_images.clear(); p->png_chunks.clear();
+  int64_t png_scan = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2122,6 +2208,27 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   for (int i = 0; i < n; i++) {
     ParsedJpeg &j = p->parsed[i];
     DB_CHECK_ARG(streams[i] && lengths[i] > 0, "decoders.image: sample %d is empty", i);
+    if (IsPngStream(streams[i], lengths[i])) {
+      // PNG: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu decodes its IDAT run (the staged range)
+      // into the decode window, and the post pass behind it is shared
+      dalib200::PngImage pim;
+      int rc = ParsePng(streams[i], lengths[i], j, &pim, &p->png_chunks, (int)p->png_images.size());
+      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
+      JpegImage &im = p->images[i];
+      memset(&im, 0, sizeof(im));
+      im.width = j.width; im.height = j.height; im.out_type = output_type;
+      im.unit_begin = im.unit_end = (int)p->units.size();
+      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
+      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
+      pim.sample = i;
+      pim.raw_off = (int64_t)raw;
+      pim.scan_off = png_scan;
+      png_scan += (int64_t)Align((size_t)pim.scan_bytes, 16);
+      p->png_images.push_back(pim);
+      p->src_ptr.push_back(streams[i] + j.scan_begin);
+      raw += Align(j.scan_end - j.scan_begin, 16);
+      continue;
+    }
     int rc = ParseHeaders(streams[i], lengths[i], j, true);
     if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
     auto unsupported = [&](const char *what) { SetLastError("decoders.image: sample %d: %s", i, what); return DALIB200_ERROR_UNSUPPORTED; };
@@ -2293,54 +2400,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       im.plane_off[c] = planes;
       planes += Align((size_t)im.plane_w[c] * im.plane_h[c], 16);
     }
-    // ---- output geometry: orientation, region of interest, decode window, post pass
-    const int orient = p->adjust_orientation ? j.orientation : 1;
-    const int W = j.width, H = j.height;
-    const int OW = orient >= 5 ? H : W, OH = orient >= 5 ? W : H;          // oriented image size
-    int rx0 = 0, ry0 = 0, rx1 = OW, ry1 = OH;                              // region of interest, oriented coordinates
-    if (rois && rois[i].use_roi) {
-      rx0 = rois[i].x0; ry0 = rois[i].y0; rx1 = rois[i].x1; ry1 = rois[i].y1;
-      if (!(0 <= rx0 && rx0 < rx1 && rx1 <= OW && 0 <= ry0 && ry0 < ry1 && ry1 <= OH)) {
-        SetLastError("decoders.image: sample %d: ROI [%d, %d) x [%d, %d) must be non-empty and fit within the image bounds (%d x %d)",
-                     i, rx0, rx1, ry0, ry1, OW, OH);
-        return DALIB200_ERROR_INVALID_ARGUMENT;
-      }
-    }
-    // source rectangle of the region (the EXIF transforms map rectangles to rectangles)
-    int sx0, sx1, sy0, sy1;
-    {
-      auto src_of = [&](int fy, int fx, int &sy, int &sx) {
-        switch (orient) {
-          case 2: sy = fy; sx = W - 1 - fx; break;
-          case 3: sy = H - 1 - fy; sx = W - 1 - fx; break;
-          case 4: sy = H - 1 - fy; sx = fx; break;
-          case 5: sy = fx; sx = fy; break;
-          case 6: sy = H - 1 - fx; sx = fy; break;
-          case 7: sy = H - 1 - fx; sx = W - 1 - fy; break;
-          case 8: sy = fx; sx = W - 1 - fy; break;
-          default: sy = fy; sx = fx; break;
-        }
-      };
-      int ay, ax, by_, bx_;
-      src_of(ry0, rx0, ay, ax); src_of(ry1 - 1, rx1 - 1, by_, bx_);
-      sy0 = std::min(ay, by_); sy1 = std::max(ay, by_) + 1; sx0 = std::min(ax, bx_); sx1 = std::max(ax, bx_) + 1;
-    }
-    const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
-    p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
-    im.win_x0 = sx0 & ~7; im.win_y0 = sy0;
-    im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0; im.win_h = sy1 - sy0;
-    JpegGeo &ge = p->geo[i];
-    ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
-    ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
-    // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
-    ge.planar_ok = j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
-                   output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
-    const bool planes_only = rois && rois[i].planes_only;
-    if (planes_only && !ge.planar_ok) {
-      SetLastError("decoders.image: sample %d: planes_only needs a 3-component 4:2:0 YCbCr stream without orientation, RGB u8 output", i);
-      return DALIB200_ERROR_UNSUPPORTED;
-    }
-    p->planes_only[i] = planes_only;
+    if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
     // MCUs the IDCT has to produce: the window plus the neighbours the (fancy) chroma upsampling reads
     {
       const int mw = 8 * j.hmax, mh = 8 * j.vmax, ex = 2 * j.hmax, ey = 2 * j.vmax;
@@ -2359,6 +2419,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   }
   DB_CHECK_ARG(raw < (1ull << 32) && clean < (1ull << 32), "decoders.image: batch of encoded data exceeds 4 GiB");
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
+  p->png_scan_bytes = png_scan;
   p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
   for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
     if ((size_t)u.clean_off + u.raw_len + clean_read_behind(p->log2_sub) > p->clean_alloc) {
@@ -2671,6 +2732,42 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     if ((rc = LaunchProgressive(a, ps))) return rc;
     DB_CUDA(cudaEventRecord(p->prog_join, ps));
   }
+  if (!p->png_images.empty()) {
+    // PNG samples (png.cu): the inflate is a serial chain per image, so the stage is forked onto a stream of its own behind the upload
+    // and the status clear, runs beside the JPEG samples' kernels and is joined in front of the post pass.  It writes only the PNG
+    // samples' decode windows, its scanline scratch and their status words.
+    using namespace dalib200;
+    if ((rc = GrowDevice(p->d_png_scan, p->d_png_scan_cap, (size_t)p->png_scan_bytes + 16))) return rc;
+    if (!p->png_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->png_stream, cudaStreamNonBlocking));
+    cudaStream_t ps = p->png_stream;
+    DB_CUDA(cudaEventRecord(p->png_fork, s));
+    DB_CUDA(cudaStreamWaitEvent(ps, p->png_fork, 0));
+    if (p->png_pending) { DB_CUDA(cudaEventSynchronize(p->png_uploaded)); p->png_pending = false; }
+    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
+    int64_t px = 0;
+    for (PngImage &pi : p->png_images) {
+      const JpegImage &im = hi[pi.sample];
+      pi.out = im.out; pi.out_type = im.out_type;
+      pi.win_x0 = im.win_x0; pi.win_y0 = im.win_y0; pi.win_w = im.win_w; pi.win_h = im.win_h;
+      pi.first_px = px;
+      px += (int64_t)im.win_w * im.win_h;
+    }
+    const size_t npi = p->png_images.size(), nch = p->png_chunks.size();
+    const size_t o_chunk = Align(sizeof(PngImage) * npi, 16), pbytes = Align(o_chunk + sizeof(PngChunk) * nch, 16);
+    if ((rc = p->png_arena.Reserve(pbytes))) return rc;
+    memcpy(p->png_arena.host, p->png_images.data(), sizeof(PngImage) * npi);
+    memcpy(p->png_arena.host + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
+    if ((rc = p->png_arena.Upload(pbytes, ps))) return rc;
+    DB_CUDA(cudaEventRecord(p->png_uploaded, ps));
+    p->png_pending = true;
+    PngLaunch a;
+    a.d_images = reinterpret_cast<const PngImage *>(p->png_arena.dev); a.nimages = (int)npi;
+    a.d_chunks = reinterpret_cast<const PngChunk *>(p->png_arena.dev + o_chunk); a.nchunks = (int)nch;
+    a.total_px = px;
+    a.d_raw = d_raw; a.d_scan = p->d_png_scan; a.d_status = p->d_status;
+    if ((rc = LaunchPng(a, ps))) return rc;
+    DB_CUDA(cudaEventRecord(p->png_join, ps));
+  }
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
   if (any_units) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
@@ -2741,6 +2838,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
       CountLaunch();
     }
   }
+  if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png_join, 0));       // the PNG samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

@@ -52,28 +52,30 @@ int dalib200ProfilingEnable(int on);
 int dalib200ProfilingCollect(char *names, int name_stride, float *ms, int max, int *count);
 
 /* ------------------------------------------------------------------------------------------------
- * JPEG decode (Huffman + dequant + IDCT + chroma upsampling + YCbCr->RGB): baseline sequential (self-synchronising parallel entropy
- * decode) and progressive (SOF2: scans in dependency waves, one warp per scan; spectral selection + successive approximation).
+ * Image decode.  JPEG (Huffman + dequant + IDCT + chroma upsampling + YCbCr->RGB): baseline sequential (self-synchronising parallel
+ * entropy decode) and progressive (SOF2: scans in dependency waves, one warp per scan; spectral selection + successive approximation).
+ * PNG (detected by its signature; IDAT CRCs, inflate + unfilter, colour conversion, bit-exact with cv2.imdecode).  Both formats may be
+ * mixed in one batch of a plan.
  * Replaces: imgcodec::ImageDecoder<MixedBackend>::RunImplImpl -> nvimgcodecDecoderDecode
  *           (dali/operators/imgcodec/image_decoder.h:613-882) and ParseSample (:473-499).
- * Host work: marker/table parse only.  Device work: everything arithmetic. */
+ * Host work: marker / table / chunk-header parse only.  Device work: everything arithmetic. */
 typedef struct dalib200JpegPlan dalib200JpegPlan;
 
 typedef struct {
   int32_t width, height;        /* decoded image size */
-  int32_t components;           /* 1 or 3 */
+  int32_t components;           /* JPEG: 1, 3 or 4; PNG: channels of the file (palette: 3) */
   int32_t subsampling;          /* (hmax<<4)|vmax of the luma sampling factors, e.g. 0x22 = 4:2:0 */
   int32_t restart_interval;
   int32_t orientation;          /* EXIF orientation, 1 = none */
 } dalib200JpegInfo;
 
-/* header-only parse: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
+/* header-only parse of a JPEG or PNG stream: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info);
 
 int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch);
 int dalib200JpegPlanDestroy(dalib200JpegPlan *plan);
 /* Parses n encoded streams (host pointers) and builds the per-sample descriptors.  The streams are BORROWED until
- * dalib200JpegUpload returns (it packs the entropy-coded segments into the plan's pinned staging buffer, in groups, and
+ * dalib200JpegUpload returns (it packs the entropy-coded segments / IDAT runs into the plan's pinned staging buffer, in groups, and
  * issues the H2D copy of each group as soon as it is packed).  Output shapes via ...GetInfo().
  * fancy_upsampling != 0 selects libjpeg "fancy" (triangle) chroma upsampling -- the reference CPU
  * backend's behaviour; 0 = box replication. */
@@ -86,13 +88,14 @@ int dalib200JpegPlanGetInfo(const dalib200JpegPlan *plan, int sample, dalib200Jp
  *   dtype                DALIB200_UINT8 | DALIB200_FLOAT     (ConvertSatNorm: u8 * (1 / 255), convert.h:118-128)
  *   adjust_orientation   apply the EXIF orientation (image_decoder.h:211,678-679,806)
  *   rois[i]              region of interest of sample i in OUTPUT (oriented) pixel coordinates, [x0, x1) x [y0, y1)
- *                        (imgcodec.h:26-44, image_decoder.h:681-716); only the MCUs under the region are transformed.
+ *                        (imgcodec.h:26-44, image_decoder.h:681-716); only the MCUs (PNG: pixels) under the region are
+ *                        transformed.
  * The result equals the full decode followed by orientation, crop and conversion, bit for bit. */
 typedef struct { int32_t output_type, fancy_upsampling, dtype, adjust_orientation; } dalib200JpegParams;
 typedef struct {
   int32_t use_roi, x0, y0, x1, y1;
   int32_t planes_only;        /* skip upsampling + colour conversion for this sample: the caller reads the component planes
-                                 (dalib200JpegPlanGetPlanes -> dalib200ResampleLaunchPlanar); 4:2:0 YCbCr streams only */
+                                 (dalib200JpegPlanGetPlanes -> dalib200ResampleLaunchPlanar); 4:2:0 YCbCr JPEG streams only */
 } dalib200JpegRoi;
 /* The decoder's planar output of a sample: 8-bit planes, Cb / Cr at half resolution (4:2:0), rows padded to a multiple of 16 bytes.
  * Only the MCUs under the sample's region of interest hold data.  crop_x / crop_y: filled by the caller (window the resampler treats

@@ -1,7 +1,7 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize and progressive JPEG kernels are EXECUTED on the host -- their bodies are single
-// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h), so a launch is a loop over blocks and threads around
+// of the 3-D resize, progressive JPEG and PNG kernels are EXECUTED on the host -- their bodies are single
+// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h), so a launch is a loop over blocks and threads around
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
 // end to end without a GPU -- descriptor upload, temporaries, stage order, grid-stride loops, wave ranges, arena offsets -- and
 // tests/test_launch_emul_cpu.py compares what lands in "device" memory with the oracle.
@@ -16,6 +16,7 @@
 #include "../../include/dali_b200.h"
 #include "../../dali_b200/csrc/resample3d_core.h"
 #include "../../dali_b200/csrc/jpeg_prog_core.h"
+#include "../../dali_b200/csrc/png_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -65,10 +66,10 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[3];
+static long g_emulated[6];
 long emul_launch_count(int which) { return g_emulated[which]; }
 
-// kernels of dali_b200/csrc/resample3d.cu and jpeg_prog.cu, thread by thread
+// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu and png.cu, thread by thread
 static void run_resample3d_pass(Dim3 g, Dim3 b, void **args) {
   const R3Pass *passes = *static_cast<const R3Pass **>(args[0]);
   const int32_t *tab = *static_cast<const int32_t **>(args[1]);
@@ -114,6 +115,51 @@ static void run_prog_dc(Dim3 g, Dim3 b, void **args) {
       }
 }
 
+static void run_png_crc(Dim3 g, Dim3 b, void **args) {
+  const PngChunk *chunks = *static_cast<const PngChunk **>(args[0]);
+  const int nchunks = *static_cast<int *>(args[1]);
+  const PngImage *images = *static_cast<const PngImage **>(args[2]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[3]);
+  int32_t *status = *static_cast<int32_t **>(args[4]);
+  uint32_t table[256];
+  for (uint32_t i = 0; i < 256; i++) table[i] = png_crc_table_entry(i);
+  for (int k = 0; k < (int)(g.x * b.x) && k < nchunks; k++) {
+    const PngImage &im = images[chunks[k].image];
+    if (!png_chunk_crc_ok(raw + im.raw_off + chunks[k].off - 4, chunks[k].len, table)) status[im.sample] = 1;
+  }
+}
+static void run_png_inflate(Dim3 g, Dim3, void **args) {
+  const PngImage *images = *static_cast<const PngImage **>(args[0]);
+  const PngChunk *chunks = *static_cast<const PngChunk **>(args[1]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[2]);
+  uint8_t *scan = *static_cast<uint8_t **>(args[3]);
+  int32_t *status = *static_cast<int32_t **>(args[4]);
+  PngWork *w = new PngWork;
+  for (int bx = (int)g.x - 1; bx >= 0; bx--) {             // one working thread per block, blocks in no particular order
+    const PngImage &im = images[bx];
+    if (status[im.sample]) continue;
+    if (png_inflate_unfilter(im, chunks, raw, scan + im.scan_off, *w)) status[im.sample] = 1;
+  }
+  delete w;
+}
+static void run_png_color(Dim3 g, Dim3 b, void **args) {
+  const PngImage *images = *static_cast<const PngImage **>(args[0]);
+  const int nimages = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  const uint8_t *scan = *static_cast<const uint8_t **>(args[3]);
+  const int64_t step = (int64_t)g.x * b.x;
+  for (unsigned bx = 0; bx < g.x; bx++)
+    for (unsigned tx = 0; tx < b.x; tx++)
+      for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
+        int lo = 0, hi = nimages - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
+        const PngImage &im = images[lo];
+        const int64_t lp = e - im.first_px;
+        const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
+        png_pixel(im, scan + im.scan_off, lx, ly);
+      }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -121,6 +167,9 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_r3 = !strcmp(name, "_ZN8dalib20022resample3d_pass_kernelEPKNS_6R3PassEPKii");
   const bool is_scan = !strcmp(name, "_ZN8dalib20016prog_scan_kernelEPKNS_8ProgScanEiPKNS_9ProgImageEPKNS_8ProgHuffEPKhPsPi");
   const bool is_dc = !strcmp(name, "_ZN8dalib20014prog_dc_kernelEPKNS_9ProgImageEPKlilPKsPsPi");
+  const bool is_png_crc = !strcmp(name, "_ZN8dalib20014png_crc_kernelEPKNS_8PngChunkEiPKNS_8PngImageEPKhPi");
+  const bool is_png_inflate = !strcmp(name, "_ZN8dalib20018png_inflate_kernelEPKNS_8PngImageEPKNS_8PngChunkEPKhPhPi");
+  const bool is_png_color = !strcmp(name, "_ZN8dalib20016png_color_kernelEPKNS_8PngImageEilPKh");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -128,6 +177,9 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   if (is_r3) { run_resample3d_pass(grid, block, args); g_emulated[0]++; }
   else if (is_scan) { run_prog_scan(grid, block, args); g_emulated[1]++; }
   else if (is_dc) { run_prog_dc(grid, block, args); g_emulated[2]++; }
+  else if (is_png_crc) { run_png_crc(grid, block, args); g_emulated[3]++; }
+  else if (is_png_inflate) { run_png_inflate(grid, block, args); g_emulated[4]++; }
+  else if (is_png_color) { run_png_color(grid, block, args); g_emulated[5]++; }
   return 0;
 }
 }  // extern "C"

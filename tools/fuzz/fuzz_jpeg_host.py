@@ -19,6 +19,10 @@ seeds += [synth(33, 47, prog=True), synth(40, 24, rst=2, prog=True), synth(17, 1
 # 4-component streams (CMYK, YCCK, no Adobe marker; baseline and progressive; 4:4:4 and subsampled), written by Pillow
 cmyk = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "tests", "golden", "jpeg_cmyk.npz"))
 seeds += [bytearray(cmyk[f"enc_{k}"].tobytes()) for k in range(len(cmyk.files) // 4) if str(cmyk[f"name_{k}"]).endswith("61x77")]
+# PNG streams (every colour type, Adam7, split IDAT runs, eXIf): the chunk walk of the planner
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "tests"))
+import png_streams
+seeds += [bytearray(s) for _, s in png_streams.corpus()[::6]]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()

@@ -14,7 +14,8 @@ F="-gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17 -Xcompiler -fPIC,-fsa
 $NVCC $F -c "$ROOT/dali_b200/csrc/jpeg.cu" -o "$OUT/jpeg.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/common.cu" -o "$OUT/common.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/jpeg_prog.cu" -o "$OUT/jpeg_prog.o"
-$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
+$NVCC $F -c "$ROOT/dali_b200/csrc/png.cu" -o "$OUT/png.o"
+$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
 gcc -shared -fPIC -O1 -o "$OUT/cuda_stub.so" "$HERE/cuda_stub.c"
 # the progressive scan decoder itself (the body of prog_scan_kernel, compiled for the host by tools/emul) under ASAN + UBSAN on mutated
 # progressive streams: garbage Huffman codes, runs past the band, truncated scans, markers inside the data must stay inside the arena
