@@ -23,9 +23,9 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): J (encoded bytes) + H*W*3 (decoded image).
 //
-// The plan also takes PNG streams (detected by their signature): png_plan.h walks their chunks at set-up, png.cu decodes them into
-// the same decode windows on a stream of its own, and the post pass below serves both formats.  A PNG sample has no units,
-// subsequences or MCUs, so every kernel of this file skips it.
+// The plan also takes PNG and TIFF streams (detected by their signatures): png_plan.h walks their chunks and tiff_plan.h their IFD at
+// set-up, png.cu and tiff.cu decode them into the same decode windows on streams of their own, and the post pass below serves every
+// format.  A PNG or TIFF sample has no units, subsequences or MCUs, so every kernel of this file skips it.
 #include "common.cuh"
 #include <algorithm>
 #include <cstring>
@@ -1660,10 +1660,12 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 // progressive streams: planner + launch interface of jpeg_prog.cu (included here, behind the kernels, so that their line tables stay put)
 #include "jpeg_prog.h"
 #include "jpeg_prog_plan.h"
-// EXIF orientation (shared with the PNG planner); PNG streams: planner + launch interface of png.cu
+// EXIF orientation (shared with the PNG planner); PNG and TIFF streams: planners + launch interfaces of png.cu and tiff.cu
 #include "exif.h"
 #include "png.h"
 #include "png_plan.h"
+#include "tiff.h"
+#include "tiff_plan.h"
 namespace {
 
 struct ParsedJpeg {
@@ -1672,6 +1674,7 @@ struct ParsedJpeg {
   int hmax = 0, vmax = 0;
   bool progressive = false, jfif = false;
   bool png = false;           // a PNG stream (png_plan.h): width / height / ncomp / orientation / scan range only
+  bool tiff = false;          // a TIFF stream (tiff_plan.h): the same fields
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
   HostHuff dc[4], ac[4];
@@ -1783,6 +1786,23 @@ int ParsePng(const uint8_t *p, size_t n, ParsedJpeg &j, PngImage *im, std::vecto
   const int rc = PlanPng(p, n, image, im ? im : &tmp, chunks ? *chunks : tmpc, &info, &err);
   if (rc) { SetLastError("%s", err.c_str()); return rc; }
   j.png = true;
+  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
+  j.hs[0] = j.vs[0] = 1;
+  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
+  return DALIB200_SUCCESS;
+}
+
+// TIFF stream (tiff_plan.h), as ParsePng; `dec_base` / `dec_bytes`: the image's range of the decoded-segment scratch
+int ParseTiff(const uint8_t *p, size_t n, ParsedJpeg &j, TiffImage *im, std::vector<TiffSeg> *segs, int image, int64_t dec_base,
+              int64_t *dec_bytes) {
+  TiffImage tmp;
+  std::vector<TiffSeg> tmps;
+  TiffInfo info;
+  int64_t tmpd;
+  std::string err;
+  const int rc = PlanTiff(p, n, image, im ? im : &tmp, segs ? *segs : tmps, dec_base, dec_bytes ? dec_bytes : &tmpd, &info, &err);
+  if (rc) { SetLastError("%s", err.c_str()); return rc; }
+  j.tiff = true;
   j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
   j.hs[0] = j.vs[0] = 1;
   j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
@@ -1931,6 +1951,16 @@ struct dalib200JpegPlan {
   cudaEvent_t png_uploaded = nullptr, png_fork = nullptr, png_join = nullptr;
   cudaStream_t png_stream = nullptr;
   bool png_pending = false;
+  // TIFF samples: decoded by tiff.cu on a stream of their own, like the PNG samples
+  std::vector<dalib200::TiffImage> tiff_images;
+  std::vector<dalib200::TiffSeg> tiff_segs;
+  int64_t tiff_dec_bytes = 0;
+  uint8_t *d_tiff_dec = nullptr; size_t d_tiff_dec_cap = 0;    // decoded segments (grow only)
+  uint8_t *d_tiff_slots = nullptr; size_t d_tiff_slots_cap = 0; // segment working memory (grow only)
+  dalib200::DescArena tiff_arena;
+  cudaEvent_t tiff_uploaded = nullptr, tiff_fork = nullptr, tiff_join = nullptr;
+  cudaStream_t tiff_stream = nullptr;
+  bool tiff_pending = false;
 };
 
 namespace {
@@ -1978,7 +2008,7 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
-    if (j.png) {                   // decoded by png.cu: no IDCT / colour work
+    if (j.png || j.tiff) {         // decoded by png.cu / tiff.cu: no IDCT / colour work
       p->first_work[i] = work; p->first_fused[i] = fused; p->first_quad[i] = quads; p->first_item[i] = items;
       continue;
     }
@@ -2040,7 +2070,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   const int output_type = p->output_type;
   const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
   p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
-  if (j.png) {                   // any window: png_color produces pixels one by one
+  if (j.png || j.tiff) {         // any window: png_color / tiff_color produce pixels one by one
     im.win_x0 = sx0; im.win_w = sx1 - sx0;
   } else {
     im.win_x0 = sx0 & ~7; im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0;
@@ -2050,7 +2080,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
   ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
   // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
-  ge.planar_ok = !j.png && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
+  ge.planar_ok = !j.png && !j.tiff && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
                  output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
   const bool planes_only = rois && rois[i].planes_only;
   if (planes_only && !ge.planar_ok) {
@@ -2067,7 +2097,8 @@ extern "C" {
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info) try {
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
-  int rc = IsPngStream(data, len) ? ParsePng(data, len, j, nullptr, nullptr, 0) : ParseHeaders(data, len, j, false);
+  int rc = IsPngStream(data, len) ? ParsePng(data, len, j, nullptr, nullptr, 0)
+           : IsTiffStream(data, len) ? ParseTiff(data, len, j, nullptr, nullptr, 0, 0, nullptr) : ParseHeaders(data, len, j, false);
   if (rc) return rc;
   FillInfo(j, info);
   return DALIB200_SUCCESS;
@@ -2084,7 +2115,10 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
       cudaEventCreateWithFlags(&p->prog_join, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->png_uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->png_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->png_join, cudaEventDisableTiming) != cudaSuccess) {
+      cudaEventCreateWithFlags(&p->png_join, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->tiff_uploaded, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->tiff_fork, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->tiff_join, cudaEventDisableTiming) != cudaSuccess) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2106,6 +2140,13 @@ int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (p->png_join) cudaEventDestroy(p->png_join);
   p->png_arena.Free();
   if (p->d_png_scan) cudaFree(p->d_png_scan);
+  if (p->tiff_stream) { cudaStreamSynchronize(p->tiff_stream); cudaStreamDestroy(p->tiff_stream); }
+  if (p->tiff_uploaded) { cudaEventSynchronize(p->tiff_uploaded); cudaEventDestroy(p->tiff_uploaded); }
+  if (p->tiff_fork) cudaEventDestroy(p->tiff_fork);
+  if (p->tiff_join) cudaEventDestroy(p->tiff_join);
+  p->tiff_arena.Free();
+  if (p->d_tiff_dec) cudaFree(p->d_tiff_dec);
+  if (p->d_tiff_slots) cudaFree(p->d_tiff_slots);
   if (p->h_stage) cudaFreeHost(p->h_stage);
   if (p->h_images) cudaFreeHost(p->h_images);
   if (p->h_status) cudaFreeHost(p->h_status);
@@ -2186,6 +2227,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->prog_total_blocks = 0;
   p->png_images.clear(); p->png_chunks.clear();
   int64_t png_scan = 0;
+  p->tiff_images.clear(); p->tiff_segs.clear();
+  int64_t tiff_dec = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2225,6 +2268,26 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       pim.scan_off = png_scan;
       png_scan += (int64_t)Align((size_t)pim.scan_bytes, 16);
       p->png_images.push_back(pim);
+      p->src_ptr.push_back(streams[i] + j.scan_begin);
+      raw += Align(j.scan_end - j.scan_begin, 16);
+      continue;
+    }
+    if (IsTiffStream(streams[i], lengths[i])) {
+      // TIFF: as PNG; tiff.cu decodes its segments (the staged range is their span) into the decode window
+      dalib200::TiffImage tim;
+      int64_t dec_bytes = 0;
+      int rc = ParseTiff(streams[i], lengths[i], j, &tim, &p->tiff_segs, (int)p->tiff_images.size(), tiff_dec, &dec_bytes);
+      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
+      JpegImage &im = p->images[i];
+      memset(&im, 0, sizeof(im));
+      im.width = j.width; im.height = j.height; im.out_type = output_type;
+      im.unit_begin = im.unit_end = (int)p->units.size();
+      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
+      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
+      tim.sample = i;
+      tim.raw_off = (int64_t)raw;
+      tiff_dec += dec_bytes;
+      p->tiff_images.push_back(tim);
       p->src_ptr.push_back(streams[i] + j.scan_begin);
       raw += Align(j.scan_end - j.scan_begin, 16);
       continue;
@@ -2420,6 +2483,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   DB_CHECK_ARG(raw < (1ull << 32) && clean < (1ull << 32), "decoders.image: batch of encoded data exceeds 4 GiB");
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
   p->png_scan_bytes = png_scan;
+  p->tiff_dec_bytes = tiff_dec;
+  DB_CHECK_ARG(p->tiff_segs.size() < (1ull << 31), "decoders.image: batch of more than 2^31 TIFF segments");
   p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
   for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
     if ((size_t)u.clean_off + u.raw_len + clean_read_behind(p->log2_sub) > p->clean_alloc) {
@@ -2768,6 +2833,43 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     if ((rc = LaunchPng(a, ps))) return rc;
     DB_CUDA(cudaEventRecord(p->png_join, ps));
   }
+  if (!p->tiff_images.empty()) {
+    // TIFF samples (tiff.cu): forked onto a stream of their own as the PNG samples are, so that a TIFF written as one big strip (a serial
+    // chain) runs beside the JPEG kernels.  It writes only the TIFF samples' decode windows, its scratch and their status words.
+    using namespace dalib200;
+    const int nseg = (int)p->tiff_segs.size();
+    if ((rc = GrowDevice(p->d_tiff_dec, p->d_tiff_dec_cap, (size_t)p->tiff_dec_bytes + 16))) return rc;
+    if ((rc = GrowDevice(p->d_tiff_slots, p->d_tiff_slots_cap, (size_t)TiffSlotCount(nseg) * kTiffSlotBytes))) return rc;
+    if (!p->tiff_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->tiff_stream, cudaStreamNonBlocking));
+    cudaStream_t ts = p->tiff_stream;
+    DB_CUDA(cudaEventRecord(p->tiff_fork, s));
+    DB_CUDA(cudaStreamWaitEvent(ts, p->tiff_fork, 0));
+    if (p->tiff_pending) { DB_CUDA(cudaEventSynchronize(p->tiff_uploaded)); p->tiff_pending = false; }
+    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
+    int64_t px = 0;
+    for (TiffImage &ti : p->tiff_images) {
+      const JpegImage &im = hi[ti.sample];
+      ti.out = im.out; ti.out_type = im.out_type;
+      ti.win_x0 = im.win_x0; ti.win_y0 = im.win_y0; ti.win_w = im.win_w; ti.win_h = im.win_h;
+      ti.first_px = px;
+      px += (int64_t)im.win_w * im.win_h;
+    }
+    const size_t nti = p->tiff_images.size();
+    const size_t o_seg = Align(sizeof(TiffImage) * nti, 16), tbytes = Align(o_seg + sizeof(TiffSeg) * nseg, 16);
+    if ((rc = p->tiff_arena.Reserve(tbytes))) return rc;
+    memcpy(p->tiff_arena.host, p->tiff_images.data(), sizeof(TiffImage) * nti);
+    memcpy(p->tiff_arena.host + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
+    if ((rc = p->tiff_arena.Upload(tbytes, ts))) return rc;
+    DB_CUDA(cudaEventRecord(p->tiff_uploaded, ts));
+    p->tiff_pending = true;
+    TiffLaunch a;
+    a.d_images = reinterpret_cast<const TiffImage *>(p->tiff_arena.dev); a.nimages = (int)nti;
+    a.d_segs = reinterpret_cast<const TiffSeg *>(p->tiff_arena.dev + o_seg); a.nsegs = nseg;
+    a.total_px = px;
+    a.d_raw = d_raw; a.d_dec = p->d_tiff_dec; a.d_slots = p->d_tiff_slots; a.d_status = p->d_status;
+    if ((rc = LaunchTiff(a, ts))) return rc;
+    DB_CUDA(cudaEventRecord(p->tiff_join, ts));
+  }
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
   if (any_units) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
@@ -2839,6 +2941,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     }
   }
   if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png_join, 0));       // the PNG samples' windows and status are in place
+  if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff_join, 0));     // the TIFF samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

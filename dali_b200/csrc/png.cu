@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(32) png_inflate_kernel(const PngImage *__restr
   if (threadIdx.x != 0) return;
   const PngImage &im = images[blockIdx.x];
   if (status[im.sample]) return;                              // a CRC error: the data is not decoded
-  PngWork w;
+  InflateWork w;
   if (png_inflate_unfilter(im, chunks, raw, scan + im.scan_off, w)) status[im.sample] = 1;
 }
 

@@ -15,6 +15,7 @@
 #ifndef DALI_B200_CSRC_PNG_CORE_H_
 #define DALI_B200_CSRC_PNG_CORE_H_
 #include <stdint.h>
+#include "inflate.h"
 
 #if defined(__CUDACC__)
 #define PNG_HD __host__ __device__ __forceinline__
@@ -90,97 +91,9 @@ PNG_HD uint32_t png_crc_table_entry(uint32_t i) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
-// Inflate.  Bit reader over the IDAT payloads as one stream, hopping the 12-byte gaps (CRC, length, type) between chunks.  Bytes past
-// the last payload read as zero; `used` counts the bits consumed, so running past the data is detected exactly.
-struct PngBits {
-  const uint8_t *raw;          // the image's staged bytes
-  const PngChunk *chunks;
-  int k, kend;                 // current chunk, end of the image's chunks
-  uint32_t pos;                // next byte inside chunk k
-  uint64_t acc;                // LSB first
-  int nbits;
-  int64_t used, avail;         // bits consumed / bits of data in all payloads
-};
-PNG_HD void pbits_fill(PngBits &b) {
-  while (b.nbits <= 56) {
-    while (b.k < b.kend && b.pos >= b.chunks[b.k].len) { b.k++; b.pos = 0; }
-    uint32_t v = 0;
-    if (b.k < b.kend) v = b.raw[b.chunks[b.k].off + b.pos++];
-    b.acc |= (uint64_t)v << b.nbits;
-    b.nbits += 8;
-  }
-}
-PNG_HD uint32_t pbits_get(PngBits &b, int n) {        // n <= 32
-  if (b.nbits < n) pbits_fill(b);
-  const uint32_t v = n ? (uint32_t)(b.acc & ((1ull << n) - 1)) : 0u;
-  b.acc >>= n; b.nbits -= n; b.used += n;
-  return v;
-}
-PNG_HD bool pbits_dry(const PngBits &b) { return b.used > b.avail; }
-
-// Canonical Huffman code (RFC 1951 3.2.2) as zlib's puff.c decodes it, with a 9-bit first-level table in front.
-constexpr int kPngLutBits = 9;
-struct PngHuff {
-  uint16_t lut[1 << kPngLutBits];    // (length << 9) | symbol for codes of at most 9 bits, 0 = longer code or no code
-  uint16_t count[16];                // codes of each length
-  uint16_t symbol[288];              // symbols in canonical order
-};
-
-// builds the code from `n` code lengths; returns false for an over-subscribed set, or an incomplete one that is not a single code
-// of length 1 or that may not be incomplete at all (zlib inflate_table: a single length-1 code is accepted for the literal / length
-// and distance codes, never for the code-length code; a code without any symbol is left empty)
-PNG_HD bool png_build(PngHuff &h, const uint8_t *len, int n, bool allow_incomplete) {
-  for (int l = 0; l < 16; l++) h.count[l] = 0;
-  for (int s = 0; s < n; s++) h.count[len[s]]++;
-  for (int i = 0; i < (1 << kPngLutBits); i++) h.lut[i] = 0;
-  if (h.count[0] == n) return true;                       // no codes: any use of it is an undefined symbol
-  int left = 1, maxlen = 0;
-  for (int l = 1; l < 16; l++) {
-    left <<= 1; left -= h.count[l];
-    if (left < 0) return false;
-    if (h.count[l]) maxlen = l;
-  }
-  if (left > 0 && !(allow_incomplete && maxlen == 1)) return false;
-  uint16_t offs[16];
-  offs[1] = 0;
-  for (int l = 1; l < 15; l++) offs[l + 1] = offs[l] + h.count[l];
-  // canonical codes: first code of length l = (first code of length l - 1 + count[l - 1]) << 1
-  uint16_t next[16];
-  int code = 0;
-  for (int l = 1; l < 16; l++) { code = (code + (l > 1 ? h.count[l - 1] : 0)) << 1; next[l] = (uint16_t)code; }
-  for (int s = 0; s < n; s++) {
-    const int l = len[s];
-    if (!l) continue;
-    h.symbol[offs[l]++] = (uint16_t)s;
-    const uint32_t c = next[l]++;
-    if (l <= kPngLutBits) {
-      uint32_t r = 0;                                       // the stream sends the code MSB first into an LSB-first bit order
-      for (int i = 0; i < l; i++) r |= ((c >> i) & 1u) << (l - 1 - i);
-      for (uint32_t e = r; e < (1u << kPngLutBits); e += 1u << l) h.lut[e] = (uint16_t)((l << 9) | s);
-    }
-  }
-  return true;
-}
-
-// next symbol, -1 = no such code
-PNG_HD int png_decode(PngBits &b, const PngHuff &h) {
-  if (b.nbits < 16) pbits_fill(b);
-  const uint16_t e = h.lut[b.acc & ((1u << kPngLutBits) - 1)];
-  if (e) { const int l = e >> 9; b.acc >>= l; b.nbits -= l; b.used += l; return e & 511; }
-  int code = 0, first = 0, index = 0;                    // puff.c decode(): one bit at a time
-  for (int l = 1; l < 16; l++) {
-    code |= (int)((b.acc >> (l - 1)) & 1u);
-    const int cnt = h.count[l];
-    if (code - cnt < first) { b.acc >>= l; b.nbits -= l; b.used += l; return h.symbol[index + (code - first)]; }
-    index += cnt; first += cnt; first <<= 1; code <<= 1;
-  }
-  return -1;
-}
-
-struct PngWork { PngHuff lit, dist, cl; uint8_t lens[288 + 32]; };     // the kernel's working memory (per image)
-
-// Inflates the image's zlib stream into `scan` (im.scan_bytes bytes).  Returns 0, or 1 for a malformed stream.  Reads stay inside
-// the chunks' payloads; writes stay inside [scan, scan + scan_bytes).
+// Inflates the image's zlib stream into `scan` (im.scan_bytes bytes): inflate.h over the IDAT payloads read as one stream, hopping the
+// 12-byte gaps (CRC, length, type) between chunks.  Returns 0, or 1 for a malformed stream.  Reads stay inside the chunks' payloads;
+// writes stay inside [scan, scan + scan_bytes).
 //
 // The stream's tail follows libpng + zlib (pinned against cv2 by tests/test_png_cpu.py):
 //   * the data running out before the end of the zlib stream is an error, before or after the image is complete ("Not enough image
@@ -189,112 +102,15 @@ struct PngWork { PngHuff lit, dist, cl; uint8_t lens[288 + 32]; };     // the ke
 //     bad Adler-32 trailer met before that is an error;
 //   * once a byte beyond the image (a surplus) would be produced, libpng only drains the rest of the stream: malformed data or a bad
 //     trailer there is a warning, so the rest is decoded without output ("draining") and only its end is required.
-PNG_HD int png_inflate(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, PngWork &w) {
-  PngBits b;
-  b.raw = raw + im.raw_off; b.chunks = chunks; b.k = im.chunk_begin; b.kend = im.chunk_end; b.pos = 0; b.acc = 0; b.nbits = 0; b.used = 0;
-  b.avail = 0;
-  for (int k = im.chunk_begin; k < im.chunk_end; k++) b.avail += 8 * (int64_t)chunks[k].len;
-  const int64_t total = im.scan_bytes;
-  int64_t out = 0;                                        // bytes produced, surplus included
-  bool drain = false;
-  uint32_t s1 = 1, s2 = 0, nmod = 0;                      // Adler-32
-  auto put = [&](uint8_t v) {
-    if (out < total) {
-      scan[out] = v;
-      s1 += v; s2 += s1;
-      if (++nmod == 5552) { s1 %= 65521u; s2 %= 65521u; nmod = 0; }
-    } else {
-      drain = true;
-    }
-    out++;
-  };
-  auto bad = [&] { return drain ? 0 : 1; };               // malformed data: an error unless libpng is only draining
-  pbits_get(b, 16);                                       // CMF / FLG, checked by the planner
-  bool last = false;
-  while (!last) {
-    last = pbits_get(b, 1) != 0;
-    const uint32_t type = pbits_get(b, 2);
-    if (pbits_dry(b)) return 1;
-    if (type == 0) {                                      // stored
-      const int drop = b.nbits & 7;                       // to the byte boundary
-      pbits_get(b, drop);
-      const uint32_t len = pbits_get(b, 16), nlen = pbits_get(b, 16);
-      if (pbits_dry(b)) return 1;
-      if ((len ^ 0xFFFFu) != nlen) return bad();
-      for (uint32_t i = 0; i < len; i++) {
-        const uint8_t v = (uint8_t)pbits_get(b, 8);
-        if (pbits_dry(b)) return 1;
-        put(v);
-      }
-    } else if (type == 1 || type == 2) {
-      if (type == 1) {                                    // fixed codes (RFC 1951 3.2.6)
-        for (int s = 0; s < 288; s++) w.lens[s] = s < 144 ? 8 : s < 256 ? 9 : s < 280 ? 7 : 8;
-        png_build(w.lit, w.lens, 288, true);
-        for (int s = 0; s < 32; s++) w.lens[s] = 5;      // 30 and 31 complete the code; decoding one is an error
-        png_build(w.dist, w.lens, 32, true);
-      } else {                                            // dynamic codes (3.2.7)
-        const int nlen = (int)pbits_get(b, 5) + 257, ndist = (int)pbits_get(b, 5) + 1, ncode = (int)pbits_get(b, 4) + 4;
-        if (pbits_dry(b)) return 1;
-        if (nlen > 286 || ndist > 30) return bad();
-        const uint8_t order[19] = { 16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15 };
-        uint8_t cl[19];
-        for (int i = 0; i < 19; i++) cl[order[i]] = i < ncode ? (uint8_t)pbits_get(b, 3) : 0;
-        if (pbits_dry(b)) return 1;
-        if (!png_build(w.cl, cl, 19, false)) return bad();
-        int i = 0;
-        while (i < nlen + ndist) {
-          const int sym = png_decode(b, w.cl);
-          if (pbits_dry(b)) return 1;
-          if (sym < 0) return bad();
-          if (sym < 16) { w.lens[i++] = (uint8_t)sym; continue; }
-          int rep, v = 0;
-          if (sym == 16) { if (i == 0) return bad(); v = w.lens[i - 1]; rep = 3 + (int)pbits_get(b, 2); }
-          else if (sym == 17) rep = 3 + (int)pbits_get(b, 3);
-          else rep = 11 + (int)pbits_get(b, 7);
-          if (pbits_dry(b)) return 1;
-          if (i + rep > nlen + ndist) return bad();
-          while (rep--) w.lens[i++] = (uint8_t)v;
-        }
-        if (w.lens[256] == 0) return bad();               // no end-of-block code
-        if (!png_build(w.lit, w.lens, nlen, true)) return bad();
-        if (!png_build(w.dist, w.lens + nlen, ndist, true)) return bad();
-      }
-      while (true) {
-        const int sym = png_decode(b, w.lit);
-        if (pbits_dry(b)) return 1;
-        if (sym < 0) return bad();
-        if (sym < 256) { put((uint8_t)sym); continue; }
-        if (sym == 256) break;
-        const int li = sym - 257;
-        if (li >= 29) return bad();                       // 286, 287
-        int len;
-        if (li < 8) len = 3 + li;
-        else if (li == 28) len = 258;
-        else { const int e = (li >> 2) - 1; len = ((4 + (li & 3)) << e) + 3 + (int)pbits_get(b, e); }
-        const int ds = png_decode(b, w.dist);
-        if (pbits_dry(b)) return 1;
-        if (ds < 0 || ds >= 30) return bad();
-        int dist;
-        if (ds < 4) dist = ds + 1;
-        else { const int e = (ds >> 1) - 1; dist = ((2 + (ds & 1)) << e) + 1 + (int)pbits_get(b, e); }
-        if (pbits_dry(b)) return 1;
-        if (dist > out) return bad();                     // a distance behind the output start
-        for (int k = 0; k < len; k++) put(out < total ? scan[out - dist] : 0);     // past the image only the count matters
-      }
-    } else {
-      return bad();                                       // block type 3
-    }
-  }
-  if (out < total) return 1;                              // the stream ends before the image does
-  pbits_get(b, b.nbits & 7);                              // the Adler-32 trailer
-  uint32_t adler = 0;
-  for (int i = 0; i < 4; i++) adler = (adler << 8) | pbits_get(b, 8);
-  if (pbits_dry(b)) return 1;
-  return adler != (((s2 % 65521u) << 16) | (s1 % 65521u)) ? bad() : 0;
+PNG_HD int png_inflate(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
+  InflateBits<PngChunk> b;
+  ibits_init(b, raw + im.raw_off, chunks, im.chunk_begin, im.chunk_end);
+  ibits_get(b, 16);                                       // CMF / FLG, checked by the planner
+  return inflate_zlib<false>(b, scan, im.scan_bytes, w);
 }
 
 // png_inflate, then the unfilter in place.  Returns 0, or 1 for a malformed stream or filter byte.
-PNG_HD int png_inflate_unfilter(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, PngWork &w) {
+PNG_HD int png_inflate_unfilter(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
   if (png_inflate(im, chunks, raw, scan, w)) return 1;
   // unfilter in place, pass by pass (filter types 0..4 of the PNG specification, 9.2); bpp = bytes of a whole pixel, at least 1
   const int bpp = (im.spp * im.depth + 7) >> 3;

@@ -116,7 +116,7 @@ inline int PlanPng(const uint8_t *p, size_t n, int image, PngImage *im, std::vec
   for (size_t k = first_chunk; k < chunks.size() && got < 2; k++)
     for (uint32_t i = 0; i < chunks[k].len && got < 2; i++) zh[got++] = p[info->stage_begin + chunks[k].off + i];
   if (got < 2) return bad("IDAT data ends inside the zlib header");
-  if ((zh[0] & 15) != 8 || (zh[0] >> 4) > 7 || ((zh[0] << 8) | zh[1]) % 31 != 0 || (zh[1] & 0x20)) return bad("bad zlib header");
+  if (!zlib_header_ok(zh[0], zh[1])) return bad("bad zlib header");
   // scanline layout, pass by pass
   int64_t off = 0;
   for (int ps = 0; ps < (im->interlace ? 7 : 1); ps++) {

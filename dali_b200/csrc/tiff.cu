@@ -1,0 +1,79 @@
+// dali_b200/csrc/tiff.cu -- TIFF decoding inside decoders.image: segment decode, colour conversion.
+//
+// The planner (tiff_plan.h) walks the IFD on the host and builds the segment table; the image data itself is only touched here:
+//   tiff_segment  one lane per segment (strip or tile of one plane): LZW / Deflate / PackBits / raw copy into plan scratch, then the
+//                 horizontal predictor undone row by row (tiff_decode_segment, tiff_core.h).  Each thread owns a kTiffSlotBytes slot of
+//                 plan-owned global memory for the LZW string starts or the inflate tables, so that the kernel keeps no stack frame.
+//   tiff_color    one thread per output pixel: gathers the samples from their segments and planes and applies libtiff's RGBA rules
+//                 and cv2's GRAY rule, into the decode window
+// Orientation, region of interest, YCbCr and float output are the JPEG path's post pass over that window (jpeg.cu jpeg_post_kernel).
+#include "common.cuh"
+#include "tiff.h"
+#include <algorithm>
+
+namespace dalib200 {
+
+// tiff_segment runs one warp per CTA, and `lanes` working lanes in each warp (the others return).  A segment is a serial chain whose
+// lanes diverge from each other's codes at once, so lanes of one warp share its issue slots: with few segments (a batch of images
+// stored as one strip each) every segment gets a warp of its own, spread over all SMs; with many, the warps fill up to 32 lanes.
+struct TiffSegGeometry { int warps, lanes; };
+TiffSegGeometry tiff_seg_geometry(int nsegs) {
+  const int resident = NumSMs() * 32;                         // one-warp CTAs: at most 32 resident per SM
+  constexpr int kMaxWorkers = 33792;                          // working lanes (and 16 KB slots) in all: 540 MB of slots at most
+  TiffSegGeometry g;
+  g.lanes = std::max(1, std::min(32, (nsegs + resident - 1) / resident));
+  g.warps = std::max(1, std::min((nsegs + g.lanes - 1) / g.lanes, std::min(resident, kMaxWorkers / g.lanes)));
+  return g;
+}
+
+__global__ void __launch_bounds__(32) tiff_segment_kernel(const TiffImage *__restrict__ images, const TiffSeg *__restrict__ segs,
+                                                          int nsegs, int lanes, const uint8_t *__restrict__ raw, uint8_t *dec,
+                                                          uint8_t *slots, int32_t *status) {
+  if ((int)threadIdx.x >= lanes) return;
+  const int w = blockIdx.x * lanes + threadIdx.x;             // working lane, and its slot
+  void *slot = slots + (size_t)w * kTiffSlotBytes;
+  for (int k = w; k < nsegs; k += gridDim.x * lanes) {
+    const TiffSeg &s = segs[k];
+    const TiffImage &im = images[s.image];
+    if (*(volatile int32_t *)&status[im.sample]) continue;   // another segment of the image failed: the image is not decoded
+    if (tiff_decode_segment(im, s, raw, dec + s.dec_off, slot)) status[im.sample] = 1;
+  }
+}
+
+__global__ void __launch_bounds__(256) tiff_color_kernel(const TiffImage *__restrict__ images, int nimages, int64_t total,
+                                                         const TiffSeg *__restrict__ segs, const uint8_t *__restrict__ dec) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
+    int lo = 0, hi = nimages - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
+    const TiffImage &im = images[lo];
+    const int64_t lp = e - im.first_px;
+    const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
+    tiff_pixel(im, segs, dec, lx, ly);
+  }
+}
+
+int TiffSlotCount(int nsegs) {
+  const TiffSegGeometry g = tiff_seg_geometry(nsegs);
+  return g.warps * g.lanes;
+}
+
+int LaunchTiff(const TiffLaunch &a, cudaStream_t s) {
+  if (a.nimages == 0) return DALIB200_SUCCESS;
+  if (a.nsegs > 0) {
+    ProfScope ps_("tiff_segment", s);
+    const TiffSegGeometry g = tiff_seg_geometry(a.nsegs);
+    tiff_segment_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.d_segs, a.nsegs, g.lanes, a.d_raw, a.d_dec, a.d_slots, a.d_status);
+    CountLaunch();
+  }
+  if (a.total_px > 0) {
+    const int grid = (int)std::min<int64_t>((a.total_px + 255) / 256, (int64_t)NumSMs() * 16);
+    ProfScope ps_("tiff_color", s);
+    tiff_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_segs, a.d_dec);
+    CountLaunch();
+  }
+  DB_CUDA(cudaGetLastError());
+  return DALIB200_SUCCESS;
+}
+
+}  // namespace dalib200

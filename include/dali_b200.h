@@ -54,8 +54,10 @@ int dalib200ProfilingCollect(char *names, int name_stride, float *ms, int max, i
 /* ------------------------------------------------------------------------------------------------
  * Image decode.  JPEG (Huffman + dequant + IDCT + chroma upsampling + YCbCr->RGB): baseline sequential (self-synchronising parallel
  * entropy decode) and progressive (SOF2: scans in dependency waves, one warp per scan; spectral selection + successive approximation).
- * PNG (detected by its signature; IDAT CRCs, inflate + unfilter, colour conversion, bit-exact with cv2.imdecode).  Both formats may be
- * mixed in one batch of a plan.
+ * PNG (detected by its signature; IDAT CRCs, inflate + unfilter, colour conversion, bit-exact with cv2.imdecode).
+ * TIFF (detected by its header; first IFD, strips or tiles, LZW / Deflate / PackBits / none, one GPU lane per segment, colour
+ * conversion, bit-exact with cv2.imdecode; unsupported layouts fail with DALIB200_ERROR_UNSUPPORTED).  All formats may be mixed in one
+ * batch of a plan.
  * Replaces: imgcodec::ImageDecoder<MixedBackend>::RunImplImpl -> nvimgcodecDecoderDecode
  *           (dali/operators/imgcodec/image_decoder.h:613-882) and ParseSample (:473-499).
  * Host work: marker / table / chunk-header parse only.  Device work: everything arithmetic. */
@@ -63,13 +65,13 @@ typedef struct dalib200JpegPlan dalib200JpegPlan;
 
 typedef struct {
   int32_t width, height;        /* decoded image size */
-  int32_t components;           /* JPEG: 1, 3 or 4; PNG: channels of the file (palette: 3) */
+  int32_t components;           /* JPEG: 1, 3 or 4; PNG, TIFF: channels of the file (palette: 3) */
   int32_t subsampling;          /* (hmax<<4)|vmax of the luma sampling factors, e.g. 0x22 = 4:2:0 */
   int32_t restart_interval;
   int32_t orientation;          /* EXIF orientation, 1 = none */
 } dalib200JpegInfo;
 
-/* header-only parse of a JPEG or PNG stream: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
+/* header-only parse of a JPEG, PNG or TIFF stream: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info);
 
 int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch);
@@ -88,7 +90,7 @@ int dalib200JpegPlanGetInfo(const dalib200JpegPlan *plan, int sample, dalib200Jp
  *   dtype                DALIB200_UINT8 | DALIB200_FLOAT     (ConvertSatNorm: u8 * (1 / 255), convert.h:118-128)
  *   adjust_orientation   apply the EXIF orientation (image_decoder.h:211,678-679,806)
  *   rois[i]              region of interest of sample i in OUTPUT (oriented) pixel coordinates, [x0, x1) x [y0, y1)
- *                        (imgcodec.h:26-44, image_decoder.h:681-716); only the MCUs (PNG: pixels) under the region are
+ *                        (imgcodec.h:26-44, image_decoder.h:681-716); only the MCUs (PNG, TIFF: pixels) under the region are
  *                        transformed.
  * The result equals the full decode followed by orientation, crop and conversion, bit for bit. */
 typedef struct { int32_t output_type, fancy_upsampling, dtype, adjust_orientation; } dalib200JpegParams;

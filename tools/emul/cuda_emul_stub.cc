@@ -1,7 +1,7 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG and PNG kernels are EXECUTED on the host -- their bodies are single
-// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h), so a launch is a loop over blocks and threads around
+// of the 3-D resize, progressive JPEG, PNG and TIFF kernels are EXECUTED on the host -- their bodies are single
+// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h), so a launch is a loop over blocks and threads around
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
 // end to end without a GPU -- descriptor upload, temporaries, stage order, grid-stride loops, wave ranges, arena offsets -- and
 // tests/test_launch_emul_cpu.py compares what lands in "device" memory with the oracle.
@@ -17,6 +17,7 @@
 #include "../../dali_b200/csrc/resample3d_core.h"
 #include "../../dali_b200/csrc/jpeg_prog_core.h"
 #include "../../dali_b200/csrc/png_core.h"
+#include "../../dali_b200/csrc/tiff_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -66,10 +67,10 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[6];
+static long g_emulated[8];
 long emul_launch_count(int which) { return g_emulated[which]; }
 
-// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu and png.cu, thread by thread
+// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu and tiff.cu, thread by thread
 static void run_resample3d_pass(Dim3 g, Dim3 b, void **args) {
   const R3Pass *passes = *static_cast<const R3Pass **>(args[0]);
   const int32_t *tab = *static_cast<const int32_t **>(args[1]);
@@ -134,7 +135,7 @@ static void run_png_inflate(Dim3 g, Dim3, void **args) {
   const uint8_t *raw = *static_cast<const uint8_t **>(args[2]);
   uint8_t *scan = *static_cast<uint8_t **>(args[3]);
   int32_t *status = *static_cast<int32_t **>(args[4]);
-  PngWork *w = new PngWork;
+  InflateWork *w = new InflateWork;
   for (int bx = (int)g.x - 1; bx >= 0; bx--) {             // one working thread per block, blocks in no particular order
     const PngImage &im = images[bx];
     if (status[im.sample]) continue;
@@ -160,6 +161,44 @@ static void run_png_color(Dim3 g, Dim3 b, void **args) {
       }
 }
 
+static void run_tiff_segment(Dim3 g, Dim3 b, void **args) {
+  const TiffImage *images = *static_cast<const TiffImage **>(args[0]);
+  const TiffSeg *segs = *static_cast<const TiffSeg **>(args[1]);
+  const int nsegs = *static_cast<int *>(args[2]);
+  const int lanes = *static_cast<int *>(args[3]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[4]);
+  uint8_t *dec = *static_cast<uint8_t **>(args[5]);
+  uint8_t *slots = *static_cast<uint8_t **>(args[6]);
+  int32_t *status = *static_cast<int32_t **>(args[7]);
+  for (int bx = (int)g.x - 1; bx >= 0; bx--)                 // blocks of a launch run in no particular order: take the reverse one
+    for (int tx = 0; tx < (int)b.x && tx < lanes; tx++) {
+      const int w = bx * lanes + tx;
+      for (int k = w; k < nsegs; k += (int)g.x * lanes) {
+        const TiffImage &im = images[segs[k].image];
+        if (status[im.sample]) continue;
+        if (tiff_decode_segment(im, segs[k], raw, dec + segs[k].dec_off, slots + (size_t)w * kTiffSlotBytes)) status[im.sample] = 1;
+      }
+    }
+}
+static void run_tiff_color(Dim3 g, Dim3 b, void **args) {
+  const TiffImage *images = *static_cast<const TiffImage **>(args[0]);
+  const int nimages = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  const TiffSeg *segs = *static_cast<const TiffSeg **>(args[3]);
+  const uint8_t *dec = *static_cast<const uint8_t **>(args[4]);
+  const int64_t step = (int64_t)g.x * b.x;
+  for (unsigned bx = 0; bx < g.x; bx++)
+    for (unsigned tx = 0; tx < b.x; tx++)
+      for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
+        int lo = 0, hi = nimages - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
+        const TiffImage &im = images[lo];
+        const int64_t lp = e - im.first_px;
+        const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
+        tiff_pixel(im, segs, dec, lx, ly);
+      }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -170,6 +209,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_png_crc = !strcmp(name, "_ZN8dalib20014png_crc_kernelEPKNS_8PngChunkEiPKNS_8PngImageEPKhPi");
   const bool is_png_inflate = !strcmp(name, "_ZN8dalib20018png_inflate_kernelEPKNS_8PngImageEPKNS_8PngChunkEPKhPhPi");
   const bool is_png_color = !strcmp(name, "_ZN8dalib20016png_color_kernelEPKNS_8PngImageEilPKh");
+  const bool is_tiff_segment = !strcmp(name, "_ZN8dalib20019tiff_segment_kernelEPKNS_9TiffImageEPKNS_7TiffSegEiiPKhPhS8_Pi");
+  const bool is_tiff_color = !strcmp(name, "_ZN8dalib20017tiff_color_kernelEPKNS_9TiffImageEilPKNS_7TiffSegEPKh");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -180,6 +221,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_png_crc) { run_png_crc(grid, block, args); g_emulated[3]++; }
   else if (is_png_inflate) { run_png_inflate(grid, block, args); g_emulated[4]++; }
   else if (is_png_color) { run_png_color(grid, block, args); g_emulated[5]++; }
+  else if (is_tiff_segment) { run_tiff_segment(grid, block, args); g_emulated[6]++; }
+  else if (is_tiff_color) { run_tiff_color(grid, block, args); g_emulated[7]++; }
   return 0;
 }
 }  // extern "C"

@@ -34,7 +34,7 @@ extern "C" int emul_png_decode(const uint8_t *data, size_t len, int out_type, ui
   int status = 0;
   for (const PngChunk &c : chunks)                                    // png_crc_kernel: one thread per chunk
     if (!png_chunk_crc_ok(staged + im.raw_off + c.off - 4, c.len, table)) status = -1;
-  PngWork *w = new PngWork;
+  InflateWork *w = new InflateWork;
   if (!status && png_inflate_unfilter(im, chunks.data(), staged, scan, *w)) status = -1;
   delete w;
   im.out = out; im.out_type = out_type;

@@ -23,6 +23,9 @@ seeds += [bytearray(cmyk[f"enc_{k}"].tobytes()) for k in range(len(cmyk.files) /
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "..", "tests"))
 import png_streams
 seeds += [bytearray(s) for _, s in png_streams.corpus()[::6]]
+# TIFF streams (strips, tiles, planes, both byte orders, every codec): the IFD walk and the segment table of the planner
+import tiff_streams
+seeds += [bytearray(s) for _, s in tiff_streams.corpus()[::8]]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()
