@@ -1,5 +1,6 @@
 // dali_b200/csrc/common.cu -- error state, descriptor arena, launch accounting.
 #include "common.cuh"
+#include <algorithm>
 #include <mutex>
 #include <nvtx3/nvToolsExt.h>
 #include <cstring>
@@ -54,6 +55,14 @@ int NumSMs() {
       n = 132;
   }
   return n;
+}
+
+SerialLanes SerialLaneGeometry(int nchains, int max_workers) {
+  const int resident = NumSMs() * 32;                         // one-warp CTAs: at most 32 resident per SM
+  SerialLanes g;
+  g.lanes = std::max(1, std::min(32, (nchains + resident - 1) / resident));
+  g.warps = std::max(1, std::min((nchains + g.lanes - 1) / g.lanes, std::min(resident, max_workers / g.lanes)));
+  return g;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -40,6 +40,13 @@ struct DescArena {
 
 int NumSMs();
 
+// Launch shape of a kernel whose working lanes each run one serial chain (tiff_segment, webp_entropy): one warp per CTA and `lanes`
+// working lanes in each warp (the others return).  Serial chains diverge from each other at once, so lanes of one warp share its issue
+// slots: with few chains every chain gets a warp of its own, spread over all SMs; with more chains than resident warps, the warps fill
+// up to 32 lanes.  At most `max_workers` lanes in all.
+struct SerialLanes { int warps, lanes; };
+SerialLanes SerialLaneGeometry(int nchains, int max_workers);
+
 // Optional per-launch timing (CUDA events on the launching stream), switched on by dalib200ProfilingEnable.
 // bench.py uses it to time the dominant kernel live inside the timed region.
 void ProfBegin(const char *name, cudaStream_t s);

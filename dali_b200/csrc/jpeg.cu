@@ -23,9 +23,10 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): J (encoded bytes) + H*W*3 (decoded image).
 //
-// The plan also takes PNG and TIFF streams (detected by their signatures): png_plan.h walks their chunks and tiff_plan.h their IFD at
-// set-up, png.cu and tiff.cu decode them into the same decode windows on streams of their own, and the post pass below serves every
-// format.  A PNG or TIFF sample has no units, subsequences or MCUs, so every kernel of this file skips it.
+// The plan also takes PNG, TIFF and lossy WebP streams (detected by their signatures): png_plan.h walks their chunks, tiff_plan.h their
+// IFD and webp_plan.h their RIFF chunks and VP8 headers at set-up, png.cu, tiff.cu and webp.cu decode them into the same decode windows
+// on streams of their own, and the post pass below serves every format.  A PNG, TIFF or WebP sample has no units, subsequences or MCUs,
+// so every kernel of this file skips it.
 #include "common.cuh"
 #include <algorithm>
 #include <cstring>
@@ -1660,12 +1661,15 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 // progressive streams: planner + launch interface of jpeg_prog.cu (included here, behind the kernels, so that their line tables stay put)
 #include "jpeg_prog.h"
 #include "jpeg_prog_plan.h"
-// EXIF orientation (shared with the PNG planner); PNG and TIFF streams: planners + launch interfaces of png.cu and tiff.cu
+// EXIF orientation (shared with the PNG and WebP planners); PNG, TIFF and WebP streams: planners + launch interfaces of png.cu, tiff.cu
+// and webp.cu
 #include "exif.h"
 #include "png.h"
 #include "png_plan.h"
 #include "tiff.h"
 #include "tiff_plan.h"
+#include "webp.h"
+#include "webp_plan.h"
 namespace {
 
 struct ParsedJpeg {
@@ -1675,6 +1679,7 @@ struct ParsedJpeg {
   bool progressive = false, jfif = false;
   bool png = false;           // a PNG stream (png_plan.h): width / height / ncomp / orientation / scan range only
   bool tiff = false;          // a TIFF stream (tiff_plan.h): the same fields
+  bool webp = false;          // a lossy WebP stream (webp_plan.h): the same fields
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
   HostHuff dc[4], ac[4];
@@ -1805,6 +1810,22 @@ int ParseTiff(const uint8_t *p, size_t n, ParsedJpeg &j, TiffImage *im, std::vec
   j.tiff = true;
   j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
   j.hs[0] = j.vs[0] = 1;
+  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
+  return DALIB200_SUCCESS;
+}
+
+// lossy WebP stream (webp_plan.h), as ParsePng; `scratch_base` / `scratch_bytes`: the image's range of the WebP scratch.  The
+// subsampling reported is 4:2:0 (VP8's only layout).
+int ParseWebp(const uint8_t *p, size_t n, ParsedJpeg &j, WebpImage *im, int image, int64_t scratch_base, int64_t *scratch_bytes) {
+  WebpImage tmp;
+  WebpInfo info;
+  int64_t tmpb;
+  std::string err;
+  const int rc = PlanWebp(p, n, image, im ? im : &tmp, scratch_base, scratch_bytes ? scratch_bytes : &tmpb, &info, &err);
+  if (rc) { SetLastError("%s", err.c_str()); return rc; }
+  j.webp = true;
+  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
+  j.hs[0] = j.vs[0] = 2;
   j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
   return DALIB200_SUCCESS;
 }
@@ -1961,6 +1982,14 @@ struct dalib200JpegPlan {
   cudaEvent_t tiff_uploaded = nullptr, tiff_fork = nullptr, tiff_join = nullptr;
   cudaStream_t tiff_stream = nullptr;
   bool tiff_pending = false;
+  // WebP samples: decoded by webp.cu on a stream of their own, like the PNG and TIFF samples
+  std::vector<dalib200::WebpImage> webp_images;
+  int64_t webp_scratch_bytes = 0;
+  uint8_t *d_webp_scratch = nullptr; size_t d_webp_scratch_cap = 0;   // coefficients, macroblocks, planes (grow only)
+  dalib200::DescArena webp_arena;
+  cudaEvent_t webp_uploaded = nullptr, webp_fork = nullptr, webp_join = nullptr;
+  cudaStream_t webp_stream = nullptr;
+  bool webp_pending = false;
 };
 
 namespace {
@@ -2008,7 +2037,7 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
-    if (j.png || j.tiff) {         // decoded by png.cu / tiff.cu: no IDCT / colour work
+    if (j.png || j.tiff || j.webp) {   // decoded by png.cu / tiff.cu / webp.cu: no IDCT / colour work
       p->first_work[i] = work; p->first_fused[i] = fused; p->first_quad[i] = quads; p->first_item[i] = items;
       continue;
     }
@@ -2070,7 +2099,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   const int output_type = p->output_type;
   const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
   p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
-  if (j.png || j.tiff) {         // any window: png_color / tiff_color produce pixels one by one
+  if (j.png || j.tiff || j.webp) {   // any window: png_color / tiff_color / webp_color produce pixels one by one
     im.win_x0 = sx0; im.win_w = sx1 - sx0;
   } else {
     im.win_x0 = sx0 & ~7; im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0;
@@ -2080,7 +2109,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
   ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
   // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
-  ge.planar_ok = !j.png && !j.tiff && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
+  ge.planar_ok = !j.png && !j.tiff && !j.webp && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
                  output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
   const bool planes_only = rois && rois[i].planes_only;
   if (planes_only && !ge.planar_ok) {
@@ -2098,7 +2127,8 @@ int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info)
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
   int rc = IsPngStream(data, len) ? ParsePng(data, len, j, nullptr, nullptr, 0)
-           : IsTiffStream(data, len) ? ParseTiff(data, len, j, nullptr, nullptr, 0, 0, nullptr) : ParseHeaders(data, len, j, false);
+           : IsTiffStream(data, len) ? ParseTiff(data, len, j, nullptr, nullptr, 0, 0, nullptr)
+           : IsWebpStream(data, len) ? ParseWebp(data, len, j, nullptr, 0, 0, nullptr) : ParseHeaders(data, len, j, false);
   if (rc) return rc;
   FillInfo(j, info);
   return DALIB200_SUCCESS;
@@ -2118,7 +2148,10 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
       cudaEventCreateWithFlags(&p->png_join, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->tiff_uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->tiff_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->tiff_join, cudaEventDisableTiming) != cudaSuccess) {
+      cudaEventCreateWithFlags(&p->tiff_join, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->webp_uploaded, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->webp_fork, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&p->webp_join, cudaEventDisableTiming) != cudaSuccess) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2147,6 +2180,12 @@ int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   p->tiff_arena.Free();
   if (p->d_tiff_dec) cudaFree(p->d_tiff_dec);
   if (p->d_tiff_slots) cudaFree(p->d_tiff_slots);
+  if (p->webp_stream) { cudaStreamSynchronize(p->webp_stream); cudaStreamDestroy(p->webp_stream); }
+  if (p->webp_uploaded) { cudaEventSynchronize(p->webp_uploaded); cudaEventDestroy(p->webp_uploaded); }
+  if (p->webp_fork) cudaEventDestroy(p->webp_fork);
+  if (p->webp_join) cudaEventDestroy(p->webp_join);
+  p->webp_arena.Free();
+  if (p->d_webp_scratch) cudaFree(p->d_webp_scratch);
   if (p->h_stage) cudaFreeHost(p->h_stage);
   if (p->h_images) cudaFreeHost(p->h_images);
   if (p->h_status) cudaFreeHost(p->h_status);
@@ -2229,6 +2268,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   int64_t png_scan = 0;
   p->tiff_images.clear(); p->tiff_segs.clear();
   int64_t tiff_dec = 0;
+  p->webp_images.clear();
+  int64_t webp_scratch = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2288,6 +2329,26 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       tim.raw_off = (int64_t)raw;
       tiff_dec += dec_bytes;
       p->tiff_images.push_back(tim);
+      p->src_ptr.push_back(streams[i] + j.scan_begin);
+      raw += Align(j.scan_end - j.scan_begin, 16);
+      continue;
+    }
+    if (IsWebpStream(streams[i], lengths[i])) {
+      // WebP: as PNG; webp.cu decodes its VP8 payload (the staged range) into the decode window
+      dalib200::WebpImage wim;
+      int64_t bytes = 0;
+      int rc = ParseWebp(streams[i], lengths[i], j, &wim, (int)p->webp_images.size(), webp_scratch, &bytes);
+      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
+      JpegImage &im = p->images[i];
+      memset(&im, 0, sizeof(im));
+      im.width = j.width; im.height = j.height; im.out_type = output_type;
+      im.unit_begin = im.unit_end = (int)p->units.size();
+      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
+      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
+      wim.sample = i;
+      wim.raw_off = (int64_t)raw;
+      webp_scratch += bytes;
+      p->webp_images.push_back(wim);
       p->src_ptr.push_back(streams[i] + j.scan_begin);
       raw += Align(j.scan_end - j.scan_begin, 16);
       continue;
@@ -2484,6 +2545,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
   p->png_scan_bytes = png_scan;
   p->tiff_dec_bytes = tiff_dec;
+  p->webp_scratch_bytes = webp_scratch;
   DB_CHECK_ARG(p->tiff_segs.size() < (1ull << 31), "decoders.image: batch of more than 2^31 TIFF segments");
   p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
   for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
@@ -2870,6 +2932,38 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     if ((rc = LaunchTiff(a, ts))) return rc;
     DB_CUDA(cudaEventRecord(p->tiff_join, ts));
   }
+  if (!p->webp_images.empty()) {
+    // WebP samples (webp.cu): forked onto a stream of their own as the PNG and TIFF samples are; the entropy decode of an image is a
+    // serial chain.  It writes only the WebP samples' decode windows, its scratch and their status words.
+    using namespace dalib200;
+    if ((rc = GrowDevice(p->d_webp_scratch, p->d_webp_scratch_cap, (size_t)p->webp_scratch_bytes + 16))) return rc;
+    if (!p->webp_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->webp_stream, cudaStreamNonBlocking));
+    cudaStream_t ws = p->webp_stream;
+    DB_CUDA(cudaEventRecord(p->webp_fork, s));
+    DB_CUDA(cudaStreamWaitEvent(ws, p->webp_fork, 0));
+    if (p->webp_pending) { DB_CUDA(cudaEventSynchronize(p->webp_uploaded)); p->webp_pending = false; }
+    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
+    int64_t px = 0;
+    for (WebpImage &wi : p->webp_images) {
+      const JpegImage &im = hi[wi.sample];
+      wi.out = im.out; wi.out_type = im.out_type;
+      wi.win_x0 = im.win_x0; wi.win_y0 = im.win_y0; wi.win_w = im.win_w; wi.win_h = im.win_h;
+      wi.first_px = px;
+      px += (int64_t)im.win_w * im.win_h;
+    }
+    const size_t nwi = p->webp_images.size(), wbytes = Align(sizeof(WebpImage) * nwi, 16);
+    if ((rc = p->webp_arena.Reserve(wbytes))) return rc;
+    memcpy(p->webp_arena.host, p->webp_images.data(), sizeof(WebpImage) * nwi);
+    if ((rc = p->webp_arena.Upload(wbytes, ws))) return rc;
+    DB_CUDA(cudaEventRecord(p->webp_uploaded, ws));
+    p->webp_pending = true;
+    WebpLaunch a;
+    a.d_images = reinterpret_cast<const WebpImage *>(p->webp_arena.dev); a.nimages = (int)nwi;
+    a.total_px = px;
+    a.d_raw = d_raw; a.d_scratch = p->d_webp_scratch; a.d_status = p->d_status;
+    if ((rc = LaunchWebp(a, ws))) return rc;
+    DB_CUDA(cudaEventRecord(p->webp_join, ws));
+  }
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
   if (any_units) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
@@ -2942,6 +3036,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   }
   if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png_join, 0));       // the PNG samples' windows and status are in place
   if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff_join, 0));     // the TIFF samples' windows and status are in place
+  if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp_join, 0));     // the WebP samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

@@ -13,18 +13,9 @@
 
 namespace dalib200 {
 
-// tiff_segment runs one warp per CTA, and `lanes` working lanes in each warp (the others return).  A segment is a serial chain whose
-// lanes diverge from each other's codes at once, so lanes of one warp share its issue slots: with few segments (a batch of images
-// stored as one strip each) every segment gets a warp of its own, spread over all SMs; with many, the warps fill up to 32 lanes.
-struct TiffSegGeometry { int warps, lanes; };
-TiffSegGeometry tiff_seg_geometry(int nsegs) {
-  const int resident = NumSMs() * 32;                         // one-warp CTAs: at most 32 resident per SM
-  constexpr int kMaxWorkers = 33792;                          // working lanes (and 16 KB slots) in all: 540 MB of slots at most
-  TiffSegGeometry g;
-  g.lanes = std::max(1, std::min(32, (nsegs + resident - 1) / resident));
-  g.warps = std::max(1, std::min((nsegs + g.lanes - 1) / g.lanes, std::min(resident, kMaxWorkers / g.lanes)));
-  return g;
-}
+// tiff_segment: one working lane per segment (SerialLaneGeometry); each lane owns a 16 KB slot, so the lanes are capped at 33 792
+// (540 MB of slots at most)
+constexpr int kTiffMaxWorkers = 33792;
 
 __global__ void __launch_bounds__(32) tiff_segment_kernel(const TiffImage *__restrict__ images, const TiffSeg *__restrict__ segs,
                                                           int nsegs, int lanes, const uint8_t *__restrict__ raw, uint8_t *dec,
@@ -54,7 +45,7 @@ __global__ void __launch_bounds__(256) tiff_color_kernel(const TiffImage *__rest
 }
 
 int TiffSlotCount(int nsegs) {
-  const TiffSegGeometry g = tiff_seg_geometry(nsegs);
+  const SerialLanes g = SerialLaneGeometry(nsegs, kTiffMaxWorkers);
   return g.warps * g.lanes;
 }
 
@@ -62,7 +53,7 @@ int LaunchTiff(const TiffLaunch &a, cudaStream_t s) {
   if (a.nimages == 0) return DALIB200_SUCCESS;
   if (a.nsegs > 0) {
     ProfScope ps_("tiff_segment", s);
-    const TiffSegGeometry g = tiff_seg_geometry(a.nsegs);
+    const SerialLanes g = SerialLaneGeometry(a.nsegs, kTiffMaxWorkers);
     tiff_segment_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.d_segs, a.nsegs, g.lanes, a.d_raw, a.d_dec, a.d_slots, a.d_status);
     CountLaunch();
   }

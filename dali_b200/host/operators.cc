@@ -111,7 +111,7 @@ static std::vector<const void *> FramePtrs(const TL &tl, const FrameList &f, siz
 
 // =============================================================================================== decoders.image
 DALI_SCHEMA(decoders__Image)
-    .DocStr("Decodes JPEG, PNG and TIFF images on the GPU (JPEG: Huffman + IDCT + upsampling + colour conversion; PNG: inflate + unfilter + colour conversion; TIFF: LZW / Deflate / PackBits per strip or tile + colour conversion; all in CUDA).")
+    .DocStr("Decodes JPEG, PNG, TIFF and lossy WebP images on the GPU (JPEG: Huffman + IDCT + upsampling + colour conversion; PNG: inflate + unfilter + colour conversion; TIFF: LZW / Deflate / PackBits per strip or tile + colour conversion; WebP: VP8 entropy decode + intra reconstruction + loop filter + colour conversion; all in CUDA).")
     .NumInput(1).NumOutput(1)
     .AddOptionalArg("output_type", "Colour space of the output image.", DALI_RGB)
     .AddOptionalArg("dtype", "Output data type.", DALI_UINT8)
@@ -306,7 +306,7 @@ struct CropWindowArgs {
       .AddOptionalArg("rounding", "round | truncate", std::string("round"))
 
 DALI_SCHEMA(decoders__ImageCrop)
-    .DocStr("Decodes JPEG, PNG and TIFF images on the GPU and extracts a fixed crop window; only the JPEG blocks under the window are transformed.")
+    .DocStr("Decodes JPEG, PNG, TIFF and lossy WebP images on the GPU and extracts a fixed crop window; only the JPEG blocks under the window are transformed.")
     .NumInput(1).NumOutput(1)
     DALIB200_DECODER_ARGS() DALIB200_CROP_ARGS();
 
@@ -364,7 +364,7 @@ static std::vector<RandomCropGenerator> MakeCropGeneratorsImpl(const OpSpec &spe
 }
 
 DALI_SCHEMA(decoders__ImageRandomCrop)
-    .DocStr("Decodes JPEG, PNG and TIFF images on the GPU and extracts a randomly placed window of random area and aspect ratio.")
+    .DocStr("Decodes JPEG, PNG, TIFF and lossy WebP images on the GPU and extracts a randomly placed window of random area and aspect ratio.")
     .NumInput(1).NumOutput(1)
     DALIB200_DECODER_ARGS() DALIB200_RANDOM_CROP_ARGS();
 
@@ -387,7 +387,7 @@ DALI_REGISTER_OPERATOR(decoders__ImageRandomCrop, ImageDecoderRandomCropMixed, M
 // (normalized by default) or as `start` / `rel_start` / `end` / `rel_end` / `shape` / `rel_shape` arguments, axes (1, 0) =
 // (x, y) by default ("WH").
 DALI_SCHEMA(decoders__ImageSlice)
-    .DocStr("Decodes JPEG, PNG and TIFF images on the GPU and extracts a region of interest given by anchor and shape.")
+    .DocStr("Decodes JPEG, PNG, TIFF and lossy WebP images on the GPU and extracts a region of interest given by anchor and shape.")
     .NumInput(1, 3).NumOutput(1)
     DALIB200_DECODER_ARGS()
     .AddOptionalArg("axes", "Order of the dimensions of anchor and shape.", std::vector<int>{1, 0})

@@ -56,8 +56,10 @@ int dalib200ProfilingCollect(char *names, int name_stride, float *ms, int max, i
  * entropy decode) and progressive (SOF2: scans in dependency waves, one warp per scan; spectral selection + successive approximation).
  * PNG (detected by its signature; IDAT CRCs, inflate + unfilter, colour conversion, bit-exact with cv2.imdecode).
  * TIFF (detected by its header; first IFD, strips or tiles, LZW / Deflate / PackBits / none, one GPU lane per segment, colour
- * conversion, bit-exact with cv2.imdecode; unsupported layouts fail with DALIB200_ERROR_UNSUPPORTED).  All formats may be mixed in one
- * batch of a plan.
+ * conversion, bit-exact with cv2.imdecode; unsupported layouts fail with DALIB200_ERROR_UNSUPPORTED).
+ * Lossy WebP (detected by its RIFF header; VP8 key frame: one GPU lane per image for the entropy decode, macroblock-wavefront
+ * reconstruction and loop filter, fancy upsampling, bit-exact with cv2.imdecode; lossless and animated WebP fail with
+ * DALIB200_ERROR_UNSUPPORTED).  All formats may be mixed in one batch of a plan.
  * Replaces: imgcodec::ImageDecoder<MixedBackend>::RunImplImpl -> nvimgcodecDecoderDecode
  *           (dali/operators/imgcodec/image_decoder.h:613-882) and ParseSample (:473-499).
  * Host work: marker / table / chunk-header parse only.  Device work: everything arithmetic. */
@@ -65,13 +67,13 @@ typedef struct dalib200JpegPlan dalib200JpegPlan;
 
 typedef struct {
   int32_t width, height;        /* decoded image size */
-  int32_t components;           /* JPEG: 1, 3 or 4; PNG, TIFF: channels of the file (palette: 3) */
-  int32_t subsampling;          /* (hmax<<4)|vmax of the luma sampling factors, e.g. 0x22 = 4:2:0 */
+  int32_t components;           /* JPEG: 1, 3 or 4; PNG, TIFF: channels of the file (palette: 3); WebP: 3, 4 with alpha */
+  int32_t subsampling;          /* (hmax<<4)|vmax of the luma sampling factors, e.g. 0x22 = 4:2:0 (WebP: always 0x22) */
   int32_t restart_interval;
   int32_t orientation;          /* EXIF orientation, 1 = none */
 } dalib200JpegInfo;
 
-/* header-only parse of a JPEG, PNG or TIFF stream: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
+/* header-only parse of a JPEG, PNG, TIFF or WebP stream: the analogue of nvimgcodecCodeStreamGetImageInfo (image_decoder.h:482) */
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info);
 
 int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch);

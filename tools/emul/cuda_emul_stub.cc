@@ -1,7 +1,8 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG and TIFF kernels are EXECUTED on the host -- their bodies are single
-// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h), so a launch is a loop over blocks and threads around
+// of the 3-D resize, progressive JPEG, PNG, TIFF and WebP kernels are EXECUTED on the host -- their bodies are single
+// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h), so a launch is a
+// loop over blocks and threads around
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
 // end to end without a GPU -- descriptor upload, temporaries, stage order, grid-stride loops, wave ranges, arena offsets -- and
 // tests/test_launch_emul_cpu.py compares what lands in "device" memory with the oracle.
@@ -10,6 +11,7 @@
 #define _GNU_SOURCE
 #endif
 #include <dlfcn.h>
+#include <algorithm>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -18,6 +20,7 @@
 #include "../../dali_b200/csrc/jpeg_prog_core.h"
 #include "../../dali_b200/csrc/png_core.h"
 #include "../../dali_b200/csrc/tiff_core.h"
+#include "../../dali_b200/csrc/webp_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -67,10 +70,10 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[8];
+static long g_emulated[12];
 long emul_launch_count(int which) { return g_emulated[which]; }
 
-// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu and tiff.cu, thread by thread
+// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu, tiff.cu and webp.cu, thread by thread
 static void run_resample3d_pass(Dim3 g, Dim3 b, void **args) {
   const R3Pass *passes = *static_cast<const R3Pass **>(args[0]);
   const int32_t *tab = *static_cast<const int32_t **>(args[1]);
@@ -199,6 +202,61 @@ static void run_tiff_color(Dim3 g, Dim3 b, void **args) {
       }
 }
 
+static void run_webp_entropy(Dim3 g, Dim3 b, void **args) {
+  const WebpImage *images = *static_cast<const WebpImage **>(args[0]);
+  const int nimages = *static_cast<int *>(args[1]);
+  const int lanes = *static_cast<int *>(args[2]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[3]);
+  uint8_t *scratch = *static_cast<uint8_t **>(args[4]);
+  int32_t *status = *static_cast<int32_t **>(args[5]);
+  for (int bx = (int)g.x - 1; bx >= 0; bx--)                 // blocks of a launch run in no particular order: take the reverse one
+    for (int tx = 0; tx < (int)b.x && tx < lanes; tx++)
+      for (int k = bx * lanes + tx; k < nimages; k += (int)g.x * lanes) {
+        const WebpImage &im = images[k];
+        if (webp_entropy(im, raw, reinterpret_cast<WebpMb *>(scratch + im.mb_off), reinterpret_cast<int16_t *>(scratch + im.coef_off),
+                         reinterpret_cast<uint32_t *>(scratch + im.ctx_off)))
+          status[im.sample] = 1;
+      }
+}
+// webp_wave_kernel<false / true>: one block per image; the macroblocks of each diagonal run in REVERSE thread order, so that a
+// dependency between two macroblocks of one diagonal shows up as a mismatch
+static void run_webp_wave(Dim3 g, Dim3 b, void **args, bool filter) {
+  const WebpImage *images = *static_cast<const WebpImage **>(args[0]);
+  uint8_t *scratch = *static_cast<uint8_t **>(args[1]);
+  const int32_t *status = *static_cast<const int32_t **>(args[2]);
+  for (int bx = (int)g.x - 1; bx >= 0; bx--) {
+    const WebpImage &im = images[bx];
+    if (status[im.sample] || (filter && im.filter_type == 0)) continue;
+    const WebpMb *mbs = reinterpret_cast<const WebpMb *>(scratch + im.mb_off);
+    const int16_t *coef = reinterpret_cast<const int16_t *>(scratch + im.coef_off);
+    for (int d = 0; d < im.mb_w + 2 * (im.mb_h - 1); d++) {
+      const int y_lo = std::max(0, (d - im.mb_w + 2) / 2), y_hi = std::min(im.mb_h - 1, d / 2);
+      for (int tx = (int)b.x - 1; tx >= 0; tx--)
+        for (int y = y_lo + tx; y <= y_hi; y += (int)b.x) {
+          if (filter) webp_filter_mb(im, mbs, scratch, d - 2 * y, y);
+          else webp_recon_mb(im, mbs, coef, scratch, d - 2 * y, y);
+        }
+    }
+  }
+}
+static void run_webp_color(Dim3 g, Dim3 b, void **args) {
+  const WebpImage *images = *static_cast<const WebpImage **>(args[0]);
+  const int nimages = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  uint8_t *scratch = *static_cast<uint8_t **>(args[3]);
+  const int64_t step = (int64_t)g.x * b.x;
+  for (unsigned bx = 0; bx < g.x; bx++)
+    for (unsigned tx = 0; tx < b.x; tx++)
+      for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
+        int lo = 0, hi = nimages - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
+        const WebpImage &im = images[lo];
+        const int64_t lp = e - im.first_px;
+        const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
+        webp_pixel(im, scratch, lx, ly);
+      }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -211,6 +269,10 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_png_color = !strcmp(name, "_ZN8dalib20016png_color_kernelEPKNS_8PngImageEilPKh");
   const bool is_tiff_segment = !strcmp(name, "_ZN8dalib20019tiff_segment_kernelEPKNS_9TiffImageEPKNS_7TiffSegEiiPKhPhS8_Pi");
   const bool is_tiff_color = !strcmp(name, "_ZN8dalib20017tiff_color_kernelEPKNS_9TiffImageEilPKNS_7TiffSegEPKh");
+  const bool is_webp_entropy = !strcmp(name, "_ZN8dalib20019webp_entropy_kernelEPKNS_9WebpImageEiiPKhPhPi");
+  const bool is_webp_recon = !strcmp(name, "_ZN8dalib20016webp_wave_kernelILb0EEEvPKNS_9WebpImageEPhPKi");
+  const bool is_webp_filter = !strcmp(name, "_ZN8dalib20016webp_wave_kernelILb1EEEvPKNS_9WebpImageEPhPKi");
+  const bool is_webp_color = !strcmp(name, "_ZN8dalib20017webp_color_kernelEPKNS_9WebpImageEilPh");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -223,6 +285,10 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_png_color) { run_png_color(grid, block, args); g_emulated[5]++; }
   else if (is_tiff_segment) { run_tiff_segment(grid, block, args); g_emulated[6]++; }
   else if (is_tiff_color) { run_tiff_color(grid, block, args); g_emulated[7]++; }
+  else if (is_webp_entropy) { run_webp_entropy(grid, block, args); g_emulated[8]++; }
+  else if (is_webp_recon) { run_webp_wave(grid, block, args, false); g_emulated[9]++; }
+  else if (is_webp_filter) { run_webp_wave(grid, block, args, true); g_emulated[10]++; }
+  else if (is_webp_color) { run_webp_color(grid, block, args); g_emulated[11]++; }
   return 0;
 }
 }  // extern "C"

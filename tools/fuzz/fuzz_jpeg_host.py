@@ -26,6 +26,16 @@ seeds += [bytearray(s) for _, s in png_streams.corpus()[::6]]
 # TIFF streams (strips, tiles, planes, both byte orders, every codec): the IFD walk and the segment table of the planner
 import tiff_streams
 seeds += [bytearray(s) for _, s in tiff_streams.corpus()[::8]]
+# WebP streams (simple and VP8X, alpha, EXIF, every partition count, simple and normal filter): the RIFF walk and the VP8 header parse.
+# Written by Pillow and libwebp's encoder only: cv2's WebP encoder throws (and catches) C++ exceptions, which the preloaded ASAN
+# runtime cannot intercept in cv2's module
+import webp_streams
+wimg = [np.random.default_rng(k).integers(0, 256, (h, w, 3), dtype=np.uint8) for k, (h, w) in enumerate([(1, 1), (17, 33), (40, 56)])]
+seeds += [bytearray(webp_streams.pil_webp(a, quality=q, method=m)) for a in wimg for q, m in ((20, 0), (90, 4))]
+seeds += [bytearray(webp_streams.pil_webp(np.dstack([wimg[1], wimg[1][..., 0]]), quality=60)),
+          bytearray(webp_streams.pil_webp(wimg[2], quality=60, exif=webp_streams.exif_orientation(6)))]
+if webp_streams.libwebp():
+    seeds += [bytearray(webp_streams.libwebp_encode(wimg[2], 60.0, partitions=3, method=2, filter_type=t)) for t in (0, 1)]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()
