@@ -91,6 +91,17 @@ def synth_image(h, w, seed):
     return np.clip(img, 0, 255).astype(np.uint8)
 
 
+def random_crop_window(seed, sample_idx, H, W, area=(0.08, 1.0), aspect=(3 / 4, 4 / 3), num_attempts=10, ncalls=1):
+    """(anchor_y, anchor_x, h, w) of the ncalls-th window the library's random crop generator draws for sample_idx: the one that
+    decoders.image_random_crop / random_resized_crop with this seed use in their ncalls-th iteration (host code only; the generator
+    is pinned to the reference's by tests/test_host_cpu.py where oracle/_ref exists)."""
+    from dali_b200 import backend
+    w = (C.c_int * (4 * ncalls))()
+    assert backend.lib().dalihTestRandomCrop(C.c_int64(seed), int(sample_idx), int(H), int(W), C.c_float(aspect[0]), C.c_float(aspect[1]),
+                                             C.c_float(area[0]), C.c_float(area[1]), int(num_attempts), int(ncalls), w) == 0
+    return tuple(w[4 * (ncalls - 1):4 * ncalls])
+
+
 def jpeg_decode(streams, output_type=capi.RGB, fancy=True, plan=None, want_coefs=False):
     torch = _torch()
     n = len(streams)

@@ -247,15 +247,11 @@ def test_exif_orientation_matches_libjpeg_consumers():
         assert np.array_equal(outs[o - 1], po.exif_transform(dec, o)[r[1]:r[3], r[0]:r[2]]), f"orientation {o} + roi"
 
 
-def _index_exact_convert(src, ot):
-    """The u8 RGB / BGR / GRAY outputs are pure channel selections of the decode (GRAY: the Y plane itself)."""
-    return np.ascontiguousarray(src[..., ::-1]) if ot == capi.BGR else src
-
-
 def test_output_type_and_dtype_conversion_match_reference_convert():
-    """Every output type and dtype against the reference's convert functors (oracle/_ref); where _ref is absent the YCbCr and float
-    conversions have no restatement to compare with, and only the index-exact u8 RGB / BGR / GRAY outputs are compared."""
+    """Every output type and dtype against the float32 and float64 forms of the convert functors (tests/pointwise_ref.py) and, where
+    present, the reference's own functors (oracle/_ref)."""
     import gpu_helpers as g
+    import pointwise_ref as pr
     ref = po.have_ref()
     streams = _variant_streams()
     full = [po.jpeg_decode(s) for s in streams]
@@ -266,23 +262,17 @@ def test_output_type_and_dtype_conversion_match_reference_convert():
             assert status == [0] * len(streams)
             for i in range(len(streams)):
                 src = gray[i] if ot == capi.GRAY else full[i]           # GRAY is decoded as the Y plane (image_decoder.h:537-540)
+                pr.check_decoder_output(outs[i], src, ot, fl, f"type {ot} dtype {dt} sample {i}")
                 if ref:
-                    want = po.ref_decoder_convert(src, it, fl)
-                elif not fl and ot != capi.YCbCr:
-                    want = _index_exact_convert(src, ot)
-                else:
-                    assert outs[i].dtype == (np.float32 if fl else np.uint8)
-                    continue
-                assert outs[i].dtype == want.dtype and np.array_equal(outs[i], want), f"type {ot} dtype {dt} sample {i}"
-    # everything at once: orientation + ROI + YCbCr float (without _ref: orientation + ROI + BGR u8)
+                    assert np.array_equal(outs[i], po.ref_decoder_convert(src, it, fl)), f"type {ot} dtype {dt} sample {i}"
+    # everything at once: orientation + ROI + YCbCr float
     s6 = po.with_exif_orientation(streams[0], 6)
     win = np.ascontiguousarray(po.exif_transform(full[0], 6)[9:260, 3:150])
+    out, status = g.jpeg_decode_ex([s6], output_type=capi.YCbCr, dtype=capi.FLOAT, rois=[(3, 9, 150, 260)])
+    assert status == [0]
+    pr.check_decoder_output(out[0], win, capi.YCbCr, True, "orientation 6 + roi")
     if ref:
-        out, _ = g.jpeg_decode_ex([s6], output_type=capi.YCbCr, dtype=capi.FLOAT, rois=[(3, 9, 150, 260)])
         assert np.array_equal(out[0], po.ref_decoder_convert(win, po.IT_YCBCR, True))
-    else:
-        out, _ = g.jpeg_decode_ex([s6], output_type=capi.BGR, dtype=capi.UINT8, rois=[(3, 9, 150, 260)])
-        assert np.array_equal(out[0], _index_exact_convert(win, capi.BGR))
 
 
 def test_truncated_stream_status_gray_tail_and_pipeline_error():

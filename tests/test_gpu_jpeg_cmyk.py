@@ -10,6 +10,7 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from dali_b200 import capi  # noqa: E402
+import pointwise_ref as pr  # noqa: E402
 from oracle import pyoracle as po  # noqa: E402
 
 
@@ -142,8 +143,8 @@ def test_exif_orientations(golden_dir):
 
 
 def test_ycbcr_and_float_outputs(golden_dir):
-    """As for 3-component streams: the post pass converts the RGB (GRAY) decode.  Compared with the reference's convert functors
-    (oracle/_ref) where present; otherwise u8 RGB / BGR / GRAY index-exactly and float RGB / BGR / GRAY as u8 * (1 / 255) in float32."""
+    """As for 3-component streams: the post pass converts the RGB (GRAY) decode.  Compared with the float32 and float64 forms of the
+    convert functors (tests/pointwise_ref.py) and, where present, the reference's own functors (oracle/_ref)."""
     import gpu_helpers as g
     from jpeg_cmyk_streams import photoshop_ycck
     fx = _fixtures(golden_dir)
@@ -159,16 +160,9 @@ def test_ycbcr_and_float_outputs(golden_dir):
             assert status == [0] * len(streams)
             for i in range(len(streams)):
                 src = gray[i] if ot == capi.GRAY else full[i]
-                assert outs[i].dtype == (np.float32 if fl else np.uint8) and outs[i].shape[:2] == src.shape[:2]
+                pr.check_decoder_output(outs[i], src, ot, fl, f"type {ot} dtype {dt} sample {i}")
                 if ref:
-                    want = po.ref_decoder_convert(src, it, fl)
-                elif ot == capi.YCbCr:
-                    continue
-                else:
-                    want = np.ascontiguousarray(src[..., ::-1]) if ot == capi.BGR else src
-                    if fl:
-                        want = want.astype(np.float32) * np.float32(1.0 / 255)
-                assert np.array_equal(outs[i], want), f"type {ot} dtype {dt} sample {i}"
+                    assert np.array_equal(outs[i], po.ref_decoder_convert(src, it, fl)), f"type {ot} dtype {dt} sample {i}"
 
 
 def test_truncated_cmyk_stream_sets_its_status():

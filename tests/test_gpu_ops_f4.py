@@ -1,13 +1,15 @@
 """-m gpu parity tests of the remaining per-pixel / geometry operators (SURVEY 8f rank 4) through the public API:
 brightness_contrast, color_twist, flip, crop, slice, rotate, resize_crop_mirror -- each against the reference's own CPU code
-(oracle/_ref) or, for pure index arithmetic, numpy.  Bit-exact.  Where oracle/_ref is absent, color_twist, the rotate warp and
-resize_crop_mirror are compared with the oracle's restatements instead (pinned to the reference by tests/golden/*_ref.npz), and the
-rotate canvas / matrix come from the library's own host code (pinned to the reference by tests/test_host_cpu.py where _ref exists)."""
+(oracle/_ref) or, for pure index arithmetic, numpy.  Bit-exact.  brightness_contrast is always compared with the float32 restatement
+of tests/pointwise_ref.py as well.  Where oracle/_ref is absent, color_twist, the rotate warp and resize_crop_mirror are compared with
+the oracle's restatements instead (pinned to the reference by tests/golden/*_ref.npz), and the rotate canvas / matrix come from the
+library's own host code (pinned to the reference by tests/test_host_cpu.py where _ref exists)."""
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
+import pointwise_ref as pr  # noqa: E402
 from oracle import pyoracle as po  # noqa: E402
 
 
@@ -56,7 +58,10 @@ def test_brightness_contrast_and_color_twist():
         fn.color_twist(x, hue=25.0, saturation=1.4, contrast=cos, brightness=brs),
         fn.color_twist(x, hue=-70.0, saturation=0.5, dtype=types.FLOAT)), extra_sources=(br, co))
     for i, im in enumerate(imgs):
-        if REF:          # brightness_contrast has no restatement outside the reference
+        assert np.array_equal(a[i], pr.brightness_contrast(im, float(br[i]), 0.1, float(co[i]))), i
+        want = pr.brightness_contrast(im, 1.2, 0.0, 0.9, 100.0, out_float=True)
+        assert b[i].dtype == np.float32 and np.array_equal(b[i].view(np.uint32), want.view(np.uint32)), i
+        if REF:
             assert np.array_equal(a[i], po.ref_brightness_contrast(im, float(br[i]), 0.1, float(co[i]))), i
             want = po.ref_brightness_contrast(im, 1.2, 0.0, 0.9, 100.0, out_float=True)
             assert np.array_equal(b[i].view(np.uint32), want.view(np.uint32)), i

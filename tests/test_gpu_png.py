@@ -10,6 +10,7 @@ pytestmark = pytest.mark.gpu
 from dali_b200 import capi  # noqa: E402
 import png_oracle as pngo  # noqa: E402
 import png_streams as ps  # noqa: E402
+import pointwise_ref as pr  # noqa: E402
 from oracle import pyoracle as po  # noqa: E402
 
 
@@ -32,8 +33,8 @@ def test_corpus_rgb_bgr_gray(corpus):
 
 
 def test_corpus_ycbcr_and_float(corpus):
-    """YCbCr and float are the post pass over the RGB (GRAY) decode, as for JPEG: compared with the reference's convert functors where
-    present, otherwise float RGB / BGR / GRAY as u8 * (1 / 255) in float32"""
+    """YCbCr and float are the post pass over the RGB (GRAY) decode, as for JPEG: compared with the float32 and float64 forms of the
+    convert functors (tests/pointwise_ref.py) and, where present, the reference's own functors"""
     import gpu_helpers as g
     streams, want, names = corpus
     ref = po.have_ref()
@@ -43,16 +44,9 @@ def test_corpus_ycbcr_and_float(corpus):
             assert status == [0] * len(streams)
             for i, o in enumerate(outs):
                 src = want[i][1][..., None] if ot == capi.GRAY else want[i][0]
+                pr.check_decoder_output(o, src, ot, fl, (names[i], ot, dt))
                 if ref:
-                    w = po.ref_decoder_convert(src, it, fl)
-                elif ot == capi.YCbCr:
-                    assert o.shape == src.shape
-                    continue
-                else:
-                    w = np.ascontiguousarray(src[..., ::-1]) if ot == capi.BGR else src
-                    if fl:
-                        w = w.astype(np.float32) * np.float32(1.0 / 255)
-                assert np.array_equal(o, w), (names[i], ot, dt)
+                    assert np.array_equal(o, po.ref_decoder_convert(src, it, fl)), (names[i], ot, dt)
 
 
 def test_roi_windows_equal_crops_of_the_full_decode():
@@ -79,8 +73,9 @@ def test_roi_windows_equal_crops_of_the_full_decode():
 
 def test_crop_operators_on_png():
     """fn.decoders.image_crop / image_random_crop / image_slice on PNG samples equal the expected windows of the full decode: the
-    crop anchor and slice rounding of the reference (as tests/test_gpu_pipeline.py checks them for JPEG); the random window against
-    the reference's generator where its compiled kernels are present, otherwise its shape and placement inside the image"""
+    crop anchor and slice rounding of the reference (as tests/test_gpu_pipeline.py checks them for JPEG); the random window is the one
+    the library's generator draws for the seed (and the reference's generator, where its compiled kernels are present)"""
+    import gpu_helpers as g
     from dali_b200 import fn, pipeline_def
     streams = [np.frombuffer(ps.encode(ps.samples(h, w, 2, 8, 60 + h), 2, 8, filters="mixed", interlace=h % 2 == 1), np.uint8)
                for h, w in ((120, 160), (77, 95), (64, 64))]
@@ -113,13 +108,10 @@ def test_crop_operators_on_png():
         sx, sy = float(shapes[i][0]), float(shapes[i][1])
         assert np.array_equal(c[i], f[rnd(ay * H):rnd((ay + sy) * H), rnd(ax * W):rnd((ax + sx) * W)]), i
         assert np.array_equal(d[i], f[16:56, 30:60]), i
+        wy, wx, wh, ww = g.random_crop_window(1234, i, H, W, area=(0.1, 0.9))
+        assert b[i].shape == (wh, ww, 3) and np.array_equal(b[i], f[wy:wy + wh, wx:wx + ww]), i
         if po.have_ref():
-            wy, wx, wh, ww = po.ref_random_crop(1234, i, H, W, area=(0.1, 0.9), ncalls=1)[0]
-            assert np.array_equal(b[i], f[wy:wy + wh, wx:wx + ww]), i
-        else:
-            h, w = b[i].shape[:2]
-            assert 0.1 * H * W * 0.9 <= h * w <= H * W, (i, b[i].shape)
-            assert any(np.array_equal(f[y:y + h, x:x + w], b[i]) for y in range(H - h + 1) for x in range(W - w + 1)), i
+            assert po.ref_random_crop(1234, i, H, W, area=(0.1, 0.9), ncalls=1)[0] == (wy, wx, wh, ww), i
 
 
 def test_exif_orientations():
