@@ -41,6 +41,8 @@ EXPORTS = [
     "dalib200GenericPlanCreate", "dalib200GenericPlanDestroy", "dalib200MultiplyAddSetup", "dalib200WindowCopySetup", "dalib200GenericLaunch",
     "dalib200MelPlanCreate", "dalib200MelPlanDestroy", "dalib200MelPlanSetup", "dalib200MelLaunch", "dalib200MelPlanSetTensorCores",
     "dalib200SpectrogramMelSupported", "dalib200SpectrogramMelLaunch",
+    "dalib200JpegDistortPlanCreate", "dalib200JpegDistortPlanDestroy", "dalib200JpegDistortPlanSetup", "dalib200JpegDistortLaunch",
+    "dalib200JpegDistortDebugGetCoefficients",
 ]
 
 
@@ -60,6 +62,10 @@ class JpegRoi(C.Structure):
 class PlanarImage(C.Structure):
     _fields_ = [("y", C.c_void_p), ("cb", C.c_void_p), ("cr", C.c_void_p), ("pitch_y", C.c_int32), ("pitch_c", C.c_int32),
                 ("width", C.c_int32), ("height", C.c_int32), ("crop_x", C.c_int32), ("crop_y", C.c_int32)]
+
+
+class JpegDistortSample(C.Structure):
+    _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("quality", C.c_int32)]
 
 
 class FilterDesc(C.Structure):

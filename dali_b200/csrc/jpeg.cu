@@ -28,6 +28,7 @@
 // on streams of their own, and the post pass below serves every format.  A PNG, TIFF or WebP sample has no units, subsequences or MCUs,
 // so every kernel of this file skips it.
 #include "common.cuh"
+#include "jpeg_recon.h"
 #include <algorithm>
 #include <cstring>
 #include <map>
@@ -41,7 +42,6 @@ constexpr int kLutWords = 2 * kDcLutSize + 2 * kAcLutSize;          // DC0 DC1 A
 constexpr int kSyncThreads = 256;            // subsequences per synchronisation block
 constexpr int kChunkBytes = 4096;            // un-stuffing chunk
 constexpr uint32_t kCleanPad = 32;           // zero bytes behind the clean stream of every unit (at least: units are 16-byte aligned)
-constexpr int kMaxBlocksPerMcu = 10;
 constexpr int kMaxLog2Sub = 10;              // largest subsequence: 2^10 bits = 128 bytes
 
 // Huffman tables as the device sees them.  The first-level LUTs (one 32-bit entry per 10-bit prefix, see make_entry) are
@@ -64,46 +64,6 @@ struct TableSet {             // the 4 tables a baseline scan can reference: DC0
   HuffSlow slow[4];
 };
 __host__ __device__ inline int LutOffset(int t) { return t < 2 ? t * kDcLutSize : 2 * kDcLutSize + (t - 2) * kAcLutSize; }
-
-struct QuantSet { uint16_t q[4][64]; };       // natural order
-
-// Colour space of the decoded components (libjpeg default_decompress_parms).  Decided once per image by the plan; the kernels read
-// nothing else to pick the conversion.
-enum JpegColor : int32_t {
-  kColorGray = 0,     // 1 component
-  kColorYCbCr = 1,    // 3 components
-  kColorRGB = 2,      // 3 components: Adobe transform 0, or R/G/B component ids without JFIF / Adobe markers
-  kColorCMYK = 3,     // 4 components: Adobe transform 0, or no Adobe marker
-  kColorYCCK = 4,     // 4 components: any other Adobe transform (components 0..2 are the YCbCr of 255 - C, 255 - M, 255 - Y)
-};
-
-struct JpegImage {
-  uint8_t *out;               // HWC u8
-  int32_t width, height, ncomp;
-  int32_t hs[4], vs[4], hmax, vmax;
-  int32_t mcux, mcuy, bpm;    // MCUs per row / column, blocks per MCU
-  int32_t blk_comp[kMaxBlocksPerMcu];      // component of each block in the MCU
-  int32_t blk_dc[kMaxBlocksPerMcu], blk_ac[kMaxBlocksPerMcu];   // table index (0..3) into TableSet
-  int32_t blk_x[kMaxBlocksPerMcu], blk_y[kMaxBlocksPerMcu];     // block offset inside the MCU (in blocks)
-  int32_t tq[4];
-  int32_t restart_interval;
-  int32_t table_set, quant_set;
-  int32_t unit_begin, unit_end;            // segments (restart intervals or the whole scan)
-  int32_t subseq_begin;                    // first global subsequence
-  int32_t nsub;                            // upper bound of subsequences (from raw length)
-  int32_t block_begin;                     // first sync block
-  int32_t wblock_begin;                    // first block of the write pass (kWriteThreads subsequences each)
-  int64_t coef_off;                        // int16 offset into the coefficient arena
-  int64_t plane_off[4];                    // byte offsets into the plane arena
-  int32_t plane_w[4], plane_h[4];          // padded plane sizes (multiples of the MCU)
-  int32_t out_type, fancy;
-  int32_t color;                           // JpegColor
-  int32_t fast_color;                      // 1: color_fast_kernel, 2: idct_color_420 (4:2:0 fancy -> RGB / BGR), 0: color_kernel
-  // decode window: the pixels [win_x0, win_x0 + win_w) x [win_y0, win_y0 + win_h) of the (un-oriented) image are produced, `out`
-  // is a tight win_h x win_w x C buffer (the caller's sample, or plan scratch when a post pass follows).  win_x0 % 8 == 0.
-  int32_t win_x0, win_y0, win_w, win_h;
-  int32_t mcu_x0, mcu_y0, mcu_nx, mcu_ny;  // MCUs whose blocks the IDCT transforms (window + chroma upsampling halo)
-};
 
 // Post pass of one sample (decoders.image with output_type / dtype / orientation / unaligned ROI handling): gathers the
 // oriented region of interest from the decoded window and converts colour space and type
@@ -1420,25 +1380,6 @@ __global__ void __launch_bounds__(128, 10) color_fast_kernel(const JpegImage *__
 // The IDCT of band m leaves its last luma and chroma rows in carry row m & 1 as well, where band m + 1 finds them while the IDCT of
 // band m + 1 is already overwriting the band rows.  A segment that does not start at the top first transforms the band above it.  The
 // horizontal halo is the edge column of the chroma blocks of the MCUs left and right of the strip.
-constexpr int kFusedMcus = 16;                     // 256 luma columns per strip
-constexpr int kFusedMaxBands = 24;
-constexpr int kFusedThreads = 128;                 // >= 6 * kFusedMcus + 4 blocks: one IDCT per thread and band
-constexpr int kFusedCPitch = 8 * kFusedMcus + 16;  // chroma tile: byte 8 + (i - 8 * first MCU column) holds chroma column i
-
-struct FusedGeo { int mx0, mx_end, nstrips, m0, nbands, nseg, seg_len; };
-__host__ __device__ inline FusedGeo fused_geo(const JpegImage &im) {
-  FusedGeo g;
-  const int wx1 = im.win_x0 + im.win_w, wy1 = im.win_y0 + im.win_h, last = im.mcuy - 1;
-  g.mx0 = im.win_x0 >> 4; g.mx_end = ((wx1 - 1) >> 4) + 1;                  // MCU columns that hold window pixels
-  g.nstrips = (g.mx_end - g.mx0 + kFusedMcus - 1) / kFusedMcus;
-  g.m0 = (im.win_y0 + 1) >> 4; if (g.m0 > last) g.m0 = last;                // band of row win_y0: min((y + 1) >> 4, last)
-  const int m1 = wy1 >> 4;
-  g.nbands = (m1 < last ? m1 : last) - g.m0 + 1;
-  g.nseg = (g.nbands + kFusedMaxBands - 1) / kFusedMaxBands;
-  g.seg_len = (g.nbands + g.nseg - 1) / g.nseg;
-  return g;
-}
-
 // the 16 upsampled chroma samples of luma columns 2 * i0 .. 2 * i0 + 15 from the near / far chroma tile rows; c = tile byte of column i0
 __device__ __forceinline__ void fancy_row16(const uint8_t *near, const uint8_t *far, int c, int i0, int dw, int *v) {
   const uint2 a = *reinterpret_cast<const uint2 *>(near + c), b = *reinterpret_cast<const uint2 *>(far + c);
@@ -1646,6 +1587,54 @@ __global__ void __launch_bounds__(256) jpeg_post_kernel(const JpegPost *__restri
       op[0] = post_cvt<Out>(r); op[1] = post_cvt<Out>(g); op[2] = post_cvt<Out>(b);
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Reconstruct stage on the host: path choice, work lists, launches (jpeg_recon.h)
+void ReconAddImage(JpegImage &im, bool fancy, bool planes_only, ReconTotals &t, int64_t *first_work, int64_t *first_fused,
+                   int64_t *first_quad, int64_t *first_item) {
+  im.fast_color = im.ncomp == 3 && im.color == kColorYCbCr && (im.out_type == DALIB200_RGB || im.out_type == DALIB200_BGR) &&
+                  ((im.hmax == 2 && im.vmax <= 2) || (im.hmax == 1 && im.vmax <= 2));
+  if (im.fast_color && fancy && im.hmax == 2 && im.vmax == 2 && (im.width + 1) / 2 > 2) im.fast_color = 2;    // idct_color_420
+  if (planes_only) im.fast_color = 1;                                   // IDCT into the planes, no colour work items
+  *first_work = t.work;
+  *first_fused = t.fused;
+  *first_quad = t.quads;
+  *first_item = t.items;
+  if (im.fast_color == 2) {
+    const FusedGeo g = fused_geo(im);
+    t.fused += (int64_t)g.nstrips * g.nseg;
+    return;
+  }
+  t.work += (int64_t)im.mcu_nx * im.mcu_ny * im.bpm;
+  if (planes_only) return;
+  if (im.fast_color) t.items += (int64_t)((im.win_w + kColorSeg - 1) / kColorSeg) * im.win_h;
+  else t.quads += (int64_t)((im.win_w + 3) / 4) * im.win_h;
+}
+
+int LaunchReconstruct(const ReconLaunch &a, cudaStream_t s) {
+  const int sms = NumSMs();
+  const int64_t total_blocks = a.totals.work;
+  const int grid = (int)std::min<int64_t>((total_blocks + 127) / 128, (int64_t)sms * 32);
+  if (total_blocks > 0) {
+    ProfScope ps_("jpeg_idct", s);
+    idct_kernel<<<grid, 128, 0, s>>>(a.d_images, a.d_first_work, a.nimages, total_blocks, a.d_coef, a.d_dc, a.d_quants, a.d_planes);
+  }
+  if (a.totals.fused > 0) {
+    { ProfScope ps_("jpeg_idct_color", s); idct_color_420<<<(int)a.totals.fused, kFusedThreads, 0, s>>>(a.d_images, a.d_first_fused, a.nimages, a.d_coef, a.d_dc, a.d_quants); }
+    CountLaunch();
+  }
+  if (a.totals.quads > 0) {
+    const int grid2 = (int)std::min<int64_t>((a.totals.quads + 255) / 256, (int64_t)sms * 32);
+    { ProfScope ps_("jpeg_upsample_color_generic", s); color_kernel<<<grid2, 256, 0, s>>>(a.d_images, a.d_first_quad, a.nimages, a.totals.quads, a.d_planes); }
+    CountLaunch();
+  }
+  if (a.totals.items > 0) {
+    const int grid3 = (int)std::min<int64_t>(a.totals.items, (int64_t)sms * 64);
+    { ProfScope ps_("jpeg_upsample_color", s); color_fast_kernel<<<grid3, 128, 0, s>>>(a.d_images, a.d_first_item, a.nimages, a.totals.items, a.d_planes); }
+    CountLaunch();
+  }
+  return DALIB200_SUCCESS;
 }
 
 }  // namespace dalib200
@@ -2015,7 +2004,8 @@ namespace {
 void BuildWorkLists(dalib200JpegPlan *p) {
   const int n = p->n;
   p->posts.clear(); p->post_sample.clear(); p->post_off.clear();
-  int64_t work = 0, fused = 0, post_px = 0, quads = 0, items = 0;
+  ReconTotals t;
+  int64_t post_px = 0;
   size_t post_bytes = 0;
   for (int i = 0; i < n; i++) {
     JpegImage &im = p->images[i];
@@ -2038,29 +2028,13 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
     if (j.png || j.tiff || j.webp) {   // decoded by png.cu / tiff.cu / webp.cu: no IDCT / colour work
-      p->first_work[i] = work; p->first_fused[i] = fused; p->first_quad[i] = quads; p->first_item[i] = items;
+      p->first_work[i] = t.work; p->first_fused[i] = t.fused; p->first_quad[i] = t.quads; p->first_item[i] = t.items;
       continue;
     }
-    im.fast_color = j.ncomp == 3 && im.color == kColorYCbCr && (im.out_type == DALIB200_RGB || im.out_type == DALIB200_BGR) &&
-                    ((j.hmax == 2 && j.vmax <= 2) || (j.hmax == 1 && j.vmax <= 2));
-    if (im.fast_color && p->fancy && j.hmax == 2 && j.vmax == 2 && (j.width + 1) / 2 > 2) im.fast_color = 2;    // idct_color_420
-    if (planes_only) im.fast_color = 1;                                   // IDCT into the planes, no colour work items
-    p->first_work[i] = work;
-    p->first_fused[i] = fused;
-    p->first_quad[i] = quads;
-    p->first_item[i] = items;
-    if (im.fast_color == 2) {
-      const FusedGeo g = fused_geo(im);
-      fused += (int64_t)g.nstrips * g.nseg;
-      continue;
-    }
-    work += (int64_t)im.mcu_nx * im.mcu_ny * im.bpm;
-    if (planes_only) continue;
-    if (im.fast_color) items += (int64_t)((im.win_w + kColorSeg - 1) / kColorSeg) * im.win_h;
-    else quads += (int64_t)((im.win_w + 3) / 4) * im.win_h;
+    ReconAddImage(im, p->fancy != 0, planes_only, t, &p->first_work[i], &p->first_fused[i], &p->first_quad[i], &p->first_item[i]);
   }
-  p->total_work = work; p->total_fused = fused; p->total_post_px = post_px; p->post_bytes = post_bytes; p->total_quads = quads;
-  p->total_items = items;
+  p->total_work = t.work; p->total_fused = t.fused; p->total_post_px = post_px; p->post_bytes = post_bytes; p->total_quads = t.quads;
+  p->total_items = t.items;
 }
 
 // Output geometry of sample i: orientation, region of interest, decode window, post pass.  Returns a DALIB200 status.
@@ -3011,28 +2985,14 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   { ProfScope ps_("jpeg_truncation_fixup", s); truncation_fixup_kernel<<<p->n, 256, 0, s>>>(cx); }
   CountLaunch();
   {
-    const int64_t total_blocks = p->total_work;
-    const auto *d_work = reinterpret_cast<const int64_t *>(p->d_stage + p->off_work);
-    const int grid = (int)std::min<int64_t>((total_blocks + 127) / 128, (int64_t)sms * 32);
-    if (total_blocks > 0) {
-      ProfScope ps_("jpeg_idct", s);
-      idct_kernel<<<grid, 128, 0, s>>>(d_images, d_work, p->n, total_blocks, p->d_coef, p->d_dc, d_quants, p->d_planes);
-    }
-    if (p->total_fused > 0) {
-      const auto *d_fused = reinterpret_cast<const int64_t *>(p->d_stage + p->off_fused);
-      { ProfScope ps_("jpeg_idct_color", s); idct_color_420<<<(int)p->total_fused, kFusedThreads, 0, s>>>(d_images, d_fused, p->n, p->d_coef, p->d_dc, d_quants); }
-      CountLaunch();
-    }
-    if (p->total_quads > 0) {
-      const int grid2 = (int)std::min<int64_t>((p->total_quads + 255) / 256, (int64_t)sms * 32);
-      { ProfScope ps_("jpeg_upsample_color_generic", s); color_kernel<<<grid2, 256, 0, s>>>(d_images, d_quads, p->n, p->total_quads, p->d_planes); }
-      CountLaunch();
-    }
-    if (p->total_items > 0) {
-      const int grid3 = (int)std::min<int64_t>(p->total_items, (int64_t)sms * 64);
-      { ProfScope ps_("jpeg_upsample_color", s); color_fast_kernel<<<grid3, 128, 0, s>>>(d_images, d_items, p->n, p->total_items, p->d_planes); }
-      CountLaunch();
-    }
+    ReconLaunch ra;
+    ra.d_images = d_images; ra.nimages = p->n;
+    ra.totals.work = p->total_work; ra.totals.fused = p->total_fused; ra.totals.quads = p->total_quads; ra.totals.items = p->total_items;
+    ra.d_first_work = reinterpret_cast<const int64_t *>(p->d_stage + p->off_work);
+    ra.d_first_fused = reinterpret_cast<const int64_t *>(p->d_stage + p->off_fused);
+    ra.d_first_quad = d_quads; ra.d_first_item = d_items;
+    ra.d_coef = p->d_coef; ra.d_dc = p->d_dc; ra.d_quants = d_quants; ra.d_planes = p->d_planes;
+    if ((rc = LaunchReconstruct(ra, s))) return rc;
   }
   if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png_join, 0));       // the PNG samples' windows and status are in place
   if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff_join, 0));     // the TIFF samples' windows and status are in place

@@ -1769,6 +1769,68 @@ class ColorTwistGPU : public PointwiseBase {
 };
 DALI_REGISTER_OPERATOR(ColorTwist, ColorTwistGPU, GPU);
 
+// =============================================================================================== JpegCompressionDistortion
+// dali/operators/image/distortion/jpeg_compression_distortion_op.{h,cc}: every image (every frame of a sequence, at its sample's
+// quality) goes through a JPEG encode + decode, bit-exact with cv2.imencode(".jpg", quality) + cv2.imdecode.
+DALI_SCHEMA(JpegCompressionDistortion)
+    .DocStr("Introduces JPEG compression artifacts to RGB images: each image is JPEG-encoded at `quality` and decoded again.")
+    .NumInput(1).NumOutput(1).AllowSequences()
+    .AddOptionalArg("quality", "JPEG compression quality from 1 (lowest) to 100 (highest).", 50, true);
+
+class JpegCompressionDistortionGPU : public Operator<GPUBackend> {
+ public:
+  explicit JpegCompressionDistortionGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
+  ~JpegCompressionDistortionGPU() override { dalib200JpegDistortPlanDestroy(plan_); }
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    DALI_ENFORCE(in.type() == DALI_UINT8, "JpegCompressionDistortion: the input must be uint8");
+    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "JpegCompressionDistortion");
+    std::vector<dalib200JpegDistortSample> s;
+    kept_.clear();
+    for (int k = 0; k < frames_.num_frames(); k++) {
+      DALI_ENFORCE(frames_.c[k] == 3, "JpegCompressionDistortion: the input must have 3 channels (channel-last RGB), got ", frames_.c[k]);
+      if (frames_.h[k] == 0 || frames_.w[k] == 0) continue;        // nothing to compress
+      const int q = spec_.GetArgument<int>("quality", &ws, frames_.sample_of_frame[k]);
+      DALI_ENFORCE(q >= 1 && q <= 100, "JpegCompressionDistortion: quality must be in [1, 100], got ", q, " for sample ",
+                   frames_.sample_of_frame[k]);
+      s.push_back({ frames_.h[k], frames_.w[k], q });
+      kept_.push_back(k);
+    }
+    const int n = static_cast<int>(s.size());
+    if (n > plan_cap_) {
+      dalib200JpegDistortPlanDestroy(plan_); plan_ = nullptr;
+      plan_cap_ = std::max(n, max_batch_size_);
+      CheckStatus(dalib200JpegDistortPlanCreate(&plan_, plan_cap_), "JpegCompressionDistortion");
+    }
+    if (plan_) CheckStatus(dalib200JpegDistortPlanSetup(plan_, n, s.data()), "JpegCompressionDistortion");
+    out.resize(1);
+    out[0].shape = in.shape(); out[0].type = DALI_UINT8;
+    return true;
+  }
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(in.GetLayout());
+    if (kept_.empty()) return;
+    const auto ip = FramePtrs(in, frames_, 1);
+    std::vector<const void *> src(kept_.size());
+    std::vector<void *> dst(kept_.size());
+    for (size_t i = 0; i < kept_.size(); i++) {
+      const int k = kept_[i];
+      src[i] = ip[k];
+      dst[i] = static_cast<uint8_t *>(out.raw_mutable_tensor(frames_.sample_of_frame[k])) + frames_.frame_offset_elems[k];
+    }
+    CheckStatus(dalib200JpegDistortLaunch(plan_, src.data(), dst.data(), ws.stream()), "JpegCompressionDistortion");
+  }
+ private:
+  dalib200JpegDistortPlan *plan_ = nullptr;
+  int plan_cap_ = 0;
+  FrameList frames_;
+  std::vector<int> kept_;                    // frames with pixels, in plan order
+};
+DALI_REGISTER_OPERATOR(JpegCompressionDistortion, JpegCompressionDistortionGPU, GPU);
+
 // =============================================================================================== Flip / Crop / Slice
 // Window copies of interleaved u8 images (dali/operators/generic/flip.{h,cc}, image/crop/crop.{h,cc}, generic/slice/slice.{h,cc}).
 class WindowOpBase : public GenericOpBase {

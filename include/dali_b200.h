@@ -155,6 +155,25 @@ int dalib200JpegStatusFetch(const dalib200JpegPlan *plan, int32_t *status_out, i
 int dalib200JpegDebugGetCoefficients(dalib200JpegPlan *plan, int sample, int16_t *out, size_t count);
 
 /* ------------------------------------------------------------------------------------------------
+ * JPEG compression distortion (fn.jpeg_compression_distortion): every RGB u8 image is JPEG-compressed at its quality and decoded
+ * again, bit-exact with cv2.imdecode(cv2.imencode(".jpg", img, {IMWRITE_JPEG_QUALITY, quality}), IMREAD_COLOR) (libjpeg-turbo
+ * defaults: 4:2:0, islow DCT, the Annex K tables scaled by the quality, fancy upsampling).  No entropy-coded stream is written: the
+ * quantised coefficients go straight to the decoder's reconstruct kernels.
+ * Replaces: JpegCompressionDistortion (dali/operators/image/distortion/jpeg_compression_distortion_op*.{h,cc}). */
+typedef struct dalib200JpegDistortPlan dalib200JpegDistortPlan;
+typedef struct { int32_t height, width, quality; } dalib200JpegDistortSample;
+
+int dalib200JpegDistortPlanCreate(dalib200JpegDistortPlan **plan, int max_batch);
+int dalib200JpegDistortPlanDestroy(dalib200JpegDistortPlan *plan);
+/* quality in [1, 100]; each side in [1, 65500] (libjpeg's limit); otherwise DALIB200_ERROR_INVALID_ARGUMENT */
+int dalib200JpegDistortPlanSetup(dalib200JpegDistortPlan *plan, int n, const dalib200JpegDistortSample *samples);
+/* in_ptrs[i] / out_ptrs[i]: device HWC RGB u8 [height][width][3]; in and out must not overlap */
+int dalib200JpegDistortLaunch(dalib200JpegDistortPlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
+/* Test accessor: the quantised coefficients of one sample after a launch (MCU order Y00 Y01 Y10 Y11 Cb Cr, natural order per block,
+ * absolute DC), as the JPEG stream cv2.imencode writes would hold them.  Synchronises. */
+int dalib200JpegDistortDebugGetCoefficients(dalib200JpegDistortPlan *plan, int sample, int16_t *out, size_t count);
+
+/* ------------------------------------------------------------------------------------------------
  * Separable resampling (fused two-pass).  Replaces kernels::ResampleGPU / SeparableResamplingGPUImpl::Run
  * (dali/kernels/imgproc/resample/separable_impl.h:110-203) and BatchResamplingSetup::SetupBatch
  * (resampling_setup.cc:347-418); numerics follow the CPU kernel SeparableResampleCPU

@@ -12,6 +12,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."
 from dali_b200 import capi  # noqa: E402
 
 rng = np.random.default_rng(int(sys.argv[1]) if len(sys.argv) > 1 else 0)
+jd_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 1])
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
 L = capi.lib()
 MILD = float(os.environ.get("FUZZ_BAD_SCALE", "1"))      # < 1: fewer adversarial values per call -> more set-ups reach their deep paths
@@ -61,7 +62,7 @@ def note(name, rc):
     hist[(name, "ok" if rc == 0 else "err")] = hist.get((name, "ok" if rc == 0 else "err"), 0) + 1
 
 
-plans = {k: plan(k, 8) for k in ("Resample", "Resample3D", "Cmn", "Warp", "Pointwise", "Spectrogram", "Mel", "Signal", "Generic")}
+plans = {k: plan(k, 8) for k in ("Resample", "Resample3D", "Cmn", "Warp", "Pointwise", "Spectrogram", "Mel", "Signal", "Generic", "JpegDistort")}
 for it in range(N):
     n = int(rng.integers(0, 9)) if rng.random() < 0.9 else int(rng.choice([9, 100, -1]))
     m = max(n, 1) if n < 64 else 8
@@ -233,4 +234,14 @@ for it in range(N):
     note("window_copy", rc)
     if rc == 0:
         launch("window_copy", L.dalib200GenericLaunch, plans["Generic"].handle, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
+    # ---- jpeg compression distortion: drawn from a generator of its own, so the draws of the entry points above stay as they were
+    rng, main_rng = jd_rng, rng
+    JD = (capi.JpegDistortSample * m)()
+    for s in JD:
+        s.height, s.width, s.quality = dim(), dim(), code(range(1, 101))
+    rc = L.dalib200JpegDistortPlanSetup(plans["JpegDistort"].handle, n, JD)
+    note("jpeg_distort", rc)
+    if rc == 0:
+        launch("jpeg_distort", L.dalib200JpegDistortLaunch, plans["JpegDistort"].handle, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
+    rng = main_rng
 print("seed", sys.argv[1] if len(sys.argv) > 1 else 0, "iterations", N, "- no sanitizer report;", {f"{k[0]}:{k[1]}": v for k, v in sorted(hist.items())})
