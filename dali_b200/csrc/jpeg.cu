@@ -1661,14 +1661,20 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 #include "webp_plan.h"
 namespace {
 
+// The formats the plan takes, told apart by their signatures.  PNG, TIFF and WebP samples are planned by png_plan.h, tiff_plan.h and
+// webp_plan.h and decoded by png.cu, tiff.cu and webp.cu; everything else is parsed as JPEG.
+enum class Format { kJpeg, kPng, kTiff, kWebp };
+
+Format DetectFormat(const uint8_t *p, size_t n) {
+  return IsPngStream(p, n) ? Format::kPng : IsTiffStream(p, n) ? Format::kTiff : IsWebpStream(p, n) ? Format::kWebp : Format::kJpeg;
+}
+
 struct ParsedJpeg {
   int width = 0, height = 0, ncomp = 0, precision = 8;
   int cid[4] = {0}, hs[4] = {0}, vs[4] = {0}, tq[4] = {0};
   int hmax = 0, vmax = 0;
   bool progressive = false, jfif = false;
-  bool png = false;           // a PNG stream (png_plan.h): width / height / ncomp / orientation / scan range only
-  bool tiff = false;          // a TIFF stream (tiff_plan.h): the same fields
-  bool webp = false;          // a lossy WebP stream (webp_plan.h): the same fields
+  Format format = Format::kJpeg;   // PNG, TIFF, WebP: width / height / ncomp / orientation / scan range and hs[0] / vs[0] only
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
   HostHuff dc[4], ac[4];
@@ -1770,55 +1776,6 @@ int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
   return DALIB200_SUCCESS;
 }
 
-// PNG stream (png_plan.h): fills the fields of `j` the plan reads for every sample (size, components, orientation, staged byte
-// range); `im` / `chunks`, when given, receive the device descriptors of batch image `image`.  Returns a DALIB200 status.
-int ParsePng(const uint8_t *p, size_t n, ParsedJpeg &j, PngImage *im, std::vector<PngChunk> *chunks, int image) {
-  PngImage tmp;
-  std::vector<PngChunk> tmpc;
-  PngInfo info;
-  std::string err;
-  const int rc = PlanPng(p, n, image, im ? im : &tmp, chunks ? *chunks : tmpc, &info, &err);
-  if (rc) { SetLastError("%s", err.c_str()); return rc; }
-  j.png = true;
-  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
-  j.hs[0] = j.vs[0] = 1;
-  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
-  return DALIB200_SUCCESS;
-}
-
-// TIFF stream (tiff_plan.h), as ParsePng; `dec_base` / `dec_bytes`: the image's range of the decoded-segment scratch
-int ParseTiff(const uint8_t *p, size_t n, ParsedJpeg &j, TiffImage *im, std::vector<TiffSeg> *segs, int image, int64_t dec_base,
-              int64_t *dec_bytes) {
-  TiffImage tmp;
-  std::vector<TiffSeg> tmps;
-  TiffInfo info;
-  int64_t tmpd;
-  std::string err;
-  const int rc = PlanTiff(p, n, image, im ? im : &tmp, segs ? *segs : tmps, dec_base, dec_bytes ? dec_bytes : &tmpd, &info, &err);
-  if (rc) { SetLastError("%s", err.c_str()); return rc; }
-  j.tiff = true;
-  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
-  j.hs[0] = j.vs[0] = 1;
-  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
-  return DALIB200_SUCCESS;
-}
-
-// lossy WebP stream (webp_plan.h), as ParsePng; `scratch_base` / `scratch_bytes`: the image's range of the WebP scratch.  The
-// subsampling reported is 4:2:0 (VP8's only layout).
-int ParseWebp(const uint8_t *p, size_t n, ParsedJpeg &j, WebpImage *im, int image, int64_t scratch_base, int64_t *scratch_bytes) {
-  WebpImage tmp;
-  WebpInfo info;
-  int64_t tmpb;
-  std::string err;
-  const int rc = PlanWebp(p, n, image, im ? im : &tmp, scratch_base, scratch_bytes ? scratch_bytes : &tmpb, &info, &err);
-  if (rc) { SetLastError("%s", err.c_str()); return rc; }
-  j.webp = true;
-  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
-  j.hs[0] = j.vs[0] = 2;
-  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
-  return DALIB200_SUCCESS;
-}
-
 void FillInfo(const ParsedJpeg &j, dalib200JpegInfo *info) {
   info->width = j.width; info->height = j.height;
   info->components = j.ncomp;
@@ -1886,6 +1843,50 @@ void BuildDeviceTable(const HostHuff &h, uint32_t *lut, uint16_t *lut16, HuffSlo
 
 }  // namespace
 
+// A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP), for samples whose decode is a serial chain per
+// image: it runs on a stream of its own, so that those chains overlap the JPEG kernels.  Its order on the caller's stream s:
+//   Begin(s)   after the status clear: fork (s -> stage stream), then wait until the previous upload of the pinned arena is done;
+//   Upload()   the arena, filled by the caller, goes to the device on the stage stream; then the stage's kernels;
+//   End()      join event, which s waits on in front of the first kernel that reads the stage's result (dc_scan for the progressive
+//              stage, jpeg_post for the others).
+// A stage with no sample in the batch is not touched: no stream is created, no event recorded.
+struct SideStage {
+  dalib200::DescArena arena;
+  cudaStream_t stream = nullptr;            // created at the first launch that has samples for the stage
+  cudaEvent_t uploaded = nullptr, fork = nullptr, join = nullptr;
+  bool pending = false;                     // `uploaded` is recorded: the H2D copy may still read the arena
+
+  bool Create() {
+    return cudaEventCreateWithFlags(&uploaded, cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) == cudaSuccess &&
+           cudaEventCreateWithFlags(&join, cudaEventDisableTiming) == cudaSuccess;
+  }
+  void Destroy() {
+    if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+    if (uploaded) { cudaEventSynchronize(uploaded); cudaEventDestroy(uploaded); }
+    if (fork) cudaEventDestroy(fork);
+    if (join) cudaEventDestroy(join);
+    arena.Free();
+  }
+  int Begin(cudaStream_t s) {
+    if (!stream) DB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    DB_CUDA(cudaEventRecord(fork, s));
+    DB_CUDA(cudaStreamWaitEvent(stream, fork, 0));
+    if (pending) { DB_CUDA(cudaEventSynchronize(uploaded)); pending = false; }
+    return DALIB200_SUCCESS;
+  }
+  int Upload(size_t bytes) {
+    if (int rc = arena.Upload(bytes, stream)) return rc;
+    DB_CUDA(cudaEventRecord(uploaded, stream));
+    pending = true;
+    return DALIB200_SUCCESS;
+  }
+  int End() {
+    DB_CUDA(cudaEventRecord(join, stream));
+    return DALIB200_SUCCESS;
+  }
+};
+
 struct JpegGeo { int orient = 1, rx0 = 0, ry0 = 0, rx1 = 0, ry1 = 0, out_c = 3; bool direct = true, planar_ok = false; };
 
 struct dalib200JpegPlan {
@@ -1948,37 +1949,25 @@ struct dalib200JpegPlan {
   std::vector<int> prog_wave_begin;
   std::vector<int64_t> prog_first_blk;
   int64_t prog_total_blocks = 0;
-  dalib200::DescArena prog_arena;
-  cudaEvent_t prog_uploaded = nullptr, prog_fork = nullptr, prog_join = nullptr;
-  cudaStream_t prog_stream = nullptr;      // the scans are serial chains on one warp each: they run beside the baseline entropy stage
-  bool prog_pending = false;
-  // PNG samples: decoded by png.cu on a stream of their own into the same decode windows; the post pass is shared
+  SideStage prog;                           // the scans are serial chains on one warp each: they run beside the baseline entropy stage
+  // PNG samples: decoded by png.cu into the same decode windows; the post pass is shared
   std::vector<dalib200::PngImage> png_images;
   std::vector<dalib200::PngChunk> png_chunks;
   int64_t png_scan_bytes = 0;
   uint8_t *d_png_scan = nullptr; size_t d_png_scan_cap = 0;   // filtered scanlines (grow only)
-  dalib200::DescArena png_arena;
-  cudaEvent_t png_uploaded = nullptr, png_fork = nullptr, png_join = nullptr;
-  cudaStream_t png_stream = nullptr;
-  bool png_pending = false;
-  // TIFF samples: decoded by tiff.cu on a stream of their own, like the PNG samples
+  SideStage png;
+  // TIFF samples: decoded by tiff.cu, like the PNG samples
   std::vector<dalib200::TiffImage> tiff_images;
   std::vector<dalib200::TiffSeg> tiff_segs;
   int64_t tiff_dec_bytes = 0;
   uint8_t *d_tiff_dec = nullptr; size_t d_tiff_dec_cap = 0;    // decoded segments (grow only)
   uint8_t *d_tiff_slots = nullptr; size_t d_tiff_slots_cap = 0; // segment working memory (grow only)
-  dalib200::DescArena tiff_arena;
-  cudaEvent_t tiff_uploaded = nullptr, tiff_fork = nullptr, tiff_join = nullptr;
-  cudaStream_t tiff_stream = nullptr;
-  bool tiff_pending = false;
-  // WebP samples: decoded by webp.cu on a stream of their own, like the PNG and TIFF samples
+  SideStage tiff;
+  // WebP samples: decoded by webp.cu, like the PNG and TIFF samples
   std::vector<dalib200::WebpImage> webp_images;
   int64_t webp_scratch_bytes = 0;
   uint8_t *d_webp_scratch = nullptr; size_t d_webp_scratch_cap = 0;   // coefficients, macroblocks, planes (grow only)
-  dalib200::DescArena webp_arena;
-  cudaEvent_t webp_uploaded = nullptr, webp_fork = nullptr, webp_join = nullptr;
-  cudaStream_t webp_stream = nullptr;
-  bool webp_pending = false;
+  SideStage webp;
 };
 
 namespace {
@@ -2027,7 +2016,7 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
-    if (j.png || j.tiff || j.webp) {   // decoded by png.cu / tiff.cu / webp.cu: no IDCT / colour work
+    if (j.format != Format::kJpeg) {   // decoded by png.cu / tiff.cu / webp.cu: no IDCT / colour work
       p->first_work[i] = t.work; p->first_fused[i] = t.fused; p->first_quad[i] = t.quads; p->first_item[i] = t.items;
       continue;
     }
@@ -2035,6 +2024,59 @@ void BuildWorkLists(dalib200JpegPlan *p) {
   }
   p->total_work = t.work; p->total_fused = t.fused; p->total_post_px = post_px; p->post_bytes = post_bytes; p->total_quads = t.quads;
   p->total_items = t.items;
+}
+
+// PNG, TIFF or WebP sample `sample` (format f): its planner appends its descriptors to the plan's stage and advances the stage's scratch,
+// its staged bytes go to `raw_off` of the raw staging area, and `j` receives the fields the plan reads for every sample.  Returns a
+// DALIB200 status.
+int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t len, int sample, int64_t raw_off, ParsedJpeg &j) {
+  StreamInfo info;
+  std::string err;
+  int rc;
+  auto add = [&](auto &images, auto &im) { im.sample = sample; im.raw_off = raw_off; images.push_back(im); };
+  if (f == Format::kPng) {
+    PngImage im;
+    if (!(rc = PlanPng(data, len, (int)p->png_images.size(), &im, p->png_chunks, &info, &err))) {
+      im.scan_off = p->png_scan_bytes;
+      p->png_scan_bytes += (int64_t)Align((size_t)im.scan_bytes, 16);
+      add(p->png_images, im);
+    }
+  } else if (f == Format::kTiff) {
+    TiffImage im;
+    int64_t bytes = 0;
+    if (!(rc = PlanTiff(data, len, (int)p->tiff_images.size(), &im, p->tiff_segs, p->tiff_dec_bytes, &bytes, &info, &err))) {
+      p->tiff_dec_bytes += bytes;
+      add(p->tiff_images, im);
+    }
+  } else {
+    WebpImage im;
+    int64_t bytes = 0;
+    if (!(rc = PlanWebp(data, len, (int)p->webp_images.size(), &im, p->webp_scratch_bytes, &bytes, &info, &err))) {
+      p->webp_scratch_bytes += bytes;
+      add(p->webp_images, im);
+    }
+  }
+  if (rc) { SetLastError("%s", err.c_str()); return rc; }
+  j.format = f;
+  j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
+  j.hs[0] = j.vs[0] = f == Format::kWebp ? 2 : 1;      // reported subsampling: WebP is 4:2:0 (VP8's only layout)
+  j.scan_begin = info.stage_begin; j.scan_end = info.stage_end;
+  return DALIB200_SUCCESS;
+}
+
+// The decode window and output pointer of every PNG, TIFF or WebP image, from its sample's JpegImage as patched for this launch (`hi`).
+// Returns the pixel total; each image's first_px is its prefix, by which the colour kernel finds the image of a pixel.
+template <typename Image>
+int64_t FillWindows(std::vector<Image> &images, const JpegImage *hi) {
+  int64_t px = 0;
+  for (Image &d : images) {
+    const JpegImage &im = hi[d.sample];
+    d.out = im.out; d.out_type = im.out_type;
+    d.win_x0 = im.win_x0; d.win_y0 = im.win_y0; d.win_w = im.win_w; d.win_h = im.win_h;
+    d.first_px = px;
+    px += (int64_t)im.win_w * im.win_h;
+  }
+  return px;
 }
 
 // Output geometry of sample i: orientation, region of interest, decode window, post pass.  Returns a DALIB200 status.
@@ -2073,7 +2115,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   const int output_type = p->output_type;
   const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
   p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
-  if (j.png || j.tiff || j.webp) {   // any window: png_color / tiff_color / webp_color produce pixels one by one
+  if (j.format != Format::kJpeg) {   // any window: png_color / tiff_color / webp_color produce pixels one by one
     im.win_x0 = sx0; im.win_w = sx1 - sx0;
   } else {
     im.win_x0 = sx0 & ~7; im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0;
@@ -2083,7 +2125,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   ge.orient = orient; ge.rx0 = rx0; ge.ry0 = ry0; ge.rx1 = rx1; ge.ry1 = ry1; ge.out_c = out_c;
   ge.direct = orient == 1 && p->dtype == DALIB200_UINT8 && output_type != DALIB200_YCbCr && im.win_x0 == sx0 && im.win_x0 + im.win_w == sx1;
   // decode -> resize without the RGB image (the caller consumes the planes): 4:2:0 YCbCr, fancy upsampling, plain RGB u8 request
-  ge.planar_ok = !j.png && !j.tiff && !j.webp && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
+  ge.planar_ok = j.format == Format::kJpeg && j.ncomp == 3 && im.color == kColorYCbCr && j.hmax == 2 && j.vmax == 2 && p->fancy && orient == 1 && j.width > 4 &&
                  output_type == DALIB200_RGB && p->dtype == DALIB200_UINT8;
   const bool planes_only = rois && rois[i].planes_only;
   if (planes_only && !ge.planar_ok) {
@@ -2100,9 +2142,9 @@ extern "C" {
 int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info) try {
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
-  int rc = IsPngStream(data, len) ? ParsePng(data, len, j, nullptr, nullptr, 0)
-           : IsTiffStream(data, len) ? ParseTiff(data, len, j, nullptr, nullptr, 0, 0, nullptr)
-           : IsWebpStream(data, len) ? ParseWebp(data, len, j, nullptr, 0, 0, nullptr) : ParseHeaders(data, len, j, false);
+  const Format f = DetectFormat(data, len);
+  dalib200JpegPlan descs;                   // receives the descriptors of a PNG, TIFF or WebP stream; no device resources
+  int rc = f == Format::kJpeg ? ParseHeaders(data, len, j, false) : PlanSideSample(&descs, f, data, len, 0, 0, j);
   if (rc) return rc;
   FillInfo(j, info);
   return DALIB200_SUCCESS;
@@ -2114,18 +2156,7 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->img_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->prog_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->prog_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->prog_join, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->png_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->png_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->png_join, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->tiff_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->tiff_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->tiff_join, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->webp_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->webp_fork, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->webp_join, cudaEventDisableTiming) != cudaSuccess) {
+      !p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create()) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2136,35 +2167,13 @@ int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
   if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   if (p->img_uploaded) { cudaEventSynchronize(p->img_uploaded); cudaEventDestroy(p->img_uploaded); }
-  if (p->prog_stream) { cudaStreamSynchronize(p->prog_stream); cudaStreamDestroy(p->prog_stream); }
-  if (p->prog_uploaded) { cudaEventSynchronize(p->prog_uploaded); cudaEventDestroy(p->prog_uploaded); }
-  if (p->prog_fork) cudaEventDestroy(p->prog_fork);
-  if (p->prog_join) cudaEventDestroy(p->prog_join);
-  p->prog_arena.Free();
-  if (p->png_stream) { cudaStreamSynchronize(p->png_stream); cudaStreamDestroy(p->png_stream); }
-  if (p->png_uploaded) { cudaEventSynchronize(p->png_uploaded); cudaEventDestroy(p->png_uploaded); }
-  if (p->png_fork) cudaEventDestroy(p->png_fork);
-  if (p->png_join) cudaEventDestroy(p->png_join);
-  p->png_arena.Free();
-  if (p->d_png_scan) cudaFree(p->d_png_scan);
-  if (p->tiff_stream) { cudaStreamSynchronize(p->tiff_stream); cudaStreamDestroy(p->tiff_stream); }
-  if (p->tiff_uploaded) { cudaEventSynchronize(p->tiff_uploaded); cudaEventDestroy(p->tiff_uploaded); }
-  if (p->tiff_fork) cudaEventDestroy(p->tiff_fork);
-  if (p->tiff_join) cudaEventDestroy(p->tiff_join);
-  p->tiff_arena.Free();
-  if (p->d_tiff_dec) cudaFree(p->d_tiff_dec);
-  if (p->d_tiff_slots) cudaFree(p->d_tiff_slots);
-  if (p->webp_stream) { cudaStreamSynchronize(p->webp_stream); cudaStreamDestroy(p->webp_stream); }
-  if (p->webp_uploaded) { cudaEventSynchronize(p->webp_uploaded); cudaEventDestroy(p->webp_uploaded); }
-  if (p->webp_fork) cudaEventDestroy(p->webp_fork);
-  if (p->webp_join) cudaEventDestroy(p->webp_join);
-  p->webp_arena.Free();
-  if (p->d_webp_scratch) cudaFree(p->d_webp_scratch);
+  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp }) st->Destroy();
   if (p->h_stage) cudaFreeHost(p->h_stage);
   if (p->h_images) cudaFreeHost(p->h_images);
   if (p->h_status) cudaFreeHost(p->h_status);
   void *bufs[] = { p->d_stage, p->d_clean, p->d_chunk, p->d_unit_len, p->d_state, p->d_n, p->d_coef, p->d_dc, p->d_planes, p->d_status,
-                   p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk };
+                   p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk, p->d_png_scan,
+                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch };
   for (void *b : bufs) if (b) cudaFree(b);
   delete p;
   return DALIB200_SUCCESS;
@@ -2238,12 +2247,9 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->first_item.assign(n, 0);
   p->prog_images.clear(); p->prog_scans.clear(); p->prog_huff.clear(); p->prog_wave_begin.clear(); p->prog_first_blk.clear();
   p->prog_total_blocks = 0;
-  p->png_images.clear(); p->png_chunks.clear();
-  int64_t png_scan = 0;
-  p->tiff_images.clear(); p->tiff_segs.clear();
-  int64_t tiff_dec = 0;
-  p->webp_images.clear();
-  int64_t webp_scratch = 0;
+  p->png_images.clear(); p->png_chunks.clear(); p->png_scan_bytes = 0;
+  p->tiff_images.clear(); p->tiff_segs.clear(); p->tiff_dec_bytes = 0;
+  p->webp_images.clear(); p->webp_scratch_bytes = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2266,70 +2272,27 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   for (int i = 0; i < n; i++) {
     ParsedJpeg &j = p->parsed[i];
     DB_CHECK_ARG(streams[i] && lengths[i] > 0, "decoders.image: sample %d is empty", i);
-    if (IsPngStream(streams[i], lengths[i])) {
-      // PNG: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu decodes its IDAT run (the staged range)
-      // into the decode window, and the post pass behind it is shared
-      dalib200::PngImage pim;
-      int rc = ParsePng(streams[i], lengths[i], j, &pim, &p->png_chunks, (int)p->png_images.size());
-      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
+    auto sample_error = [&](int rc, const std::string &what) { SetLastError("decoders.image: sample %d: %s", i, what.c_str()); return rc; };
+    const Format f = DetectFormat(streams[i], lengths[i]);
+    if (f != Format::kJpeg) {
+      // PNG, TIFF, WebP: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu / tiff.cu / webp.cu decode its
+      // staged range (the IDAT run, the span of the segments, the VP8 payload) into the decode window, and the post pass behind it is
+      // shared
+      int rc = PlanSideSample(p, f, streams[i], lengths[i], i, (int64_t)raw, j);
+      if (rc) return sample_error(rc, dalib200GetLastError());
       JpegImage &im = p->images[i];
       memset(&im, 0, sizeof(im));
       im.width = j.width; im.height = j.height; im.out_type = output_type;
       im.unit_begin = im.unit_end = (int)p->units.size();
       im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
       if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
-      pim.sample = i;
-      pim.raw_off = (int64_t)raw;
-      pim.scan_off = png_scan;
-      png_scan += (int64_t)Align((size_t)pim.scan_bytes, 16);
-      p->png_images.push_back(pim);
-      p->src_ptr.push_back(streams[i] + j.scan_begin);
-      raw += Align(j.scan_end - j.scan_begin, 16);
-      continue;
-    }
-    if (IsTiffStream(streams[i], lengths[i])) {
-      // TIFF: as PNG; tiff.cu decodes its segments (the staged range is their span) into the decode window
-      dalib200::TiffImage tim;
-      int64_t dec_bytes = 0;
-      int rc = ParseTiff(streams[i], lengths[i], j, &tim, &p->tiff_segs, (int)p->tiff_images.size(), tiff_dec, &dec_bytes);
-      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
-      JpegImage &im = p->images[i];
-      memset(&im, 0, sizeof(im));
-      im.width = j.width; im.height = j.height; im.out_type = output_type;
-      im.unit_begin = im.unit_end = (int)p->units.size();
-      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
-      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
-      tim.sample = i;
-      tim.raw_off = (int64_t)raw;
-      tiff_dec += dec_bytes;
-      p->tiff_images.push_back(tim);
-      p->src_ptr.push_back(streams[i] + j.scan_begin);
-      raw += Align(j.scan_end - j.scan_begin, 16);
-      continue;
-    }
-    if (IsWebpStream(streams[i], lengths[i])) {
-      // WebP: as PNG; webp.cu decodes its VP8 payload (the staged range) into the decode window
-      dalib200::WebpImage wim;
-      int64_t bytes = 0;
-      int rc = ParseWebp(streams[i], lengths[i], j, &wim, (int)p->webp_images.size(), webp_scratch, &bytes);
-      if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
-      JpegImage &im = p->images[i];
-      memset(&im, 0, sizeof(im));
-      im.width = j.width; im.height = j.height; im.out_type = output_type;
-      im.unit_begin = im.unit_end = (int)p->units.size();
-      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
-      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
-      wim.sample = i;
-      wim.raw_off = (int64_t)raw;
-      webp_scratch += bytes;
-      p->webp_images.push_back(wim);
       p->src_ptr.push_back(streams[i] + j.scan_begin);
       raw += Align(j.scan_end - j.scan_begin, 16);
       continue;
     }
     int rc = ParseHeaders(streams[i], lengths[i], j, true);
-    if (rc) { std::string m = dalib200GetLastError(); SetLastError("decoders.image: sample %d: %s", i, m.c_str()); return rc; }
-    auto unsupported = [&](const char *what) { SetLastError("decoders.image: sample %d: %s", i, what); return DALIB200_ERROR_UNSUPPORTED; };
+    if (rc) return sample_error(rc, dalib200GetLastError());
+    auto unsupported = [&](const char *what) { return sample_error(DALIB200_ERROR_UNSUPPORTED, what); };
     // multi-scan streams -- progressive, or a sequential frame whose components come in separate scans -- take the scan-by-scan entropy
     // stage (jpeg_prog.cu); `prog` below means exactly that
     const bool prog = j.progressive || (j.ncomp > 1 && j.scan_ncomp != j.ncomp);
@@ -2445,7 +2408,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       std::string perr;
       const size_t first_new = p->prog_scans.size();
       rc = dalib200::PlanProgressive(d, lengths[i], sb, (int)p->prog_images.size(), &pim, p->prog_scans, p->prog_huff, prog_table_cache, &perr);
-      if (rc) { SetLastError("decoders.image: sample %d: %s", i, perr.c_str()); return rc; }
+      if (rc) return sample_error(rc, perr);
       for (size_t k = first_new; k < p->prog_scans.size(); k++)
         if ((size_t)p->prog_scans[k].data_off + p->prog_scans[k].data_len > se - sb) {
           // a scan that runs into the trimmed end-of-image marker ends in front of it
@@ -2517,9 +2480,6 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   }
   DB_CHECK_ARG(raw < (1ull << 32) && clean < (1ull << 32), "decoders.image: batch of encoded data exceeds 4 GiB");
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
-  p->png_scan_bytes = png_scan;
-  p->tiff_dec_bytes = tiff_dec;
-  p->webp_scratch_bytes = webp_scratch;
   DB_CHECK_ARG(p->tiff_segs.size() < (1ull << 31), "decoders.image: batch of more than 2^31 TIFF segments");
   p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
   for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
@@ -2800,143 +2760,91 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   // (the clean stream is zero-padded behind every unit by the scatter kernel itself: no memset of the 129 MB buffer)
   DB_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(int32_t) * p->n, s));
   DB_CUDA(cudaMemsetAsync(p->d_chain_count, 0, sizeof(uint32_t) * 8, s));
+  const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
   if (!p->prog_images.empty()) {
     // progressive samples: scans wave by wave into the same coefficient arena, DC left as differences for dc_scan (jpeg_prog.cu).
-    // A scan is a serial chain on ONE warp (milliseconds for a large image) that leaves the GPU empty: the stage is forked onto a
-    // stream of its own here, behind the upload and the status clear, runs beside the baseline samples' entropy kernels and is joined
-    // in front of dc_scan.  It touches only the progressive samples' ranges of the coefficient / DC arenas and their status words.
-    using namespace dalib200;
-    if (!p->prog_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->prog_stream, cudaStreamNonBlocking));
-    cudaStream_t ps = p->prog_stream;
-    DB_CUDA(cudaEventRecord(p->prog_fork, s));
-    DB_CUDA(cudaStreamWaitEvent(ps, p->prog_fork, 0));
-    if (p->prog_pending) { DB_CUDA(cudaEventSynchronize(p->prog_uploaded)); p->prog_pending = false; }
+    // A scan is a serial chain on ONE warp (milliseconds for a large image) that leaves the GPU empty: the stage runs beside the
+    // baseline samples' entropy kernels and is joined in front of dc_scan.  It touches only the progressive samples' ranges of the
+    // coefficient / DC arenas and their status words.
+    SideStage &st = p->prog;
+    if ((rc = st.Begin(s))) return rc;
     const size_t npi = p->prog_images.size(), nsc = p->prog_scans.size(), nh = p->prog_huff.size();
     const size_t o_img = 0, o_scan = Align(o_img + sizeof(ProgImage) * npi, 16), o_huff = Align(o_scan + sizeof(ProgScan) * nsc, 16),
                  o_blk = Align(o_huff + sizeof(ProgHuff) * nh, 16), pbytes = Align(o_blk + sizeof(int64_t) * npi, 16);
-    if ((rc = p->prog_arena.Reserve(pbytes))) return rc;
-    memcpy(p->prog_arena.host + o_img, p->prog_images.data(), sizeof(ProgImage) * npi);
-    memcpy(p->prog_arena.host + o_scan, p->prog_scans.data(), sizeof(ProgScan) * nsc);
-    memcpy(p->prog_arena.host + o_huff, p->prog_huff.data(), sizeof(ProgHuff) * nh);
-    memcpy(p->prog_arena.host + o_blk, p->prog_first_blk.data(), sizeof(int64_t) * npi);
-    if ((rc = p->prog_arena.Upload(pbytes, ps))) return rc;
-    DB_CUDA(cudaEventRecord(p->prog_uploaded, ps));
-    p->prog_pending = true;
+    if ((rc = st.arena.Reserve(pbytes))) return rc;
+    memcpy(st.arena.host + o_img, p->prog_images.data(), sizeof(ProgImage) * npi);
+    memcpy(st.arena.host + o_scan, p->prog_scans.data(), sizeof(ProgScan) * nsc);
+    memcpy(st.arena.host + o_huff, p->prog_huff.data(), sizeof(ProgHuff) * nh);
+    memcpy(st.arena.host + o_blk, p->prog_first_blk.data(), sizeof(int64_t) * npi);
+    if ((rc = st.Upload(pbytes))) return rc;
     ProgLaunch a;
-    a.d_images = reinterpret_cast<const ProgImage *>(p->prog_arena.dev + o_img); a.nimages = (int)npi;
-    a.d_scans = reinterpret_cast<const ProgScan *>(p->prog_arena.dev + o_scan);
-    a.d_huff = reinterpret_cast<const ProgHuff *>(p->prog_arena.dev + o_huff);
-    a.d_first_blk = reinterpret_cast<const int64_t *>(p->prog_arena.dev + o_blk);
+    a.d_images = reinterpret_cast<const ProgImage *>(st.arena.dev + o_img); a.nimages = (int)npi;
+    a.d_scans = reinterpret_cast<const ProgScan *>(st.arena.dev + o_scan);
+    a.d_huff = reinterpret_cast<const ProgHuff *>(st.arena.dev + o_huff);
+    a.d_first_blk = reinterpret_cast<const int64_t *>(st.arena.dev + o_blk);
     a.total_blocks = p->prog_total_blocks;
     a.wave_begin = &p->prog_wave_begin; a.h_images = &p->prog_images;
     a.d_raw = d_raw; a.d_coef = p->d_coef; a.d_dc = p->d_dc; a.d_status = p->d_status;
-    if ((rc = LaunchProgressive(a, ps))) return rc;
-    DB_CUDA(cudaEventRecord(p->prog_join, ps));
+    if ((rc = LaunchProgressive(a, st.stream)) || (rc = st.End())) return rc;
   }
   if (!p->png_images.empty()) {
-    // PNG samples (png.cu): the inflate is a serial chain per image, so the stage is forked onto a stream of its own behind the upload
-    // and the status clear, runs beside the JPEG samples' kernels and is joined in front of the post pass.  It writes only the PNG
-    // samples' decode windows, its scanline scratch and their status words.
-    using namespace dalib200;
+    // PNG samples (png.cu): the inflate is a serial chain per image.  The stage writes only the PNG samples' decode windows, its
+    // scanline scratch and their status words.
+    SideStage &st = p->png;
     if ((rc = GrowDevice(p->d_png_scan, p->d_png_scan_cap, (size_t)p->png_scan_bytes + 16))) return rc;
-    if (!p->png_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->png_stream, cudaStreamNonBlocking));
-    cudaStream_t ps = p->png_stream;
-    DB_CUDA(cudaEventRecord(p->png_fork, s));
-    DB_CUDA(cudaStreamWaitEvent(ps, p->png_fork, 0));
-    if (p->png_pending) { DB_CUDA(cudaEventSynchronize(p->png_uploaded)); p->png_pending = false; }
-    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
-    int64_t px = 0;
-    for (PngImage &pi : p->png_images) {
-      const JpegImage &im = hi[pi.sample];
-      pi.out = im.out; pi.out_type = im.out_type;
-      pi.win_x0 = im.win_x0; pi.win_y0 = im.win_y0; pi.win_w = im.win_w; pi.win_h = im.win_h;
-      pi.first_px = px;
-      px += (int64_t)im.win_w * im.win_h;
-    }
+    if ((rc = st.Begin(s))) return rc;
+    const int64_t px = FillWindows(p->png_images, hi);
     const size_t npi = p->png_images.size(), nch = p->png_chunks.size();
     const size_t o_chunk = Align(sizeof(PngImage) * npi, 16), pbytes = Align(o_chunk + sizeof(PngChunk) * nch, 16);
-    if ((rc = p->png_arena.Reserve(pbytes))) return rc;
-    memcpy(p->png_arena.host, p->png_images.data(), sizeof(PngImage) * npi);
-    memcpy(p->png_arena.host + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
-    if ((rc = p->png_arena.Upload(pbytes, ps))) return rc;
-    DB_CUDA(cudaEventRecord(p->png_uploaded, ps));
-    p->png_pending = true;
+    if ((rc = st.arena.Reserve(pbytes))) return rc;
+    memcpy(st.arena.host, p->png_images.data(), sizeof(PngImage) * npi);
+    memcpy(st.arena.host + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
+    if ((rc = st.Upload(pbytes))) return rc;
     PngLaunch a;
-    a.d_images = reinterpret_cast<const PngImage *>(p->png_arena.dev); a.nimages = (int)npi;
-    a.d_chunks = reinterpret_cast<const PngChunk *>(p->png_arena.dev + o_chunk); a.nchunks = (int)nch;
+    a.d_images = reinterpret_cast<const PngImage *>(st.arena.dev); a.nimages = (int)npi;
+    a.d_chunks = reinterpret_cast<const PngChunk *>(st.arena.dev + o_chunk); a.nchunks = (int)nch;
     a.total_px = px;
     a.d_raw = d_raw; a.d_scan = p->d_png_scan; a.d_status = p->d_status;
-    if ((rc = LaunchPng(a, ps))) return rc;
-    DB_CUDA(cudaEventRecord(p->png_join, ps));
+    if ((rc = LaunchPng(a, st.stream)) || (rc = st.End())) return rc;
   }
   if (!p->tiff_images.empty()) {
-    // TIFF samples (tiff.cu): forked onto a stream of their own as the PNG samples are, so that a TIFF written as one big strip (a serial
-    // chain) runs beside the JPEG kernels.  It writes only the TIFF samples' decode windows, its scratch and their status words.
-    using namespace dalib200;
+    // TIFF samples (tiff.cu): a TIFF written as one big strip is a serial chain.  The stage writes only the TIFF samples' decode
+    // windows, its scratch and their status words.
+    SideStage &st = p->tiff;
     const int nseg = (int)p->tiff_segs.size();
     if ((rc = GrowDevice(p->d_tiff_dec, p->d_tiff_dec_cap, (size_t)p->tiff_dec_bytes + 16))) return rc;
     if ((rc = GrowDevice(p->d_tiff_slots, p->d_tiff_slots_cap, (size_t)TiffSlotCount(nseg) * kTiffSlotBytes))) return rc;
-    if (!p->tiff_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->tiff_stream, cudaStreamNonBlocking));
-    cudaStream_t ts = p->tiff_stream;
-    DB_CUDA(cudaEventRecord(p->tiff_fork, s));
-    DB_CUDA(cudaStreamWaitEvent(ts, p->tiff_fork, 0));
-    if (p->tiff_pending) { DB_CUDA(cudaEventSynchronize(p->tiff_uploaded)); p->tiff_pending = false; }
-    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
-    int64_t px = 0;
-    for (TiffImage &ti : p->tiff_images) {
-      const JpegImage &im = hi[ti.sample];
-      ti.out = im.out; ti.out_type = im.out_type;
-      ti.win_x0 = im.win_x0; ti.win_y0 = im.win_y0; ti.win_w = im.win_w; ti.win_h = im.win_h;
-      ti.first_px = px;
-      px += (int64_t)im.win_w * im.win_h;
-    }
+    if ((rc = st.Begin(s))) return rc;
+    const int64_t px = FillWindows(p->tiff_images, hi);
     const size_t nti = p->tiff_images.size();
     const size_t o_seg = Align(sizeof(TiffImage) * nti, 16), tbytes = Align(o_seg + sizeof(TiffSeg) * nseg, 16);
-    if ((rc = p->tiff_arena.Reserve(tbytes))) return rc;
-    memcpy(p->tiff_arena.host, p->tiff_images.data(), sizeof(TiffImage) * nti);
-    memcpy(p->tiff_arena.host + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
-    if ((rc = p->tiff_arena.Upload(tbytes, ts))) return rc;
-    DB_CUDA(cudaEventRecord(p->tiff_uploaded, ts));
-    p->tiff_pending = true;
+    if ((rc = st.arena.Reserve(tbytes))) return rc;
+    memcpy(st.arena.host, p->tiff_images.data(), sizeof(TiffImage) * nti);
+    memcpy(st.arena.host + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
+    if ((rc = st.Upload(tbytes))) return rc;
     TiffLaunch a;
-    a.d_images = reinterpret_cast<const TiffImage *>(p->tiff_arena.dev); a.nimages = (int)nti;
-    a.d_segs = reinterpret_cast<const TiffSeg *>(p->tiff_arena.dev + o_seg); a.nsegs = nseg;
+    a.d_images = reinterpret_cast<const TiffImage *>(st.arena.dev); a.nimages = (int)nti;
+    a.d_segs = reinterpret_cast<const TiffSeg *>(st.arena.dev + o_seg); a.nsegs = nseg;
     a.total_px = px;
     a.d_raw = d_raw; a.d_dec = p->d_tiff_dec; a.d_slots = p->d_tiff_slots; a.d_status = p->d_status;
-    if ((rc = LaunchTiff(a, ts))) return rc;
-    DB_CUDA(cudaEventRecord(p->tiff_join, ts));
+    if ((rc = LaunchTiff(a, st.stream)) || (rc = st.End())) return rc;
   }
   if (!p->webp_images.empty()) {
-    // WebP samples (webp.cu): forked onto a stream of their own as the PNG and TIFF samples are; the entropy decode of an image is a
-    // serial chain.  It writes only the WebP samples' decode windows, its scratch and their status words.
-    using namespace dalib200;
+    // WebP samples (webp.cu): the entropy decode of an image is a serial chain.  The stage writes only the WebP samples' decode
+    // windows, its scratch and their status words.
+    SideStage &st = p->webp;
     if ((rc = GrowDevice(p->d_webp_scratch, p->d_webp_scratch_cap, (size_t)p->webp_scratch_bytes + 16))) return rc;
-    if (!p->webp_stream) DB_CUDA(cudaStreamCreateWithFlags(&p->webp_stream, cudaStreamNonBlocking));
-    cudaStream_t ws = p->webp_stream;
-    DB_CUDA(cudaEventRecord(p->webp_fork, s));
-    DB_CUDA(cudaStreamWaitEvent(ws, p->webp_fork, 0));
-    if (p->webp_pending) { DB_CUDA(cudaEventSynchronize(p->webp_uploaded)); p->webp_pending = false; }
-    const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
-    int64_t px = 0;
-    for (WebpImage &wi : p->webp_images) {
-      const JpegImage &im = hi[wi.sample];
-      wi.out = im.out; wi.out_type = im.out_type;
-      wi.win_x0 = im.win_x0; wi.win_y0 = im.win_y0; wi.win_w = im.win_w; wi.win_h = im.win_h;
-      wi.first_px = px;
-      px += (int64_t)im.win_w * im.win_h;
-    }
+    if ((rc = st.Begin(s))) return rc;
+    const int64_t px = FillWindows(p->webp_images, hi);
     const size_t nwi = p->webp_images.size(), wbytes = Align(sizeof(WebpImage) * nwi, 16);
-    if ((rc = p->webp_arena.Reserve(wbytes))) return rc;
-    memcpy(p->webp_arena.host, p->webp_images.data(), sizeof(WebpImage) * nwi);
-    if ((rc = p->webp_arena.Upload(wbytes, ws))) return rc;
-    DB_CUDA(cudaEventRecord(p->webp_uploaded, ws));
-    p->webp_pending = true;
+    if ((rc = st.arena.Reserve(wbytes))) return rc;
+    memcpy(st.arena.host, p->webp_images.data(), sizeof(WebpImage) * nwi);
+    if ((rc = st.Upload(wbytes))) return rc;
     WebpLaunch a;
-    a.d_images = reinterpret_cast<const WebpImage *>(p->webp_arena.dev); a.nimages = (int)nwi;
+    a.d_images = reinterpret_cast<const WebpImage *>(st.arena.dev); a.nimages = (int)nwi;
     a.total_px = px;
     a.d_raw = d_raw; a.d_scratch = p->d_webp_scratch; a.d_status = p->d_status;
-    if ((rc = LaunchWebp(a, ws))) return rc;
-    DB_CUDA(cudaEventRecord(p->webp_join, ws));
+    if ((rc = LaunchWebp(a, st.stream)) || (rc = st.End())) return rc;
   }
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
   if (any_units) {
@@ -2980,7 +2888,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   { ProfScope ps_("jpeg_huff_scan", s); huff_scan_kernel<<<p->n, 1024, 0, s>>>(cx); }
   CountLaunch();
   if (any_units && p->total_blocks_write > 0) { ProfScope ps_("jpeg_huff_write", s); huff_write_kernel<<<p->total_blocks_write, kWriteThreads, wsmem, s>>>(cx); }
-  if (!p->prog_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->prog_join, 0));      // the progressive samples' coefficients and DC differences are in place
+  if (!p->prog_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->prog.join, 0));      // the progressive samples' coefficients and DC differences are in place
   { ProfScope ps_("jpeg_dc_scan", s); dc_scan_kernel<<<p->n, 1024, 0, s>>>(d_images, p->d_dc); }
   { ProfScope ps_("jpeg_truncation_fixup", s); truncation_fixup_kernel<<<p->n, 256, 0, s>>>(cx); }
   CountLaunch();
@@ -2994,9 +2902,9 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     ra.d_coef = p->d_coef; ra.d_dc = p->d_dc; ra.d_quants = d_quants; ra.d_planes = p->d_planes;
     if ((rc = LaunchReconstruct(ra, s))) return rc;
   }
-  if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png_join, 0));       // the PNG samples' windows and status are in place
-  if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff_join, 0));     // the TIFF samples' windows and status are in place
-  if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp_join, 0));     // the WebP samples' windows and status are in place
+  if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png.join, 0));       // the PNG samples' windows and status are in place
+  if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff.join, 0));     // the TIFF samples' windows and status are in place
+  if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp.join, 0));     // the WebP samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

@@ -15,6 +15,7 @@
 #include "../../include/dali_b200.h"
 #include "exif.h"
 #include "png_core.h"
+#include "stream_info.h"
 
 namespace dalib200 {
 
@@ -32,18 +33,14 @@ inline uint32_t PngCrc32(const uint8_t *p, size_t n) {
 // It also keeps every row size and pixel offset of png_core.h far inside 32 bits.
 constexpr uint32_t kPngMaxSide = 1000000;
 
-struct PngInfo {
-  int width = 0, height = 0, components = 0, orientation = 1;
-  size_t stage_begin = 0, stage_end = 0;   // the bytes the device reads: the first IDAT's type field .. the last IDAT's CRC
-};
-
-// Plans image `image` (its chunks are appended to `chunks`, offsets relative to stage_begin).  Returns a DALIB200 status.
-inline int PlanPng(const uint8_t *p, size_t n, int image, PngImage *im, std::vector<PngChunk> &chunks, PngInfo *info, std::string *err) {
+// Plans image `image` (its chunks are appended to `chunks`, offsets relative to stage_begin).  The staged bytes, info->stage_begin ..
+// stage_end, run from the first IDAT's type field to the last IDAT's CRC.  Returns a DALIB200 status.
+inline int PlanPng(const uint8_t *p, size_t n, int image, PngImage *im, std::vector<PngChunk> &chunks, StreamInfo *info, std::string *err) {
   auto bad = [&](const char *m) { if (err) *err = std::string("PNG: ") + m; return DALIB200_ERROR_BAD_DATA; };
   auto be32 = [](const uint8_t *q) { return ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | q[3]; };
   if (!IsPngStream(p, n)) return bad("missing signature");
   memset(im, 0, sizeof(*im));
-  *info = PngInfo();
+  *info = StreamInfo();
   const int first_chunk = (int)chunks.size();
   bool have_ihdr = false, have_iend = false;
   int idat_state = 0;                                   // 0: none yet, 1: in the IDAT run, 2: behind it

@@ -16,6 +16,7 @@
 #include <string>
 #include <vector>
 #include "../../include/dali_b200.h"
+#include "stream_info.h"
 #include "tiff_core.h"
 
 namespace dalib200 {
@@ -30,15 +31,11 @@ constexpr uint32_t kTiffMaxSide = 1u << 20;
 constexpr uint64_t kTiffMaxPixels = 1ull << 30;
 constexpr uint32_t kTiffMaxTile = 512;      // tile side allowed beyond the image's (rounded up to 16)
 
-struct TiffInfo {
-  int width = 0, height = 0, components = 0, orientation = 1;
-  size_t stage_begin = 0, stage_end = 0;   // the bytes the device reads: the span of the segments
-};
-
 // Plans image `image`: its segments are appended to `segs`, offsets relative to stage_begin, decoded bytes from `dec_base` on in the
-// scratch buffer (16-byte aligned each); *dec_bytes receives the image's decoded size.  Returns a DALIB200 status.
+// scratch buffer (16-byte aligned each); *dec_bytes receives the image's decoded size.  The staged bytes, info->stage_begin ..
+// stage_end, are the span of the segments.  Returns a DALIB200 status.
 inline int PlanTiff(const uint8_t *p, size_t n, int image, TiffImage *im, std::vector<TiffSeg> &segs, int64_t dec_base, int64_t *dec_bytes,
-                    TiffInfo *info, std::string *err) {
+                    StreamInfo *info, std::string *err) {
   auto fail = [&](int rc, const std::string &m) { if (err) *err = "TIFF: " + m; return rc; };
   auto bad = [&](const std::string &m) { return fail(DALIB200_ERROR_BAD_DATA, m); };
   auto unsupported = [&](const std::string &m) { return fail(DALIB200_ERROR_UNSUPPORTED, m); };
@@ -51,7 +48,7 @@ inline int PlanTiff(const uint8_t *p, size_t n, int image, TiffImage *im, std::v
               : ((uint32_t)p[o + 3] << 24) | ((uint32_t)p[o + 2] << 16) | ((uint32_t)p[o + 1] << 8) | p[o];
   };
   memset(im, 0, sizeof(*im));
-  *info = TiffInfo();
+  *info = StreamInfo();
   if (n < 8) return bad("truncated header");
   const uint32_t ifd = u32(4);
   if (ifd < 8 || (uint64_t)ifd + 2 > n) return bad("IFD offset outside the stream");

@@ -14,16 +14,12 @@
 #include <string>
 #include "../../include/dali_b200.h"
 #include "exif.h"
+#include "stream_info.h"
 #include "webp_core.h"
 
 namespace dalib200 {
 
 inline bool IsWebpStream(const uint8_t *p, size_t n) { return n >= 12 && !memcmp(p, "RIFF", 4) && !memcmp(p + 8, "WEBP", 4); }
-
-struct WebpInfo {
-  int width = 0, height = 0, components = 0, orientation = 1;
-  size_t stage_begin = 0, stage_end = 0;   // the bytes the device reads: from behind the frame header to the end of the input
-};
 
 // RFC 6386 section 14.1 (libwebp kDcTable / kAcTable)
 static const uint8_t kWebpDcTable[128] = {
@@ -268,8 +264,9 @@ inline int64_t WebpScratchBytes(int mb_w, int mb_h) {
 }
 
 // Plans image `image`: its scratch ranges start at `scratch_base` (*scratch_bytes receives their size), its staged bytes are given by
-// info->stage_begin / stage_end (partition offsets are relative to stage_begin).  Returns a DALIB200 status.
-inline int PlanWebp(const uint8_t *p, size_t n, int image, WebpImage *im, int64_t scratch_base, int64_t *scratch_bytes, WebpInfo *info,
+// info->stage_begin / stage_end, from behind the frame header to the end of the input (partition offsets are relative to stage_begin).
+// Returns a DALIB200 status.
+inline int PlanWebp(const uint8_t *p, size_t n, int image, WebpImage *im, int64_t scratch_base, int64_t *scratch_bytes, StreamInfo *info,
                     std::string *err) {
   (void)image;
   auto fail = [&](int rc, const std::string &m) { if (err) *err = "WebP: " + m; return rc; };
@@ -279,7 +276,7 @@ inline int PlanWebp(const uint8_t *p, size_t n, int image, WebpImage *im, int64_
   auto le24 = [&](size_t o) { return (uint32_t)p[o] | ((uint32_t)p[o + 1] << 8) | ((uint32_t)p[o + 2] << 16); };
   auto tag = [&](size_t o, const char *t) { return !memcmp(p + o, t, 4); };
   memset(im, 0, sizeof(*im));
-  *info = WebpInfo();
+  *info = StreamInfo();
   if (!IsWebpStream(p, n)) return bad("missing RIFF / WEBP header");
   // ---- RIFF (libwebp ParseRIFF): at least one chunk header, inside the data.  Bytes behind the RIFF are still data to the VP8
   // decoder: libwebp hands it everything from the frame header to the end of the input (see the partitions below).

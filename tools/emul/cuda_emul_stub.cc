@@ -6,15 +6,26 @@
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
 // end to end without a GPU -- descriptor upload, temporaries, stage order, grid-stride loops, wave ranges, arena offsets -- and
 // tests/test_launch_emul_cpu.py compares what lands in "device" memory with the oracle.
+//
+// DALIB200_EMUL_TRACE=<file> also writes the stream-ordering calls to <file>, one line each, in host call order: event creation,
+// record, stream wait, synchronisation and destruction, stream creation, synchronisation and destruction, cudaMemsetAsync, H2D
+// cudaMemcpyAsync and every kernel launch (by its demangled name).  Events and streams are renumbered by first appearance (e0, e1, ...,
+// s0, s1, ...; a destroyed handle's number is not reused), so two runs of one batch give the same text, and
+// tests/test_decoder_stage_order_emul_cpu.py can check the order of the decoder's side stages from it.
 //   g++ -std=c++17 -O2 -ffp-contract=off -shared -fPIC -I/usr/local/cuda/include tools/emul/cuda_emul_stub.cc -ldl
 #ifndef _GNU_SOURCE
 #define _GNU_SOURCE
 #endif
+#include <cxxabi.h>
 #include <dlfcn.h>
-#include <algorithm>
 #include <stdint.h>
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
+#include <map>
+#include <mutex>
+#include <string>
 #include "../../include/dali_b200.h"
 #include "../../dali_b200/csrc/resample3d_core.h"
 #include "../../dali_b200/csrc/jpeg_prog_core.h"
@@ -26,12 +37,41 @@ using namespace dalib200;
 typedef int cudaError_t;
 struct Dim3 { unsigned x, y, z; };
 
+// ---- call trace (DALIB200_EMUL_TRACE)
+static FILE *trace_file() {
+  static FILE *f = [] { const char *p = getenv("DALIB200_EMUL_TRACE"); return p && *p ? fopen(p, "w") : nullptr; }();
+  return f;
+}
+static std::mutex g_trace_mu;
+static std::map<const void *, int> g_events, g_streams;
+static int g_nevents = 0, g_nstreams = 0;
+static int ev(const void *e) { auto it = g_events.find(e); return it != g_events.end() ? it->second : (g_events[e] = g_nevents++); }
+static int st(const void *s) { auto it = g_streams.find(s); return it != g_streams.end() ? it->second : (g_streams[s] = g_nstreams++); }
+static int forget(std::map<const void *, int> &m, int id, const void *h) { m.erase(h); return id; }   // the allocator may reuse h
+#define TRACE(...)                                                                                            \
+  do {                                                                                                        \
+    if (FILE *f_ = trace_file()) {                                                                            \
+      std::lock_guard<std::mutex> l_(g_trace_mu);                                                             \
+      fprintf(f_, __VA_ARGS__); fputc('\n', f_); fflush(f_);                                                  \
+    }                                                                                                         \
+  } while (0)
+// "dalib200::jpeg_post_kernel<float>" of "_ZN8dalib20016jpeg_post_kernelIfEEvPKNS_8JpegPostEil": no return type, no parameters
+static std::string kernel_name(const char *mangled) {
+  int rc = 0;
+  char *d = abi::__cxa_demangle(mangled, nullptr, nullptr, &rc);
+  std::string s = rc == 0 && d ? d : *mangled ? mangled : "?";
+  free(d);
+  s = s.substr(0, s.find('('));
+  if (!s.compare(0, 5, "void ")) s = s.substr(5);
+  return s;
+}
+
 extern "C" {
-cudaError_t cudaEventCreateWithFlags(void **e, unsigned) { *e = malloc(8); return 0; }
-cudaError_t cudaEventCreate(void **e) { *e = malloc(8); return 0; }
-cudaError_t cudaEventDestroy(void *e) { free(e); return 0; }
-cudaError_t cudaEventSynchronize(void *) { return 0; }
-cudaError_t cudaEventRecord(void *, void *) { return 0; }
+cudaError_t cudaEventCreateWithFlags(void **e, unsigned) { *e = malloc(8); TRACE("event_create e%d", ev(*e)); return 0; }
+cudaError_t cudaEventCreate(void **e) { *e = malloc(8); TRACE("event_create e%d", ev(*e)); return 0; }
+cudaError_t cudaEventDestroy(void *e) { TRACE("event_destroy e%d", forget(g_events, ev(e), e)); free(e); return 0; }
+cudaError_t cudaEventSynchronize(void *e) { TRACE("event_sync e%d", ev(e)); return 0; }
+cudaError_t cudaEventRecord(void *e, void *s) { TRACE("record e%d s%d", ev(e), st(s)); return 0; }
 cudaError_t cudaEventQuery(void *) { return 0; }
 cudaError_t cudaHostAlloc(void **p, size_t n, unsigned) { *p = calloc(n ? n : 1, 1); return *p ? 0 : 2; }
 cudaError_t cudaMallocHost(void **p, size_t n) { *p = calloc(n ? n : 1, 1); return *p ? 0 : 2; }
@@ -48,9 +88,13 @@ cudaError_t cudaGetLastError(void) { const int e = g_last_error; g_last_error = 
 cudaError_t cudaPeekAtLastError(void) { return g_last_error; }
 const char *cudaGetErrorName(cudaError_t e) { return e == 9 ? "cudaErrorInvalidConfiguration" : e ? "cudaErrorUnknown" : "cudaSuccess"; }
 const char *cudaGetErrorString(cudaError_t e) { return e == 9 ? "invalid configuration argument (emulated launch)" : e ? "error" : "no error"; }
-cudaError_t cudaStreamSynchronize(void *) { return 0; }
-cudaError_t cudaMemsetAsync(void *p, int v, size_t n, void *) { memset(p, v, n); return 0; }
-cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, int, void *) { memmove(d, s, n); return 0; }
+cudaError_t cudaStreamSynchronize(void *s) { TRACE("stream_sync s%d", st(s)); return 0; }
+cudaError_t cudaMemsetAsync(void *p, int v, size_t n, void *s) { TRACE("memset s%d %zu", st(s), n); memset(p, v, n); return 0; }
+cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, int kind, void *stream) {
+  if (kind == 1) TRACE("h2d s%d %zu", st(stream), n);          // cudaMemcpyHostToDevice
+  memmove(d, s, n);
+  return 0;
+}
 cudaError_t cudaMemcpy(void *d, const void *s, size_t n, int) { memmove(d, s, n); return 0; }
 cudaError_t cudaMemset(void *p, int v, size_t n) { memset(p, v, n); return 0; }
 cudaError_t cudaDeviceSynchronize(void) { return 0; }
@@ -62,16 +106,17 @@ struct stubPtrAttr { int type; int device; void *devp; void *hostp; };
 cudaError_t cudaPointerGetAttributes(stubPtrAttr *a, const void *p) { a->type = 0; a->device = 0; a->devp = 0; a->hostp = (void *)p; return 0; }
 cudaError_t cudaGetDriverEntryPoint(const char *, void **fn, unsigned long long, int *status) { *fn = 0; if (status) *status = 1; return 0; }
 cudaError_t cudaEventElapsedTime(float *ms, void *, void *) { *ms = 0; return 0; }
-cudaError_t cudaStreamCreateWithFlags(void **s, unsigned) { *s = malloc(8); return 0; }
-cudaError_t cudaStreamCreate(void **s) { *s = malloc(8); return 0; }
-cudaError_t cudaStreamDestroy(void *s) { free(s); return 0; }
-cudaError_t cudaStreamWaitEvent(void *, void *, unsigned) { return 0; }
+cudaError_t cudaStreamCreateWithFlags(void **s, unsigned) { *s = malloc(8); TRACE("stream_create s%d", st(*s)); return 0; }
+cudaError_t cudaStreamCreate(void **s) { *s = malloc(8); TRACE("stream_create s%d", st(*s)); return 0; }
+cudaError_t cudaStreamDestroy(void *s) { TRACE("stream_destroy s%d", forget(g_streams, st(s), s)); free(s); return 0; }
+cudaError_t cudaStreamWaitEvent(void *s, void *e, unsigned) { TRACE("wait s%d e%d", st(s), ev(e)); return 0; }
 cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
 static long g_emulated[12];
 long emul_launch_count(int which) { return g_emulated[which]; }
+void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
 // kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu, tiff.cu and webp.cu, thread by thread
 static void run_resample3d_pass(Dim3 g, Dim3 b, void **args) {
@@ -257,10 +302,11 @@ static void run_webp_color(Dim3 g, Dim3 b, void **args) {
       }
 }
 
-cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *) {
+cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *stream) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
   const char *name = func && dladdr(func, &di) && di.dli_sname && di.dli_saddr == func ? di.dli_sname : "";
+  TRACE("launch %s s%d", kernel_name(name).c_str(), st(stream));
   const bool is_r3 = !strcmp(name, "_ZN8dalib20022resample3d_pass_kernelEPKNS_6R3PassEPKii");
   const bool is_scan = !strcmp(name, "_ZN8dalib20016prog_scan_kernelEPKNS_8ProgScanEiPKNS_9ProgImageEPKNS_8ProgHuffEPKhPsPi");
   const bool is_dc = !strcmp(name, "_ZN8dalib20014prog_dc_kernelEPKNS_9ProgImageEPKlilPKsPsPi");

@@ -20,7 +20,7 @@ using namespace dalib200;
 extern "C" int emul_png_decode(const uint8_t *data, size_t len, int out_type, uint8_t *out, int *info) {
   PngImage im;
   std::vector<PngChunk> chunks;
-  PngInfo pi;
+  StreamInfo pi;
   std::string err;
   const int rc = PlanPng(data, len, 0, &im, chunks, &pi, &err);
   if (rc) return rc;

@@ -20,7 +20,7 @@ using namespace dalib200;
 extern "C" int emul_tiff_decode(const uint8_t *data, size_t len, int out_type, uint8_t *out, int *info) {
   TiffImage im;
   std::vector<TiffSeg> segs;
-  TiffInfo ti;
+  StreamInfo ti;
   int64_t dec_bytes = 0;
   std::string err;
   const int rc = PlanTiff(data, len, 0, &im, segs, 0, &dec_bytes, &ti, &err);

@@ -19,7 +19,7 @@ using namespace dalib200;
 // status (a partition that runs out of data).
 extern "C" int emul_webp_decode(const uint8_t *data, size_t len, int out_type, uint8_t *out, int *info) {
   WebpImage im;
-  WebpInfo wi;
+  StreamInfo wi;
   int64_t scratch_bytes = 0;
   std::string err;
   const int rc = PlanWebp(data, len, 0, &im, 0, &scratch_bytes, &wi, &err);
@@ -54,7 +54,7 @@ extern "C" int emul_webp_decode(const uint8_t *data, size_t len, int out_type, u
 // used, number of 4x4-predicted macroblocks, number of distinct segments used }.  Returns the planner's status, or -1.
 extern "C" int emul_webp_header(const uint8_t *data, size_t len, int *h) {
   WebpImage im;
-  WebpInfo wi;
+  StreamInfo wi;
   int64_t scratch_bytes = 0;
   const int rc = PlanWebp(data, len, 0, &im, 0, &scratch_bytes, &wi, nullptr);
   if (rc) return rc;
