@@ -1,0 +1,63 @@
+// dali_b200/csrc/bitmap.cu -- BMP and PNM decoding inside decoders.image: serial unpack of RLE / ASCII images, colour conversion.
+//
+// The planner (bitmap_plan.h) parses the headers on the host; the pixel data itself is only touched here:
+//   bitmap_unpack  one lane per RLE4 / RLE8 BMP or ASCII PNM image (SerialLaneGeometry): expands it into an 8-bit plane of plan scratch
+//                  (bitmap_unpack, bitmap_core.h).  Not launched for a batch whose images are all uncompressed.
+//   bitmap_color   16 window pixels per thread, read from the staged raster (uncompressed images: no scratch, no copy) or from the plane,
+//                  converted to RGB / BGR / GRAY and written with 16-byte stores into the decode window
+// Orientation, region of interest, YCbCr and float output are the JPEG path's post pass over that window (jpeg.cu jpeg_post_kernel).
+#include "common.cuh"
+#include "bitmap.h"
+#include <algorithm>
+
+namespace dalib200 {
+
+__global__ void __launch_bounds__(32) bitmap_unpack_kernel(const BitmapImage *__restrict__ images, const int32_t *__restrict__ list,
+                                                           int nlist, int lanes, const uint8_t *__restrict__ raw, uint8_t *scratch,
+                                                           int32_t *status) {
+  if ((int)threadIdx.x >= lanes) return;
+  for (int k = blockIdx.x * lanes + threadIdx.x; k < nlist; k += gridDim.x * lanes) {
+    const BitmapImage &im = images[list[k]];
+    if (bitmap_unpack(im, raw + im.raw_off, scratch + im.plane_off)) status[im.sample] = 1;
+  }
+}
+
+__global__ void __launch_bounds__(256) bitmap_color_kernel(const BitmapImage *__restrict__ images, int nimages, int64_t total,
+                                                           const uint8_t *__restrict__ raw, const uint8_t *__restrict__ scratch) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
+    int lo = 0, hi = nimages - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_grp <= e) lo = mid; else hi = mid - 1; }
+    const BitmapImage &im = images[lo];
+    bitmap_group(im, im.unpack == kBitmapDirect ? raw + im.raw_off : scratch + im.plane_off, e - im.first_grp);
+  }
+}
+
+int64_t BitmapGroups(std::vector<BitmapImage> &images) {
+  int64_t g = 0;
+  for (BitmapImage &d : images) {
+    d.first_grp = g;
+    g += ((int64_t)d.win_w * d.win_h + kBitmapGroup - 1) / kBitmapGroup;
+  }
+  return g;
+}
+
+int LaunchBitmap(const BitmapLaunch &a, cudaStream_t s) {
+  if (a.nimages == 0) return DALIB200_SUCCESS;
+  if (a.nunpack > 0) {
+    const SerialLanes g = SerialLaneGeometry(a.nunpack, 1 << 30);
+    ProfScope ps_("bitmap_unpack", s);
+    bitmap_unpack_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.d_unpack, a.nunpack, g.lanes, a.d_raw, a.d_scratch, a.d_status);
+    CountLaunch();
+  }
+  if (a.total_groups > 0) {
+    const int grid = (int)std::min<int64_t>((a.total_groups + 255) / 256, (int64_t)NumSMs() * 16);
+    ProfScope ps_("bitmap_color", s);
+    bitmap_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_groups, a.d_raw, a.d_scratch);
+    CountLaunch();
+  }
+  DB_CUDA(cudaGetLastError());
+  return DALIB200_SUCCESS;
+}
+
+}  // namespace dalib200

@@ -23,10 +23,10 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): J (encoded bytes) + H*W*3 (decoded image).
 //
-// The plan also takes PNG, TIFF and lossy WebP streams (detected by their signatures): png_plan.h walks their chunks, tiff_plan.h their
-// IFD and webp_plan.h their RIFF chunks and VP8 headers at set-up, png.cu, tiff.cu and webp.cu decode them into the same decode windows
-// on streams of their own, and the post pass below serves every format.  A PNG, TIFF or WebP sample has no units, subsequences or MCUs,
-// so every kernel of this file skips it.
+// The plan also takes PNG, TIFF, lossy WebP, BMP and PNM streams (detected by their signatures): png_plan.h, tiff_plan.h, webp_plan.h
+// and bitmap_plan.h read their headers at set-up, png.cu, tiff.cu, webp.cu and bitmap.cu decode them into the same decode windows on
+// streams of their own, and the post pass below serves every format.  Such a sample has no units, subsequences or MCUs, so every kernel
+// of this file skips it.
 #include "common.cuh"
 #include "jpeg_recon.h"
 #include <algorithm>
@@ -1659,14 +1659,18 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 #include "tiff_plan.h"
 #include "webp.h"
 #include "webp_plan.h"
+// BMP and PNM streams: planner + launch interface of bitmap.cu
+#include "bitmap.h"
+#include "bitmap_plan.h"
 namespace {
 
-// The formats the plan takes, told apart by their signatures.  PNG, TIFF and WebP samples are planned by png_plan.h, tiff_plan.h and
-// webp_plan.h and decoded by png.cu, tiff.cu and webp.cu; everything else is parsed as JPEG.
-enum class Format { kJpeg, kPng, kTiff, kWebp };
+// The formats the plan takes, told apart by their signatures.  PNG, TIFF, WebP and BMP / PNM samples are planned by png_plan.h,
+// tiff_plan.h, webp_plan.h and bitmap_plan.h and decoded by png.cu, tiff.cu, webp.cu and bitmap.cu; everything else is parsed as JPEG.
+enum class Format { kJpeg, kPng, kTiff, kWebp, kBitmap };
 
 Format DetectFormat(const uint8_t *p, size_t n) {
-  return IsPngStream(p, n) ? Format::kPng : IsTiffStream(p, n) ? Format::kTiff : IsWebpStream(p, n) ? Format::kWebp : Format::kJpeg;
+  return IsPngStream(p, n) ? Format::kPng : IsTiffStream(p, n) ? Format::kTiff : IsWebpStream(p, n) ? Format::kWebp
+       : IsBitmapStream(p, n) ? Format::kBitmap : Format::kJpeg;
 }
 
 struct ParsedJpeg {
@@ -1674,7 +1678,7 @@ struct ParsedJpeg {
   int cid[4] = {0}, hs[4] = {0}, vs[4] = {0}, tq[4] = {0};
   int hmax = 0, vmax = 0;
   bool progressive = false, jfif = false;
-  Format format = Format::kJpeg;   // PNG, TIFF, WebP: width / height / ncomp / orientation / scan range and hs[0] / vs[0] only
+  Format format = Format::kJpeg;   // PNG, TIFF, WebP, BMP / PNM: width / height / ncomp / orientation / scan range and hs[0] / vs[0] only
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
   HostHuff dc[4], ac[4];
@@ -1843,8 +1847,9 @@ void BuildDeviceTable(const HostHuff &h, uint32_t *lut, uint16_t *lut16, HuffSlo
 
 }  // namespace
 
-// A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP), for samples whose decode is a serial chain per
-// image: it runs on a stream of its own, so that those chains overlap the JPEG kernels.  Its order on the caller's stream s:
+// A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP, BMP / PNM), for samples whose decode is a serial
+// chain per image or needs no JPEG kernel: it runs on a stream of its own, so that its work overlaps the JPEG kernels.  Its order on the
+// caller's stream s:
 //   Begin(s)   after the status clear: fork (s -> stage stream), then wait until the previous upload of the pinned arena is done;
 //   Upload()   the arena, filled by the caller, goes to the device on the stage stream; then the stage's kernels;
 //   End()      join event, which s waits on in front of the first kernel that reads the stage's result (dc_scan for the progressive
@@ -1968,6 +1973,12 @@ struct dalib200JpegPlan {
   int64_t webp_scratch_bytes = 0;
   uint8_t *d_webp_scratch = nullptr; size_t d_webp_scratch_cap = 0;   // coefficients, macroblocks, planes (grow only)
   SideStage webp;
+  // BMP and PNM samples: decoded by bitmap.cu, like the PNG, TIFF and WebP samples
+  std::vector<dalib200::BitmapImage> bitmap_images;
+  std::vector<int32_t> bitmap_unpack;       // the RLE / ASCII images among them
+  int64_t bitmap_scratch_bytes = 0;
+  uint8_t *d_bitmap_scratch = nullptr; size_t d_bitmap_scratch_cap = 0;   // unpacked planes (grow only)
+  SideStage bitmap;
 };
 
 namespace {
@@ -2016,7 +2027,7 @@ void BuildWorkLists(dalib200JpegPlan *p) {
       p->posts.push_back(po); p->post_sample.push_back(i); p->post_off.push_back(post_bytes);
       post_bytes += Align((size_t)im.win_w * im.win_h * po.src_c, 256);
     }
-    if (j.format != Format::kJpeg) {   // decoded by png.cu / tiff.cu / webp.cu: no IDCT / colour work
+    if (j.format != Format::kJpeg) {   // decoded by png.cu / tiff.cu / webp.cu / bitmap.cu: no IDCT / colour work
       p->first_work[i] = t.work; p->first_fused[i] = t.fused; p->first_quad[i] = t.quads; p->first_item[i] = t.items;
       continue;
     }
@@ -2026,9 +2037,9 @@ void BuildWorkLists(dalib200JpegPlan *p) {
   p->total_items = t.items;
 }
 
-// PNG, TIFF or WebP sample `sample` (format f): its planner appends its descriptors to the plan's stage and advances the stage's scratch,
-// its staged bytes go to `raw_off` of the raw staging area, and `j` receives the fields the plan reads for every sample.  Returns a
-// DALIB200 status.
+// PNG, TIFF, WebP, BMP or PNM sample `sample` (format f): its planner appends its descriptors to the plan's stage and advances the
+// stage's scratch, its staged bytes go to `raw_off` of the raw staging area, and `j` receives the fields the plan reads for every sample.
+// Returns a DALIB200 status.
 int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t len, int sample, int64_t raw_off, ParsedJpeg &j) {
   StreamInfo info;
   std::string err;
@@ -2048,12 +2059,20 @@ int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t le
       p->tiff_dec_bytes += bytes;
       add(p->tiff_images, im);
     }
-  } else {
+  } else if (f == Format::kWebp) {
     WebpImage im;
     int64_t bytes = 0;
     if (!(rc = PlanWebp(data, len, (int)p->webp_images.size(), &im, p->webp_scratch_bytes, &bytes, &info, &err))) {
       p->webp_scratch_bytes += bytes;
       add(p->webp_images, im);
+    }
+  } else {
+    BitmapImage im;
+    int64_t bytes = 0;
+    if (!(rc = PlanBitmap(data, len, &im, p->bitmap_scratch_bytes, &bytes, &info, &err))) {
+      p->bitmap_scratch_bytes += bytes;
+      if (im.unpack != kBitmapDirect) p->bitmap_unpack.push_back((int32_t)p->bitmap_images.size());
+      add(p->bitmap_images, im);
     }
   }
   if (rc) { SetLastError("%s", err.c_str()); return rc; }
@@ -2064,8 +2083,8 @@ int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t le
   return DALIB200_SUCCESS;
 }
 
-// The decode window and output pointer of every PNG, TIFF or WebP image, from its sample's JpegImage as patched for this launch (`hi`).
-// Returns the pixel total; each image's first_px is its prefix, by which the colour kernel finds the image of a pixel.
+// The decode window and output pointer of every PNG, TIFF, WebP, BMP or PNM image, from its sample's JpegImage as patched for this
+// launch (`hi`).  Returns the pixel total; each image's first_px is its prefix, by which the colour kernel finds the image of a pixel.
 template <typename Image>
 int64_t FillWindows(std::vector<Image> &images, const JpegImage *hi) {
   int64_t px = 0;
@@ -2115,7 +2134,7 @@ int PlanGeometry(dalib200JpegPlan *p, int i, const dalib200JpegRoi *rois, const 
   const int output_type = p->output_type;
   const int out_c = output_type == DALIB200_GRAY ? 1 : 3;
   p->out_shape[3 * i] = ry1 - ry0; p->out_shape[3 * i + 1] = rx1 - rx0; p->out_shape[3 * i + 2] = out_c;
-  if (j.format != Format::kJpeg) {   // any window: png_color / tiff_color / webp_color produce pixels one by one
+  if (j.format != Format::kJpeg) {   // any window: png_color / tiff_color / webp_color / bitmap_color produce pixels one by one
     im.win_x0 = sx0; im.win_w = sx1 - sx0;
   } else {
     im.win_x0 = sx0 & ~7; im.win_w = std::min(W, (sx1 + 7) & ~7) - im.win_x0;
@@ -2143,7 +2162,7 @@ int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info)
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
   const Format f = DetectFormat(data, len);
-  dalib200JpegPlan descs;                   // receives the descriptors of a PNG, TIFF or WebP stream; no device resources
+  dalib200JpegPlan descs;                   // receives the descriptors of a PNG, TIFF, WebP, BMP or PNM stream; no device resources
   int rc = f == Format::kJpeg ? ParseHeaders(data, len, j, false) : PlanSideSample(&descs, f, data, len, 0, 0, j);
   if (rc) return rc;
   FillInfo(j, info);
@@ -2156,7 +2175,8 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&p->img_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      !p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create()) {
+      !p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() ||
+      !p->bitmap.Create()) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2167,13 +2187,13 @@ int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
   if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   if (p->img_uploaded) { cudaEventSynchronize(p->img_uploaded); cudaEventDestroy(p->img_uploaded); }
-  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp }) st->Destroy();
+  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp, &p->bitmap }) st->Destroy();
   if (p->h_stage) cudaFreeHost(p->h_stage);
   if (p->h_images) cudaFreeHost(p->h_images);
   if (p->h_status) cudaFreeHost(p->h_status);
   void *bufs[] = { p->d_stage, p->d_clean, p->d_chunk, p->d_unit_len, p->d_state, p->d_n, p->d_coef, p->d_dc, p->d_planes, p->d_status,
                    p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk, p->d_png_scan,
-                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch };
+                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch, p->d_bitmap_scratch };
   for (void *b : bufs) if (b) cudaFree(b);
   delete p;
   return DALIB200_SUCCESS;
@@ -2250,6 +2270,7 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->png_images.clear(); p->png_chunks.clear(); p->png_scan_bytes = 0;
   p->tiff_images.clear(); p->tiff_segs.clear(); p->tiff_dec_bytes = 0;
   p->webp_images.clear(); p->webp_scratch_bytes = 0;
+  p->bitmap_images.clear(); p->bitmap_unpack.clear(); p->bitmap_scratch_bytes = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2275,9 +2296,9 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     auto sample_error = [&](int rc, const std::string &what) { SetLastError("decoders.image: sample %d: %s", i, what.c_str()); return rc; };
     const Format f = DetectFormat(streams[i], lengths[i]);
     if (f != Format::kJpeg) {
-      // PNG, TIFF, WebP: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu / tiff.cu / webp.cu decode its
-      // staged range (the IDAT run, the span of the segments, the VP8 payload) into the decode window, and the post pass behind it is
-      // shared
+      // PNG, TIFF, WebP, BMP, PNM: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu / tiff.cu / webp.cu /
+      // bitmap.cu decode its staged range (the IDAT run, the span of the segments, the VP8 payload, the pixel array or raster) into the
+      // decode window, and the post pass behind it is shared
       int rc = PlanSideSample(p, f, streams[i], lengths[i], i, (int64_t)raw, j);
       if (rc) return sample_error(rc, dalib200GetLastError());
       JpegImage &im = p->images[i];
@@ -2846,6 +2867,28 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     a.d_raw = d_raw; a.d_scratch = p->d_webp_scratch; a.d_status = p->d_status;
     if ((rc = LaunchWebp(a, st.stream)) || (rc = st.End())) return rc;
   }
+  if (!p->bitmap_images.empty()) {
+    // BMP and PNM samples (bitmap.cu): mostly uncompressed rasters read straight from the staged bytes; RLE and ASCII images are
+    // unpacked first, one serial lane each.  The stage writes only the BMP / PNM samples' decode windows, its scratch and their status
+    // words.
+    SideStage &st = p->bitmap;
+    if ((rc = GrowDevice(p->d_bitmap_scratch, p->d_bitmap_scratch_cap, (size_t)p->bitmap_scratch_bytes + 16))) return rc;
+    if ((rc = st.Begin(s))) return rc;
+    FillWindows(p->bitmap_images, hi);
+    const int64_t groups = BitmapGroups(p->bitmap_images);
+    const size_t nbi = p->bitmap_images.size(), nun = p->bitmap_unpack.size();
+    const size_t o_un = Align(sizeof(BitmapImage) * nbi, 16), bbytes = Align(o_un + sizeof(int32_t) * nun, 16);
+    if ((rc = st.arena.Reserve(bbytes))) return rc;
+    memcpy(st.arena.host, p->bitmap_images.data(), sizeof(BitmapImage) * nbi);
+    memcpy(st.arena.host + o_un, p->bitmap_unpack.data(), sizeof(int32_t) * nun);
+    if ((rc = st.Upload(bbytes))) return rc;
+    BitmapLaunch a;
+    a.d_images = reinterpret_cast<const BitmapImage *>(st.arena.dev); a.nimages = (int)nbi;
+    a.d_unpack = reinterpret_cast<const int32_t *>(st.arena.dev + o_un); a.nunpack = (int)nun;
+    a.total_groups = groups;
+    a.d_raw = d_raw; a.d_scratch = p->d_bitmap_scratch; a.d_status = p->d_status;
+    if ((rc = LaunchBitmap(a, st.stream)) || (rc = st.End())) return rc;
+  }
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
   if (any_units) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
@@ -2905,6 +2948,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png.join, 0));       // the PNG samples' windows and status are in place
   if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff.join, 0));     // the TIFF samples' windows and status are in place
   if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp.join, 0));     // the WebP samples' windows and status are in place
+  if (!p->bitmap_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->bitmap.join, 0)); // the BMP / PNM samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

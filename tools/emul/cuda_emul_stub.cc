@@ -1,8 +1,8 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG, TIFF and WebP kernels are EXECUTED on the host -- their bodies are single
-// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h), so a launch is a
-// loop over blocks and threads around
+// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP and BMP / PNM kernels are EXECUTED on the host -- their bodies are single
+// host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h, bitmap_core.h), so a
+// launch is a loop over blocks and threads around
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
 // end to end without a GPU -- descriptor upload, temporaries, stage order, grid-stride loops, wave ranges, arena offsets -- and
 // tests/test_launch_emul_cpu.py compares what lands in "device" memory with the oracle.
@@ -32,6 +32,7 @@
 #include "../../dali_b200/csrc/png_core.h"
 #include "../../dali_b200/csrc/tiff_core.h"
 #include "../../dali_b200/csrc/webp_core.h"
+#include "../../dali_b200/csrc/bitmap_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -114,11 +115,11 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[12];
+static long g_emulated[14];
 long emul_launch_count(int which) { return g_emulated[which]; }
 void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
-// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu, tiff.cu and webp.cu, thread by thread
+// kernels of dali_b200/csrc/resample3d.cu, jpeg_prog.cu, png.cu, tiff.cu, webp.cu and bitmap.cu, thread by thread
 static void run_resample3d_pass(Dim3 g, Dim3 b, void **args) {
   const R3Pass *passes = *static_cast<const R3Pass **>(args[0]);
   const int32_t *tab = *static_cast<const int32_t **>(args[1]);
@@ -302,6 +303,38 @@ static void run_webp_color(Dim3 g, Dim3 b, void **args) {
       }
 }
 
+static void run_bitmap_unpack(Dim3 g, Dim3 b, void **args) {
+  const BitmapImage *images = *static_cast<const BitmapImage **>(args[0]);
+  const int32_t *list = *static_cast<const int32_t **>(args[1]);
+  const int nlist = *static_cast<int *>(args[2]);
+  const int lanes = *static_cast<int *>(args[3]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[4]);
+  uint8_t *scratch = *static_cast<uint8_t **>(args[5]);
+  int32_t *status = *static_cast<int32_t **>(args[6]);
+  for (int bx = (int)g.x - 1; bx >= 0; bx--)                 // blocks of a launch run in no particular order: take the reverse one
+    for (int tx = 0; tx < (int)b.x && tx < lanes; tx++)
+      for (int k = bx * lanes + tx; k < nlist; k += (int)g.x * lanes) {
+        const BitmapImage &im = images[list[k]];
+        if (bitmap_unpack(im, raw + im.raw_off, scratch + im.plane_off)) status[im.sample] = 1;
+      }
+}
+static void run_bitmap_color(Dim3 g, Dim3 b, void **args) {
+  const BitmapImage *images = *static_cast<const BitmapImage **>(args[0]);
+  const int nimages = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[3]);
+  const uint8_t *scratch = *static_cast<const uint8_t **>(args[4]);
+  const int64_t step = (int64_t)g.x * b.x;
+  for (unsigned bx = 0; bx < g.x; bx++)
+    for (unsigned tx = 0; tx < b.x; tx++)
+      for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
+        int lo = 0, hi = nimages - 1;
+        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_grp <= e) lo = mid; else hi = mid - 1; }
+        const BitmapImage &im = images[lo];
+        bitmap_group(im, im.unpack == kBitmapDirect ? raw + im.raw_off : scratch + im.plane_off, e - im.first_grp);
+      }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *stream) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -319,6 +352,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_webp_recon = !strcmp(name, "_ZN8dalib20016webp_wave_kernelILb0EEEvPKNS_9WebpImageEPhPKi");
   const bool is_webp_filter = !strcmp(name, "_ZN8dalib20016webp_wave_kernelILb1EEEvPKNS_9WebpImageEPhPKi");
   const bool is_webp_color = !strcmp(name, "_ZN8dalib20017webp_color_kernelEPKNS_9WebpImageEilPh");
+  const bool is_bitmap_unpack = !strcmp(name, "_ZN8dalib20020bitmap_unpack_kernelEPKNS_11BitmapImageEPKiiiPKhPhPi");
+  const bool is_bitmap_color = !strcmp(name, "_ZN8dalib20019bitmap_color_kernelEPKNS_11BitmapImageEilPKhS4_");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -335,6 +370,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_webp_recon) { run_webp_wave(grid, block, args, false); g_emulated[9]++; }
   else if (is_webp_filter) { run_webp_wave(grid, block, args, true); g_emulated[10]++; }
   else if (is_webp_color) { run_webp_color(grid, block, args); g_emulated[11]++; }
+  else if (is_bitmap_unpack) { run_bitmap_unpack(grid, block, args); g_emulated[12]++; }
+  else if (is_bitmap_color) { run_bitmap_color(grid, block, args); g_emulated[13]++; }
   return 0;
 }
 }  // extern "C"

@@ -36,6 +36,9 @@ seeds += [bytearray(webp_streams.pil_webp(np.dstack([wimg[1], wimg[1][..., 0]]),
           bytearray(webp_streams.pil_webp(wimg[2], quality=60, exif=webp_streams.exif_orientation(6)))]
 if webp_streams.libwebp():
     seeds += [bytearray(webp_streams.libwebp_encode(wimg[2], 60.0, partitions=3, method=2, filter_type=t)) for t in (0, 1)]
+# BMP and PNM streams (every header size, palettes, bitfields, RLE4 / RLE8, P1 - P6, comments): the header parse of the planner
+import bitmap_streams
+seeds += [bytearray(s) for n, s in bitmap_streams.corpus() if len(s) < 100000][::7]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()

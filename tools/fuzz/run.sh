@@ -3,7 +3,7 @@
 # ROI and descriptor build of dalib200JpegGetInfo / dalib200JpegPlanSetupEx) under AddressSanitizer, without a GPU: jpeg.cu + common.cu
 # are built with -fsanitize=address and the handful of CUDA runtime calls the host side makes are replaced by a preloaded stub
 # (cuda_stub.c: events = no-ops, pinned / device allocations = malloc, so that ASAN's red zones surround them).
-# Inputs: valid baseline and progressive streams (4:2:0 / 4:4:4 / 4:2:2 / gray / CMYK / YCCK, restart intervals, EXIF orientations), PNG, TIFF and WebP streams with byte flips, truncation,
+# Inputs: valid baseline and progressive streams (4:2:0 / 4:4:4 / 4:2:2 / gray / CMYK / YCCK, restart intervals, EXIF orientations), PNG, TIFF, WebP, BMP and PNM streams with byte flips, truncation,
 # corrupted segment lengths, wrapping EXIF offsets, inserted / deleted bytes, markers sprinkled into the entropy data.
 # A finding is an ASAN report on stderr (non-zero exit).
 set -e
@@ -17,7 +17,8 @@ $NVCC $F -c "$ROOT/dali_b200/csrc/jpeg_prog.cu" -o "$OUT/jpeg_prog.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/png.cu" -o "$OUT/png.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/tiff.cu" -o "$OUT/tiff.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/webp.cu" -o "$OUT/webp.o"
-$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
+$NVCC $F -c "$ROOT/dali_b200/csrc/bitmap.cu" -o "$OUT/bitmap.o"
+$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" "$OUT/bitmap.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
 gcc -shared -fPIC -O1 -o "$OUT/cuda_stub.so" "$HERE/cuda_stub.c"
 # the progressive scan decoder itself (the body of prog_scan_kernel, compiled for the host by tools/emul) under ASAN + UBSAN on mutated
 # progressive streams: garbage Huffman codes, runs past the band, truncated scans, markers inside the data must stay inside the arena
