@@ -245,12 +245,15 @@ def csc(imgs, in_type, out_type):
     return [o.cpu().numpy() for o in outs]
 
 
-def spectrogram(sigs, nfft=None, window_length=512, window_step=256, power=2, center=True, reflect=True, layout="ft", window_fn=None):
+def spectrogram(sigs, nfft=None, window_length=512, window_step=256, power=2, center=True, reflect=True, layout="ft", window_fn=None,
+                plan=None):
+    """plan: an existing capi.Plan("Spectrogram", ...) to set up again (default: a fresh one)."""
     torch = _torch()
     n = len(sigs)
     args = capi.SpectrogramArgs(nfft or window_length, window_length, window_step, power, int(center), int(reflect), int(layout == "ft"))
     lens = (C.c_int64 * n)(*[int(s.size) for s in sigs])
-    plan = capi.Plan("Spectrogram", max(n, 1))
+    if plan is None:
+        plan = capi.Plan("Spectrogram", max(n, 1))
     wf = None
     if window_fn is not None:
         wfa = np.ascontiguousarray(window_fn, np.float32)
