@@ -9,7 +9,9 @@
 //                separately), cosine tables table.h:27-112 (double on the host), liftering mfcc.h:36-41, mfcc.cc:52-72.
 //                Same order, same tables -> bit-exact.
 //   Normalize    dali/operators/math/normalize/normalize.cc: out = (in - mean) * scale / sqrt(var + eps) + shift over the reduced
-//                axes of a 2-D sample; the mean / variance sums are tree reductions here (tolerance: 1e-5 relative).
+//                axes of a 2-D sample; the mean / variance sums are tree reductions over the deviations from the group's first
+//                element (a constant group gives `shift`), checked against a float64 statement with a per-element bound
+//                (tests/audio_tail_f64.py).
 //   NonsilentRegion  dali/operators/audio/nonsilence_op.h:60-130 + dali/kernels/signal/moving_mean_square.cc:55-77: moving mean
 //                square with a RUNNING float sum (add the new square, emit, subtract the oldest), restarted every `reset_interval`
 //                samples; threshold = reference * 10^(cutoff_db / 10) with reference = the maximum of the moving mean square by
@@ -297,17 +299,21 @@ __global__ void __launch_bounds__(256) normalize_kernel(const SigDesc *__restric
     if (mode == 0) { cnt = d.rows * d.cols; stride = 1; base = 0; }
     else if (mode == 1) { cnt = d.cols; stride = 1; base = g * d.cols; }
     else { cnt = d.rows; stride = d.cols; base = g; }
+    // The sums run over the deviations from the group's first element: a constant group then has mean and variance exactly 0 (a
+    // float mean of equal values need not equal them, and (x - mean)^2 > 0 would turn a constant row into +-scale), and an offset
+    // shared by the whole group (DC) does not enter the rounding of the sums.
+    const float x0 = __ldg(d.in + base);
     float sum = 0.0f;
-    for (int64_t e = threadIdx.x; e < cnt; e += blockDim.x) sum += __ldg(d.in + base + e * stride);
-    const float mean = block_sum(sum, sh) / (float)cnt;
+    for (int64_t e = threadIdx.x; e < cnt; e += blockDim.x) sum += __ldg(d.in + base + e * stride) - x0;
+    const float mean = block_sum(sum, sh) / (float)cnt;                 // of the deviations
     float sq = 0.0f;
-    for (int64_t e = threadIdx.x; e < cnt; e += blockDim.x) { const float x = __ldg(d.in + base + e * stride) - mean; sq += x * x; }
+    for (int64_t e = threadIdx.x; e < cnt; e += blockDim.x) { const float x = (__ldg(d.in + base + e * stride) - x0) - mean; sq += x * x; }
     const float var = block_sum(sq, sh) / (float)max((int64_t)1, cnt - ddof);
     const float sd = sqrtf(var + eps);
     const float mul = sd != 0.0f ? scale / sd : 0.0f;
     for (int64_t e = threadIdx.x; e < cnt; e += blockDim.x) {
       const int64_t i = base + e * stride;
-      d.out[i] = (__ldg(d.in + i) - mean) * mul + shift;
+      d.out[i] = ((__ldg(d.in + i) - x0) - mean) * mul + shift;
     }
     __syncthreads();
   }
