@@ -225,13 +225,42 @@ def test_mel_filter_bank_bit_exact():
             assert np.array_equal(bits(o), bits(po.mel_filter_bank(s, nf, sr, fl, fh, formula, norm))), (nf, formula)
 
 
+def _mel_f64(spec, nf, sr, fl, fh, formula, norm):
+    """The float64 mel filter bank (tests/image_f64.py mel_weights: triangles between mel-spaced edges at the bin frequencies) applied to
+    a spectrogram, and its bound: the weights' own bound times the powers, plus 2 (nterms + 16) u sum_b w P for the float32 sums
+    (nterms = the filter's non-zero weights; u = 2^-24; 16 for the ~2^-21 split products of the tensor-core path)."""
+    import image_f64 as F
+    W, B = F.mel_weights(spec.shape[0], nf, sr, fl, fh, formula == "htk", norm)
+    P = spec.astype(np.float64)
+    nterms = (W != 0).sum(axis=1, keepdims=True)
+    want = W @ P
+    return want, B @ P + 2 * (nterms + 16) * 2.0 ** -24 * want
+
+
+def test_mel_filter_bank_default_path_f64():
+    """The default (banded, non-tensor-core) mel kernel against the float64 statement of the weights, within the bound."""
+    import gpu_helpers as g
+    import image_f64 as F
+    rng = np.random.default_rng(65)
+    specs = [po.spectrogram(_clip(rng, n), nfft=1024, window_length=1024, window_step=256) for n in (16000, 5000)]
+    specs[0][:, 10:20] *= np.float32(1e-12)
+    for (nf, sr, fl, fh, formula, norm) in [(128, 16000.0, 0.0, 8000.0, "slaney", True), (80, 16000.0, 20.0, 7600.0, "htk", False),
+                                            (200, 44100.0, 0.0, 0.0, "slaney", True), (13, 22050.0, 100.0, 9000.0, "htk", True)]:
+        got = g.mel_filter_bank(specs, nf, sr, fl, fh, formula, norm)
+        for s, o in zip(specs, got):
+            want, tol = _mel_f64(s, nf, sr, fl, fh, formula, norm)
+            F.check(o, want, tol, (nf, formula))
+
+
 def test_mel_filter_bank_tensor_core_path():
     """The optional dense-GEMM path on the tensor cores (TF32 x 3 split, FP32 accumulate): same weights, different summation
     order.  Weights and powers are >= 0, so every output element gets a bound relative to its own float64 value,
-    2 (nterms + 16) u sum_b w P (nterms = the filter's non-zero weights; u = 2^-24; 16 for the ~2^-21 split products): a bound
-    relative to the row maximum would not see a wrong quiet frame, and frames 120 dB below the rest are included.  Also nfilter not a
-    multiple of 16 / above 128 and window counts that are not multiples of the 64-column tile."""
+    2 (nterms + 16) u sum_b w P against the float32 weights the kernel multiplies (nterms = the filter's non-zero weights; u = 2^-24; 16
+    for the ~2^-21 split products): a bound relative to the row maximum would not see a wrong quiet frame, and frames 120 dB below the
+    rest are included.  The same outputs are also held to the float64 statement of the weights (_mel_f64), which does not rest on the
+    restatement's weights.  Also nfilter not a multiple of 16 / above 128 and window counts that are not multiples of the 64-column tile."""
     import gpu_helpers as g
+    import image_f64 as F
     rng = np.random.default_rng(64)
     specs = [po.spectrogram(_clip(rng, n), nfft=1024, window_length=1024, window_step=256) for n in (16000, 5000, 160000, 700)]
     specs[0][:, 10:20] *= np.float32(1e-12)                             # 120 dB below the other frames
@@ -243,6 +272,8 @@ def test_mel_filter_bank_tensor_core_path():
         W = po.mel_weights(specs[0].shape[0], nf, sr, fl, fh, formula, norm).astype(np.float64)
         nterms = (W != 0).sum(axis=1, keepdims=True)
         for s, o in zip(specs, got):
+            want64, tol64 = _mel_f64(s, nf, sr, fl, fh, formula, norm)
+            F.check(o, want64, tol64, (nf, formula, "float64 weights"))
             want = W @ s.astype(np.float64)
             tol = 2 * (nterms + 16) * 2.0 ** -24 * want
             err = np.abs(o - want)
