@@ -130,6 +130,7 @@ struct RsDesc {
   int32_t use_stream;        // this sample is processed by resample_stream_kernel (decided at launch)
   int32_t tile_walk;         // the tile kernel may use the row walk (tile step count fits)
   int32_t walk_slots;        // > 0: vertical pass by the row walk with this many accumulator slots (see walk_vertical_u8)
+  int32_t walk_off;          // streamed samples: per-chunk offsets of the walk records in the table arena (see BuildWalkRecords)
   int64_t first_tile;
   // planar 4:2:0 YCbCr source (decoder planes, see resample_planar_kernel): the sample is the window [crop_y, +in_h) x [crop_x, +in_w)
   // of an img_h x img_w image
@@ -468,17 +469,24 @@ __global__ void __launch_bounds__(256) resample_fused_kernel(const RsDesc *__res
 // run the row walk (see walk_vertical_u8) over the ring, keep the open output rows in registers ACROSS chunks of 8 output
 // rows (so there is no vertical overlap between chunks: every source byte is loaded and converted once per strip), park each
 // finished output row in shared memory and, every 8 rows, run the horizontal pass from there.  The producer runs ahead
-// across chunk and item boundaries, so HBM latency is hidden by the ring, not by occupancy.
+// across chunk and item boundaries, so HBM latency is hidden by the ring, not by occupancy.  The walk tables of a chunk
+// (see BuildWalkRecords) are precomputed in the plan; the producer copies them into one of two record buffers ahead of the
+// chunk's rows.
 constexpr int kStRowBytes = 2048;         // one source row segment
-constexpr int kStSlotRows = 8;            // ring slot = TWO consecutive source rows of a chunk: one mbarrier wait / proxy fence / arrive
+constexpr int kStSlotRows = 4;            // ring slot = FOUR consecutive source rows of a chunk: one mbarrier wait / proxy fence / arrive
                                           // per slot instead of per row (the per-row synchronisation stalled the walk)
-constexpr int kStStages = 2;
+constexpr int kStStages = 5;              // 4 slots (16 rows) in flight while one is read: the most that fits 2 CTAs / SM
 constexpr int kStTH = 8;                  // output rows per chunk
+constexpr int kStSeg = 7 * kStTH;         // output rows per work item (a multiple of kStTH: chunk c of a sample starts at row c * kStTH)
 constexpr int kStConsumers = 256;
 constexpr int kStThreads = kStConsumers + 32;
 constexpr int kStSlotBytes = kStSlotRows * kStRowBytes;
-constexpr int kStSmemBytes = kStTH * kStRowBytes * 4 + kStStages * kStSlotBytes + kWalkMax * kWalkSlots * 16 + kWalkMax * 4 +
-                             2 * kStStages * 8;
+// walk records of one chunk: ent[kWalkMax][kWalkSlots] float2 (c, RN(-2^23 c)) of the tap that slot s takes from step j, or zeros,
+// then fin[kWalkMax] (byte s = chunk-local output row that slot s completes at step j, 0xFF = none)
+constexpr int kWalkEntBytes = kWalkMax * kWalkSlots * 8;
+constexpr int kWalkRecBytes = kWalkEntBytes + kWalkMax * 4;
+constexpr int kStSmemBytes = kStTH * kStRowBytes * 4 + kStStages * kStSlotBytes + 2 * kWalkRecBytes + (2 * kStStages + 4) * 8;
+static_assert(2 * (kStSmemBytes + 1024) <= 228 * 1024, "two streaming CTAs must fit one SM");
 
 struct RsItem { int32_t sample, ox0, tw, oy0, oy1; };
 
@@ -502,20 +510,21 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
   extern __shared__ __align__(128) uint8_t st_smem[];
   float *tmp2 = reinterpret_cast<float *>(st_smem);                               // [4 row pairs][RE][2]
   uint8_t *ring = st_smem + kStTH * kStRowBytes * 4;
-  float2 (*ent)[kWalkSlots] = reinterpret_cast<float2 (*)[kWalkSlots]>(ring + kStStages * kStSlotBytes);   // (c, -2^23 c) per step, slot
-  uint32_t *fin = reinterpret_cast<uint32_t *>(ring + kStStages * kStSlotBytes + kWalkMax * kWalkSlots * 16);
-  uint64_t *full = reinterpret_cast<uint64_t *>(fin + kWalkMax);
+  uint8_t *recs = ring + kStStages * kStSlotBytes;                                // [2][kWalkRecBytes]
+  uint64_t *full = reinterpret_cast<uint64_t *>(recs + 2 * kWalkRecBytes);
   uint64_t *empty = full + kStStages;
+  uint64_t *rfull = empty + kStStages, *rempty = rfull + 2;                       // the two record buffers
   const int tid = threadIdx.x;
   if (tid == 0) {
     for (int s = 0; s < kStStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], kStConsumers / 32); }
+    for (int s = 0; s < 2; s++) { mbar_init(&rfull[s], 1); mbar_init(&rempty[s], kStConsumers / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   if (tid >= kStConsumers) {
     // ------------------------------------------------------------------ producer warp: one lane issues the bulk copies
     if (tid == kStConsumers) {
-      uint32_t stage = 0, par = 1;
+      uint32_t stage = 0, par = 1, rb = 0, rpar = 1;
       for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
         const RsItem it = items[item];
         const RsDesc &d = descs[it.sample];
@@ -526,14 +535,23 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
         const int64_t pitch = (int64_t)d.in_w * d.C;
         const uint8_t *src0 = static_cast<const uint8_t *>(d.in) + g.e0;
         const int ustart = idx_y[it.oy0];
-        // the same chunking as the consumers: slots pair the rows of ONE chunk (a chunk with an odd row count ends with a half slot)
+        // the same chunking as the consumers: slots group the rows of ONE chunk (a chunk ends with a partial slot)
         for (int cy0 = it.oy0; cy0 < it.oy1; cy0 += kStTH) {
           const int th = min(kStTH, it.oy1 - cy0);
           const int cs = cy0 == it.oy0 ? ustart : idx_y[cy0 - 1] + Sy;
           const int J = idx_y[cy0 + th - 1] + Sy - cs;
+          {
+            const int32_t *rec = tab + tab[d.walk_off + cy0 / kStTH];
+            const uint32_t fin_bytes = (uint32_t)((J + 3) & ~3) * 4u;
+            mbar_wait(&rempty[rb], rpar);
+            mbar_expect_tx(&rfull[rb], (uint32_t)J * kWalkSlots * 8u + fin_bytes);
+            bulk_g2s(recs + rb * kWalkRecBytes, rec, (uint32_t)J * kWalkSlots * 8u, &rfull[rb]);
+            bulk_g2s(recs + rb * kWalkRecBytes + kWalkEntBytes, rec + J * kWalkSlots * 2, fin_bytes, &rfull[rb]);
+            if (++rb == 2) { rb = 0; rpar ^= 1u; }
+          }
           for (int j = 0; j < J; j += kStSlotRows) {
             const int nr = min(kStSlotRows, J - j);
-            mbar_wait_backoff(&empty[stage], par);
+            mbar_wait(&empty[stage], par);
             mbar_expect_tx(&full[stage], (uint32_t)(g.bytes * nr));
             for (int q = 0; q < nr; q++) {
               const int row = by + min(max(cs + j + q, 0), ey - 1);
@@ -549,15 +567,14 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
   // -------------------------------------------------------------------- consumers
   constexpr int NW = 2;
   const int lane = tid & 31;
-  uint32_t stage = 0, par = 0;
+  uint32_t stage = 0, par = 0, rb = 0, rpar = 0;
   for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
     const RsItem it = items[item];
     const RsDesc &d = descs[it.sample];
     if (!d.use_stream) continue;
-    const int C = d.C, Sx = d.support[0], Sy = d.support[1], W = d.walk_slots;
+    const int C = d.C, Sx = d.support[0], Sy = d.support[1];
     const int32_t *idx_x = tab + d.idx_off[0], *idx_y = tab + d.idx_off[1];
     const float *coef_x = reinterpret_cast<const float *>(tab + d.coef_off[0]);
-    const float *coef_y = reinterpret_cast<const float *>(tab + d.coef_off[1]);
     const int bx = d.base[0], ex = d.extent[0];
     const StripGeom g = strip_geom(d, idx_x, it.ox0, it.tw);
     const int RE = g.bytes, words = g.bytes >> 2;
@@ -577,24 +594,12 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
       const int th = min(kStTH, it.oy1 - cy0);
       const int cs = cy0 == it.oy0 ? ustart : idx_y[cy0 - 1] + Sy;
       const int J = idx_y[cy0 + th - 1] + Sy - cs;
-      // ---- chunk tables
-      for (int e = tid; e < J * kWalkSlots; e += kStConsumers) (&ent[0][0])[e] = make_float2(0.f, 0.f);
-      for (int j = tid; j < J; j += kStConsumers) fin[j] = 0xFFFFFFFFu;
-      consumer_bar();
-      for (int e = tid; e < (th + kWalkSlots) * Sy; e += kStConsumers) {
-        const int tl = e / Sy, k = e - tl * Sy, t = cy0 + tl;
-        if (t < it.oy1) {
-          const int j = idx_y[t] + k - cs;
-          if (j >= 0 && j < J) {
-            const float c = coef_y[(int64_t)t * Sy + k];
-            ent[j][t % W] = make_float2(c, mul_rn(c, -8388608.0f));
-            if (k == Sy - 1) reinterpret_cast<uint8_t *>(&fin[j])[t % W] = (uint8_t)tl;
-          }
-        }
-      }
-      consumer_bar();
-      // ---- stage A: row walk over the ring.  All WMAX slots are updated unconditionally (a closed slot has c = d = 0 and
-      //      adds +0, which is exact); the only data-dependent branch is the rare "row finished" one.
+      // ---- the chunk's walk records, copied in by the producer
+      const float2 (*ent)[kWalkSlots] = reinterpret_cast<const float2 (*)[kWalkSlots]>(recs + rb * kWalkRecBytes);
+      const uint32_t *fin = reinterpret_cast<const uint32_t *>(recs + rb * kWalkRecBytes + kWalkEntBytes);
+      mbar_wait(&rfull[rb], rpar);
+      // ---- stage A: row walk over the ring.  Closed slots (c = d = 0, exact zeros) are skipped by a CTA-uniform branch;
+      //      the only other data-dependent branch is the rare "row finished" one.
       for (int j2 = 0; j2 < J; j2 += kStSlotRows) {
         mbar_wait(&full[stage], par);
         const uint32_t *rw = reinterpret_cast<const uint32_t *>(ring + stage * kStSlotBytes);
@@ -668,6 +673,11 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
         }
         }            // rows of the slot
       }
+      // release the record buffer to the producer's next bulk copy (the async proxy), as a ring slot is released
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&rempty[rb]);
+      if (++rb == 2) { rb = 0; rpar ^= 1u; }
       consumer_bar();
       // ---- stage B: horizontal pass of the chunk's th rows, two rows per packed operation
       const int npair = (th + 1) >> 1;
@@ -701,7 +711,7 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_stream_kernel(const Rs
           if (t0 + 1 < th) out[((int64_t)(cy0 + t0 + 1) * d.out_w + ox) * C + c] = rs_store_cvt<Out>(a[p].y, he);
         }
       }
-      // no barrier here: the next chunk's table fill is separated from its walk (which overwrites tmp2) by consumer_bar()
+      consumer_bar();   // the next chunk's walk overwrites the parked rows
     }
   }
 }
@@ -792,10 +802,9 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_planar_kernel(const Rs
   for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
     const RsItem it = items[item];
     const RsDesc &d = descs[it.sample];
-    const int C = 3, Sx = d.support[0], Sy = d.support[1], W = d.walk_slots;
+    const int C = 3, Sx = d.support[0], Sy = d.support[1];
     const int32_t *idx_x = tab + d.idx_off[0], *idx_y = tab + d.idx_off[1];
     const float *coef_x = reinterpret_cast<const float *>(tab + d.coef_off[0]);
-    const float *coef_y = reinterpret_cast<const float *>(tab + d.coef_off[1]);
     const int bx = d.base[0], ex = d.extent[0];
     const PlanarGeom g = planar_geom(d, idx_x, it.ox0, it.tw);
     const int RE = g.npx * 3;
@@ -818,20 +827,11 @@ __global__ void __launch_bounds__(kStThreads, 2) resample_planar_kernel(const Rs
       const int th = min(kStTH, it.oy1 - cy0);
       const int cs = cy0 == it.oy0 ? ustart : idx_y[cy0 - 1] + Sy;
       const int J = idx_y[cy0 + th - 1] + Sy - cs;
-      // ---- chunk tables
-      for (int e = tid; e < J * kWalkSlots; e += kStConsumers) (&ent[0][0])[e] = make_float2(0.f, 0.f);
-      for (int j = tid; j < J; j += kStConsumers) fin[j] = 0xFFFFFFFFu;
-      consumer_bar();
-      for (int e = tid; e < (th + kWalkSlots) * Sy; e += kStConsumers) {
-        const int tl = e / Sy, k = e - tl * Sy, t = cy0 + tl;
-        if (t < it.oy1) {
-          const int j = idx_y[t] + k - cs;
-          if (j >= 0 && j < J) {
-            const float c = coef_y[(int64_t)t * Sy + k];
-            ent[j][t % W] = make_float2(c, mul_rn(c, -8388608.0f));
-            if (k == Sy - 1) reinterpret_cast<uint8_t *>(&fin[j])[t % W] = (uint8_t)tl;
-          }
-        }
+      // ---- the chunk's walk records from the plan (see BuildWalkRecords)
+      {
+        const int32_t *rec = tab + tab[d.walk_off + cy0 / kStTH];
+        for (int e = tid; e < J * kWalkSlots * 2; e += kStConsumers) reinterpret_cast<int32_t *>(&ent[0][0])[e] = rec[e];
+        for (int j = tid; j < J; j += kStConsumers) fin[j] = (uint32_t)rec[J * kWalkSlots * 2 + j];
       }
       consumer_bar();
       // ---- stage A: row walk over the ring, pixels produced on the fly
@@ -974,6 +974,7 @@ struct dalib200ResamplePlan {
   std::vector<int32_t> tables;                 // host copy of the table arena (idx, coef bits, flags)
   std::vector<int32_t> uploaded_tables;        // what the device arena currently holds
   std::map<TableKey, AxisTableRef> cache;      // dedup of axis tables within a batch
+  std::map<int, int> walk_cache;               // vertical axis table offset -> its walk records (BuildWalkRecords)
   std::vector<int> order0;
   int64_t total_tiles = 0;
   DescArena desc_arena, table_arena, item_arena;
@@ -1104,6 +1105,59 @@ int BuildHorzFlags(std::vector<int32_t> &arena, int idx_off, int ow, int iw, int
   return off;
 }
 
+// Walk records of the streaming kernels for one vertical axis: the tables stage A of resample_stream_kernel and resample_planar_kernel
+// walks by.  Chunks of kStTH output rows restart at every kStSeg-row work item, as the kernels' chunks do.  The records of a chunk
+// cover the steps j = 0..J-1 of its row walk: ent[j][s] = (c, RN(-2^23 c)) of the tap that accumulator slot s takes at step j, or exact
+// zeros for a closed slot (the kernels skip a slot with c == 0), and fin[j], whose byte s is the chunk-local output row that slot s
+// completes at step j (0xFF: none).  -2^23 c is a power-of-two scaling of c, so the host product is the device's mul.rn bit for bit.
+// Layout: one arena word offset per chunk, then per chunk (16-byte aligned, for the bulk copies) ent[J][kWalkSlots] as float2 and
+// fin[J] padded to a multiple of 4 words.  Returns the offset of the per-chunk offsets, or -1 if the arena would exceed its limit.
+int BuildWalkRecords(std::vector<int32_t> &arena, int idx_off, int coef_off, int out_h, int Sy, int W) {
+  const std::vector<int32_t> iy(arena.begin() + idx_off, arena.begin() + idx_off + out_h);
+  const std::vector<int32_t> cw(arena.begin() + coef_off, arena.begin() + coef_off + static_cast<size_t>(out_h) * Sy);
+  auto chunk_steps = [&](int o, int c0, int c1, int &cs) {
+    cs = c0 == o ? iy[o] : iy[c0 - 1] + Sy;
+    return iy[c1 - 1] + Sy - cs;
+  };
+  const int nchunks = (out_h + kStTH - 1) / kStTH;
+  int64_t words = static_cast<int64_t>(arena.size()) + nchunks;
+  for (int o = 0; o < out_h; o += kStSeg)
+    for (int c0 = o, o1 = std::min(o + kStSeg, out_h), cs; c0 < o1; c0 += kStTH) {
+      const int J = chunk_steps(o, c0, std::min(c0 + kStTH, o1), cs);
+      words += 3 + static_cast<int64_t>(J) * kWalkSlots * 2 + ((J + 3) & ~3);
+    }
+  if (words >= (int64_t{1} << 26)) return -1;
+  const int off = static_cast<int>(arena.size());
+  arena.resize(arena.size() + nchunks);
+  for (int o = 0; o < out_h; o += kStSeg) {
+    const int o1 = std::min(o + kStSeg, out_h);
+    for (int c0 = o; c0 < o1; c0 += kStTH) {
+      int cs;
+      const int J = chunk_steps(o, c0, std::min(c0 + kStTH, o1), cs);
+      arena.resize((arena.size() + 3) & ~static_cast<size_t>(3));
+      const size_t r = arena.size(), rf = r + static_cast<size_t>(J) * kWalkSlots * 2;
+      arena[off + c0 / kStTH] = static_cast<int32_t>(r);
+      arena.resize(rf + ((J + 3) & ~3), -1);
+      std::fill(arena.begin() + r, arena.begin() + rf, 0);
+      uint8_t *fin = reinterpret_cast<uint8_t *>(arena.data() + rf);
+      // rows open during the chunk: from its first row up to the first one that opens after the chunk's last step
+      for (int t = c0; t < o1 && iy[t] < cs + J; t++) {
+        for (int k = 0; k < Sy; k++) {
+          const int j = iy[t] + k - cs;
+          if (j < 0 || j >= J) continue;
+          float c;
+          memcpy(&c, &cw[static_cast<size_t>(t) * Sy + k], sizeof(c));
+          const float d = c * -8388608.0f;
+          memcpy(&arena[r + (static_cast<size_t>(j) * kWalkSlots + t % W) * 2], &c, sizeof(c));
+          memcpy(&arena[r + (static_cast<size_t>(j) * kWalkSlots + t % W) * 2 + 1], &d, sizeof(d));
+          if (k == Sy - 1) fin[4 * j + t % W] = static_cast<uint8_t>(t - c0);
+        }
+      }
+    }
+  }
+  return off;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1152,6 +1206,7 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
   p->path.assign(n, 0);
   p->tables.clear();
   p->cache.clear();
+  p->walk_cache.clear();
   int64_t tiles = 0;
   for (int i = 0; i < n; i++) {
     const auto &s = samples[i];
@@ -1296,7 +1351,7 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
           if (ok) { stw = t; break; }
           if (t == 1) break;
         }
-        const int seg = 7 * kStTH;
+        const int seg = kStSeg;
         bool ok = stw > 0;
         for (int o = 0; o < s.out_h && ok; o += seg) {
           int o1 = std::min(o + seg, s.out_h);
@@ -1305,6 +1360,16 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
             int cs = c0 == o ? iy[o] : iy[c0 - 1] + Sy;
             ok = iy[c1 - 1] + Sy - cs <= kWalkMax;
           }
+        }
+        if (ok) {   // (ix / iy are not used below: the arena may move)
+          auto wc = p->walk_cache.find(d.idx_off[1]);
+          if (wc != p->walk_cache.end()) {
+            d.walk_off = wc->second;
+          } else {
+            d.walk_off = BuildWalkRecords(p->tables, d.idx_off[1], d.coef_off[1], s.out_h, Sy, W);
+            p->walk_cache[d.idx_off[1]] = d.walk_off;
+          }
+          ok = d.walk_off >= 0;
         }
         if (ok) {
           p->stream_ok[i] = 1;
