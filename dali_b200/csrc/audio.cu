@@ -564,13 +564,12 @@ struct dalib200SpectrogramPlan {
   int64_t total_groups = 0;
   DescArena arena;           // descriptors
   float *d_window = nullptr; float2 *d_twiddle = nullptr;
-  int tw_nfft = 0, win_cap = 0;
+  int tw_nfft = 0;
+  size_t win_cap = 0;
   std::vector<float> window;
   bool window_dirty = true;
   size_t smem = 0;
   bool smem_set = false;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
   std::vector<float> preemph;    // per-sample coefficients of the fused pre-emphasis; empty = off
 };
 
@@ -589,8 +588,6 @@ struct dalib200MelPlan {
   int64_t total_items_mma = 0;
   std::vector<int64_t> first_item_mma;
   dalib200MelArgs args{};
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 namespace {
@@ -678,16 +675,12 @@ int dalib200SpectrogramPlanCreate(dalib200SpectrogramPlan **plan, int max_batch)
   p->max_batch = max_batch;
   int rc = p->arena.Reserve(sizeof(SpecDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("SpectrogramPlanCreate: cudaEventCreate failed"); p->arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200SpectrogramPlanDestroy(dalib200SpectrogramPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   if (p->d_window) cudaFree(p->d_window);
   if (p->d_twiddle) cudaFree(p->d_twiddle);
@@ -764,7 +757,6 @@ static int MelUploadTables(dalib200MelPlan *p, dalib200Stream_t stream, size_t *
 static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200MelPlan *mel,
                                  void *const *mel_out_ptrs, dalib200Stream_t stream) {
   if (p->n == 0 || p->total_groups == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
   const SpecParams &P = p->P;
   const bool pow2 = (P.nfft & (P.nfft - 1)) == 0;
   if (p->tw_nfft != P.nfft) {
@@ -782,27 +774,21 @@ static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *
     p->tw_nfft = P.nfft;
   }
   if (p->window_dirty) {
-    if (p->win_cap < P.win_len) {
-      if (p->d_window) cudaFree(p->d_window);
-      p->d_window = nullptr;
-      DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&p->d_window), sizeof(float) * P.win_len));
-      p->win_cap = P.win_len;
-    }
+    if (int rc = GrowDevice(p->d_window, p->win_cap, (size_t)P.win_len)) return rc;
     DB_CUDA(cudaMemcpyAsync(p->d_window, p->window.data(), sizeof(float) * P.win_len, cudaMemcpyHostToDevice, stream));
     DB_CUDA(cudaStreamSynchronize(stream));
     p->window_dirty = false;
   }
   const bool pre = !p->preemph.empty();
-  auto *hd = reinterpret_cast<SpecDesc *>(p->arena.host);
+  SpecDesc *hd;
+  int rc = p->arena.Stage(sizeof(SpecDesc) * p->n, &hd);
+  if (rc) return rc;
   for (int i = 0; i < p->n; i++) {
     hd[i] = p->descs[i]; hd[i].in = static_cast<const float *>(in_ptrs[i]);
     hd[i].out = out_ptrs ? static_cast<float *>(out_ptrs[i]) : nullptr;
     hd[i].preemph = pre ? p->preemph[i] : 0.0f;
   }
-  int rc = p->arena.Upload(sizeof(SpecDesc) * p->n, stream);
-  if (rc) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
+  if ((rc = p->arena.Upload(sizeof(SpecDesc) * p->n, stream))) return rc;
   static const bool radix2_only = getenv("DALIB200_STFT_RADIX2") != nullptr;
   if (P.nfft == 1024 && (!radix2_only || mel)) {
     // register-resident 32 x 32 FFT, one warp per pair of frames (16 frames per CTA = the grouping the descriptors were built with)
@@ -817,14 +803,12 @@ static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *
     const int grid = (int)std::min<int64_t>(p->total_groups, (int64_t)NumSMs() * 2);
     MelTables mt{};
     if (mel) {
-      if (mel->pending) { DB_CUDA(cudaEventSynchronize(mel->uploaded)); mel->pending = false; }
       size_t o_up = 0, o_down = 0;
       if ((rc = MelUploadTables(mel, stream, &o_up, &o_down))) return rc;
-      auto *md = reinterpret_cast<MelDesc *>(mel->arena.host);
+      MelDesc *md;
+      if ((rc = mel->arena.Stage(sizeof(MelDesc) * mel->n, &md))) return rc;
       for (int i = 0; i < mel->n; i++) { md[i] = mel->descs[i]; md[i].in = nullptr; md[i].out = static_cast<float *>(mel_out_ptrs[i]); }
       if ((rc = mel->arena.Upload(sizeof(MelDesc) * mel->n, stream))) return rc;
-      DB_CUDA(cudaEventRecord(mel->uploaded, stream));
-      mel->pending = true;
       mt.ends = reinterpret_cast<const int32_t *>(mel->tables.dev);
       mt.w_up = reinterpret_cast<const float *>(mel->tables.dev + o_up);
       mt.w_down = reinterpret_cast<const float *>(mel->tables.dev + o_down);
@@ -888,16 +872,12 @@ int dalib200MelPlanCreate(dalib200MelPlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   int rc = p->arena.Reserve(sizeof(MelDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("MelPlanCreate: cudaEventCreate failed"); p->arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200MelPlanDestroy(dalib200MelPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free(); p->tables.Free(); p->dense.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -950,11 +930,12 @@ static int MelUploadTables(dalib200MelPlan *p, dalib200Stream_t stream, size_t *
   const size_t tbytes = o_down + p->h_down.size() * 4;
   *o_up_out = o_up; *o_down_out = o_down;
   if (p->tables_dirty) {
-    int rc = p->tables.Reserve(tbytes);
+    uint8_t *h;
+    int rc = p->tables.Stage(tbytes, &h);
     if (rc) return rc;
-    memcpy(p->tables.host, p->h_ends.data(), p->h_ends.size() * 4);
-    memcpy(p->tables.host + o_up, p->h_up.data(), p->h_up.size() * 4);
-    memcpy(p->tables.host + o_down, p->h_down.data(), p->h_down.size() * 4);
+    memcpy(h, p->h_ends.data(), p->h_ends.size() * 4);
+    memcpy(h + o_up, p->h_up.data(), p->h_up.size() * 4);
+    memcpy(h + o_down, p->h_down.data(), p->h_down.size() * 4);
     rc = p->tables.Upload(tbytes, stream);
     if (rc) return rc;
     p->tables_dirty = false;
@@ -965,33 +946,29 @@ static int MelUploadTables(dalib200MelPlan *p, dalib200Stream_t stream, size_t *
 int dalib200MelLaunch(dalib200MelPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && in_ptrs && out_ptrs, "MelLaunch: null argument");
   if (p->n == 0 || p->total_items == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
   size_t o_up = 0, o_down = 0;
-  {
-    const int rc = MelUploadTables(p, stream, &o_up, &o_down);
-    if (rc) return rc;
-  }
-  auto *hd = reinterpret_cast<MelDesc *>(p->arena.host);
+  int rc = MelUploadTables(p, stream, &o_up, &o_down);
+  if (rc) return rc;
+  MelDesc *hd;
+  if ((rc = p->arena.Stage(sizeof(MelDesc) * p->n, &hd))) return rc;
   for (int i = 0; i < p->n; i++) {
     hd[i] = p->descs[i]; hd[i].in = static_cast<const float *>(in_ptrs[i]); hd[i].out = static_cast<float *>(out_ptrs[i]);
     if (p->tensor_cores) hd[i].first_item = p->first_item_mma[i];
   }
-  int rc = p->arena.Upload(sizeof(MelDesc) * p->n, stream);
-  if (rc) return rc;
+  if ((rc = p->arena.Upload(sizeof(MelDesc) * p->n, stream))) return rc;
   if (p->tensor_cores) {
     const int mblocks = (p->nfilter + kMmM - 1) / kMmM;
     if (p->dense_dirty) {
       p->kpad = (p->nbin + kMmK - 1) / kMmK * kMmK; p->mpad = mblocks * kMmM;
       const size_t wbytes = (size_t)p->mpad * p->kpad * 4, total = wbytes + sizeof(int2) * mblocks;
-      rc = p->dense.Reserve(total);
-      if (rc) return rc;
-      float *w = reinterpret_cast<float *>(p->dense.host);
+      float *w;
+      if ((rc = p->dense.Stage(total, &w))) return rc;
       memset(w, 0, wbytes);
       for (int m = 0; m < p->nfilter; m++) {
         for (int b = p->h_ends[m]; b < p->h_ends[m + 1]; b++) w[(size_t)m * p->kpad + b] = p->h_up[b];
         for (int b = p->h_ends[m + 1]; b < p->h_ends[m + 2]; b++) w[(size_t)m * p->kpad + b] = p->h_down[b];
       }
-      int2 *kr = reinterpret_cast<int2 *>(p->dense.host + wbytes);
+      int2 *kr = reinterpret_cast<int2 *>(reinterpret_cast<uint8_t *>(w) + wbytes);
       for (int mb = 0; mb < mblocks; mb++) {
         const int m0 = mb * kMmM, m1 = std::min(p->nfilter, m0 + kMmM);
         kr[mb] = make_int2(p->h_ends[m0] / kMmK, (p->h_ends[m1 + 1] + kMmK - 1) / kMmK);
@@ -1000,8 +977,6 @@ int dalib200MelLaunch(dalib200MelPlan *p, const void *const *in_ptrs, void *cons
       if (rc) return rc;
       p->dense_dirty = false;
     }
-    DB_CUDA(cudaEventRecord(p->uploaded, stream));
-    p->pending = true;
     const int grid = (int)std::min<int64_t>(p->total_items_mma, (int64_t)NumSMs() * 8);
     ProfScope ps_("mel_filter_bank_mma", stream);
     mel_mma_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items_mma, p->nfilter, p->nbin,
@@ -1011,8 +986,6 @@ int dalib200MelLaunch(dalib200MelPlan *p, const void *const *in_ptrs, void *cons
     DB_CUDA(cudaGetLastError());
     return DALIB200_SUCCESS;
   }
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 32);
   ProfScope ps_("mel_filter_bank", stream);
   mel_kernel<<<grid, 128, 0, stream>>>(reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items, p->nfilter,

@@ -350,8 +350,6 @@ struct dalib200SignalPlan {
   std::vector<SigDesc> descs;
   int64_t total_items = 0;
   DescArena arena;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
   // ToDecibels
   float mul_log2 = 0, s_ref = 1, min_ratio = 1e-8f; bool ref_max = false;
   uint32_t *d_max = nullptr; size_t d_max_cap = 0;
@@ -376,15 +374,6 @@ struct dalib200SignalPlan {
 };
 
 namespace {
-int GrowF(float *&p, size_t &cap, size_t need) {
-  if (need <= cap) return DALIB200_SUCCESS;
-  if (p) cudaFree(p);
-  p = nullptr; cap = 0;
-  DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&p), need * sizeof(float)));
-  cap = need;
-  return DALIB200_SUCCESS;
-}
-
 // dali/kernels/signal/dct/table.h:27-112
 void FillCosineTable(float *table, int64_t n, int ndct, int type, bool normalize) {
   int64_t idx = 0;
@@ -418,12 +407,6 @@ void FillCosineTable(float *table, int64_t n, int ndct, int type, bool normalize
       for (int64_t i = 0; i < n; i++) table[idx++] = static_cast<float>(f * std::cos(phase_mul * (i + 0.5) * (k + 0.5)));
   }
 }
-
-int UploadDescs(dalib200SignalPlan *p) {
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->arena.Reserve(sizeof(SigDesc) * std::max(1, p->n));
-  return rc;
-}
 }  // namespace
 
 extern "C" {
@@ -432,16 +415,12 @@ int dalib200SignalPlanCreate(dalib200SignalPlan **plan, int max_batch) try {
   DB_CHECK_ARG(plan && max_batch > 0, "SignalPlanCreate: bad arguments");
   auto *p = new dalib200SignalPlan();
   p->max_batch = max_batch;
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("SignalPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200SignalPlanDestroy(dalib200SignalPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   if (p->d_max) cudaFree(p->d_max);
   if (p->d_table) cudaFree(p->d_table);
@@ -624,14 +603,11 @@ int dalib200PreemphasisSetup(dalib200SignalPlan *p, int n, const int64_t *length
 } DB_API_CATCH
 
 static int PreemphasisLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) {
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->arena.Reserve(sizeof(PeDesc) * p->n);
+  PeDesc *h;
+  int rc = p->arena.Stage(sizeof(PeDesc) * p->n, &h);
   if (rc) return rc;
-  PeDesc *h = reinterpret_cast<PeDesc *>(p->arena.host);
   for (int i = 0; i < p->n; i++) { h[i] = p->pe[i]; h[i].in = in_ptrs[i]; h[i].out = static_cast<float *>(out_ptrs[i]); }
   if ((rc = p->arena.Upload(sizeof(PeDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const PeDesc *d = reinterpret_cast<const PeDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
   ProfScope ps_("preemphasis_filter", stream);
@@ -646,11 +622,10 @@ int dalib200NonsilentLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, v
                             dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && p->kind == SIG_NONSILENT && (p->n == 0 || (in_ptrs && begin_ptrs && length_ptrs)), "NonsilentLaunch: call NonsilentSetup first");
   if (p->n == 0) return DALIB200_SUCCESS;
-  int rc = GrowF(p->d_mms, p->d_mms_cap, (size_t)p->mms_total);
+  int rc = GrowDevice(p->d_mms, p->d_mms_cap, (size_t)p->mms_total);
   if (rc) return rc;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  if ((rc = p->arena.Reserve(sizeof(NsDesc) * p->n))) return rc;
-  NsDesc *h = reinterpret_cast<NsDesc *>(p->arena.host);
+  NsDesc *h;
+  if ((rc = p->arena.Stage(sizeof(NsDesc) * p->n, &h))) return rc;
   int64_t off = 0;
   for (int i = 0; i < p->n; i++) {
     h[i] = p->ns[i];
@@ -659,8 +634,6 @@ int dalib200NonsilentLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, v
     off += p->ns[i].n;
   }
   if ((rc = p->arena.Upload(sizeof(NsDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const NsDesc *d = reinterpret_cast<const NsDesc *>(p->arena.dev);
   { ProfScope ps_("nonsilent_mms", stream); nonsilent_mms_kernel<<<(unsigned)((p->total_items + 127) / 128), 128, 0, stream>>>(d, p->n, p->total_items); }
   CountLaunch();
@@ -671,19 +644,16 @@ int dalib200NonsilentLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, v
 } DB_API_CATCH
 
 static int AudioResampleLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) {
-  int rc = GrowF(p->d_lookup, p->d_lookup_cap, p->ar_lookup.size());
+  int rc = GrowDevice(p->d_lookup, p->d_lookup_cap, p->ar_lookup.size());
   if (rc) return rc;
   if (p->lookup_dirty) {
     DB_CUDA(cudaMemcpyAsync(p->d_lookup, p->ar_lookup.data(), p->ar_lookup.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
     p->lookup_dirty = false;
   }
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  if ((rc = p->arena.Reserve(sizeof(ArDesc) * p->n))) return rc;
-  ArDesc *h = reinterpret_cast<ArDesc *>(p->arena.host);
+  ArDesc *h;
+  if ((rc = p->arena.Stage(sizeof(ArDesc) * p->n, &h))) return rc;
   for (int i = 0; i < p->n; i++) { h[i] = p->ar[i]; h[i].in = static_cast<const float *>(in_ptrs[i]); h[i].out = static_cast<float *>(out_ptrs[i]); }
   if ((rc = p->arena.Upload(sizeof(ArDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   ArWindow w{ p->ar_scale, p->ar_center, p->ar_lobes, p->d_lookup };
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 8);
   ProfScope ps_("audio_resample", stream);
@@ -699,13 +669,11 @@ int dalib200SignalLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void
   if (p->n == 0 || p->total_items == 0) return DALIB200_SUCCESS;
   if (p->kind == SIG_RESAMPLE) return AudioResampleLaunch(p, in_ptrs, out_ptrs, stream);
   if (p->kind == SIG_PREEMPH) return PreemphasisLaunch(p, in_ptrs, out_ptrs, stream);
-  int rc = UploadDescs(p);
+  SigDesc *h;
+  int rc = p->arena.Stage(sizeof(SigDesc) * p->n, &h);
   if (rc) return rc;
-  SigDesc *h = reinterpret_cast<SigDesc *>(p->arena.host);
   for (int i = 0; i < p->n; i++) { h[i] = p->descs[i]; h[i].in = static_cast<const float *>(in_ptrs[i]); h[i].out = static_cast<float *>(out_ptrs[i]); }
   if ((rc = p->arena.Upload(sizeof(SigDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const SigDesc *d = reinterpret_cast<const SigDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
   if (p->kind == SIG_TODB) {
@@ -725,7 +693,7 @@ int dalib200SignalLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void
     { ProfScope ps_("to_decibels", stream); todb_kernel<<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->mul_log2, p->s_ref, p->min_ratio, smax); }
     CountLaunch();
   } else if (p->kind == SIG_MFCC) {
-    if ((rc = GrowF(p->d_table, p->d_table_cap, p->h_table.size()))) return rc;
+    if ((rc = GrowDevice(p->d_table, p->d_table_cap, p->h_table.size()))) return rc;
     if (p->table_dirty) {
       // pageable source: the copy is staged by the runtime before the call returns
       DB_CUDA(cudaMemcpyAsync(p->d_table, p->h_table.data(), p->h_table.size() * sizeof(float), cudaMemcpyHostToDevice, stream));

@@ -242,8 +242,6 @@ struct dalib200CmnPlan {
   int out_dtype = DALIB200_FLOAT, out_layout = DALIB200_LAYOUT_CHW, out_c = 3;
   int64_t total_units = 0, total_elems = 0;
   DescArena arena;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 extern "C" {
@@ -254,16 +252,12 @@ int dalib200CmnPlanCreate(dalib200CmnPlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   int rc = p->arena.Reserve(sizeof(CmnDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("CmnPlanCreate: cudaEventCreate failed"); p->arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200CmnPlanDestroy(dalib200CmnPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -277,8 +271,8 @@ int dalib200CmnPlanSetup(dalib200CmnPlan *p, int n, const dalib200CmnSample *sam
                "CropMirrorNormalize: output type %d not supported (FLOAT, FLOAT16)", out_dtype);
   DB_CHECK_ARG(out_layout == DALIB200_LAYOUT_HWC || out_layout == DALIB200_LAYOUT_CHW, "CropMirrorNormalize: bad layout");
   DB_CHECK_ARG(out_channels >= 1 && out_channels <= 4, "CropMirrorNormalize: 1..4 output channels supported, got %d", out_channels);
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<CmnDesc *>(p->arena.host);
+  CmnDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(CmnDesc) * n, &descs)) return rc;
   int64_t units = 0, elems = 0;
   for (int i = 0; i < n; i++) {
     const auto &s = samples[i];
@@ -310,16 +304,14 @@ int dalib200CmnPlanSetup(dalib200CmnPlan *p, int n, const dalib200CmnSample *sam
 int dalib200CmnLaunch(dalib200CmnPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && in_ptrs && out_ptrs, "CmnLaunch: null argument");
   if (p->n == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<CmnDesc *>(p->arena.host);
+  CmnDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(CmnDesc) * p->n, &descs)) return rc;
   for (int i = 0; i < p->n; i++) {
     descs[i].in = static_cast<const uint8_t *>(in_ptrs[i]);
     descs[i].out = out_ptrs[i];
   }
   int rc = p->arena.Upload(sizeof(CmnDesc) * p->n, stream);
   if (rc) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const CmnDesc *dd = reinterpret_cast<const CmnDesc *>(p->arena.dev);
   const int sms = NumSMs();
   if (p->total_units > 0) {

@@ -19,32 +19,51 @@ void SetLastError(const char *fmt, ...) {
   tls_error = buf;
 }
 
-int DescArena::Reserve(size_t bytes) {
-  if (bytes <= cap) return DALIB200_SUCCESS;
-  size_t ncap = cap ? cap : 4096;
+int PinnedStage::Grow(size_t bytes, uint8_t **dev) {
+  if (pending_) { DB_CUDA(cudaEventSynchronize(uploaded_)); pending_ = false; }
+  if (bytes <= cap_) return DALIB200_SUCCESS;
+  size_t ncap = cap_ ? cap_ : 4096;
   while (ncap < bytes) ncap *= 2;
   uint8_t *nh = nullptr, *nd = nullptr;
   DB_CUDA(cudaMallocHost(reinterpret_cast<void **>(&nh), ncap));
-  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&nd), ncap);
-  if (e != cudaSuccess) { cudaFreeHost(nh); DB_CUDA(e); }
-  // NOTE: a previous launch may still be reading the old device arena; cudaFree synchronises the
-  // device implicitly, so growing is safe (it only happens while shapes are still warming up).
-  if (host) cudaFreeHost(host);
-  if (dev) cudaFree(dev);
-  host = nh; dev = nd; cap = ncap;
+  if (dev) {
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&nd), ncap);
+    if (e != cudaSuccess) { cudaFreeHost(nh); DB_CUDA(e); }
+    // NOTE: a previous launch may still be reading the old device arena; cudaFree synchronises the
+    // device implicitly, so growing is safe (it only happens while shapes are still warming up).
+    if (*dev) cudaFree(*dev);
+    *dev = nd;
+  }
+  if (host_) cudaFreeHost(host_);
+  host_ = nh; cap_ = ncap;
   return DALIB200_SUCCESS;
+}
+
+int PinnedStage::Record(cudaStream_t s) {
+  cudaError_t e = uploaded_ ? cudaSuccess : cudaEventCreateWithFlags(&uploaded_, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventRecord(uploaded_, s);
+  if (e != cudaSuccess) cudaStreamSynchronize(s);       // nothing to wait on later: the copies must be over before the buffer is reused
+  DB_CUDA(e);
+  pending_ = true;
+  return DALIB200_SUCCESS;
+}
+
+void PinnedStage::Free() {
+  if (uploaded_) { cudaEventSynchronize(uploaded_); cudaEventDestroy(uploaded_); }
+  if (host_) cudaFreeHost(host_);
+  host_ = nullptr; cap_ = 0; uploaded_ = nullptr; pending_ = false;
 }
 
 int DescArena::Upload(size_t bytes, cudaStream_t s) {
   if (bytes == 0) return DALIB200_SUCCESS;
-  DB_CUDA(cudaMemcpyAsync(dev, host, bytes, cudaMemcpyHostToDevice, s));
-  return DALIB200_SUCCESS;
+  DB_CUDA(cudaMemcpyAsync(dev, host_, bytes, cudaMemcpyHostToDevice, s));
+  return Record(s);
 }
 
 void DescArena::Free() {
-  if (host) cudaFreeHost(host);
+  PinnedStage::Free();
   if (dev) cudaFree(dev);
-  host = dev = nullptr; cap = 0;
+  dev = nullptr;
 }
 
 int NumSMs() {

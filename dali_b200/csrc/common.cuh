@@ -29,15 +29,6 @@ inline void CountLaunch(int n = 1) { g_launch_count.fetch_add(n, std::memory_ord
                              cudaGetErrorString(e__));                                          \
     return DALIB200_ERROR_CUDA; } } while (0)
 
-// A grow-only pinned-host + device arena for per-batch descriptors: one H2D copy per launch.
-struct DescArena {
-  uint8_t *host = nullptr, *dev = nullptr;
-  size_t cap = 0;
-  int Reserve(size_t bytes);
-  int Upload(size_t bytes, cudaStream_t s);   // async H2D of the first `bytes`
-  void Free();
-};
-
 int NumSMs();
 
 // Launch shape of a kernel whose working lanes each run one serial chain (tiff_segment, webp_entropy): one warp per CTA and `lanes`
@@ -207,12 +198,63 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const void *tmap, int c0,
 
 }  // namespace dalib200
 
-// The C-ABI never lets a C++ exception escape (std::bad_alloc / std::length_error from a host-side table of absurd size would otherwise
-// terminate the caller's process): every entry point is a function-try-block closed by this handler.  (Kept at the end of the header
-// so that the line tables of the device code above do not move.)
+// Host-only declarations: kept at the end of the header so that the line tables of the device code above do not move.
+#include <algorithm>
 #include <exception>
 #include <new>
 namespace dalib200 {
+// Grow-only pinned host memory that per-batch data is staged in for asynchronous copies to the device.  It keeps the one rule that
+// makes reusing it safe: the host side is not rewritten while a copy may still be reading it.  Stage() hands the host side out only
+// after the copies covered by the last Record() have finished.  The event behind that is created at the first Record().
+class PinnedStage {
+ public:
+  // Waits for the last recorded copies, grows the buffer to at least `bytes` (doubling from 4 KiB; a grown buffer does not keep its
+  // contents) and sets *host to its host side.
+  template <typename T> int Stage(size_t bytes, T **host) {
+    const int rc = Grow(bytes, nullptr);
+    *host = reinterpret_cast<T *>(host_);
+    return rc;
+  }
+  int Record(cudaStream_t s);   // after the caller's copies out of the buffer are enqueued on s
+  void Free();                  // waits for the last recorded copies, then frees the buffer and the event
+
+ protected:
+  int Grow(size_t bytes, uint8_t **dev);   // Stage's wait and growth; grows *dev to the same capacity when dev is given
+  uint8_t *host_ = nullptr;
+  size_t cap_ = 0;
+
+ private:
+  cudaEvent_t uploaded_ = nullptr;
+  bool pending_ = false;
+};
+
+// A pinned stage with a device copy of the same capacity, for per-batch descriptors: one H2D copy per launch.
+class DescArena : public PinnedStage {
+ public:
+  uint8_t *dev = nullptr;
+  int Reserve(size_t bytes) { return Grow(bytes, &dev); }    // Stage without the host pointer (e.g. max_batch at plan creation)
+  template <typename T> int Stage(size_t bytes, T **host) {
+    const int rc = Reserve(bytes);
+    *host = reinterpret_cast<T *>(host_);
+    return rc;
+  }
+  int Upload(size_t bytes, cudaStream_t s);   // async H2D of the first `bytes`, then Record(s)
+  void Free();
+};
+
+// A grow-only device buffer of `cap` elements: when `need` exceeds it, it is replaced (contents not kept) by one of need + need / 4,
+// at least 4096, elements.  cudaFree waits for the device, so launches still reading the old buffer finish first.
+template <typename T>
+int GrowDevice(T *&ptr, size_t &cap, size_t need) {
+  if (need <= cap) return DALIB200_SUCCESS;
+  const size_t ncap = std::max(need + need / 4, (size_t)4096);
+  if (ptr) cudaFree(ptr);
+  ptr = nullptr; cap = 0;
+  DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&ptr), ncap * sizeof(T)));
+  cap = ncap;
+  return DALIB200_SUCCESS;
+}
+
 // a * b * c < 2^31 for non-negative extents, without overflowing on the way (the kernels index a sample with 32-bit arithmetic)
 inline bool ElementsFit31(int64_t a, int64_t b, int64_t c) {
   const int64_t lim = (int64_t{1} << 31) - 1;
@@ -222,6 +264,8 @@ inline bool ElementsFit31(int64_t a, int64_t b, int64_t c) {
   return a * b <= lim / c;
 }
 }  // namespace dalib200
+// The C-ABI never lets a C++ exception escape (std::bad_alloc / std::length_error from a host-side table of absurd size would otherwise
+// terminate the caller's process): every entry point is a function-try-block closed by this handler.
 #define DB_API_CATCH                                                                                                       \
   catch (const std::bad_alloc &) { ::dalib200::SetLastError("out of host memory"); return DALIB200_ERROR_INTERNAL; }      \
   catch (const std::exception &e__) { ::dalib200::SetLastError("unexpected C++ exception: %s", e__.what()); return DALIB200_ERROR_INTERNAL; } \

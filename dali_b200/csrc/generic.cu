@@ -154,8 +154,6 @@ struct dalib200GenericPlan {
   int pad_elem = 1; uint32_t pad_fill = 0;
   int64_t total_items = 0;
   DescArena arena;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 extern "C" {
@@ -164,16 +162,12 @@ int dalib200GenericPlanCreate(dalib200GenericPlan **plan, int max_batch) try {
   DB_CHECK_ARG(plan && max_batch > 0, "GenericPlanCreate: bad arguments");
   auto *p = new dalib200GenericPlan();
   p->max_batch = max_batch;
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("GenericPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200GenericPlanDestroy(dalib200GenericPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -258,14 +252,11 @@ int dalib200PadSetup(dalib200GenericPlan *p, int n, int ndim, int elem_size, con
 } DB_API_CATCH
 
 static int PadLaunch(dalib200GenericPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) {
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->arena.Reserve(sizeof(PadDesc) * p->n);
+  PadDesc *h;
+  int rc = p->arena.Stage(sizeof(PadDesc) * p->n, &h);
   if (rc) return rc;
-  PadDesc *h = reinterpret_cast<PadDesc *>(p->arena.host);
   for (int i = 0; i < p->n; i++) { h[i] = p->pad[i]; h[i].in = static_cast<const uint8_t *>(in_ptrs[i]); h[i].out = static_cast<uint8_t *>(out_ptrs[i]); }
   if ((rc = p->arena.Upload(sizeof(PadDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const PadDesc *d = reinterpret_cast<const PadDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
   ProfScope ps_("pad", stream);
@@ -281,14 +272,11 @@ int dalib200GenericLaunch(dalib200GenericPlan *p, const void *const *in_ptrs, vo
   DB_CHECK_ARG(p && p->kind != 0 && (p->n == 0 || (in_ptrs && out_ptrs)), "GenericLaunch: call a ...Setup function first");
   if (p->n == 0 || p->total_items == 0) return DALIB200_SUCCESS;
   if (p->kind == 3) return PadLaunch(p, in_ptrs, out_ptrs, stream);
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->arena.Reserve(sizeof(GenDesc) * p->n);
+  GenDesc *h;
+  int rc = p->arena.Stage(sizeof(GenDesc) * p->n, &h);
   if (rc) return rc;
-  GenDesc *h = reinterpret_cast<GenDesc *>(p->arena.host);
   for (int i = 0; i < p->n; i++) { h[i] = p->descs[i]; h[i].in = static_cast<const uint8_t *>(in_ptrs[i]); h[i].out = out_ptrs[i]; }
   if ((rc = p->arena.Upload(sizeof(GenDesc) * p->n, stream))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const GenDesc *d = reinterpret_cast<const GenDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
   if (p->kind == 1) {

@@ -1850,25 +1850,22 @@ void BuildDeviceTable(const HostHuff &h, uint32_t *lut, uint16_t *lut16, HuffSlo
 // A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP, BMP / PNM), for samples whose decode is a serial
 // chain per image or needs no JPEG kernel: it runs on a stream of its own, so that its work overlaps the JPEG kernels.  Its order on the
 // caller's stream s:
-//   Begin(s)   after the status clear: fork (s -> stage stream), then wait until the previous upload of the pinned arena is done;
-//   Upload()   the arena, filled by the caller, goes to the device on the stage stream; then the stage's kernels;
+//   Begin(s)   after the status clear: fork (s -> stage stream);
+//   the caller stages the arena and uploads it on the stage stream, then launches the stage's kernels there;
 //   End()      join event, which s waits on in front of the first kernel that reads the stage's result (dc_scan for the progressive
 //              stage, jpeg_post for the others).
 // A stage with no sample in the batch is not touched: no stream is created, no event recorded.
 struct SideStage {
   dalib200::DescArena arena;
   cudaStream_t stream = nullptr;            // created at the first launch that has samples for the stage
-  cudaEvent_t uploaded = nullptr, fork = nullptr, join = nullptr;
-  bool pending = false;                     // `uploaded` is recorded: the H2D copy may still read the arena
+  cudaEvent_t fork = nullptr, join = nullptr;
 
   bool Create() {
-    return cudaEventCreateWithFlags(&uploaded, cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) == cudaSuccess &&
+    return cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) == cudaSuccess &&
            cudaEventCreateWithFlags(&join, cudaEventDisableTiming) == cudaSuccess;
   }
   void Destroy() {
     if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
-    if (uploaded) { cudaEventSynchronize(uploaded); cudaEventDestroy(uploaded); }
     if (fork) cudaEventDestroy(fork);
     if (join) cudaEventDestroy(join);
     arena.Free();
@@ -1877,13 +1874,6 @@ struct SideStage {
     if (!stream) DB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     DB_CUDA(cudaEventRecord(fork, s));
     DB_CUDA(cudaStreamWaitEvent(stream, fork, 0));
-    if (pending) { DB_CUDA(cudaEventSynchronize(uploaded)); pending = false; }
-    return DALIB200_SUCCESS;
-  }
-  int Upload(size_t bytes) {
-    if (int rc = arena.Upload(bytes, stream)) return rc;
-    DB_CUDA(cudaEventRecord(uploaded, stream));
-    pending = true;
     return DALIB200_SUCCESS;
   }
   int End() {
@@ -1927,7 +1917,7 @@ struct dalib200JpegPlan {
   int total_blocks_sync = 0, total_blocks_write = 0;
   int log2_sub = 10;
   // staging (pinned) and device buffers -- grow only
-  uint8_t *h_stage = nullptr; size_t h_stage_cap = 0;
+  dalib200::PinnedStage h_stage;            // descriptors and tables, then the scan bytes (JpegUpload): d_stage's layout
   uint8_t *d_stage = nullptr; size_t d_stage_cap = 0;
   size_t desc_bytes = 0, off_images = 0, off_units = 0, off_tables = 0, off_quants = 0, off_quads = 0, off_items = 0, off_work = 0, off_fused = 0, off_blkimg = 0, off_wblkimg = 0, off_raw = 0;
   uint8_t *d_clean = nullptr; size_t d_clean_cap = 0;
@@ -1944,9 +1934,8 @@ struct dalib200JpegPlan {
   int32_t *d_status = nullptr; size_t d_status_cap = 0;
   uint32_t *d_unit_nblk = nullptr; size_t d_unit_nblk_cap = 0;
   int32_t *h_status = nullptr; size_t h_status_cap = 0;        // pinned copy of d_status (JpegStatusAsync / JpegStatusFetch)
-  cudaEvent_t uploaded = nullptr, img_uploaded = nullptr;
-  uint8_t *h_images = nullptr; size_t h_images_cap = 0;
-  bool pending = false, img_pending = false, staged = false, smem_opted = false;
+  dalib200::PinnedStage h_images;           // this launch's JpegImage and JpegPost descriptors (they carry the output pointers)
+  bool staged = false, smem_opted = false;
   // progressive (SOF2) samples: their entropy stage runs in jpeg_prog.cu, everything behind it is shared
   std::vector<dalib200::ProgImage> prog_images;
   std::vector<dalib200::ProgScan> prog_scans;     // sorted by wave
@@ -1982,17 +1971,6 @@ struct dalib200JpegPlan {
 };
 
 namespace {
-
-template <typename T>
-int GrowDevice(T *&ptr, size_t &cap, size_t need) {
-  if (need <= cap) return DALIB200_SUCCESS;
-  size_t ncap = std::max(need + need / 4, (size_t)4096);
-  if (ptr) cudaFree(ptr);
-  ptr = nullptr; cap = 0;
-  DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&ptr), ncap * sizeof(T)));
-  cap = ncap;
-  return DALIB200_SUCCESS;
-}
 
 inline size_t Align(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -2173,10 +2151,7 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
   DB_CHECK_ARG(plan && max_batch > 0, "JpegPlanCreate: bad arguments");
   auto *p = new dalib200JpegPlan();
   p->max_batch = max_batch;
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&p->img_uploaded, cudaEventDisableTiming) != cudaSuccess ||
-      !p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() ||
-      !p->bitmap.Create()) {
+  if (!p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() || !p->bitmap.Create()) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2185,11 +2160,9 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
 
 int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
-  if (p->img_uploaded) { cudaEventSynchronize(p->img_uploaded); cudaEventDestroy(p->img_uploaded); }
   for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp, &p->bitmap }) st->Destroy();
-  if (p->h_stage) cudaFreeHost(p->h_stage);
-  if (p->h_images) cudaFreeHost(p->h_images);
+  p->h_stage.Free();
+  p->h_images.Free();
   if (p->h_status) cudaFreeHost(p->h_status);
   void *bufs[] = { p->d_stage, p->d_clean, p->d_chunk, p->d_unit_len, p->d_state, p->d_n, p->d_coef, p->d_dc, p->d_planes, p->d_status,
                    p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk, p->d_png_scan,
@@ -2218,10 +2191,12 @@ int dalib200JpegPlanSetPlanesOnly(dalib200JpegPlan *p, const uint8_t *want, uint
   DB_CHECK_ARG(p && p->staged && want && granted, "JpegPlanSetPlanesOnly: call JpegPlanSetupEx first");
   for (int i = 0; i < p->n; i++) { granted[i] = want[i] && p->geo[i].planar_ok; p->planes_only[i] = granted[i]; }
   BuildWorkLists(p);
-  memcpy(p->h_stage + p->off_quads, p->first_quad.data(), sizeof(int64_t) * p->n);
-  memcpy(p->h_stage + p->off_items, p->first_item.data(), sizeof(int64_t) * p->n);
-  memcpy(p->h_stage + p->off_work, p->first_work.data(), sizeof(int64_t) * p->n);
-  memcpy(p->h_stage + p->off_fused, p->first_fused.data(), sizeof(int64_t) * p->n);
+  uint8_t *h;
+  if (int rc = p->h_stage.Stage(p->desc_bytes, &h)) return rc;
+  memcpy(h + p->off_quads, p->first_quad.data(), sizeof(int64_t) * p->n);
+  memcpy(h + p->off_items, p->first_item.data(), sizeof(int64_t) * p->n);
+  memcpy(h + p->off_work, p->first_work.data(), sizeof(int64_t) * p->n);
+  memcpy(h + p->off_fused, p->first_fused.data(), sizeof(int64_t) * p->n);
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
@@ -2523,24 +2498,17 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->off_wblkimg = off; off += Align(sizeof(int32_t) * p->wblock_image.size(), 16);
   p->off_raw = off;
   p->desc_bytes = off;
-  const size_t total = off + raw + 64;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  if (total > p->h_stage_cap) {
-    if (p->h_stage) cudaFreeHost(p->h_stage);
-    p->h_stage = nullptr; p->h_stage_cap = 0;
-    size_t ncap = total + total / 4;
-    DB_CUDA(cudaMallocHost(reinterpret_cast<void **>(&p->h_stage), ncap));
-    p->h_stage_cap = ncap;
-  }
-  memcpy(p->h_stage + p->off_units, p->units.data(), sizeof(JpegUnit) * p->units.size());
-  memcpy(p->h_stage + p->off_tables, p->tables.data(), sizeof(TableSet) * p->tables.size());
-  memcpy(p->h_stage + p->off_quants, p->quants.data(), sizeof(QuantSet) * p->quants.size());
-  memcpy(p->h_stage + p->off_quads, p->first_quad.data(), sizeof(int64_t) * n);
-  memcpy(p->h_stage + p->off_items, p->first_item.data(), sizeof(int64_t) * n);
-  memcpy(p->h_stage + p->off_work, p->first_work.data(), sizeof(int64_t) * n);
-  memcpy(p->h_stage + p->off_fused, p->first_fused.data(), sizeof(int64_t) * n);
-  memcpy(p->h_stage + p->off_blkimg, p->block_image.data(), sizeof(int32_t) * p->block_image.size());
-  memcpy(p->h_stage + p->off_wblkimg, p->wblock_image.data(), sizeof(int32_t) * p->wblock_image.size());
+  uint8_t *h;
+  if (int rc = p->h_stage.Stage(off + raw + 64, &h)) return rc;
+  memcpy(h + p->off_units, p->units.data(), sizeof(JpegUnit) * p->units.size());
+  memcpy(h + p->off_tables, p->tables.data(), sizeof(TableSet) * p->tables.size());
+  memcpy(h + p->off_quants, p->quants.data(), sizeof(QuantSet) * p->quants.size());
+  memcpy(h + p->off_quads, p->first_quad.data(), sizeof(int64_t) * n);
+  memcpy(h + p->off_items, p->first_item.data(), sizeof(int64_t) * n);
+  memcpy(h + p->off_work, p->first_work.data(), sizeof(int64_t) * n);
+  memcpy(h + p->off_fused, p->first_fused.data(), sizeof(int64_t) * n);
+  memcpy(h + p->off_blkimg, p->block_image.data(), sizeof(int32_t) * p->block_image.size());
+  memcpy(h + p->off_wblkimg, p->wblock_image.data(), sizeof(int32_t) * p->wblock_image.size());
   // the scan bytes themselves are staged by JpegUpload, chunk by chunk, so that the H2D copy starts while later samples
   // are still being copied into the pinned buffer
   p->stage_off.resize(n);
@@ -2610,8 +2578,11 @@ int dalib200JpegUpload(dalib200JpegPlan *p, dalib200Stream_t stream) try {
   const size_t total = p->desc_bytes + p->raw_bytes;
   int rc = GrowDevice(p->d_stage, p->d_stage_cap, total + 64);
   if (rc) return rc;
+  uint8_t *h;
+  if ((rc = p->h_stage.Stage(total, &h))) return rc;
   // output pointers are patched at launch: images are uploaded there.  Descriptors and tables go first ...
-  DB_CUDA(cudaMemcpyAsync(p->d_stage + p->off_units, p->h_stage + p->off_units, p->off_raw - p->off_units, cudaMemcpyHostToDevice, stream));
+  DB_CUDA(cudaMemcpyAsync(p->d_stage + p->off_units, h + p->off_units, p->off_raw - p->off_units, cudaMemcpyHostToDevice, stream));
+  if ((rc = p->h_stage.Record(stream))) return rc;
   // Sources the caller declared stable (JpegPlanSetSourceStable) AND that are page-locked go to the device without the host
   // repack: one DMA per sample straight from the caller's buffer (no CPU memcpy, no bounce buffer -- with N ranks on one host
   // the repack of N x 100 MB per batch would otherwise saturate the host's memory system).  The kernels never read the padding
@@ -2643,8 +2614,6 @@ int dalib200JpegUpload(dalib200JpegPlan *p, dalib200Stream_t stream) try {
         const cudaError_t e = cudaMemcpyBatchAsync(dsts.data(), srcs.data(), sizes.data(), (size_t)p->n, &attr, &attr_idx, 1, &fail_idx, stream);
         if (e == cudaSuccess) {
           p->last_upload_direct = 2;
-          DB_CUDA(cudaEventRecord(p->uploaded, stream));
-          p->pending = true;
           return DALIB200_SUCCESS;
         }
         cudaGetLastError();
@@ -2663,8 +2632,6 @@ int dalib200JpegUpload(dalib200JpegPlan *p, dalib200Stream_t stream) try {
         i = j;
       }
       p->last_upload_direct = 1;
-      DB_CUDA(cudaEventRecord(p->uploaded, stream));
-      p->pending = true;
       return DALIB200_SUCCESS;
     }
   }
@@ -2689,7 +2656,7 @@ int dalib200JpegUpload(dalib200JpegPlan *p, dalib200Stream_t stream) try {
     auto work = [&]() {
       for (int i; (i = next.fetch_add(1)) < n;) {
         const size_t len = p->parsed[i].scan_end - p->parsed[i].scan_begin;
-        uint8_t *dstp = p->h_stage + p->off_raw + p->stage_off[i];
+        uint8_t *dstp = h + p->off_raw + p->stage_off[i];
         memcpy(dstp, p->src_ptr[i], len);
         memset(dstp + len, 0, Align(len, 16) - len);
         done[group_of[i]].fetch_add(1, std::memory_order_release);
@@ -2704,13 +2671,12 @@ int dalib200JpegUpload(dalib200JpegPlan *p, dalib200Stream_t stream) try {
       while (done[g].load(std::memory_order_acquire) < group_cnt[g]) std::this_thread::yield();
       const size_t b0 = group_begin[g], b1 = g + 1 < G ? group_begin[g + 1] : p->raw_bytes;
       if (err == cudaSuccess && b1 > b0)
-        err = cudaMemcpyAsync(p->d_stage + p->off_raw + b0, p->h_stage + p->off_raw + b0, b1 - b0, cudaMemcpyHostToDevice, stream);
+        err = cudaMemcpyAsync(p->d_stage + p->off_raw + b0, h + p->off_raw + b0, b1 - b0, cudaMemcpyHostToDevice, stream);
     }
     for (auto &t : th) t.join();
+    if ((rc = p->h_stage.Record(stream))) return rc;      // behind the groups enqueued before a failed copy too
     DB_CUDA(err);
   }
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
@@ -2742,19 +2708,12 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   }
   // image descriptors carry the output pointers: small separate upload from their own pinned buffer (waiting on the event of
   // the big bit-stream copy here would stall the host for the whole H2D transfer)
+  JpegImage *hi;                            // the output pointers of this launch
   {
-    if (p->img_pending) { DB_CUDA(cudaEventSynchronize(p->img_uploaded)); p->img_pending = false; }
     const size_t img_bytes = Align(sizeof(JpegImage) * p->n, 16);
-    const size_t need = img_bytes + sizeof(JpegPost) * p->posts.size();
-    if (need > p->h_images_cap) {
-      if (p->h_images) cudaFreeHost(p->h_images);
-      p->h_images = nullptr; p->h_images_cap = 0;
-      DB_CUDA(cudaMallocHost(reinterpret_cast<void **>(&p->h_images), need * 2));
-      p->h_images_cap = need * 2;
-    }
-    JpegImage *hi = reinterpret_cast<JpegImage *>(p->h_images);
+    if ((rc = p->h_images.Stage(img_bytes + sizeof(JpegPost) * p->posts.size(), &hi))) return rc;
     for (int i = 0; i < p->n; i++) { hi[i] = p->images[i]; hi[i].out = static_cast<uint8_t *>(out_ptrs[i]); }
-    JpegPost *hp = reinterpret_cast<JpegPost *>(p->h_images + img_bytes);
+    JpegPost *hp = reinterpret_cast<JpegPost *>(reinterpret_cast<uint8_t *>(hi) + img_bytes);
     for (size_t k = 0; k < p->posts.size(); k++) {
       const int i = p->post_sample[k];
       hp[k] = p->posts[k];
@@ -2762,11 +2721,11 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
       hp[k].dst = out_ptrs[i];
       hi[i].out = p->d_post + p->post_off[k];              // the decoder writes the window into scratch
     }
-    DB_CUDA(cudaMemcpyAsync(p->d_stage + p->off_images, hi, sizeof(JpegImage) * p->n, cudaMemcpyHostToDevice, stream));
-    if (!p->posts.empty())
-      DB_CUDA(cudaMemcpyAsync(p->d_posts, hp, sizeof(JpegPost) * p->posts.size(), cudaMemcpyHostToDevice, stream));
-    DB_CUDA(cudaEventRecord(p->img_uploaded, stream));
-    p->img_pending = true;
+    cudaError_t e = cudaMemcpyAsync(p->d_stage + p->off_images, hi, sizeof(JpegImage) * p->n, cudaMemcpyHostToDevice, stream);
+    if (e == cudaSuccess && !p->posts.empty())
+      e = cudaMemcpyAsync(p->d_posts, hp, sizeof(JpegPost) * p->posts.size(), cudaMemcpyHostToDevice, stream);
+    if ((rc = p->h_images.Record(stream))) return rc;
+    DB_CUDA(e);
   }
   const auto *d_images = reinterpret_cast<const JpegImage *>(p->d_stage + p->off_images);
   const auto *d_units = reinterpret_cast<const JpegUnit *>(p->d_stage + p->off_units);
@@ -2781,7 +2740,6 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   // (the clean stream is zero-padded behind every unit by the scatter kernel itself: no memset of the 129 MB buffer)
   DB_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(int32_t) * p->n, s));
   DB_CUDA(cudaMemsetAsync(p->d_chain_count, 0, sizeof(uint32_t) * 8, s));
-  const JpegImage *hi = reinterpret_cast<const JpegImage *>(p->h_images);    // the output pointers of this launch
   if (!p->prog_images.empty()) {
     // progressive samples: scans wave by wave into the same coefficient arena, DC left as differences for dc_scan (jpeg_prog.cu).
     // A scan is a serial chain on ONE warp (milliseconds for a large image) that leaves the GPU empty: the stage runs beside the
@@ -2792,12 +2750,13 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     const size_t npi = p->prog_images.size(), nsc = p->prog_scans.size(), nh = p->prog_huff.size();
     const size_t o_img = 0, o_scan = Align(o_img + sizeof(ProgImage) * npi, 16), o_huff = Align(o_scan + sizeof(ProgScan) * nsc, 16),
                  o_blk = Align(o_huff + sizeof(ProgHuff) * nh, 16), pbytes = Align(o_blk + sizeof(int64_t) * npi, 16);
-    if ((rc = st.arena.Reserve(pbytes))) return rc;
-    memcpy(st.arena.host + o_img, p->prog_images.data(), sizeof(ProgImage) * npi);
-    memcpy(st.arena.host + o_scan, p->prog_scans.data(), sizeof(ProgScan) * nsc);
-    memcpy(st.arena.host + o_huff, p->prog_huff.data(), sizeof(ProgHuff) * nh);
-    memcpy(st.arena.host + o_blk, p->prog_first_blk.data(), sizeof(int64_t) * npi);
-    if ((rc = st.Upload(pbytes))) return rc;
+    uint8_t *h;
+    if ((rc = st.arena.Stage(pbytes, &h))) return rc;
+    memcpy(h + o_img, p->prog_images.data(), sizeof(ProgImage) * npi);
+    memcpy(h + o_scan, p->prog_scans.data(), sizeof(ProgScan) * nsc);
+    memcpy(h + o_huff, p->prog_huff.data(), sizeof(ProgHuff) * nh);
+    memcpy(h + o_blk, p->prog_first_blk.data(), sizeof(int64_t) * npi);
+    if ((rc = st.arena.Upload(pbytes, st.stream))) return rc;
     ProgLaunch a;
     a.d_images = reinterpret_cast<const ProgImage *>(st.arena.dev + o_img); a.nimages = (int)npi;
     a.d_scans = reinterpret_cast<const ProgScan *>(st.arena.dev + o_scan);
@@ -2817,10 +2776,11 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     const int64_t px = FillWindows(p->png_images, hi);
     const size_t npi = p->png_images.size(), nch = p->png_chunks.size();
     const size_t o_chunk = Align(sizeof(PngImage) * npi, 16), pbytes = Align(o_chunk + sizeof(PngChunk) * nch, 16);
-    if ((rc = st.arena.Reserve(pbytes))) return rc;
-    memcpy(st.arena.host, p->png_images.data(), sizeof(PngImage) * npi);
-    memcpy(st.arena.host + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
-    if ((rc = st.Upload(pbytes))) return rc;
+    uint8_t *h;
+    if ((rc = st.arena.Stage(pbytes, &h))) return rc;
+    memcpy(h, p->png_images.data(), sizeof(PngImage) * npi);
+    memcpy(h + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
+    if ((rc = st.arena.Upload(pbytes, st.stream))) return rc;
     PngLaunch a;
     a.d_images = reinterpret_cast<const PngImage *>(st.arena.dev); a.nimages = (int)npi;
     a.d_chunks = reinterpret_cast<const PngChunk *>(st.arena.dev + o_chunk); a.nchunks = (int)nch;
@@ -2839,10 +2799,11 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     const int64_t px = FillWindows(p->tiff_images, hi);
     const size_t nti = p->tiff_images.size();
     const size_t o_seg = Align(sizeof(TiffImage) * nti, 16), tbytes = Align(o_seg + sizeof(TiffSeg) * nseg, 16);
-    if ((rc = st.arena.Reserve(tbytes))) return rc;
-    memcpy(st.arena.host, p->tiff_images.data(), sizeof(TiffImage) * nti);
-    memcpy(st.arena.host + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
-    if ((rc = st.Upload(tbytes))) return rc;
+    uint8_t *h;
+    if ((rc = st.arena.Stage(tbytes, &h))) return rc;
+    memcpy(h, p->tiff_images.data(), sizeof(TiffImage) * nti);
+    memcpy(h + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
+    if ((rc = st.arena.Upload(tbytes, st.stream))) return rc;
     TiffLaunch a;
     a.d_images = reinterpret_cast<const TiffImage *>(st.arena.dev); a.nimages = (int)nti;
     a.d_segs = reinterpret_cast<const TiffSeg *>(st.arena.dev + o_seg); a.nsegs = nseg;
@@ -2858,9 +2819,10 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     if ((rc = st.Begin(s))) return rc;
     const int64_t px = FillWindows(p->webp_images, hi);
     const size_t nwi = p->webp_images.size(), wbytes = Align(sizeof(WebpImage) * nwi, 16);
-    if ((rc = st.arena.Reserve(wbytes))) return rc;
-    memcpy(st.arena.host, p->webp_images.data(), sizeof(WebpImage) * nwi);
-    if ((rc = st.Upload(wbytes))) return rc;
+    uint8_t *h;
+    if ((rc = st.arena.Stage(wbytes, &h))) return rc;
+    memcpy(h, p->webp_images.data(), sizeof(WebpImage) * nwi);
+    if ((rc = st.arena.Upload(wbytes, st.stream))) return rc;
     WebpLaunch a;
     a.d_images = reinterpret_cast<const WebpImage *>(st.arena.dev); a.nimages = (int)nwi;
     a.total_px = px;
@@ -2878,10 +2840,11 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     const int64_t groups = BitmapGroups(p->bitmap_images);
     const size_t nbi = p->bitmap_images.size(), nun = p->bitmap_unpack.size();
     const size_t o_un = Align(sizeof(BitmapImage) * nbi, 16), bbytes = Align(o_un + sizeof(int32_t) * nun, 16);
-    if ((rc = st.arena.Reserve(bbytes))) return rc;
-    memcpy(st.arena.host, p->bitmap_images.data(), sizeof(BitmapImage) * nbi);
-    memcpy(st.arena.host + o_un, p->bitmap_unpack.data(), sizeof(int32_t) * nun);
-    if ((rc = st.Upload(bbytes))) return rc;
+    uint8_t *h;
+    if ((rc = st.arena.Stage(bbytes, &h))) return rc;
+    memcpy(h, p->bitmap_images.data(), sizeof(BitmapImage) * nbi);
+    memcpy(h + o_un, p->bitmap_unpack.data(), sizeof(int32_t) * nun);
+    if ((rc = st.arena.Upload(bbytes, st.stream))) return rc;
     BitmapLaunch a;
     a.d_images = reinterpret_cast<const BitmapImage *>(st.arena.dev); a.nimages = (int)nbi;
     a.d_unpack = reinterpret_cast<const int32_t *>(st.arena.dev + o_un); a.nunpack = (int)nun;

@@ -55,22 +55,9 @@ struct dalib200JpegDistortPlan {
   int16_t *d_dc = nullptr; size_t d_dc_cap = 0;
   uint8_t *d_planes = nullptr; size_t d_planes_cap = 0;
   DescArena arena;                           // [JdImage | JpegImage | QuantSet | five prefixes], one H2D copy per launch
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 namespace {
-
-template <typename T>
-int Grow(T *&ptr, size_t &cap, size_t need) {
-  if (need <= cap) return DALIB200_SUCCESS;
-  const size_t ncap = std::max(need + need / 4, (size_t)4096);
-  if (ptr) cudaFree(ptr);
-  ptr = nullptr; cap = 0;
-  DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&ptr), ncap * sizeof(T)));
-  cap = ncap;
-  return DALIB200_SUCCESS;
-}
 
 inline size_t Align16(size_t v) { return (v + 15) / 16 * 16; }
 
@@ -82,16 +69,12 @@ int dalib200JpegDistortPlanCreate(dalib200JpegDistortPlan **plan, int max_batch)
   DB_CHECK_ARG(plan && max_batch > 0, "JpegDistortPlanCreate: bad arguments");
   auto *p = new dalib200JpegDistortPlan();
   p->max_batch = max_batch;
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("JpegDistortPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200JpegDistortPlanDestroy(dalib200JpegDistortPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   for (void *b : { (void *)p->d_coef, (void *)p->d_dc, (void *)p->d_planes }) if (b) cudaFree(b);
   delete p;
@@ -146,16 +129,14 @@ int dalib200JpegDistortLaunch(dalib200JpegDistortPlan *p, const void *const *in_
   const int n = p->n;
   if (n == 0) return DALIB200_SUCCESS;
   int rc;
-  if ((rc = Grow(p->d_coef, p->d_coef_cap, (size_t)p->total_blocks * 64))) return rc;
-  if ((rc = Grow(p->d_dc, p->d_dc_cap, (size_t)p->total_blocks))) return rc;
-  if (p->plane_bytes > 0 && (rc = Grow(p->d_planes, p->d_planes_cap, (size_t)p->plane_bytes + 64))) return rc;
+  if ((rc = GrowDevice(p->d_coef, p->d_coef_cap, (size_t)p->total_blocks * 64))) return rc;
+  if ((rc = GrowDevice(p->d_dc, p->d_dc_cap, (size_t)p->total_blocks))) return rc;
+  if (p->plane_bytes > 0 && (rc = GrowDevice(p->d_planes, p->d_planes_cap, (size_t)p->plane_bytes + 64))) return rc;
   const size_t nq = p->quants.size();
   const size_t o_img = Align16(sizeof(JdImage) * n), o_q = o_img + Align16(sizeof(JpegImage) * n), o_pre = o_q + sizeof(QuantSet) * nq;
   const size_t pre = Align16(sizeof(int64_t) * n), bytes = o_pre + 5 * pre;
-  // the previous batch's descriptors may still be on their way to the device from the pinned buffer
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  if ((rc = p->arena.Reserve(bytes))) return rc;
-  uint8_t *h = p->arena.host;
+  uint8_t *h;
+  if ((rc = p->arena.Stage(bytes, &h))) return rc;
   JdImage *hj = reinterpret_cast<JdImage *>(h);
   JpegImage *hi = reinterpret_cast<JpegImage *>(h + o_img);
   for (int i = 0; i < n; i++) {
@@ -167,8 +148,6 @@ int dalib200JpegDistortLaunch(dalib200JpegDistortPlan *p, const void *const *in_
   for (int k = 0; k < 5; k++) memcpy(h + o_pre + k * pre, pres[k]->data(), sizeof(int64_t) * n);
   cudaStream_t s = stream;
   if ((rc = p->arena.Upload(bytes, s))) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, s));
-  p->pending = true;
   const uint8_t *dv = p->arena.dev;
   const auto *d_quants = reinterpret_cast<const QuantSet *>(dv + o_q);
   {

@@ -223,8 +223,6 @@ struct dalib200PointwisePlan {
   int mode = PW_LINEAR, out_dtype = DALIB200_UINT8, in_type = 0, out_type = 0;
   int64_t total_quads = 0;
   DescArena arena;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 namespace {
@@ -295,16 +293,12 @@ int dalib200PointwisePlanCreate(dalib200PointwisePlan **plan, int max_batch) try
   p->max_batch = max_batch;
   int rc = p->arena.Reserve(sizeof(PwDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("PointwisePlanCreate: cudaEventCreate failed"); p->arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200PointwisePlanDestroy(dalib200PointwisePlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -313,8 +307,8 @@ int dalib200PointwisePlanDestroy(dalib200PointwisePlan *p) try {
 int dalib200LinearTransformSetup(dalib200PointwisePlan *p, int n, const dalib200ColorSample *samples, int out_dtype) try {
   DB_CHECK_ARG(p && samples && n >= 0 && n <= p->max_batch, "LinearTransformSetup: bad arguments");
   DB_CHECK_ARG(out_dtype == DALIB200_UINT8 || out_dtype == DALIB200_FLOAT, "Hsv/ColorTwist: output type %d not supported", out_dtype);
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<PwDesc *>(p->arena.host);
+  PwDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(PwDesc) * n, &descs)) return rc;
   int64_t quads = 0;
   for (int i = 0; i < n; i++) {
     DB_CHECK_ARG(samples[i].num_pixels >= 0, "Hsv/ColorTwist: negative sample size");
@@ -331,8 +325,8 @@ int dalib200LinearTransformSetup(dalib200PointwisePlan *p, int n, const dalib200
 int dalib200ColorSpaceSetup(dalib200PointwisePlan *p, int n, const int64_t *num_pixels, int in_type, int out_type) try {
   DB_CHECK_ARG(p && num_pixels && n >= 0 && n <= p->max_batch, "ColorSpaceSetup: bad arguments");
   DB_CHECK_ARG(in_type >= 0 && in_type <= 3 && out_type >= 0 && out_type <= 3, "ColorSpaceConversion: unknown image type");
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<PwDesc *>(p->arena.host);
+  PwDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(PwDesc) * n, &descs)) return rc;
   int64_t quads = 0;
   for (int i = 0; i < n; i++) {
     PwDesc &d = descs[i];
@@ -348,13 +342,11 @@ int dalib200ColorSpaceSetup(dalib200PointwisePlan *p, int n, const int64_t *num_
 int dalib200PointwiseLaunch(dalib200PointwisePlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && in_ptrs && out_ptrs, "PointwiseLaunch: null argument");
   if (p->n == 0 || p->total_quads == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<PwDesc *>(p->arena.host);
+  PwDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(PwDesc) * p->n, &descs)) return rc;
   for (int i = 0; i < p->n; i++) { descs[i].in = static_cast<const uint8_t *>(in_ptrs[i]); descs[i].out = out_ptrs[i]; }
   int rc = p->arena.Upload(sizeof(PwDesc) * p->n, stream);
   if (rc) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const auto *dd = reinterpret_cast<const PwDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>((p->total_quads + 255) / 256, (int64_t)NumSMs() * 32);
   ProfScope ps_(p->mode == PW_LINEAR ? "linear_transform" : "color_space_conversion", stream);

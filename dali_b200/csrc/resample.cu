@@ -981,10 +981,7 @@ struct dalib200ResamplePlan {
   std::vector<RsItem> items;                   // strips of the samples that qualify for the streaming kernel
   std::vector<uint8_t> stream_ok;              // structural eligibility per sample (alignment is checked at launch)
   std::vector<int> path;                       // per sample: 0 = tile kernel, 1 = streaming kernel (last launch)
-  size_t tables_uploaded_words = 0;
   bool tables_dirty = true;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
   bool smem_opted[13] = { false, false, false, false, false, false, false, false, false, false, false, false, false };
   bool planar_mode = false;                    // strips sized for resample_planar_kernel (set by ...SetupPlanar)
 };
@@ -1158,6 +1155,26 @@ int BuildWalkRecords(std::vector<int32_t> &arena, int idx_off, int coef_off, int
   return off;
 }
 
+// The launch's descriptors, staged in desc_arena by the caller, go to the device, then the tables if they changed since their last
+// upload, then the streaming kernels' work items if `items` is set.
+int UploadLaunchData(dalib200ResamplePlan *p, bool items, cudaStream_t stream) {
+  auto upload = [stream](DescArena &arena, const void *src, size_t bytes) {
+    uint8_t *h;
+    int rc = arena.Stage(bytes, &h);
+    if (rc) return rc;
+    memcpy(h, src, bytes);
+    return arena.Upload(bytes, stream);
+  };
+  int rc = p->desc_arena.Upload(sizeof(RsDesc) * p->n, stream);
+  if (rc) return rc;
+  if (p->tables_dirty) {
+    if ((rc = upload(p->table_arena, p->tables.data(), p->tables.size() * sizeof(int32_t)))) return rc;
+    p->uploaded_tables = p->tables;
+    p->tables_dirty = false;
+  }
+  return items ? upload(p->item_arena, p->items.data(), p->items.size() * sizeof(RsItem)) : DALIB200_SUCCESS;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1168,16 +1185,12 @@ int dalib200ResamplePlanCreate(dalib200ResamplePlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   int rc = p->desc_arena.Reserve(sizeof(RsDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("ResamplePlanCreate: cudaEventCreate failed"); p->desc_arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200ResamplePlanDestroy(dalib200ResamplePlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->desc_arena.Free(); p->table_arena.Free(); p->item_arena.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -1406,10 +1419,9 @@ int dalib200ResamplePlanSetupPlanar(dalib200ResamplePlan *p, int n, const dalib2
 int dalib200ResampleLaunchPlanar(dalib200ResamplePlan *p, const dalib200PlanarImage *srcs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && srcs && out_ptrs, "ResampleLaunchPlanar: null argument");
   if (p->n == 0 || p->items.empty()) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->desc_arena.Reserve(sizeof(RsDesc) * p->n);
+  RsDesc *hd;
+  int rc = p->desc_arena.Stage(sizeof(RsDesc) * p->n, &hd);
   if (rc) return rc;
-  auto *hd = reinterpret_cast<RsDesc *>(p->desc_arena.host);
   int wmax = 1;
   for (int i = 0; i < p->n; i++) {
     hd[i] = p->descs[i];
@@ -1430,26 +1442,7 @@ int dalib200ResampleLaunchPlanar(dalib200ResamplePlan *p, const dalib200PlanarIm
     hd[i].crop_x = s.crop_x; hd[i].crop_y = s.crop_y;
     wmax = std::max(wmax, (int)hd[i].walk_slots);
   }
-  rc = p->desc_arena.Upload(sizeof(RsDesc) * p->n, stream);
-  if (rc) return rc;
-  if (p->tables_dirty) {
-    size_t bytes = p->tables.size() * sizeof(int32_t);
-    rc = p->table_arena.Reserve(bytes);
-    if (rc) return rc;
-    memcpy(p->table_arena.host, p->tables.data(), bytes);
-    rc = p->table_arena.Upload(bytes, stream);
-    if (rc) return rc;
-    p->uploaded_tables = p->tables;
-    p->tables_dirty = false;
-  }
-  const size_t ib = p->items.size() * sizeof(RsItem);
-  rc = p->item_arena.Reserve(ib);
-  if (rc) return rc;
-  memcpy(p->item_arena.host, p->items.data(), ib);
-  rc = p->item_arena.Upload(ib, stream);
-  if (rc) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
+  if ((rc = UploadLaunchData(p, true, stream))) return rc;
   const auto *dd = reinterpret_cast<const RsDesc *>(p->desc_arena.dev);
   const auto *tb = reinterpret_cast<const int32_t *>(p->table_arena.dev);
   const auto *di = reinterpret_cast<const RsItem *>(p->item_arena.dev);
@@ -1475,10 +1468,9 @@ int dalib200ResampleLaunchPlanar(dalib200ResamplePlan *p, const dalib200PlanarIm
 int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && in_ptrs && out_ptrs, "ResampleLaunch: null argument");
   if (p->n == 0 || p->total_tiles == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  int rc = p->desc_arena.Reserve(sizeof(RsDesc) * p->n);
+  RsDesc *hd;
+  int rc = p->desc_arena.Stage(sizeof(RsDesc) * p->n, &hd);
   if (rc) return rc;
-  auto *hd = reinterpret_cast<RsDesc *>(p->desc_arena.host);
   int nstream = 0;
   for (int i = 0; i < p->n; i++) {
     hd[i] = p->descs[i];
@@ -1490,28 +1482,7 @@ int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, 
     p->path[i] = hd[i].use_stream;
     nstream += hd[i].use_stream;
   }
-  rc = p->desc_arena.Upload(sizeof(RsDesc) * p->n, stream);
-  if (rc) return rc;
-  if (p->tables_dirty) {
-    size_t bytes = p->tables.size() * sizeof(int32_t);
-    rc = p->table_arena.Reserve(bytes);
-    if (rc) return rc;
-    memcpy(p->table_arena.host, p->tables.data(), bytes);
-    rc = p->table_arena.Upload(bytes, stream);
-    if (rc) return rc;
-    p->uploaded_tables = p->tables;
-    p->tables_dirty = false;
-  }
-  if (nstream > 0) {
-    const size_t ib = p->items.size() * sizeof(RsItem);
-    rc = p->item_arena.Reserve(ib);
-    if (rc) return rc;
-    memcpy(p->item_arena.host, p->items.data(), ib);
-    rc = p->item_arena.Upload(ib, stream);
-    if (rc) return rc;
-  }
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
+  if ((rc = UploadLaunchData(p, nstream > 0, stream))) return rc;
   const auto *dd = reinterpret_cast<const RsDesc *>(p->desc_arena.dev);
   const auto *tb = reinterpret_cast<const int32_t *>(p->table_arena.dev);
   if (nstream > 0) {

@@ -34,8 +34,6 @@ struct dalib200Resample3DPlan {
   float *tmp = nullptr;            // device temporaries of the whole batch
   size_t tmp_cap = 0;              // floats
   bool tables_dirty = true;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
 };
 
 extern "C" {
@@ -44,16 +42,12 @@ int dalib200Resample3DPlanCreate(dalib200Resample3DPlan **plan, int max_batch) t
   DB_CHECK_ARG(plan && max_batch > 0 && max_batch <= 65535, "Resample3DPlanCreate: bad arguments (1..65535 samples)");
   auto *p = new dalib200Resample3DPlan();
   p->max_batch = max_batch;
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("Resample3DPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200Resample3DPlanDestroy(dalib200Resample3DPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->pass_arena.Free(); p->table_arena.Free();
   if (p->tmp) cudaFree(p->tmp);
   delete p;
@@ -90,18 +84,13 @@ int dalib200Resample3DLaunch(dalib200Resample3DPlan *p, const void *const *in_pt
   DB_CHECK_ARG(p && (p->n == 0 || (in_ptrs && out_ptrs)), "Resample3DLaunch: null argument");
   const int n = p->n;
   if (n == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
   // temporaries: sample i owns [tmp_off, tmp_off + tmp_floats[0] + tmp_floats[1])
   size_t need = 0;
   for (const auto &s : p->samples) need += (size_t)s.tmp_floats[0] + (size_t)s.tmp_floats[1];
-  if (need > p->tmp_cap) {
-    if (p->tmp) { DB_CUDA(cudaFree(p->tmp)); p->tmp = nullptr; p->tmp_cap = 0; }     // cudaFree waits for the launches that still use it
-    DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&p->tmp), need * sizeof(float)));
-    p->tmp_cap = need;
-  }
-  int rc = p->pass_arena.Reserve(sizeof(R3Pass) * 3 * (size_t)n);
+  int rc = GrowDevice(p->tmp, p->tmp_cap, need);
   if (rc) return rc;
-  R3Pass *hp = reinterpret_cast<R3Pass *>(p->pass_arena.host);
+  R3Pass *hp;
+  if ((rc = p->pass_arena.Stage(sizeof(R3Pass) * 3 * (size_t)n, &hp))) return rc;
   size_t tmp_off = 0;
   int64_t stage_max[3] = { 0, 0, 0 };
   for (int i = 0; i < n; i++) {
@@ -121,13 +110,12 @@ int dalib200Resample3DLaunch(dalib200Resample3DPlan *p, const void *const *in_pt
   if ((rc = p->pass_arena.Upload(sizeof(R3Pass) * 3 * (size_t)n, stream))) return rc;
   if (p->tables_dirty) {
     const size_t bytes = p->tables.size() * sizeof(int32_t);
-    if ((rc = p->table_arena.Reserve(std::max<size_t>(bytes, 16)))) return rc;
-    if (bytes) memcpy(p->table_arena.host, p->tables.data(), bytes);
+    int32_t *ht;
+    if ((rc = p->table_arena.Stage(std::max<size_t>(bytes, 16), &ht))) return rc;
+    if (bytes) memcpy(ht, p->tables.data(), bytes);
     if ((rc = p->table_arena.Upload(bytes, stream))) return rc;
     p->tables_dirty = false;
   }
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const R3Pass *dp = reinterpret_cast<const R3Pass *>(p->pass_arena.dev);
   const int32_t *dt = reinterpret_cast<const int32_t *>(p->table_arena.dev);
   for (int k = 0; k < 3; k++) {

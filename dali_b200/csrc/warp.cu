@@ -384,8 +384,6 @@ struct dalib200WarpPlan {
   float border = 0;
   int64_t total_tiles = 0;
   DescArena arena;
-  cudaEvent_t uploaded = nullptr;
-  bool pending = false;
   // band kernel / tensor-map path: the map is cached per (base, stride, shape)
   std::vector<dalib200WarpSample> samples;
   CUtensorMap tmap;
@@ -430,16 +428,12 @@ int dalib200WarpPlanCreate(dalib200WarpPlan **plan, int max_batch) try {
   p->max_batch = max_batch;
   int rc = p->arena.Reserve(sizeof(WarpDesc) * max_batch);
   if (rc) { delete p; return rc; }
-  if (cudaEventCreateWithFlags(&p->uploaded, cudaEventDisableTiming) != cudaSuccess) {
-    SetLastError("WarpPlanCreate: cudaEventCreate failed"); p->arena.Free(); delete p; return DALIB200_ERROR_CUDA;
-  }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200WarpPlanDestroy(dalib200WarpPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  if (p->uploaded) { cudaEventSynchronize(p->uploaded); cudaEventDestroy(p->uploaded); }
   p->arena.Free();
   delete p;
   return DALIB200_SUCCESS;
@@ -451,8 +445,8 @@ int dalib200WarpPlanSetup(dalib200WarpPlan *p, int n, const dalib200WarpSample *
   DB_CHECK_ARG(n <= p->max_batch, "WarpPlanSetup: batch %d exceeds plan capacity %d", n, p->max_batch);
   DB_CHECK_ARG(interp == 0 || interp == 1, "WarpAffine: only NN and LINEAR interpolation are supported (got %d)", interp);
   DB_CHECK_ARG(out_dtype == DALIB200_UINT8 || out_dtype == DALIB200_FLOAT, "WarpAffine: output type %d not supported", out_dtype);
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<WarpDesc *>(p->arena.host);
+  WarpDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(WarpDesc) * n, &descs)) return rc;
   p->samples.assign(samples, samples + n);
   int64_t tiles = 0;
   for (int i = 0; i < n; i++) {
@@ -480,8 +474,8 @@ int dalib200WarpPlanSetup(dalib200WarpPlan *p, int n, const dalib200WarpSample *
 int dalib200WarpLaunch(dalib200WarpPlan *p, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream) try {
   DB_CHECK_ARG(p && in_ptrs && out_ptrs, "WarpLaunch: null argument");
   if (p->n == 0 || p->total_tiles == 0) return DALIB200_SUCCESS;
-  if (p->pending) { DB_CUDA(cudaEventSynchronize(p->uploaded)); p->pending = false; }
-  auto *descs = reinterpret_cast<WarpDesc *>(p->arena.host);
+  WarpDesc *descs;
+  if (int rc = p->arena.Stage(sizeof(WarpDesc) * p->n, &descs)) return rc;
   for (int i = 0; i < p->n; i++) { descs[i].in = static_cast<const uint8_t *>(in_ptrs[i]); descs[i].out = out_ptrs[i]; }
   // ---- band kernel: bilinear u8 -> u8, every sample 3-channel (DALIB200_WARP_GENERIC=1 forces the generic kernel: A/B runs) ...
   bool band = p->interp == 1 && p->out_dtype == DALIB200_UINT8 && !getenv("DALIB200_WARP_GENERIC");
@@ -532,8 +526,6 @@ int dalib200WarpLaunch(dalib200WarpPlan *p, const void *const *in_ptrs, void *co
   }
   int rc = p->arena.Upload(sizeof(WarpDesc) * p->n, stream);
   if (rc) return rc;
-  DB_CUDA(cudaEventRecord(p->uploaded, stream));
-  p->pending = true;
   const auto *dd = reinterpret_cast<const WarpDesc *>(p->arena.dev);
   const bool lin = p->interp == 1, clampb = !p->use_fill, u8 = p->out_dtype == DALIB200_UINT8;
   if (band) {

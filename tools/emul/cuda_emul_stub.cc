@@ -11,7 +11,9 @@
 // record, stream wait, synchronisation and destruction, stream creation, synchronisation and destruction, cudaMemsetAsync, H2D
 // cudaMemcpyAsync and every kernel launch (by its demangled name).  Events and streams are renumbered by first appearance (e0, e1, ...,
 // s0, s1, ...; a destroyed handle's number is not reused), so two runs of one batch give the same text, and
-// tests/test_decoder_stage_order_emul_cpu.py can check the order of the decoder's side stages from it.
+// tests/test_decoder_stage_order_emul_cpu.py can check the order of the decoder's side stages from it.  An H2D copy names its source:
+// p<k> for the k-th cudaMallocHost allocation (counted from 0 in allocation order), "-" for any other host memory; with that,
+// tests/test_pinned_reuse_emul_cpu.py checks that every plan waits for the last copy out of a pinned buffer before it reuses it.
 //   g++ -std=c++17 -O2 -ffp-contract=off -shared -fPIC -I/usr/local/cuda/include tools/emul/cuda_emul_stub.cc -ldl
 #ifndef _GNU_SOURCE
 #define _GNU_SOURCE
@@ -49,6 +51,17 @@ static int g_nevents = 0, g_nstreams = 0;
 static int ev(const void *e) { auto it = g_events.find(e); return it != g_events.end() ? it->second : (g_events[e] = g_nevents++); }
 static int st(const void *s) { auto it = g_streams.find(s); return it != g_streams.end() ? it->second : (g_streams[s] = g_nstreams++); }
 static int forget(std::map<const void *, int> &m, int id, const void *h) { m.erase(h); return id; }   // the allocator may reuse h
+// cudaMallocHost allocations (base -> size, number in allocation order) while they live, to name the source of an H2D copy
+static std::mutex g_pinned_mu;
+static std::map<const void *, std::pair<size_t, int>> g_pinned;
+static int g_npinned = 0;
+static int pinned_of(const void *p) {           // the allocation holding p, or -1
+  std::lock_guard<std::mutex> l(g_pinned_mu);
+  auto it = g_pinned.upper_bound(p);
+  if (it == g_pinned.begin()) return -1;
+  --it;
+  return static_cast<const char *>(p) < static_cast<const char *>(it->first) + it->second.first ? it->second.second : -1;
+}
 #define TRACE(...)                                                                                            \
   do {                                                                                                        \
     if (FILE *f_ = trace_file()) {                                                                            \
@@ -75,8 +88,18 @@ cudaError_t cudaEventSynchronize(void *e) { TRACE("event_sync e%d", ev(e)); retu
 cudaError_t cudaEventRecord(void *e, void *s) { TRACE("record e%d s%d", ev(e), st(s)); return 0; }
 cudaError_t cudaEventQuery(void *) { return 0; }
 cudaError_t cudaHostAlloc(void **p, size_t n, unsigned) { *p = calloc(n ? n : 1, 1); return *p ? 0 : 2; }
-cudaError_t cudaMallocHost(void **p, size_t n) { *p = calloc(n ? n : 1, 1); return *p ? 0 : 2; }
-cudaError_t cudaFreeHost(void *p) { free(p); return 0; }
+cudaError_t cudaMallocHost(void **p, size_t n) {
+  *p = calloc(n ? n : 1, 1);
+  if (!*p) return 2;
+  std::lock_guard<std::mutex> l(g_pinned_mu);
+  g_pinned[*p] = { n, g_npinned++ };
+  return 0;
+}
+cudaError_t cudaFreeHost(void *p) {
+  { std::lock_guard<std::mutex> l(g_pinned_mu); g_pinned.erase(p); }
+  free(p);
+  return 0;
+}
 // fresh "device" memory is filled with a pattern: a kernel that relies on zeroed memory it never cleared shows up
 cudaError_t cudaMalloc(void **p, size_t n) { *p = malloc(n ? n : 1); if (*p) memset(*p, 0xA5, n ? n : 1); return *p ? 0 : 2; }
 cudaError_t cudaFree(void *p) { free(p); return 0; }
@@ -92,7 +115,11 @@ const char *cudaGetErrorString(cudaError_t e) { return e == 9 ? "invalid configu
 cudaError_t cudaStreamSynchronize(void *s) { TRACE("stream_sync s%d", st(s)); return 0; }
 cudaError_t cudaMemsetAsync(void *p, int v, size_t n, void *s) { TRACE("memset s%d %zu", st(s), n); memset(p, v, n); return 0; }
 cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, int kind, void *stream) {
-  if (kind == 1) TRACE("h2d s%d %zu", st(stream), n);          // cudaMemcpyHostToDevice
+  if (kind == 1) {                                              // cudaMemcpyHostToDevice
+    const int h = pinned_of(s);
+    if (h >= 0) TRACE("h2d s%d %zu p%d", st(stream), n, h);
+    else TRACE("h2d s%d %zu -", st(stream), n);
+  }
   memmove(d, s, n);
   return 0;
 }
