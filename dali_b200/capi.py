@@ -28,7 +28,7 @@ EXPORTS = [
     "dalib200ResamplePlanSetupPlanar", "dalib200ResampleLaunchPlanar",
     "dalib200ResamplePlanCreate", "dalib200ResamplePlanDestroy", "dalib200ResamplePlanSetup", "dalib200ResampleLaunch",
     "dalib200ResamplePlanGetOrder",
-    "dalib200ResamplePlanGetPath",
+    "dalib200ResamplePlanGetPath", "dalib200ResamplePlanGetStreamInfo",
     "dalib200Resample3DPlanCreate", "dalib200Resample3DPlanDestroy", "dalib200Resample3DPlanSetup", "dalib200Resample3DLaunch",
     "dalib200Resample3DPlanGetOrder",
     "dalib200CmnPlanCreate", "dalib200CmnPlanDestroy", "dalib200CmnPlanSetup", "dalib200CmnLaunch",
@@ -233,6 +233,14 @@ class Plan:
                 self.handle = C.c_void_p()
         except Exception:
             pass
+
+
+def resample_stream_info(plan, sample):
+    """dalib200ResamplePlanGetStreamInfo: (eligible, walk slots W, most walk steps J of a chunk, work items) of one sample of a
+    Resample plan after set-up."""
+    info = (C.c_int32 * 4)()
+    check(lib().dalib200ResamplePlanGetStreamInfo(plan.handle, int(sample), info))
+    return tuple(info)
 
 
 def np_f32(x, n):

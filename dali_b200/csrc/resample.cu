@@ -1102,6 +1102,18 @@ int BuildHorzFlags(std::vector<int32_t> &arena, int idx_off, int ow, int iw, int
   return off;
 }
 
+// The most steps J of the row walk of one chunk, over the chunks of kStTH output rows of every kStSeg-row work item: the chunking of
+// BuildWalkRecords and of the kernels.
+int MaxChunkSteps(const int32_t *iy, int out_h, int Sy) {
+  int m = 0;
+  for (int o = 0; o < out_h; o += kStSeg)
+    for (int c0 = o, o1 = std::min(o + kStSeg, out_h); c0 < o1; c0 += kStTH) {
+      const int cs = c0 == o ? iy[o] : iy[c0 - 1] + Sy;
+      m = std::max(m, iy[std::min(c0 + kStTH, o1) - 1] + Sy - cs);
+    }
+  return m;
+}
+
 // Walk records of the streaming kernels for one vertical axis: the tables stage A of resample_stream_kernel and resample_planar_kernel
 // walks by.  Chunks of kStTH output rows restart at every kStSeg-row work item, as the kernels' chunks do.  The records of a chunk
 // cover the steps j = 0..J-1 of its row walk: ent[j][s] = (c, RN(-2^23 c)) of the tap that accumulator slot s takes at step j, or exact
@@ -1199,6 +1211,17 @@ int dalib200ResamplePlanDestroy(dalib200ResamplePlan *p) try {
 int dalib200ResamplePlanGetPath(const dalib200ResamplePlan *p, int sample) try {
   if (!p || sample < 0 || sample >= p->n) return -1;
   return p->path[sample];
+} DB_API_CATCH
+
+int dalib200ResamplePlanGetStreamInfo(const dalib200ResamplePlan *p, int sample, int32_t info[4]) try {
+  DB_CHECK_ARG(p && info && sample >= 0 && sample < p->n && sample < static_cast<int>(p->descs.size()),
+               "ResamplePlanGetStreamInfo: bad arguments");
+  const RsDesc &d = p->descs[sample];
+  info[0] = p->stream_ok[sample];
+  info[1] = d.walk_slots;
+  info[2] = d.out_h > 0 && d.out_w > 0 ? MaxChunkSteps(p->tables.data() + d.idx_off[1], d.out_h, d.support[1]) : 0;
+  info[3] = static_cast<int32_t>(std::count_if(p->items.begin(), p->items.end(), [&](const RsItem &it) { return it.sample == sample; }));
+  return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200ResamplePlanGetOrder(const dalib200ResamplePlan *p, int sample) try {
@@ -1365,15 +1388,7 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
           if (t == 1) break;
         }
         const int seg = kStSeg;
-        bool ok = stw > 0;
-        for (int o = 0; o < s.out_h && ok; o += seg) {
-          int o1 = std::min(o + seg, s.out_h);
-          for (int c0 = o; c0 < o1 && ok; c0 += kStTH) {
-            int c1 = std::min(c0 + kStTH, o1);
-            int cs = c0 == o ? iy[o] : iy[c0 - 1] + Sy;
-            ok = iy[c1 - 1] + Sy - cs <= kWalkMax;
-          }
-        }
+        bool ok = stw > 0 && MaxChunkSteps(iy, s.out_h, Sy) <= kWalkMax;
         if (ok) {   // (ix / iy are not used below: the arena may move)
           auto wc = p->walk_cache.find(d.idx_off[1]);
           if (wc != p->walk_cache.end()) {

@@ -209,6 +209,10 @@ int dalib200ResampleLaunchPlanar(dalib200ResamplePlan *plan, const dalib200Plana
 int dalib200ResamplePlanGetOrder(const dalib200ResamplePlan *plan, int sample);
 /* 1 when the sample went through the streaming (TMA ring) kernel in the last launch, 0 = tile kernel, -1 = bad index. */
 int dalib200ResamplePlanGetPath(const dalib200ResamplePlan *plan, int sample);
+/* The streaming kernel's view of a sample after set-up (read-only): info[0] = 1 when the sample is eligible (the 16-byte alignment of its
+ * input is checked at launch), info[1] = accumulator slots W of its row walk (0: no walk), info[2] = the most source rows one chunk of 8
+ * output rows walks (the sample streams only up to 96), info[3] = its work items (column strips x 56-row segments). */
+int dalib200ResamplePlanGetStreamInfo(const dalib200ResamplePlan *plan, int sample, int32_t info[4]);
 
 /* ------------------------------------------------------------------------------------------------
  * Separable resampling of volumes (DHWC), three passes.  Replaces the spatial_ndim = 3 instances of kernels::ResampleGPU /

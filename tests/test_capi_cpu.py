@@ -44,6 +44,12 @@ def test_jpeg_get_info_rejects_garbage():
     assert rc != 0 and b"SOI" in capi.lib().dalib200GetLastError()
 
 
+def test_resample_stream_info_rejects_bad_arguments():
+    info = (C.c_int32 * 4)()
+    assert capi.lib().dalib200ResamplePlanGetStreamInfo(None, 0, info) == 1
+    assert b"GetStreamInfo" in capi.lib().dalib200GetLastError()
+
+
 def test_color_twist_matrix_matches_reference_composition():
     rng = np.random.default_rng(5)
     for _ in range(300):

@@ -22,8 +22,9 @@ def _enc(img, q=90, ss=None):
     return enc.tobytes()
 
 
-def _fused(streams, out_hws, rois=None):
-    """decode (planes only where granted) + planar resample; returns (outputs, granted flags)."""
+def _fused(streams, out_hws, rois=None, filt=(capi.FILTER_LINEAR, 1, 0.0), infos=None):
+    """decode (planes only where granted) + planar resample with `filt` as min and mag filter; returns (outputs, granted flags).  infos: a
+    list that receives dalib200ResamplePlanGetStreamInfo of every sample of the planar plan."""
     import torch
     import gpu_helpers as g
     lib = capi.lib()
@@ -48,7 +49,7 @@ def _fused(streams, out_hws, rois=None):
         shapes.append(tuple(hwc))
     rs = (capi.ResampleSample * n)()
     for i in range(n):
-        g.fill_resample_sample(rs[i], shapes[i], out_hws[i], (capi.FILTER_LINEAR, 1, 0.0), (capi.FILTER_LINEAR, 1, 0.0), None)
+        g.fill_resample_sample(rs[i], shapes[i], out_hws[i], filt, filt, None)
     ok = (C.c_uint8 * n)()
     capi.check(lib.dalib200ResamplePlanSetupPlanar(rp.handle, n, rs, ok))
     granted = (C.c_uint8 * n)()
@@ -60,6 +61,8 @@ def _fused(streams, out_hws, rois=None):
         capi.check(lib.dalib200ResamplePlanSetupPlanar(rp.handle, n, rs, ok))
         for i in range(n):
             rs[i].channels = 3
+    if infos is not None:
+        infos.extend(capi.resample_stream_info(rp, i) for i in range(n))
     dec = [torch.empty(s, dtype=torch.uint8, device="cuda") for s in shapes]
     outs = [torch.zeros((hw[0], hw[1], 3), dtype=torch.uint8, device="cuda") for hw in out_hws]
     capi.check(lib.dalib200JpegUpload(jp.handle, capi.stream_handle()))
