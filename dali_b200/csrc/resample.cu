@@ -16,7 +16,9 @@
 // intermediate held in shared memory, so HBM sees the input once and the output once.
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): in_h*in_w*C*sizeof(In) + out_h*out_w*C*sizeof(Out).
+// The per-axis host setup (filters, pass order, tables) is resample_axis.h, shared with the 3-D resampler.
 #include "common.cuh"
+#include "resample_axis.h"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -24,88 +26,6 @@
 #include <tuple>
 
 namespace dalib200 {
-
-// ---------------------------------------------------------------------------------------------
-// host: filters (resampling_filters.cuh / .cu restated for the host-side table builder)
-struct RFilter {
-  const float *coeffs; int num_coeffs; float anchor; float scale;
-  void rescale(float support) { float old = scale; scale = (num_coeffs - 1) / support; anchor = anchor * old / scale; }
-  int support() const { return (int)ceilf((num_coeffs - 1) / scale); }
-  float operator()(float x) const {
-    if (!(x > -1)) return 0;
-    if (x >= num_coeffs) return 0;
-    int x0 = (int)std::floor(x), x1 = x0 + 1;
-    float d = x - x0;
-    float f0 = x0 < 0.0f ? 0 : coeffs[x0];
-    float f1 = x1 >= num_coeffs ? 0.0f : coeffs[x1];
-    float t = f1 - f0;
-    float m = d * t;
-    return f0 + m;
-  }
-};
-
-struct FilterBank {
-  float tri[3], gauss[65], lanczos[193], cubic[129];
-  RFilter base[4];
-  FilterBank() {
-    tri[0] = 0; tri[1] = 1; tri[2] = 0;
-    for (int i = 0; i < 65; i++) { float x = 4 * (i - 64 * 0.5f) / 64; gauss[i] = expf(-x * x); }
-    auto sinc = [](float x) { x = (float)(x * M_PI); if (std::fabs(x) < 1e-5f) return 1.0f - x * x * (1.0f / 6); return sinf(x) / x; };
-    for (int i = 0; i < 193; i++) {
-      float x = 2 * 3.0f * (i - 192 * 0.5f) / 192;
-      lanczos[i] = std::fabs(x) >= 3.0f ? 0.0f : sinc(x) * sinc(x / 3.0f);
-    }
-    for (int i = 0; i < 129; i++) {
-      float x = std::fabs(4 * (i - 128 * 0.5f) / 128), v;
-      if (x >= 2) v = 0;
-      else { float x2 = x * x, x3 = x2 * x; v = x > 1 ? -0.5f * x3 + 2.5f * x2 - 4.0f * x + 2.0f : 1.5f * x3 - 2.5f * x2 + 1.0f; }
-      cubic[i] = v;
-    }
-    base[0] = { tri, 3, 1, 1.0f };
-    base[1] = { gauss, 65, 1, 32.0f };
-    base[2] = { lanczos, 193, 1, 96.0f };
-    base[3] = { cubic, 129, 1, 64.0f };
-    base[2].rescale(6);
-    base[3].rescale(4);
-  }
-  RFilter get(int type, float radius) const {
-    RFilter f;
-    switch (type) {
-      case DALIB200_FILTER_LINEAR:     f = base[0]; f.rescale(std::max(1.0f, 2 * 1.0f)); return f;
-      case DALIB200_FILTER_TRIANGULAR: f = base[0]; f.rescale(std::max(1.0f, 2 * radius)); return f;
-      case DALIB200_FILTER_GAUSSIAN: { float sigma = (float)(radius * 0.5f / M_SQRT2);
-                                       f = base[1]; f.rescale(std::max(1.0f, static_cast<float>(4 * M_SQRT2) * sigma)); return f; }
-      case DALIB200_FILTER_CUBIC:      f = base[3]; f.rescale(2.0f * std::max(2.0f, radius)); return f;
-      case DALIB200_FILTER_LANCZOS3:   f = base[2]; f.rescale(2.0f * std::max(3.0f, radius)); return f;
-      default:                         f = { nullptr, 0, 0, 1 }; return f;
-    }
-  }
-};
-static const FilterBank &Filters() { static FilterBank fb; return fb; }
-
-static float DefaultRadius(int type, bool antialias, float in_size, float out_size) {
-  antialias = antialias && in_size > out_size;
-  switch (type) {
-    case DALIB200_FILTER_TRIANGULAR: return antialias ? in_size / out_size : 1;
-    case DALIB200_FILTER_GAUSSIAN:   return antialias ? in_size / out_size : 1;
-    case DALIB200_FILTER_CUBIC:      return antialias ? (2 * in_size / out_size) : 2;
-    case DALIB200_FILTER_LANCZOS3:   return antialias ? (3 * in_size / out_size) : 3;
-    default: return 1;
-  }
-}
-
-// One axis of one sample after setup.  Axis 0 = x (width), 1 = y (height) -- the reference's vec order.
-struct AxisSetup {
-  int in_size, out_size;
-  int ftype;
-  RFilter filter;
-  float origin, scale;       // origin already shifted by roi_lo when the axis is cropped
-  int roi_lo, roi_hi;
-  int base, extent;          // absolute source index = base + clamp(idx, 0, extent-1)
-  int support;               // >= 1 (NN -> 1)
-};
-
-struct AxisTableRef { int idx_off, coef_off, support; };
 
 constexpr int kTmpFloats = 24 * 1024;     // 96 KB of fp32 intermediate per CTA -> 2 CTAs / SM
 constexpr int kMaxTileH = 16;             // output rows per tile in the vertical-first order
@@ -988,120 +908,6 @@ struct dalib200ResamplePlan {
 
 namespace {
 
-// resampling_setup.cc:47-122 for one axis (dim: 0 = y params index, axis = 1 - dim)
-int SetupAxis(AxisSetup &a, int in_size, int out_size, bool use_roi, float roi_start, float roi_end,
-              dalib200FilterDesc minf, dalib200FilterDesc magf) {
-  a.in_size = in_size; a.out_size = out_size;
-  float fin = use_roi ? std::abs(roi_end - roi_start) : (float)in_size;
-  dalib200FilterDesc fd = out_size < fin ? minf : magf;
-  if (fd.antialias && fd.type == DALIB200_FILTER_LINEAR) fd.type = DALIB200_FILTER_TRIANGULAR;
-  else if (!fd.antialias && fd.type == DALIB200_FILTER_TRIANGULAR) fd.type = DALIB200_FILTER_LINEAR;
-  if (fd.radius == 0) fd.radius = DefaultRadius(fd.type, fd.antialias != 0, fin, (float)out_size);
-  a.ftype = fd.type;
-  a.filter = Filters().get(fd.type, fd.radius);
-  float rs = use_roi ? roi_start : 0, re = use_roi ? roi_end : (float)in_size;
-  a.origin = rs;
-  a.scale = (re - rs) / out_size;
-  int support = a.filter.num_coeffs ? a.filter.support() : 1;
-  if (support > 8192) a.filter.rescale(8192);
-  float lo, hi;
-  if (rs <= re) { lo = rs - a.filter.anchor; hi = re - a.filter.anchor + support; }
-  else          { lo = re - a.filter.anchor; hi = rs - a.filter.anchor + support; }
-  a.roi_lo = std::max<int>(0, std::min<int>(in_size, (int)std::floor(lo)));
-  a.roi_hi = std::max<int>(0, std::min<int>(in_size, (int)std::ceil(hi)));
-  a.support = std::max(1, a.filter.num_coeffs ? a.filter.support() : 1);
-  return 0;
-}
-
-// resampling_setup.cc:131-192 (2-D): returns the first-pass axis (0 = x / horizontal first)
-int ProcessingOrder(const AxisSetup ax[2]) {
-  float best = 1e+30f; int best_first = 0;
-  for (int first = 0; first < 2; first++) {
-    int64_t sz[2] = { ax[0].roi_hi - ax[0].roi_lo, ax[1].roi_hi - ax[1].roi_lo };
-    int axes[2] = { first, 1 - first };
-    float total = 0; bool ok = true;
-    for (int p = 0; p < 2; p++) {
-      if (total >= best) { ok = false; break; }
-      int a = axes[p];
-      sz[a] = ax[a].out_size;
-      int64_t vol = sz[0] * sz[1];
-      float mul = a == 0 ? 1.4f : 1.0f;
-      float base = (float)(ax[a].support * vol);
-      total += mul * base + vol * 3.0f;
-    }
-    if (ok && !(total >= best)) { best = total; best_first = first; }
-  }
-  return best_first;
-}
-
-// Coefficient / index table of one axis.  FIR: resampling_impl_cpu.cc:22-47.  NN (1 tap, weight 1):
-// resampling_impl_cpu.h:522-606 -- note the y coordinate is accumulated incrementally there.
-void BuildTable(std::vector<int32_t> &arena, AxisTableRef &ref, const AxisSetup &a, int axis) {
-  const int n = a.out_size, S = a.support;
-  ref.support = S;
-  ref.idx_off = (int)arena.size();
-  arena.resize(arena.size() + n);
-  ref.coef_off = (int)arena.size();
-  arena.resize(arena.size() + (size_t)n * S);
-  int32_t *idx = arena.data() + ref.idx_off;
-  float *coef = reinterpret_cast<float *>(arena.data() + ref.coef_off);
-  if (a.ftype == DALIB200_FILTER_NN) {
-    if (axis == 1) {
-      float sy = a.origin + 0.5f * a.scale;
-      for (int y = 0; y < n; y++, sy += a.scale) { idx[y] = (int)std::floor(sy); coef[y] = 1.0f; }
-    } else if (a.scale == 1) {
-      int sx0 = (int)std::floor(a.origin + 0.5f);
-      for (int x = 0; x < n; x++) { idx[x] = sx0 + x; coef[x] = 1.0f; }
-    } else {
-      for (int x = 0; x < n; x++) { idx[x] = (int)std::floor(a.origin + (x + 0.5f) * a.scale); coef[x] = 1.0f; }
-    }
-    return;
-  }
-  const RFilter &f = a.filter;
-  float s0 = a.origin;
-  s0 += 0.5f * a.scale - 0.5f - f.anchor;
-  for (int x = 0; x < n; x++) {
-    float sx0f = x * a.scale + s0;
-    int sx0 = (int)ceilf(sx0f);
-    idx[x] = sx0;
-    const float f0 = sx0 - sx0f;
-    float sum = 0;
-    for (int k = 0; k < S; k++) {
-      float c = f((f0 + k) * f.scale);
-      coef[(size_t)S * x + k] = c;
-      sum += c;
-    }
-    if (sum) for (int k = 0; k < S; k++) coef[(size_t)S * x + k] /= sum;
-  }
-}
-
-// Which output columns does the reference's horizontal pass compute in its 16-lane SSE path?
-// (resampling_impl_cpu.h:126-222,225-336) -- those round half-to-even when storing u8.
-int BuildHorzFlags(std::vector<int32_t> &arena, int idx_off, int ow, int iw, int support) {
-  int off = (int)arena.size();
-  arena.resize(arena.size() + (ow + 3) / 4);
-  const int32_t *idx = arena.data() + idx_off;      // after the resize: the arena may have moved
-  uint8_t *fl = reinterpret_cast<uint8_t *>(arena.data() + off);
-  memset(fl, 0, (size_t)((ow + 3) / 4) * 4);
-  bool flipped = idx[ow - 1] < idx[0];
-  int first = 0, last = ow - 1;
-  if (flipped) {
-    while (first < ow && idx[first] + support > iw) first++;
-    while (last >= 0 && idx[last] < 0) last--;
-  } else {
-    while (first < ow && idx[first] < 0) first++;
-    while (last >= 0 && idx[last] + support > iw) last--;
-  }
-  int bounds[4] = { std::min(first, last + 1), first, last + 1, ow };
-  int x = 0;
-  for (int r = 0; r < 4; r++) {
-    int ox1 = bounds[r];
-    for (; x + 16 <= ox1; x += 16) memset(fl + x, 1, 16);
-    for (; x < ox1; x++) fl[x] = 0;
-  }
-  return off;
-}
-
 // The most steps J of the row walk of one chunk, over the chunks of kStTH output rows of every kStSeg-row work item: the chunking of
 // BuildWalkRecords and of the kernels.
 int MaxChunkSteps(const int32_t *iy, int out_h, int Sy) {
@@ -1135,7 +941,7 @@ int BuildWalkRecords(std::vector<int32_t> &arena, int idx_off, int coef_off, int
       const int J = chunk_steps(o, c0, std::min(c0 + kStTH, o1), cs);
       words += 3 + static_cast<int64_t>(J) * kWalkSlots * 2 + ((J + 3) & ~3);
     }
-  if (words >= (int64_t{1} << 26)) return -1;
+  if (words >= kMaxTableWords) return -1;
   const int off = static_cast<int>(arena.size());
   arena.resize(arena.size() + nchunks);
   for (int o = 0; o < out_h; o += kStSeg) {
@@ -1253,11 +1059,8 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
                  "Resize: sample %d: images of 2^31 elements or more are not supported", i);
     for (int a = 0; a < 2; a++) {
       for (const dalib200FilterDesc *f : { &s.min_filter[a], &s.mag_filter[a] })
-        DB_CHECK_ARG(f->type >= DALIB200_FILTER_NN && f->type <= DALIB200_FILTER_LANCZOS3 && f->radius >= 0 && f->radius <= 1e6f,
-                     "Resize: sample %d: invalid filter (type %d, radius %g)", i, f->type, static_cast<double>(f->radius));
-      DB_CHECK_ARG(!s.use_roi[a] || (std::isfinite(s.roi_start[a]) && std::isfinite(s.roi_end[a]) && std::fabs(s.roi_start[a]) <= 1e9f &&
-                                     std::fabs(s.roi_end[a]) <= 1e9f),
-                   "Resize: sample %d: the region of interest must be finite", i);
+        DB_CHECK_ARG(FilterDescValid(*f), "Resize: sample %d: invalid filter (type %d, radius %g)", i, f->type, static_cast<double>(f->radius));
+      DB_CHECK_ARG(!s.use_roi[a] || RoiFinite(s.roi_start[a], s.roi_end[a]), "Resize: sample %d: the region of interest must be finite", i);
     }
     RsDesc &d = p->descs[i];
     memset(&d, 0, sizeof(d));
@@ -1270,26 +1073,21 @@ int dalib200ResamplePlanSetup(dalib200ResamplePlan *p, int n, const dalib200Resa
     // axis 0 = x <- params index 1 ; axis 1 = y <- params index 0
     SetupAxis(ax[0], s.in_w, s.out_w, s.use_roi[1] != 0, s.roi_start[1], s.roi_end[1], s.min_filter[1], s.mag_filter[1]);
     SetupAxis(ax[1], s.in_h, s.out_h, s.use_roi[0] != 0, s.roi_start[0], s.roi_end[0], s.min_filter[0], s.mag_filter[0]);
-    const int first = ProcessingOrder(ax);
+    int order[2];
+    ProcessingOrder(ax, 2, order);
+    const int first = order[0];
     p->order0[i] = first;
     d.vfirst = first == 1;
     for (int a = 0; a < 2; a++) {
-      if (a != first) {          // cropped to the filter footprint, origin moved (setup.cc:323-336)
-        ax[a].origin -= ax[a].roi_lo;
-        ax[a].base = ax[a].roi_lo; ax[a].extent = ax[a].roi_hi - ax[a].roi_lo;
-      } else {
-        ax[a].base = 0; ax[a].extent = ax[a].in_size;
-      }
+      CropAxis(ax[a], a == first);
       DB_CHECK_ARG(ax[a].extent > 0, "Resize: sample %d has an empty region of interest", i);
       TableKey key{ ax[a].in_size, ax[a].out_size, ax[a].ftype * 2 + a, ax[a].base, ax[a].extent, fbits(ax[a].origin),
                     fbits(ax[a].scale), fbits(ax[a].filter.scale), fbits(ax[a].filter.anchor) };
       auto it = p->cache.find(key);
       AxisTableRef ref;
       if (it == p->cache.end()) {
-        // index + coefficient tables are addressed with 32-bit offsets and live in one host / device arena: refuse absurd requests
-        // (e.g. a 2^31-wide source minified with antialiasing = millions of taps per output) instead of exhausting memory
         DB_CHECK_ARG(static_cast<int64_t>(ax[a].out_size) * (static_cast<int64_t>(ax[a].support) + 1) + static_cast<int64_t>(p->tables.size()) <
-                         (int64_t{1} << 26),
+                         kMaxTableWords,
                      "Resize: sample %d needs %lld filter taps per output along axis %d (%d -> %d): the filter tables would exceed 256 MB", i,
                      static_cast<long long>(ax[a].support), a, ax[a].in_size, ax[a].out_size);
         BuildTable(p->tables, ref, ax[a], a);
@@ -1543,41 +1341,3 @@ int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, 
 } DB_API_CATCH
 
 }  // extern "C"
-
-// ---------------------------------------------------------------------------------------------
-// The per-axis host setup exported to the 3-D planner (resample_axis.h).  Appended at the end of the file so that the line tables of
-// the kernels above do not move.
-#include "resample_axis.h"
-namespace dalib200 {
-
-int AxisSetupShared(AxisShared *s, int in_size, int out_size, bool use_roi, float roi_start, float roi_end,
-                    dalib200FilterDesc min_filter, dalib200FilterDesc mag_filter) {
-  AxisSetup a;
-  int rc = SetupAxis(a, in_size, out_size, use_roi, roi_start, roi_end, min_filter, mag_filter);
-  if (rc) return rc;
-  s->in_size = a.in_size; s->out_size = a.out_size; s->ftype = a.ftype; s->support = a.support;
-  s->roi_lo = a.roi_lo; s->roi_hi = a.roi_hi; s->origin = a.origin; s->scale = a.scale;
-  s->coeffs = a.filter.coeffs; s->num_coeffs = a.filter.num_coeffs; s->anchor = a.filter.anchor; s->fscale = a.filter.scale;
-  return 0;
-}
-
-void AxisFirTableShared(const AxisShared *s, float origin, int32_t *idx, float *coef) {
-  AxisSetup a;
-  a.in_size = s->in_size; a.out_size = s->out_size; a.ftype = s->ftype; a.support = s->support;
-  a.roi_lo = s->roi_lo; a.roi_hi = s->roi_hi; a.origin = origin; a.scale = s->scale;
-  a.filter = { s->coeffs, s->num_coeffs, s->anchor, s->fscale };
-  a.base = 0; a.extent = s->in_size;
-  std::vector<int32_t> arena;
-  AxisTableRef ref;
-  BuildTable(arena, ref, a, 0);
-  memcpy(idx, arena.data() + ref.idx_off, sizeof(int32_t) * (size_t)s->out_size);
-  memcpy(coef, arena.data() + ref.coef_off, sizeof(float) * (size_t)s->out_size * s->support);
-}
-
-void HorzSimdFlagsShared(const int32_t *idx, int ow, int iw, int support, uint8_t *flags) {
-  std::vector<int32_t> arena(idx, idx + ow);
-  int off = BuildHorzFlags(arena, 0, ow, iw, support);
-  memcpy(flags, reinterpret_cast<const uint8_t *>(arena.data() + off), (size_t)ow);
-}
-
-}  // namespace dalib200

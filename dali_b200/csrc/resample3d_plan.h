@@ -3,12 +3,11 @@
 // produces; tools/emul/resample3d_emul.cc runs the same plan through resample3d_core.h on the host.
 //
 // Restates SeparableResamplingSetup<3>::SetupSample (dali/kernels/imgproc/resample/resampling_setup.cc:271-337): filters and ROI per
-// axis (:47-122, shared with the 2-D plan through resample_axis.h), pass order by the reference's cost search (:131-192), temporaries
-// (:296-307), input cropped to the filter footprint along the non-first axes (:323-336); the passes follow SeparableResampleCPU<.., 3>
-// (separable_cpu.h:149-249), the parity target.
+// axis (:47-122), pass order by the reference's cost search (:131-192), temporaries (:296-307), input cropped to the filter footprint
+// along the non-first axes (:323-336); the passes follow SeparableResampleCPU<.., 3> (separable_cpu.h:149-249), the parity target.
+// The per-axis steps (filters, ROI, pass order, crop, tables) are the 2-D plan's, from resample_axis.h.
 #ifndef DALI_B200_CSRC_RESAMPLE3D_PLAN_H_
 #define DALI_B200_CSRC_RESAMPLE3D_PLAN_H_
-#include <cmath>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -36,30 +35,6 @@ inline bool Fit31(int64_t a, int64_t b, int64_t c, int64_t d) {
   }
   return true;
 }
-// resampling_setup.cc:131-192 for three axes: depth-first over the orders, axes tried in ascending vec order, a branch is abandoned as
-// soon as it is not cheaper than the best complete order
-inline void ProcessingOrder3(const AxisShared ax[3], int order[3]) {
-  float best = 1e+30f;
-  order[0] = 0; order[1] = 1; order[2] = 2;
-  for (int a0 = 0; a0 < 3; a0++)
-    for (int a1 = 0; a1 < 3; a1++) {
-      if (a1 == a0) continue;
-      const int seq[3] = { a0, a1, 3 - a0 - a1 };
-      int64_t sz[3] = { ax[0].roi_hi - ax[0].roi_lo, ax[1].roi_hi - ax[1].roi_lo, ax[2].roi_hi - ax[2].roi_lo };
-      float total = 0;
-      bool ok = true;
-      for (int p = 0; p < 3; p++) {
-        if (total >= best) { ok = false; break; }
-        const int a = seq[p];
-        sz[a] = ax[a].out_size;
-        const int64_t vol = sz[0] * sz[1] * sz[2];
-        const float mul = a == 0 ? 1.4f : a > 1 ? 1.2f : 1.0f;
-        const float base = static_cast<float>(ax[a].support * vol);
-        total += mul * base + vol * 3.0f;
-      }
-      if (ok && !(total >= best)) { best = total; order[0] = seq[0]; order[1] = seq[1]; order[2] = seq[2]; }
-    }
-}
 inline int ClampIdx(int v, int n) { return v < 0 ? 0 : v > n - 1 ? n - 1 : v; }
 }  // namespace r3detail
 
@@ -77,24 +52,19 @@ inline int PlanResample3D(const dalib200Resample3DSample &s, int in_dtype, int o
     return fail("volumes of 2^31 elements or more are not supported");
   for (int d = 0; d < 3; d++) {
     for (const dalib200FilterDesc *f : { &s.min_filter[d], &s.mag_filter[d] })
-      if (!(f->type >= DALIB200_FILTER_NN && f->type <= DALIB200_FILTER_LANCZOS3 && f->radius >= 0 && f->radius <= 1e6f)) return fail("invalid filter");
-    if (s.use_roi[d] && !(std::isfinite(s.roi_start[d]) && std::isfinite(s.roi_end[d]) && std::fabs(s.roi_start[d]) <= 1e9f && std::fabs(s.roi_end[d]) <= 1e9f))
-      return fail("the region of interest must be finite");
+      if (!FilterDescValid(*f)) return fail("invalid filter");
+    if (s.use_roi[d] && !RoiFinite(s.roi_start[d], s.roi_end[d])) return fail("the region of interest must be finite");
   }
   if (s.out_shape[0] == 0 || s.out_shape[1] == 0 || s.out_shape[2] == 0) return DALIB200_SUCCESS;
-  AxisShared ax[3];
+  AxisSetup ax[3];
   for (int a = 0; a < 3; a++) {          // vec axis a <- shape / params index 2 - a
     const int d = 2 - a;
-    AxisSetupShared(&ax[a], s.in_shape[d], s.out_shape[d], s.use_roi[d] != 0, s.roi_start[d], s.roi_end[d], s.min_filter[d], s.mag_filter[d]);
+    SetupAxis(ax[a], s.in_shape[d], s.out_shape[d], s.use_roi[d] != 0, s.roi_start[d], s.roi_end[d], s.min_filter[d], s.mag_filter[d]);
   }
-  ProcessingOrder3(ax, sp->order);
-  const int first = sp->order[0];
-  float origin[3];
-  int cin[3], off[3];
+  ProcessingOrder(ax, 3, sp->order);
   for (int a = 0; a < 3; a++) {
-    if (a != first) { origin[a] = ax[a].origin - ax[a].roi_lo; off[a] = ax[a].roi_lo; cin[a] = ax[a].roi_hi - ax[a].roi_lo; }
-    else { origin[a] = ax[a].origin; off[a] = 0; cin[a] = ax[a].in_size; }
-    if (cin[a] <= 0) return fail("empty region of interest");
+    CropAxis(ax[a], a == sp->order[0]);
+    if (ax[a].extent <= 0) return fail("empty region of interest");
   }
   const int64_t vstride[3] = { C, (int64_t)s.in_shape[2] * C, (int64_t)s.in_shape[1] * s.in_shape[2] * C };
   const int osz[3] = { s.out_shape[2], s.out_shape[1], s.out_shape[0] };
@@ -102,13 +72,8 @@ inline int PlanResample3D(const dalib200Resample3DSample &s, int in_dtype, int o
     const int o = (int)tables.size();
     tables.resize(tables.size() + n_out);
     int32_t *m = tables.data() + o;
-    if (a == 0) {
-      if (scale == 1) { const int sx0 = (int)std::floor(origin[0] + 0.5f); for (int x = 0; x < n_out; x++) m[x] = ClampIdx(sx0 + x, n_in); }
-      else for (int x = 0; x < n_out; x++) m[x] = ClampIdx((int)std::floor(origin[0] + (x + 0.5f) * scale), n_in);
-    } else {
-      float src = origin[a] + 0.5f * scale;
-      for (int i = 0; i < n_out; i++, src += scale) m[i] = ClampIdx((int)std::floor(src), n_in);
-    }
+    NNIndices(m, n_out, ax[a].origin, scale, a);
+    for (int i = 0; i < n_out; i++) m[i] = ClampIdx(m[i], n_in);
     return o;
   };
   const bool pure_nn = ax[0].ftype == DALIB200_FILTER_NN && ax[1].ftype == DALIB200_FILTER_NN && ax[2].ftype == DALIB200_FILTER_NN;
@@ -118,17 +83,17 @@ inline int PlanResample3D(const dalib200Resample3DSample &s, int in_dtype, int o
     p.total = (int64_t)out_sz[0] * out_sz[1] * out_sz[2] * C;
     p.flags_off = -1; p.simd_end = 0; p.idx_off = p.coef_off = 0; p.support = 1;
   };
+  int cur[3] = { ax[0].extent, ax[1].extent, ax[2].extent };
   if (pure_nn) {
     R3Pass &p = sp->pass[0];
-    common(p, cin, osz);
+    common(p, cur, osz);
     p.axis = -1;
     p.in_u8 = in_dtype == DALIB200_UINT8; p.out_u8 = out_dtype == DALIB200_UINT8;
-    for (int a = 0; a < 3; a++) { p.in_stride[a] = vstride[a]; p.in_offset += off[a] * vstride[a]; }
-    for (int a = 0; a < 3; a++) p.map_off[a] = nn_map(a, ax[a].scale, osz[a], cin[a]);
+    for (int a = 0; a < 3; a++) { p.in_stride[a] = vstride[a]; p.in_offset += ax[a].base * vstride[a]; }
+    for (int a = 0; a < 3; a++) p.map_off[a] = nn_map(a, ax[a].scale, osz[a], cur[a]);
     sp->npass = 1;
     return DALIB200_SUCCESS;
   }
-  int cur[3] = { cin[0], cin[1], cin[2] };
   for (int stage = 0; stage < 3; stage++) {
     const int a = sp->order[stage];
     int nxt[3] = { cur[0], cur[1], cur[2] };
@@ -138,7 +103,7 @@ inline int PlanResample3D(const dalib200Resample3DSample &s, int in_dtype, int o
     common(p, cur, nxt);
     p.in_u8 = stage == 0 && in_dtype == DALIB200_UINT8;
     p.out_u8 = stage == 2 && out_dtype == DALIB200_UINT8;
-    if (stage == 0) { for (int b = 0; b < 3; b++) { p.in_stride[b] = vstride[b]; p.in_offset += off[b] * vstride[b]; } }
+    if (stage == 0) { for (int b = 0; b < 3; b++) { p.in_stride[b] = vstride[b]; p.in_offset += ax[b].base * vstride[b]; } }
     else { p.in_stride[0] = C; p.in_stride[1] = (int64_t)cur[0] * C; p.in_stride[2] = (int64_t)cur[0] * cur[1] * C; }
     if (stage < 2) sp->tmp_floats[stage] = p.total;
     if (ax[a].ftype == DALIB200_FILTER_NN) {       // separable_cpu.h:219-227: ResampleNN with the other scales forced to 1
@@ -147,18 +112,13 @@ inline int PlanResample3D(const dalib200Resample3DSample &s, int in_dtype, int o
     } else {
       p.axis = a;
       const int64_t words = (int64_t)osz[a] * (ax[a].support + 1);
-      if (words + (int64_t)tables.size() >= (int64_t{1} << 26)) return fail("the filter tables would exceed 256 MB");
-      p.support = ax[a].support;
-      p.idx_off = (int)tables.size();
-      tables.resize(tables.size() + osz[a]);
-      p.coef_off = (int)tables.size();
-      tables.resize(tables.size() + (size_t)osz[a] * ax[a].support);
-      AxisFirTableShared(&ax[a], origin[a], tables.data() + p.idx_off, reinterpret_cast<float *>(tables.data() + p.coef_off));
+      if (words + (int64_t)tables.size() >= kMaxTableWords) return fail("the filter tables would exceed 256 MB");
+      AxisTableRef ref;
+      BuildTable(tables, ref, ax[a], a);
+      p.support = ref.support; p.idx_off = ref.idx_off; p.coef_off = ref.coef_off;
       if (p.out_u8) {
         if (a == 0) {
-          p.flags_off = (int)tables.size();
-          tables.resize(tables.size() + (osz[0] + 3) / 4);
-          HorzSimdFlagsShared(tables.data() + p.idx_off, osz[0], cur[0], p.support, reinterpret_cast<uint8_t *>(tables.data() + p.flags_off));
+          p.flags_off = BuildHorzFlags(tables, p.idx_off, osz[0], cur[0], p.support);
         } else {
           // ResampleVert stores rows of X * C (per slice); ResampleDepth fuses x and y of the (contiguous) temporary and output
           const int64_t flat_w = a == 1 ? (int64_t)nxt[0] * C : (int64_t)nxt[0] * nxt[1] * C;

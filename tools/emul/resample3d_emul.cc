@@ -5,7 +5,7 @@
 // (resample3d_plan.h) is plain C++.  This file compiles both with the host compiler and executes every pass element by element on host
 // memory, so that tests/test_resample3d_emul_cpu.py can compare planner + arithmetic with the reference's SeparableResampleCPU<.., 3>
 // bit for bit on a machine without a GPU.  What it cannot cover is the launch itself (descriptor upload, grid shape): that is the
-// `-m gpu` test's job.  Built by the test:  g++ -O2 -ffp-contract=off -shared -fPIC ... -ldali_b200 (AxisSetupShared & co live there).
+// `-m gpu` test's job.  Built by the test:  g++ -O2 -ffp-contract=off -shared -fPIC ...
 #include <cstdlib>
 #include <string>
 #include <vector>
