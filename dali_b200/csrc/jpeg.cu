@@ -26,7 +26,8 @@
 // The plan also takes PNG, TIFF, lossy WebP, BMP and PNM streams (detected by their signatures): png_plan.h, tiff_plan.h, webp_plan.h
 // and bitmap_plan.h read their headers at set-up, png.cu, tiff.cu, webp.cu and bitmap.cu decode them into the same decode windows on
 // streams of their own, and the post pass below serves every format.  Such a sample has no units, subsequences or MCUs, so every kernel
-// of this file skips it.
+// of this file skips it.  A lossless JPEG (SOF3) sample is parsed here and planned by ljpeg_plan.h: its restart intervals join U1 - U3 as
+// units of no JPEG image, and ljpeg.cu decodes their clean streams on a stream forked behind U3.
 #include "common.cuh"
 #include "jpeg_recon.h"
 #include <algorithm>
@@ -77,17 +78,6 @@ struct JpegPost {
   int32_t orientation;                     // EXIF 1..8
   int32_t out_type, dtype;                 // DALIB200_RGB.. / DALIB200_UINT8 | DALIB200_FLOAT
   int64_t first_px;
-};
-
-struct JpegUnit {
-  uint32_t raw_off, raw_len;               // in the staged byte buffer
-  uint32_t clean_off;                      // in the clean buffer (bytes, 16-aligned)
-  uint32_t first_chunk;                    // global chunk index
-  int32_t image;
-  int32_t first_subseq;                    // image-local
-  int32_t nsub_max;
-  int64_t slot_base;                       // first coefficient slot of this unit (image-local)
-  int64_t nslots;                          // expected number of slots (= MCUs * bpm * 64)
 };
 
 __constant__ uint8_t c_zigzag[64] = {
@@ -1213,7 +1203,7 @@ __global__ void __launch_bounds__(256) color_kernel(const JpegImage *__restrict_
       if (im.out_type == DALIB200_RGB) { px[3 * k] = r; px[3 * k + 1] = g; px[3 * k + 2] = b; }
       else if (im.out_type == DALIB200_BGR) { px[3 * k] = b; px[3 * k + 1] = g; px[3 * k + 2] = r; }
       else if (im.out_type == DALIB200_YCbCr) { px[3 * k] = yy; px[3 * k + 1] = cb; px[3 * k + 2] = cr; }
-      else if (cm == kColorRGB) px[k] = (r * 19595 + g * 38470 + b * 7471 + 32768) >> 16;
+      else if (cm == kColorRGB) px[k] = RgbJpegGray(r, g, b);
       else if (cm >= kColorCMYK) px[k] = (b * 1868 + g * 9617 + r * 4899 + 8192) >> 14;      // OpenCV icvCvt_CMYK2Gray
       else px[k] = yy;
     }
@@ -1662,11 +1652,15 @@ struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 // BMP and PNM streams: planner + launch interface of bitmap.cu
 #include "bitmap.h"
 #include "bitmap_plan.h"
+// lossless JPEG (SOF3): planner + launch interface of ljpeg.cu
+#include "ljpeg.h"
+#include "ljpeg_plan.h"
 namespace {
 
 // The formats the plan takes, told apart by their signatures.  PNG, TIFF, WebP and BMP / PNM samples are planned by png_plan.h,
 // tiff_plan.h, webp_plan.h and bitmap_plan.h and decoded by png.cu, tiff.cu, webp.cu and bitmap.cu; everything else is parsed as JPEG.
-enum class Format { kJpeg, kPng, kTiff, kWebp, kBitmap };
+// A JPEG whose frame header is SOF3 becomes kLossless once parsed: ljpeg_plan.h plans it, ljpeg.cu decodes it.
+enum class Format { kJpeg, kPng, kTiff, kWebp, kBitmap, kLossless };
 
 Format DetectFormat(const uint8_t *p, size_t n) {
   return IsPngStream(p, n) ? Format::kPng : IsTiffStream(p, n) ? Format::kTiff : IsWebpStream(p, n) ? Format::kWebp
@@ -1677,7 +1671,8 @@ struct ParsedJpeg {
   int width = 0, height = 0, ncomp = 0, precision = 8;
   int cid[4] = {0}, hs[4] = {0}, vs[4] = {0}, tq[4] = {0};
   int hmax = 0, vmax = 0;
-  bool progressive = false, jfif = false;
+  bool progressive = false, jfif = false, lossless = false;
+  int ss = 0, se = 63, ah = 0, al = 0;   // spectral selection / predictor, successive approximation / point transform of the first scan
   Format format = Format::kJpeg;   // PNG, TIFF, WebP, BMP / PNM: width / height / ncomp / orientation / scan range and hs[0] / vs[0] only
   int adobe_transform = -1, orientation = 1, restart_interval = 0;
   uint16_t qt[4][64]; bool qt_present[4] = {false, false, false, false};
@@ -1733,9 +1728,10 @@ int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
         memcpy(h.vals, s + o, cnt); o += cnt;
         h.present = true;
       }
-    } else if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
+    } else if (m == 0xC0 || m == 0xC1 || m == 0xC2 || m == 0xC3) {
       if (sl < 6) { SetLastError("JPEG: bad SOF"); return DALIB200_ERROR_BAD_DATA; }
       j.progressive = m == 0xC2;
+      j.lossless = m == 0xC3;
       j.precision = s[0]; j.height = rd16(s + 1); j.width = rd16(s + 3); j.ncomp = s[5];
       if (j.ncomp < 1 || j.ncomp > 4 || sl < 6 + 3 * j.ncomp) { SetLastError("JPEG: bad SOF component count"); return DALIB200_ERROR_BAD_DATA; }
       for (int c = 0; c < j.ncomp; c++) {
@@ -1744,8 +1740,8 @@ int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
         j.hmax = std::max(j.hmax, j.hs[c]); j.vmax = std::max(j.vmax, j.vs[c]);
       }
       got_sof = true;
-    } else if (m >= 0xC3 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC) {
-      SetLastError("JPEG: coding process 0x%02X (lossless / arithmetic / hierarchical) is not supported", m);
+    } else if (m >= 0xC5 && m <= 0xCF && m != 0xC8 && m != 0xCC) {
+      SetLastError("JPEG: coding process 0x%02X (arithmetic / hierarchical) is not supported", m);
       return DALIB200_ERROR_UNSUPPORTED;
     } else if (m == 0xDD) {
       if (sl >= 2) j.restart_interval = rd16(s);
@@ -1765,6 +1761,10 @@ int ParseHeaders(const uint8_t *p, size_t n, ParsedJpeg &j, bool need_scan) {
         for (int c = 0; c < j.ncomp; c++) if (j.cid[c] == cs) ci = c;
         if (ci < 0) { SetLastError("JPEG: SOS references an unknown component"); return DALIB200_ERROR_BAD_DATA; }
         j.scan_comp[i] = ci; j.td[i] = s[2 + 2 * i] >> 4; j.ta[i] = s[2 + 2 * i] & 15;
+      }
+      if (sl >= 4 + 2 * j.scan_ncomp) {
+        const uint8_t *t = s + 1 + 2 * j.scan_ncomp;
+        j.ss = t[0]; j.se = t[1]; j.ah = t[2] >> 4; j.al = t[2] & 15;
       }
       j.scan_begin = pos + L;
       break;
@@ -1968,6 +1968,17 @@ struct dalib200JpegPlan {
   int64_t bitmap_scratch_bytes = 0;
   uint8_t *d_bitmap_scratch = nullptr; size_t d_bitmap_scratch_cap = 0;   // unpacked planes (grow only)
   SideStage bitmap;
+  // lossless JPEG samples: their units join U1 - U3 (in `units`, skipped by every DCT kernel); ljpeg.cu decodes the clean streams on a
+  // stage forked behind U3
+  std::vector<dalib200::LjpegImage> ljpeg_images;
+  std::vector<dalib200::LjpegUnit> ljpeg_units;
+  std::vector<dalib200::LjpegTable> ljpeg_tables;
+  std::vector<dalib200::LjpegBand> ljpeg_bands;
+  int64_t ljpeg_total_sub = 0, ljpeg_diff_elems = 0;
+  int16_t *d_ljpeg_diff = nullptr; size_t d_ljpeg_diff_cap = 0;          // differences, reconstructed in place (grow only)
+  uint64_t *d_ljpeg_rec = nullptr; size_t d_ljpeg_rec_cap = 0;           // subsequence records (grow only)
+  uint32_t *d_ljpeg_first = nullptr; size_t d_ljpeg_first_cap = 0;      // first symbol of each subsequence (grow only)
+  SideStage ljpeg;
 };
 
 namespace {
@@ -2061,6 +2072,69 @@ int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t le
   return DALIB200_SUCCESS;
 }
 
+// Lossless JPEG sample `sample` (ParseHeaders found SOF3): checks the frame (ljpeg_plan.h), appends its image record, tables and
+// reconstruction bands, and one JpegUnit + LjpegUnit per restart interval, whose bytes sit at `raw` + their offset behind the scan start
+// in the raw staging area; `clean` and `chunks` advance as for a baseline unit.  Returns a DALIB200 status.
+int PlanLossless(dalib200JpegPlan *p, int sample, const uint8_t *d, size_t len, size_t raw, size_t &clean, uint32_t &chunks, ParsedJpeg &j) {
+  LjpegFrame f;
+  f.width = j.width; f.height = j.height; f.ncomp = j.ncomp; f.precision = j.precision;
+  for (int c = 0; c < 4; c++) { f.hs[c] = j.hs[c]; f.vs[c] = j.vs[c]; }
+  f.scan_ncomp = j.scan_ncomp;
+  f.scan_in_frame_order = true;
+  for (int i = 0; i < j.scan_ncomp; i++) { f.td[j.scan_comp[i]] = j.td[i]; f.scan_in_frame_order &= j.scan_comp[i] == i; }
+  f.pred = j.ss; f.se = j.se; f.ah = j.ah; f.pt = j.al;
+  f.restart_interval = j.restart_interval; f.jfif = j.jfif; f.adobe_transform = j.adobe_transform;
+  for (int t = 0; t < 4; t++) if (j.dc[t].present) { f.bits[t] = j.dc[t].bits; f.vals[t] = j.dc[t].vals; }
+  LjpegImage im;
+  std::string err;
+  if (int rc = PlanLjpegFrame(f, &im, p->ljpeg_tables, &err)) { SetLastError("%s", err.c_str()); return rc; }
+  if ((int64_t)j.width * j.height >= (1ll << 31)) { SetLastError("images of 2^31 pixels or more are not supported"); return DALIB200_ERROR_UNSUPPORTED; }
+  const size_t sb = j.scan_begin;
+  size_t se = len;
+  if (se >= sb + 2 && d[se - 2] == 0xFF && d[se - 1] == 0xD9) se -= 2;
+  j.scan_end = se;
+  const int W = j.width, H = j.height, C = j.ncomp;
+  const int lines = j.restart_interval ? j.restart_interval / W : H;
+  const int nunits = (H + lines - 1) / lines;
+  std::vector<std::pair<size_t, size_t>> segs;
+  im.bad_rst = SplitLjpegUnits(d, sb, se, nunits, segs);
+  for (const auto &sg : segs)
+    if (sg.second - sg.first > kLjpegMaxUnitBytes) {
+      SetLastError("lossless JPEG: an entropy-coded segment above %zu bytes is not supported (use restart intervals)", kLjpegMaxUnitBytes);
+      return DALIB200_ERROR_UNSUPPORTED;
+    }
+  im.sample = sample;
+  im.diff_off = p->ljpeg_diff_elems;
+  p->ljpeg_diff_elems += (int64_t)Align((size_t)W * H * C, 8);
+  const int li = (int)p->ljpeg_images.size();
+  for (int k = 0; k < nunits; k++) {
+    JpegUnit u;
+    memset(&u, 0, sizeof(u));
+    u.raw_off = (uint32_t)(raw + (segs[k].first - sb));
+    u.raw_len = (uint32_t)(segs[k].second - segs[k].first);
+    u.clean_off = (uint32_t)clean;
+    u.first_chunk = chunks;
+    u.image = sample;
+    LjpegUnit lu;
+    lu.junit = (int32_t)p->units.size(); lu.image = li;
+    lu.first_sub = p->ljpeg_total_sub;
+    lu.nsub = (int32_t)((u.raw_len + (1u << (kLjpegLog2Sub - 3)) - 1) >> (kLjpegLog2Sub - 3));
+    lu.clean_off = u.clean_off;
+    const int y0 = k * lines, y1 = std::min(H, y0 + lines);
+    lu.nsym = (int64_t)(y1 - y0) * W * C;
+    lu.sym_off = im.diff_off + (int64_t)y0 * W * C;
+    for (int c = 0; c < C; c++) p->ljpeg_bands.push_back(LjpegBand{ li, c, y0, y1 });
+    p->ljpeg_total_sub += lu.nsub;
+    clean += Align(u.raw_len + kCleanPad, 16);
+    chunks += (u.raw_len + kChunkBytes - 1) / kChunkBytes;
+    p->units.push_back(u);
+    p->ljpeg_units.push_back(lu);
+  }
+  p->ljpeg_images.push_back(im);
+  j.format = Format::kLossless;
+  return DALIB200_SUCCESS;
+}
+
 // The decode window and output pointer of every PNG, TIFF, WebP, BMP or PNM image, from its sample's JpegImage as patched for this
 // launch (`hi`).  Returns the pixel total; each image's first_px is its prefix, by which the colour kernel finds the image of a pixel.
 template <typename Image>
@@ -2151,7 +2225,7 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
   DB_CHECK_ARG(plan && max_batch > 0, "JpegPlanCreate: bad arguments");
   auto *p = new dalib200JpegPlan();
   p->max_batch = max_batch;
-  if (!p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() || !p->bitmap.Create()) {
+  if (!p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() || !p->bitmap.Create() || !p->ljpeg.Create()) {
     SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
   }
   *plan = p;
@@ -2160,13 +2234,13 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
 
 int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp, &p->bitmap }) st->Destroy();
+  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp, &p->bitmap, &p->ljpeg }) st->Destroy();
   p->h_stage.Free();
   p->h_images.Free();
   if (p->h_status) cudaFreeHost(p->h_status);
   void *bufs[] = { p->d_stage, p->d_clean, p->d_chunk, p->d_unit_len, p->d_state, p->d_n, p->d_coef, p->d_dc, p->d_planes, p->d_status,
                    p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk, p->d_png_scan,
-                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch, p->d_bitmap_scratch };
+                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch, p->d_bitmap_scratch, p->d_ljpeg_diff, p->d_ljpeg_rec, p->d_ljpeg_first };
   for (void *b : bufs) if (b) cudaFree(b);
   delete p;
   return DALIB200_SUCCESS;
@@ -2246,6 +2320,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->tiff_images.clear(); p->tiff_segs.clear(); p->tiff_dec_bytes = 0;
   p->webp_images.clear(); p->webp_scratch_bytes = 0;
   p->bitmap_images.clear(); p->bitmap_unpack.clear(); p->bitmap_scratch_bytes = 0;
+  p->ljpeg_images.clear(); p->ljpeg_units.clear(); p->ljpeg_tables.clear(); p->ljpeg_bands.clear();
+  p->ljpeg_total_sub = 0; p->ljpeg_diff_elems = 0;
   std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
@@ -2288,6 +2364,19 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     }
     int rc = ParseHeaders(streams[i], lengths[i], j, true);
     if (rc) return sample_error(rc, dalib200GetLastError());
+    if (j.lossless) {
+      // lossless JPEG: units for U1 - U3 only (the DCT kernels see no unit, subsequence or MCU of the sample); ljpeg.cu decodes them
+      JpegImage &im = p->images[i];
+      memset(&im, 0, sizeof(im));
+      im.width = j.width; im.height = j.height; im.out_type = output_type;
+      im.unit_begin = im.unit_end = (int)p->units.size();
+      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
+      if ((rc = PlanLossless(p, i, streams[i], lengths[i], raw, clean, chunks, j))) return sample_error(rc, dalib200GetLastError());
+      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
+      p->src_ptr.push_back(streams[i] + j.scan_begin);
+      raw += Align(j.scan_end - j.scan_begin, 16);
+      continue;
+    }
     auto unsupported = [&](const char *what) { return sample_error(DALIB200_ERROR_UNSUPPORTED, what); };
     // multi-scan streams -- progressive, or a sequential frame whose components come in separate scans -- take the scan-by-scan entropy
     // stage (jpeg_prog.cu); `prog` below means exactly that
@@ -2852,13 +2941,43 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     a.d_raw = d_raw; a.d_scratch = p->d_bitmap_scratch; a.d_status = p->d_status;
     if ((rc = LaunchBitmap(a, st.stream)) || (rc = st.End())) return rc;
   }
-  const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;      // false: every sample of the batch is progressive
-  if (any_units) {
+  // any_units: the batch has a baseline sample; lossless samples have units for U1 - U3 but nothing for the baseline entropy kernels
+  const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;
+  if (nunits > 0 && p->nchunks > 0) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
     { ProfScope ps_("jpeg_unstuff_count", s); unstuff_count_kernel<<<grid, 256, 0, s>>>(d_raw, d_units, nunits, p->nchunks, p->d_chunk); }
     { ProfScope ps_("jpeg_unstuff_scan", s); unstuff_scan_kernel<<<(nunits + 7) / 8, 256, 0, s>>>(d_units, nunits, p->d_chunk, p->d_unit_len); }
     { ProfScope ps_("jpeg_unstuff_scatter", s); unstuff_scatter_kernel<<<grid, 256, 0, s>>>(d_raw, d_units, nunits, p->nchunks, p->d_chunk, p->d_clean); }
     CountLaunch(3);
+  }
+  if (!p->ljpeg_images.empty()) {
+    // lossless JPEG samples (ljpeg.cu): forked behind U3, whose clean streams they read.  The stage writes only the lossless samples'
+    // decode windows, its scratch and their status words.
+    SideStage &st = p->ljpeg;
+    if ((rc = GrowDevice(p->d_ljpeg_diff, p->d_ljpeg_diff_cap, (size_t)p->ljpeg_diff_elems + 8))) return rc;
+    if ((rc = GrowDevice(p->d_ljpeg_rec, p->d_ljpeg_rec_cap, (size_t)p->ljpeg_total_sub + 1))) return rc;
+    if ((rc = GrowDevice(p->d_ljpeg_first, p->d_ljpeg_first_cap, (size_t)p->ljpeg_total_sub + 1))) return rc;
+    if ((rc = st.Begin(s))) return rc;
+    const int64_t px = FillWindows(p->ljpeg_images, hi);
+    const size_t nli = p->ljpeg_images.size(), nlu = p->ljpeg_units.size(), nlt = p->ljpeg_tables.size(), nlb = p->ljpeg_bands.size();
+    const size_t o_unit = Align(sizeof(LjpegImage) * nli, 16), o_tab = Align(o_unit + sizeof(LjpegUnit) * nlu, 16),
+                 o_band = Align(o_tab + sizeof(LjpegTable) * nlt, 16), lbytes = Align(o_band + sizeof(LjpegBand) * nlb, 16);
+    uint8_t *h;
+    if ((rc = st.arena.Stage(lbytes, &h))) return rc;
+    memcpy(h, p->ljpeg_images.data(), sizeof(LjpegImage) * nli);
+    memcpy(h + o_unit, p->ljpeg_units.data(), sizeof(LjpegUnit) * nlu);
+    memcpy(h + o_tab, p->ljpeg_tables.data(), sizeof(LjpegTable) * nlt);
+    memcpy(h + o_band, p->ljpeg_bands.data(), sizeof(LjpegBand) * nlb);
+    if ((rc = st.arena.Upload(lbytes, st.stream))) return rc;
+    LjpegLaunch a;
+    a.d_images = reinterpret_cast<const LjpegImage *>(st.arena.dev); a.nimages = (int)nli;
+    a.d_units = reinterpret_cast<const LjpegUnit *>(st.arena.dev + o_unit); a.nunits = (int)nlu;
+    a.d_tables = reinterpret_cast<const LjpegTable *>(st.arena.dev + o_tab);
+    a.d_bands = reinterpret_cast<const LjpegBand *>(st.arena.dev + o_band); a.nbands = (int)nlb;
+    a.total_sub = p->ljpeg_total_sub; a.total_px = px;
+    a.d_clean = p->d_clean; a.d_unit_clean_len = p->d_unit_len;
+    a.d_rec = p->d_ljpeg_rec; a.d_first = p->d_ljpeg_first; a.d_diff = p->d_ljpeg_diff; a.d_status = p->d_status;
+    if ((rc = LaunchLjpeg(a, st.stream)) || (rc = st.End())) return rc;
   }
   HuffCtx cx;
   cx.images = d_images; cx.nimages = p->n; cx.block_image = reinterpret_cast<const int32_t *>(p->d_stage + p->off_blkimg);
@@ -2912,6 +3031,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff.join, 0));     // the TIFF samples' windows and status are in place
   if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp.join, 0));     // the WebP samples' windows and status are in place
   if (!p->bitmap_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->bitmap.join, 0)); // the BMP / PNM samples' windows and status are in place
+  if (!p->ljpeg_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->ljpeg.join, 0));   // the lossless samples' windows and status are in place
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

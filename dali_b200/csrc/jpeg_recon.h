@@ -21,6 +21,9 @@ constexpr int kMaxBlocksPerMcu = 10;
 
 struct QuantSet { uint16_t q[4][64]; };       // natural order
 
+// GRAY of an RGB-coded JPEG pixel (libjpeg-turbo rgb_gray_convert): the baseline path's Adobe-0 / R-G-B images and lossless RGB.
+JPEG_RECON_HD int RgbJpegGray(int r, int g, int b) { return (r * 19595 + g * 38470 + b * 7471 + 32768) >> 16; }
+
 // Colour space of the decoded components (libjpeg default_decompress_parms).  Decided once per image by the plan; the kernels read
 // nothing else to pick the conversion.
 enum JpegColor : int32_t {
@@ -57,6 +60,19 @@ struct JpegImage {
   // is a tight win_h x win_w x C buffer (the caller's sample, or plan scratch when a post pass follows).  win_x0 % 8 == 0.
   int32_t win_x0, win_y0, win_w, win_h;
   int32_t mcu_x0, mcu_y0, mcu_nx, mcu_ny;  // MCUs whose blocks the IDCT transforms (window + chroma upsampling halo)
+};
+
+// An entropy-coded unit (a restart interval, or a whole scan) as U1 - U3 (jpeg.cu) un-stuff it: a baseline segment, or a restart
+// interval of a lossless sample (ljpeg.cu), which has no subsequences or slots of the baseline path.
+struct JpegUnit {
+  uint32_t raw_off, raw_len;               // in the staged byte buffer
+  uint32_t clean_off;                      // in the clean buffer (bytes, 16-aligned)
+  uint32_t first_chunk;                    // global chunk index
+  int32_t image;
+  int32_t first_subseq;                    // image-local
+  int32_t nsub_max;
+  int64_t slot_base;                       // first coefficient slot of this unit (image-local)
+  int64_t nslots;                          // expected number of slots (= MCUs * bpm * 64)
 };
 
 // idct_color_420 (jpeg.cu): work item = a strip of kFusedMcus MCU columns of one image's window, walked down one MCU row ("band") at a

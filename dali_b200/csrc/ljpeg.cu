@@ -1,0 +1,136 @@
+// dali_b200/csrc/ljpeg.cu -- lossless JPEG (SOF3) decoding inside decoders.image.
+//
+// The planner (ljpeg_plan.h) checks the frame and splits the scan into restart intervals on the host; their bytes are un-stuffed by the
+// JPEG path's U1 - U3 with every other unit of the batch.  Behind that, on the stream that ran U3:
+//   L1 + L2a  ljpeg_sync     one thread per 128-byte subsequence: speculative decode from its first bit, then the chain that carries its
+//                            exit state to the right until it agrees with the record (ljpeg_walk, ljpeg_core.h)
+//   L2b       ljpeg_scan     one CTA per unit: exclusive scan of the symbol counts, status of a short unit or a bad restart sequence
+//   L3        ljpeg_write    one thread per subsequence: decode from the true entry state, int16 differences into the arena
+//   L4        ljpeg_recon    one CTA per (image, component, restart band): the prediction as a wavefront over the diagonals x + y,
+//                            one thread per line, reconstructed in place
+//   L5        ljpeg_color    one thread per window pixel: << Pt, colour rules, into the decode window
+// Orientation, region of interest, YCbCr and float output are the JPEG path's post pass over that window (jpeg.cu jpeg_post_kernel).
+#include "common.cuh"
+#include "jpeg_recon.h"
+#include "ljpeg.h"
+#include <algorithm>
+
+namespace dalib200 {
+
+constexpr int kLjpegRecThreads = 512;
+
+__device__ __forceinline__ int ljpeg_find_unit(const LjpegUnit *u, int n, int64_t g) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (u[mid].first_sub <= g) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+
+__global__ void __launch_bounds__(256) ljpeg_sync_kernel(LjpegLaunch a) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < a.total_sub; g += step) {
+    const LjpegUnit &u = a.d_units[ljpeg_find_unit(a.d_units, a.nunits, g)];
+    ljpeg_walk(a.d_images[u.image], u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec,
+               [](uint64_t *p, uint64_t v) { return (uint64_t)atomicMax(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v); });
+  }
+}
+
+__global__ void __launch_bounds__(256) ljpeg_scan_kernel(LjpegLaunch a) {
+  __shared__ uint32_t warp_tot[8];
+  __shared__ uint32_t carry;
+  const LjpegUnit &u = a.d_units[blockIdx.x];
+  const LjpegImage &im = a.d_images[u.image];
+  const uint32_t clean_bits = a.d_unit_clean_len[u.junit] * 8u;
+  const uint32_t nsub = (clean_bits + (1u << kLjpegLog2Sub) - 1) >> kLjpegLog2Sub;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (uint32_t base = 0; base < nsub; base += blockDim.x) {
+    const uint32_t i = base + threadIdx.x;
+    const uint32_t v = i < nsub ? ljpeg_count(a.d_rec[u.first_sub + i]) : 0u;
+    uint32_t incl = v;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, incl, o); if ((threadIdx.x & 31) >= (uint32_t)o) incl += x; }
+    if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = incl;
+    __syncthreads();
+    uint32_t woff = 0, tot = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) { if (w < (int)(threadIdx.x >> 5)) woff += warp_tot[w]; tot += warp_tot[w]; }
+    if (i < nsub) a.d_first[u.first_sub + i] = carry + woff + incl - v;
+    __syncthreads();
+    if (threadIdx.x == 0) carry += tot;
+    __syncthreads();
+  }
+  // the pad bits behind the data may decode into a few more symbols, so only a SHORT count is an error; the samples it lacks are 0
+  const int64_t have = carry;
+  if (threadIdx.x == 0 && (have < u.nsym || im.bad_rst)) a.d_status[im.sample] = 1;
+  for (int64_t k = have + threadIdx.x; k < u.nsym; k += blockDim.x) a.d_diff[u.sym_off + k] = 0;
+}
+
+__global__ void __launch_bounds__(256) ljpeg_write_kernel(LjpegLaunch a) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < a.total_sub; g += step) {
+    const LjpegUnit &u = a.d_units[ljpeg_find_unit(a.d_units, a.nunits, g)];
+    const LjpegImage &im = a.d_images[u.image];
+    if (ljpeg_write(im, u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec, a.d_first[g], a.d_diff)) a.d_status[im.sample] = 1;
+  }
+}
+
+// Thread t owns line y0 + t of a strip of blockDim.x lines and reaches column x at step x + t: (x - 1, y) is its own previous sample,
+// (x, y - 1) and (x - 1, y - 1) are the samples of thread t - 1 at the previous two steps (exchanged through shared memory, one barrier
+// per step).  Thread 0 of a later strip reads the line above from the arena, where the previous strip left it.
+__global__ void __launch_bounds__(kLjpegRecThreads) ljpeg_recon_kernel(const LjpegImage *__restrict__ images, const LjpegBand *__restrict__ bands,
+                                                                       int16_t *diff) {
+  __shared__ int32_t up[2][kLjpegRecThreads];
+  const LjpegBand bd = bands[blockIdx.x];
+  const LjpegImage &im = images[bd.image];
+  const int W = im.width, C = im.ncomp, t = threadIdx.x, pred = im.pred;
+  const int32_t init = 1 << (im.precision - im.pt - 1);
+  int16_t *base = diff + im.diff_off + bd.comp;
+  for (int r0 = bd.y0; r0 < bd.y1; r0 += blockDim.x) {
+    const int rows = min((int)blockDim.x, bd.y1 - r0), y = r0 + t;
+    const bool own = t < rows, first_line = y == bd.y0;
+    int16_t *row = base + (int64_t)y * W * C;
+    const int16_t *above = row - (int64_t)W * C;
+    int32_t Ra = 0, Rb = 0, Rc = 0;
+    int32_t nxt = own ? row[0] : 0;
+    for (int d = 0; d < W + rows - 1; d++) {
+      const int x = d - t;
+      if (own && x >= 0 && x < W) {
+        Rc = Rb;
+        if (!first_line) Rb = t == 0 ? (int32_t)(uint16_t)above[(int64_t)x * C] : up[(d - 1) & 1][t - 1];
+        const int32_t v = (nxt + ljpeg_predict(pred, first_line, x, init, Ra, Rb, Rc)) & 0xFFFF;
+        if (x + 1 < W) nxt = row[(int64_t)(x + 1) * C];
+        row[(int64_t)x * C] = (int16_t)v;
+        Ra = v;
+        up[d & 1][t] = v;
+      }
+      __syncthreads();
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) ljpeg_color_kernel(const LjpegImage *__restrict__ images, int nimages, int64_t total,
+                                                          const int16_t *__restrict__ diff) {
+  const int64_t step = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
+    int lo = 0, hi = nimages - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
+    ljpeg_pixel(images[lo], diff, e - images[lo].first_px, [](int r, int g, int b) { return RgbJpegGray(r, g, b); });
+  }
+}
+
+int LaunchLjpeg(const LjpegLaunch &a, cudaStream_t s) {
+  if (a.nimages == 0) return DALIB200_SUCCESS;
+  const int sms = NumSMs();
+  auto grid_of = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sms * 16)); };
+  if (a.total_sub > 0) {
+    DB_CUDA(cudaMemsetAsync(a.d_rec, 0, sizeof(uint64_t) * a.total_sub, s));
+    { ProfScope ps_("ljpeg_sync", s); ljpeg_sync_kernel<<<grid_of(a.total_sub), 256, 0, s>>>(a); }
+  }
+  { ProfScope ps_("ljpeg_scan", s); ljpeg_scan_kernel<<<a.nunits, 256, 0, s>>>(a); }
+  if (a.total_sub > 0) { ProfScope ps_("ljpeg_write", s); ljpeg_write_kernel<<<grid_of(a.total_sub), 256, 0, s>>>(a); }
+  { ProfScope ps_("ljpeg_recon", s); ljpeg_recon_kernel<<<a.nbands, kLjpegRecThreads, 0, s>>>(a.d_images, a.d_bands, a.d_diff); }
+  { ProfScope ps_("ljpeg_color", s); ljpeg_color_kernel<<<grid_of(a.total_px), 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_diff); }
+  CountLaunch(a.total_sub > 0 ? 5 : 3);
+  DB_CUDA(cudaGetLastError());
+  return DALIB200_SUCCESS;
+}
+
+}  // namespace dalib200

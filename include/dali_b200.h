@@ -59,7 +59,9 @@ int dalib200ProfilingCollect(char *names, int name_stride, float *ms, int max, i
  * conversion, bit-exact with cv2.imdecode; unsupported layouts fail with DALIB200_ERROR_UNSUPPORTED).
  * Lossy WebP (detected by its RIFF header; VP8 key frame: one GPU lane per image for the entropy decode, macroblock-wavefront
  * reconstruction and loop filter, fancy upsampling, bit-exact with cv2.imdecode; lossless and animated WebP fail with
- * DALIB200_ERROR_UNSUPPORTED).  All formats may be mixed in one batch of a plan.
+ * DALIB200_ERROR_UNSUPPORTED).  Lossless JPEG (SOF3: precision 2..8, predictors 1..7, 1 or 3 components at 1x1 sampling, restart
+ * intervals of whole lines; self-synchronising parallel Huffman decode and a diagonal-wavefront prediction, bit-exact with cv2.imdecode;
+ * precision above 8 bits fails with DALIB200_ERROR_UNSUPPORTED).  All formats may be mixed in one batch of a plan.
  * Replaces: imgcodec::ImageDecoder<MixedBackend>::RunImplImpl -> nvimgcodecDecoderDecode
  *           (dali/operators/imgcodec/image_decoder.h:613-882) and ParseSample (:473-499).
  * Host work: marker / table / chunk-header parse only.  Device work: everything arithmetic. */

@@ -1,6 +1,7 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP and BMP / PNM kernels are EXECUTED on the host -- their bodies are single
+// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM and lossless JPEG kernels (and U2 / U3, which feed the last) are
+// EXECUTED on the host -- their bodies are single
 // host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h, bitmap_core.h), so a
 // launch is a loop over blocks and threads around
 // the same function the device runs.  All other kernels are no-ops.  With this preloaded, the real launch path of the library runs
@@ -35,6 +36,8 @@
 #include "../../dali_b200/csrc/tiff_core.h"
 #include "../../dali_b200/csrc/webp_core.h"
 #include "../../dali_b200/csrc/bitmap_core.h"
+#include "../../dali_b200/csrc/jpeg_recon.h"
+#include "../../dali_b200/csrc/ljpeg_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -142,7 +145,7 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[14];
+static long g_emulated[21];
 long emul_launch_count(int which) { return g_emulated[which]; }
 void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
@@ -362,6 +365,101 @@ static void run_bitmap_color(Dim3 g, Dim3 b, void **args) {
       }
 }
 
+// U2 / U3 of jpeg.cu as their result: each unit's clean length, and its clean stream (FF 00 -> FF, word-swapped, zero pad behind it).
+// They serve the lossless JPEG stage here; the baseline kernels that read the clean streams are not emulated.
+static uint32_t unstuff_unit(const uint8_t *raw, const JpegUnit &u, uint8_t *clean) {
+  uint32_t q = 0;
+  for (uint32_t i = 0; i < u.raw_len; i++) {
+    const uint8_t *p = raw + u.raw_off + i;
+    if (i > 0 && p[0] == 0 && p[-1] == 0xFF) continue;
+    if (clean) clean[(u.clean_off + q) ^ 3u] = p[0];
+    q++;
+  }
+  if (clean)
+    for (uint32_t e = u.clean_off + q; e < u.clean_off + ((u.raw_len + 32u + 15u) & ~15u); e++) clean[e ^ 3u] = 0;
+  return q;
+}
+static const uint8_t *g_unstuff_raw;                 // the raw buffer of the last unstuff_count launch (the scan launch has none)
+static void run_unstuff_count(void **args) { g_unstuff_raw = *static_cast<const uint8_t **>(args[0]); }
+static void run_unstuff_scan(void **args) {
+  const JpegUnit *units = *static_cast<const JpegUnit **>(args[0]);
+  const int n = *static_cast<int *>(args[1]);
+  uint32_t *len = *static_cast<uint32_t **>(args[3]);
+  for (int k = n - 1; k >= 0; k--) len[k] = unstuff_unit(g_unstuff_raw, units[k], nullptr);
+}
+static void run_unstuff_scatter(void **args) {
+  const uint8_t *raw = *static_cast<const uint8_t **>(args[0]);
+  const JpegUnit *units = *static_cast<const JpegUnit **>(args[1]);
+  const int n = *static_cast<int *>(args[2]);
+  uint8_t *clean = *static_cast<uint8_t **>(args[5]);
+  for (int k = n - 1; k >= 0; k--) unstuff_unit(raw, units[k], clean);
+}
+
+// ljpeg.cu.  ljpeg_sync and ljpeg_write take the subsequences in REVERSE order, so that a chain always meets the records of the chains
+// that started to its right first; ljpeg_recon walks each band in raster order, which keeps every dependency of the wavefront.
+static int ljpeg_unit_of(const LjpegLaunch &a, int64_t g) {
+  int k = a.nunits - 1;
+  while (a.d_units[k].first_sub > g) k--;
+  return k;
+}
+static void run_ljpeg_sync(void **args) {
+  const LjpegLaunch &a = *static_cast<const LjpegLaunch *>(args[0]);
+  auto amax = [](uint64_t *p, uint64_t v) { const uint64_t o = *p; if (v > o) *p = v; return o; };
+  for (int64_t g = a.total_sub - 1; g >= 0; g--) {
+    const LjpegUnit &u = a.d_units[ljpeg_unit_of(a, g)];
+    ljpeg_walk(a.d_images[u.image], u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec, amax);
+  }
+}
+static void run_ljpeg_scan(void **args) {
+  const LjpegLaunch &a = *static_cast<const LjpegLaunch *>(args[0]);
+  for (int k = a.nunits - 1; k >= 0; k--) {
+    const LjpegUnit &u = a.d_units[k];
+    const LjpegImage &im = a.d_images[u.image];
+    const uint32_t nsub = (a.d_unit_clean_len[u.junit] * 8u + (1u << kLjpegLog2Sub) - 1) >> kLjpegLog2Sub;
+    uint32_t run = 0;
+    for (uint32_t i = 0; i < nsub; i++) { a.d_first[u.first_sub + i] = run; run += ljpeg_count(a.d_rec[u.first_sub + i]); }
+    if ((int64_t)run < u.nsym || im.bad_rst) a.d_status[im.sample] = 1;
+    for (int64_t s = run; s < u.nsym; s++) a.d_diff[u.sym_off + s] = 0;
+  }
+}
+static void run_ljpeg_write(void **args) {
+  const LjpegLaunch &a = *static_cast<const LjpegLaunch *>(args[0]);
+  for (int64_t g = a.total_sub - 1; g >= 0; g--) {
+    const LjpegUnit &u = a.d_units[ljpeg_unit_of(a, g)];
+    const LjpegImage &im = a.d_images[u.image];
+    if (ljpeg_write(im, u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec, a.d_first[g], a.d_diff)) a.d_status[im.sample] = 1;
+  }
+}
+static void run_ljpeg_recon(Dim3 g, void **args) {
+  const LjpegImage *images = *static_cast<const LjpegImage **>(args[0]);
+  const LjpegBand *bands = *static_cast<const LjpegBand **>(args[1]);
+  int16_t *diff = *static_cast<int16_t **>(args[2]);
+  for (int bx = (int)g.x - 1; bx >= 0; bx--) {
+    const LjpegBand bd = bands[bx];
+    const LjpegImage &im = images[bd.image];
+    const int W = im.width, C = im.ncomp;
+    const int32_t init = 1 << (im.precision - im.pt - 1);
+    auto at = [&](int y, int x) -> int16_t & { return diff[im.diff_off + ((int64_t)y * W + x) * C + bd.comp]; };
+    for (int y = bd.y0; y < bd.y1; y++)
+      for (int x = 0; x < W; x++) {
+        const bool fl = y == bd.y0;
+        const int32_t Ra = x ? (uint16_t)at(y, x - 1) : 0, Rb = fl ? 0 : (uint16_t)at(y - 1, x), Rc = fl || !x ? 0 : (uint16_t)at(y - 1, x - 1);
+        at(y, x) = (int16_t)((at(y, x) + ljpeg_predict(im.pred, fl, x, init, Ra, Rb, Rc)) & 0xFFFF);
+      }
+  }
+}
+static void run_ljpeg_color(void **args) {
+  const LjpegImage *images = *static_cast<const LjpegImage **>(args[0]);
+  const int n = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  const int16_t *diff = *static_cast<const int16_t **>(args[3]);
+  for (int64_t e = total - 1; e >= 0; e--) {
+    int i = n - 1;
+    while (images[i].first_px > e) i--;
+    ljpeg_pixel(images[i], diff, e - images[i].first_px, [](int r, int gg, int b) { return RgbJpegGray(r, gg, b); });
+  }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *stream) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -381,6 +479,14 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_webp_color = !strcmp(name, "_ZN8dalib20017webp_color_kernelEPKNS_9WebpImageEilPh");
   const bool is_bitmap_unpack = !strcmp(name, "_ZN8dalib20020bitmap_unpack_kernelEPKNS_11BitmapImageEPKiiiPKhPhPi");
   const bool is_bitmap_color = !strcmp(name, "_ZN8dalib20019bitmap_color_kernelEPKNS_11BitmapImageEilPKhS4_");
+  const bool is_unstuff_count = !strcmp(name, "_ZN8dalib20020unstuff_count_kernelEPKhPKNS_8JpegUnitEijPj");
+  const bool is_unstuff_scan = !strcmp(name, "_ZN8dalib20019unstuff_scan_kernelEPKNS_8JpegUnitEiPjS3_");
+  const bool is_unstuff_scatter = !strcmp(name, "_ZN8dalib20022unstuff_scatter_kernelEPKhPKNS_8JpegUnitEijPKjPh");
+  const bool is_ljpeg_sync = !strcmp(name, "_ZN8dalib20017ljpeg_sync_kernelENS_11LjpegLaunchE");
+  const bool is_ljpeg_scan = !strcmp(name, "_ZN8dalib20017ljpeg_scan_kernelENS_11LjpegLaunchE");
+  const bool is_ljpeg_write = !strcmp(name, "_ZN8dalib20018ljpeg_write_kernelENS_11LjpegLaunchE");
+  const bool is_ljpeg_recon = !strcmp(name, "_ZN8dalib20018ljpeg_recon_kernelEPKNS_10LjpegImageEPKNS_9LjpegBandEPs");
+  const bool is_ljpeg_color = !strcmp(name, "_ZN8dalib20018ljpeg_color_kernelEPKNS_10LjpegImageEilPKs");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -399,6 +505,14 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_webp_color) { run_webp_color(grid, block, args); g_emulated[11]++; }
   else if (is_bitmap_unpack) { run_bitmap_unpack(grid, block, args); g_emulated[12]++; }
   else if (is_bitmap_color) { run_bitmap_color(grid, block, args); g_emulated[13]++; }
+  else if (is_unstuff_count) { run_unstuff_count(args); g_emulated[14]++; }
+  else if (is_unstuff_scan) { run_unstuff_scan(args); g_emulated[14]++; }
+  else if (is_unstuff_scatter) { run_unstuff_scatter(args); g_emulated[14]++; }
+  else if (is_ljpeg_sync) { run_ljpeg_sync(args); g_emulated[15]++; }
+  else if (is_ljpeg_scan) { run_ljpeg_scan(args); g_emulated[16]++; }
+  else if (is_ljpeg_write) { run_ljpeg_write(args); g_emulated[17]++; }
+  else if (is_ljpeg_recon) { run_ljpeg_recon(grid, args); g_emulated[18]++; }
+  else if (is_ljpeg_color) { run_ljpeg_color(args); g_emulated[19]++; }
   return 0;
 }
 }  // extern "C"

@@ -39,6 +39,10 @@ if webp_streams.libwebp():
 # BMP and PNM streams (every header size, palettes, bitfields, RLE4 / RLE8, P1 - P6, comments): the header parse of the planner
 import bitmap_streams
 seeds += [bytearray(s) for n, s in bitmap_streams.corpus() if len(s) < 100000][::7]
+# lossless JPEG streams (SOF3: predictors, point transforms, restart intervals, tables with codes up to 16 bits): the frame checks, the
+# table build and the split at the restart markers of ljpeg_plan.h
+import ljpeg_streams
+seeds += [bytearray(s) for n, s, _, _ in ljpeg_streams.corpus() if len(s) < 100000][::5]
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()

@@ -18,7 +18,8 @@ $NVCC $F -c "$ROOT/dali_b200/csrc/png.cu" -o "$OUT/png.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/tiff.cu" -o "$OUT/tiff.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/webp.cu" -o "$OUT/webp.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/bitmap.cu" -o "$OUT/bitmap.o"
-$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" "$OUT/bitmap.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
+$NVCC $F -c "$ROOT/dali_b200/csrc/ljpeg.cu" -o "$OUT/ljpeg.o"
+$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" "$OUT/bitmap.o" "$OUT/ljpeg.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
 gcc -shared -fPIC -O1 -o "$OUT/cuda_stub.so" "$HERE/cuda_stub.c"
 # the progressive scan decoder itself (the body of prog_scan_kernel, compiled for the host by tools/emul) under ASAN + UBSAN on mutated
 # progressive streams: garbage Huffman codes, runs past the band, truncated scans, markers inside the data must stay inside the arena
