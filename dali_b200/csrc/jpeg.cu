@@ -414,7 +414,9 @@ __device__ __forceinline__ uint32_t make_entry16(uint32_t len, uint32_t sym, boo
 }
 
 // codes longer than the first-level LUT (std tables: AC codes of 12..16 bits, < 1 % of the symbols): canonical search,
-// T.81 F.2.2.3.  `toff` = LUT word offset of the table, which identifies it.  Returns code length | symbol << 8.
+// T.81 F.2.2.3.  `toff` = LUT word offset of the table, which identifies it.  Returns code length | symbol << 8; a window that matches
+// no code gives 17 | 0, which the 5-bit length fields of make_entry / make_entry16 and the >= 32-bit window hold.  The sync, walk and
+// write passes all decode through here, so they stay in step on damaged data.
 __device__ __noinline__ uint32_t slow_lookup(const HuffSlow *__restrict__ slow, uint32_t toff, uint32_t hi, bool is_dc) {
   const int tbl = toff < 2u * kDcLutSize ? (int)(toff / kDcLutSize) : 2 + (int)((toff - 2u * kDcLutSize) / kAcLutSize);
   const HuffSlow *sl = slow + tbl;
@@ -422,12 +424,12 @@ __device__ __noinline__ uint32_t slow_lookup(const HuffSlow *__restrict__ slow, 
   if (sl->long_n > 0) {
     const int idx = min(max(code16 - sl->long_base, 0), sl->long_n - 1);
     const uint32_t e = sl->long_lut[idx];
-    return e ? e : 16u;                                      // corrupt / speculative: keep going deterministically (length 16, symbol 0)
+    return e ? e : 17u;                                      // not a code: 17 bits, symbol 0 (libjpeg jpeg_huff_decode)
   }
   uint32_t len = (is_dc ? kDcLutBits : kAcLutBits) + 1;
   while (len <= 16 && code16 >= sl->maxcode[len]) len++;
   uint32_t sym = 0;
-  if (len > 16) len = 16;                                    // corrupt / speculative: keep going deterministically
+  if (len > 16) len = 17;                                    // not a code: 17 bits, symbol 0, as libjpeg (jpeg_huff_decode)
   else sym = sl->vals[(sl->valoff[len] + (code16 >> (16 - len))) & 0xFF];
   return len | (sym << 8);
 }
@@ -995,50 +997,30 @@ __global__ void __launch_bounds__(256) truncation_fixup_kernel(HuffCtx cx) {
 
 // ============================================================================================
 // I1: dequantisation + islow IDCT (libjpeg jidctint: CONST_BITS 13, PASS1_BITS 2).  One thread per 8x8 block.
-#define FIX_0_298631336 2446
-#define FIX_0_390180644 3196
-#define FIX_0_541196100 4433
-#define FIX_0_765366865 6270
-#define FIX_0_899976223 7373
-#define FIX_1_175875602 9633
-#define FIX_1_501321110 12299
-#define FIX_1_847759065 15137
-#define FIX_1_961570560 16069
-#define FIX_2_053119869 16819
-#define FIX_2_562915447 20995
-#define FIX_3_072711026 25172
+// The arithmetic is that of libjpeg-turbo's x86 SIMD kernels (jidctint-sse2 / -avx2), which cv2.imdecode and the reference's CPU decoder
+// run; it equals the C jidctint on natural streams and parts from it where coefficients are far out of range (damaged or hostile
+// streams, 16-bit DQT): dequantised words and the sums i0 +- i4, i7 + i3, i5 + i1 wrap to 16 bits, the multiply-adds are exact in 32
+// bits, each pass saturates its output to int16 and the result to [-128, 127].  Restated in oracle/jpeg_oracle.c and tests/jpeg_idct16.py.
+__device__ __forceinline__ int wrap16(int x) { return (int)(int16_t)x; }
 
+// One 1-D pass over int16 inputs: the descaled 32-bit results (no sum leaves 32 bits for int16 inputs); the caller saturates.
 template <int SHIFT>
 __device__ __forceinline__ void idct8(int i0, int i1, int i2, int i3, int i4, int i5, int i6, int i7, int *o) {
-  int z1, z2, z3, z4, z5, tmp0, tmp1, tmp2, tmp3, tmp10, tmp11, tmp12, tmp13;
-  z2 = i2; z3 = i6;
-  z1 = (z2 + z3) * FIX_0_541196100;
-  tmp2 = z1 + z3 * (-FIX_1_847759065);
-  tmp3 = z1 + z2 * FIX_0_765366865;
-  z2 = i0; z3 = i4;
-  tmp0 = (int)((unsigned)(z2 + z3) << 13);
-  tmp1 = (int)((unsigned)(z2 - z3) << 13);
-  tmp10 = tmp0 + tmp3; tmp13 = tmp0 - tmp3; tmp11 = tmp1 + tmp2; tmp12 = tmp1 - tmp2;
-  tmp0 = i7; tmp1 = i5; tmp2 = i3; tmp3 = i1;
-  z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2; z4 = tmp1 + tmp3;
-  z5 = (z3 + z4) * FIX_1_175875602;
-  tmp0 *= FIX_0_298631336; tmp1 *= FIX_2_053119869; tmp2 *= FIX_3_072711026; tmp3 *= FIX_1_501321110;
-  z1 *= -FIX_0_899976223; z2 *= -FIX_2_562915447; z3 *= -FIX_1_961570560; z4 *= -FIX_0_390180644;
-  z3 += z5; z4 += z5;
-  tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
+  const int tmp3 = i2 * 10703 + i6 * 4433, tmp2 = i2 * 4433 - i6 * 10704;
+  const int tmp0 = wrap16(i0 + i4) * 8192, tmp1 = wrap16(i0 - i4) * 8192;
+  const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  const int z3 = wrap16(i7 + i3), z4 = wrap16(i5 + i1);
+  const int Z3 = z3 * -6436 + z4 * 9633, Z4 = z3 * 9633 + z4 * 6437;
+  const int o0 = i7 * -4927 + i1 * -7373 + Z3, o3 = i7 * -7373 + i1 * 4926 + Z4;
+  const int o1 = i5 * -4176 + i3 * -20995 + Z4, o2 = i5 * -20995 + i3 * 4177 + Z3;
   const int r = 1 << (SHIFT - 1);
-  o[0] = (tmp10 + tmp3 + r) >> SHIFT; o[7] = (tmp10 - tmp3 + r) >> SHIFT;
-  o[1] = (tmp11 + tmp2 + r) >> SHIFT; o[6] = (tmp11 - tmp2 + r) >> SHIFT;
-  o[2] = (tmp12 + tmp1 + r) >> SHIFT; o[5] = (tmp12 - tmp1 + r) >> SHIFT;
-  o[3] = (tmp13 + tmp0 + r) >> SHIFT; o[4] = (tmp13 - tmp0 + r) >> SHIFT;
+  o[0] = (t10 + o3 + r) >> SHIFT; o[7] = (t10 - o3 + r) >> SHIFT;
+  o[1] = (t11 + o2 + r) >> SHIFT; o[6] = (t11 - o2 + r) >> SHIFT;
+  o[2] = (t12 + o1 + r) >> SHIFT; o[5] = (t12 - o1 + r) >> SHIFT;
+  o[3] = (t13 + o0 + r) >> SHIFT; o[4] = (t13 - o0 + r) >> SHIFT;
 }
 
-__device__ __forceinline__ uint32_t range_limit(int x) {     // libjpeg range_limit[(x) & RANGE_MASK], table centred on 128
-  // idx = x & 1023: [0,128) -> idx + 128, [128,512) -> 255, [512,896) -> 0, [896,1024) -> idx - 896.  With y = (x + 128) & 1023
-  // this is: y < 256 -> y, y < 640 -> 255, else 0.
-  const uint32_t y = (uint32_t)(x + 128) & 1023u;
-  return y < 640u ? min(y, 255u) : 0u;
-}
+__device__ __forceinline__ uint32_t pixel(int x) { return (uint32_t)(min(max(x, -128), 127) + 128); }     // packsswb, + 128
 
 __device__ __forceinline__ int find_by_prefix(const int64_t *first, int n, int64_t v) {
   int lo = 0, hi = n - 1;
@@ -1058,7 +1040,7 @@ __device__ __forceinline__ void idct_block(const int16_t *__restrict__ coef_aren
   {
     int in[64];
     const uint4 *q4 = reinterpret_cast<const uint4 *>(q);      // 8 x u16 per row in ONE 16-byte load (the table is 16-byte aligned)
-    uint32_t q00 = 0;
+    uint32_t q00 = 0, ac_rows = 0;
 #pragma unroll
     for (int r = 0; r < 8; r++) {
       const int4 v = __ldg(src + r);
@@ -1066,27 +1048,35 @@ __device__ __forceinline__ void idct_block(const int16_t *__restrict__ coef_aren
       const int w[4] = { v.x, v.y, v.z, v.w };
       const uint32_t qw[4] = { qv.x, qv.y, qv.z, qv.w };
       if (r == 0) q00 = qv.x & 0xFFFFu;
+      else ac_rows |= (uint32_t)(v.x | v.y | v.z | v.w);
 #pragma unroll
       for (int k = 0; k < 4; k++) {
-        in[r * 8 + 2 * k] = (int)(int16_t)(w[k] & 0xFFFF) * (int)(qw[k] & 0xFFFFu);
-        in[r * 8 + 2 * k + 1] = (w[k] >> 16) * (int)(qw[k] >> 16);
+        in[r * 8 + 2 * k] = wrap16(w[k] * (int)(qw[k] & 0xFFFFu));                     // the low 16 bits of coef * q (pmullw)
+        in[r * 8 + 2 * k + 1] = wrap16((w[k] >> 16) * (int)(qw[k] >> 16));
       }
     }
-    in[0] = (int)__ldg(dc_arena + gb) * (int)q00;         // DC lives in the compact array (after prediction)
+    in[0] = wrap16((int)__ldg(dc_arena + gb) * (int)q00);  // DC lives in the compact array (after prediction)
+    // coefficients of rows 1..7 all zero: the SIMD kernels skip pass 1 and shift row 0 left by PASS1_BITS in 16 bits, which wraps
+    // where the full pass (whose outputs are then exactly in[x] << 2) saturates.  wrap16(in[x] << 2) is a multiple of 4, so feeding the
+    // full pass a quarter of it yields the wrapped value unsaturated.
+    if (ac_rows == 0) {
+#pragma unroll
+      for (int x = 0; x < 8; x++) in[x] = wrap16(in[x] * 4) >> 2;
+    }
 #pragma unroll
     for (int x = 0; x < 8; x++) {       // pass 1: columns
       int o[8];
       idct8<11>(in[x], in[8 + x], in[16 + x], in[24 + x], in[32 + x], in[40 + x], in[48 + x], in[56 + x], o);
 #pragma unroll
-      for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y];
+      for (int y = 0; y < 8; y++) ws[y * 8 + x] = min(max(o[y], -32768), 32767);       // packssdw
     }
   }
 #pragma unroll
   for (int y = 0; y < 8; y++) {         // pass 2: rows
     int o[8];
     idct8<18>(ws[y * 8], ws[y * 8 + 1], ws[y * 8 + 2], ws[y * 8 + 3], ws[y * 8 + 4], ws[y * 8 + 5], ws[y * 8 + 6], ws[y * 8 + 7], o);
-    rows[y].x = range_limit(o[0]) | (range_limit(o[1]) << 8) | (range_limit(o[2]) << 16) | (range_limit(o[3]) << 24);
-    rows[y].y = range_limit(o[4]) | (range_limit(o[5]) << 8) | (range_limit(o[6]) << 16) | (range_limit(o[7]) << 24);
+    rows[y].x = pixel(o[0]) | (pixel(o[1]) << 8) | (pixel(o[2]) << 16) | (pixel(o[3]) << 24);
+    rows[y].y = pixel(o[4]) | (pixel(o[5]) << 8) | (pixel(o[6]) << 16) | (pixel(o[7]) << 24);
   }
 }
 

@@ -60,7 +60,9 @@ __device__ const uint8_t d_prog_natural[64] = {
 static const uint8_t h_prog_natural[64] = {
    0,  1,  8, 16,  9,  2,  3, 10, 17, 24, 32, 25, 18, 11,  4,  5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13,  6,  7, 14, 21, 28,
   35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
+// zig-zag index -> natural index; a run past 63 (corrupt data) lands on 63, as on the guard entries of libjpeg's jpeg_natural_order
 PG_HD int prog_natural(int k) {
+  if (k > 63) k = 63;
 #if defined(__CUDA_ARCH__)
   return d_prog_natural[k];
 #else
@@ -177,7 +179,7 @@ PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuf
               rs &= 15;
               if (rs) {
                 z += r;
-                q[prog_natural(z & 63)] = (int16_t)pb_extend(pb_get(b, rs), rs);
+                q[prog_natural(z)] = (int16_t)pb_extend(pb_get(b, rs), rs);
               } else if (r == 15) {
                 z += 15;
               } else {
@@ -216,7 +218,7 @@ PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuf
               if (t) {
                 k += r;
                 const int v = pb_extend(pb_get(b, t), t);
-                q[prog_natural(k & 63)] = (int16_t)((uint32_t)v << s.al);
+                q[prog_natural(k)] = (int16_t)((uint32_t)v << s.al);
               } else if (r == 15) {
                 k += 15;
               } else {
@@ -243,7 +245,7 @@ PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuf
               }
               // step over already-nonzero coefficients (each takes a correction bit) and r still-zero ones
               do {
-                int16_t *tc = q + prog_natural(k & 63);
+                int16_t *tc = q + prog_natural(k);
                 if (*tc != 0) {
                   if (pb_get(b, 1) && (*tc & p1) == 0) *tc = (int16_t)(*tc >= 0 ? *tc + p1 : *tc + m1);
                 } else if (--r < 0) {
@@ -251,12 +253,12 @@ PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuf
                 }
                 k++;
               } while (k <= s.se);
-              if (t) q[prog_natural(k & 63)] = (int16_t)t;
+              if (t) q[prog_natural(k)] = (int16_t)t;
             }
           }
           if (eobrun > 0) {
             for (; k <= s.se; k++) {
-              int16_t *tc = q + prog_natural(k & 63);
+              int16_t *tc = q + prog_natural(k);
               if (*tc != 0 && pb_get(b, 1) && (*tc & p1) == 0) *tc = (int16_t)(*tc >= 0 ? *tc + p1 : *tc + m1);
             }
             eobrun--;

@@ -9,7 +9,8 @@
  * cmake/Dependencies.common.cmake:310-311 -> libjpeg-turbo).  It is restated here from the
  * published algorithms:
  *   - ITU-T T.81 Annex B (markers), C (Huffman table generation), F.2.2 (sequential decode),
- *   - libjpeg "islow" integer IDCT (Loeffler-Ligtenberg-Moschytz, CONST_BITS=13, PASS1_BITS=2),
+ *   - libjpeg "islow" integer IDCT (Loeffler-Ligtenberg-Moschytz, CONST_BITS=13, PASS1_BITS=2) in the 16-bit dataflow of
+ *     libjpeg-turbo's x86 SIMD kernels (see jo_idct_block),
  *   - libjpeg "fancy" (triangle) h2v1 / h2v2 chroma upsampling,
  *   - libjpeg fixed-point (SCALEBITS=16) YCbCr->RGB.
  * Pinned (tests/test_oracle_jpeg.py, tests/golden/) against cv2.imdecode (OpenCV 4.13 bundling
@@ -222,64 +223,82 @@ typedef struct {
   uint32_t acc;
   int nbits;
   int marker;       /* pending marker seen (stops feeding real bits) */
+  int pad;          /* the last `pad` bits of the window are zero padding supplied behind a marker or the end of the data */
+  int overrun;      /* padding bits have been CONSUMED (decoded as data) */
 } jo_bits;
 
 static void jo_fill(jo_bits *b) {
   while (b->nbits <= 24) {
-    int byte = 0;
+    int byte = 0, real = 0;
     if (!b->marker && b->pos < b->end) {
       byte = b->p[b->pos];
       if (byte == 0xFF) {
         int nx = b->pos + 1 < b->end ? b->p[b->pos + 1] : 0xD9;
-        if (nx == 0x00) { b->pos += 2; }
+        if (nx == 0x00) { b->pos += 2; real = 1; }
         else { b->marker = nx; byte = 0; }      /* do not consume the marker */
       } else {
-        b->pos++;
+        b->pos++; real = 1;
       }
     }
+    if (!real) b->pad += 8;
     b->acc |= (uint32_t)byte << (24 - b->nbits);
     b->nbits += 8;
   }
+}
+static inline void jo_drop(jo_bits *b, int n) {
+  b->acc <<= n; b->nbits -= n;
+  if (b->nbits < b->pad) { b->overrun = 1; b->pad = b->nbits; }
 }
 static inline int jo_getbits(jo_bits *b, int n) {
   if (n == 0) return 0;
   if (b->nbits < n) jo_fill(b);
   int v = (int)(b->acc >> (32 - n));
-  b->acc <<= n; b->nbits -= n;
+  jo_drop(b, n);
   return v;
 }
+/* libjpeg jdhuff.c jpeg_huff_decode: a code that matches no length up to 16 consumes 17 bits and yields symbol 0.  The macros below
+ * exist so that tests/test_jpeg_extreme_cpu.py can build variants with planted mistakes and show that its comparisons catch them. */
+#ifndef JO_BAD_CODE_BITS
+#define JO_BAD_CODE_BITS 17
+#endif
 static int jo_decode_sym(jo_bits *b, const jo_huff *h) {
-  if (b->nbits < 16) jo_fill(b);
+  if (b->nbits < 17) jo_fill(b);
   int code = 0;
   for (int l = 1; l <= 16; l++) {
     code = (int)(b->acc >> (32 - l));
     if (h->maxcode[l] >= 0 && code <= h->maxcode[l] && code >= h->mincode[l]) {
-      b->acc <<= l; b->nbits -= l;
+      jo_drop(b, l);
       return h->vals[h->valptr[l] + code - h->mincode[l]];
     }
   }
-  b->acc <<= 16; b->nbits -= 16;
-  return 0;   /* corrupt stream: libjpeg also substitutes 0 */
+  jo_drop(b, JO_BAD_CODE_BITS);
+  return 0;   /* corrupt stream: libjpeg warns and substitutes 0 */
 }
 static inline int jo_extend(int v, int s) { return (s && v < (1 << (s - 1))) ? v - (1 << s) + 1 : v; }
+
+/* Whether the last jo_entropy() decoded padding bits supplied behind a marker (or the end of the data) in any unit (restart interval or
+ * whole scan): the unit ran out of data, which libjpeg answers with zeros and the GPU decoder with status 1. */
+static int jo_overrun;
+int jpeg_oracle_overrun(void) { return jo_overrun; }
 
 /* Decode all blocks of the (single, interleaved or 1-component) scan.
  * coef[c]: int16 [bh*bw][64] natural order, quantized (NOT dequantized). */
 static int jo_entropy(jo_dec *d, int16_t *coef[4]) {
   jo_info *in = &d->info;
+  jo_overrun = 0;
   if (in->progressive) return JO_ERR_UNSUPPORTED;
   if (in->precision != 8) return JO_ERR_UNSUPPORTED;
   if (d->scan_ncomp != in->ncomp) return JO_ERR_UNSUPPORTED;   /* multi-scan baseline */
   for (int i = 0; i < d->scan_ncomp; i++)
     if (!d->dc[d->td[i]].present || !d->ac[d->ta[i]].present) return JO_ERR_FORMAT;
-  jo_bits b = { d->data, d->scan_begin, d->len, 0, 0, 0 };
+  jo_bits b = { d->data, d->scan_begin, d->len, 0, 0, 0, 0, 0 };
   int pred[4] = {0, 0, 0, 0};
   int nmcu = in->mcux * in->mcuy;
   int rst_left = in->restart_interval;
   for (int m = 0; m < nmcu; m++) {
     if (in->restart_interval && rst_left == 0) {
       /* byte align, expect RSTn */
-      b.acc = 0; b.nbits = 0;
+      b.acc = 0; b.nbits = 0; b.pad = 0;
       if (!b.marker) {
         /* skip to next marker */
         while (b.pos + 1 < b.end && !(b.p[b.pos] == 0xFF && b.p[b.pos + 1] >= 0xD0 && b.p[b.pos + 1] <= 0xD7)) b.pos++;
@@ -308,82 +327,63 @@ static int jo_entropy(jo_dec *d, int16_t *coef[4]) {
               if (r == 15) { k += 16; continue; }
               break;                              /* EOB */
             }
-            k += r;
-            if (k > 63) break;                    /* corrupt */
-            blk[jo_zigzag[k]] = (int16_t)jo_extend(jo_getbits(&b, ss), ss);
+            k += r;                               /* a run past 63 (corrupt) lands on 63: jpeg_natural_order's guard entries */
+#ifdef JO_RUN_PAST_63_BREAKS
+            if (k > 63) break;
+#endif
+            blk[jo_zigzag[k > 63 ? 63 : k]] = (int16_t)jo_extend(jo_getbits(&b, ss), ss);
             k++;
           }
         }
     }
     if (in->restart_interval) rst_left--;
   }
+  jo_overrun = b.overrun;
   return JO_OK;
 }
 
-/* ---------------------------------------------------------------- islow IDCT (libjpeg jidctint) */
-#define CONST_BITS 13
-#define PASS1_BITS 2
-#define FIX_0_298631336 2446
-#define FIX_0_390180644 3196
-#define FIX_0_541196100 4433
-#define FIX_0_765366865 6270
-#define FIX_0_899976223 7373
-#define FIX_1_175875602 9633
-#define FIX_1_501321110 12299
-#define FIX_1_847759065 15137
-#define FIX_1_961570560 16069
-#define FIX_2_053119869 16819
-#define FIX_2_562915447 20995
-#define FIX_3_072711026 25172
-#define DESCALE(x, n) (((x) + (1 << ((n) - 1))) >> (n))
+/* ---------------------------------------------------------------- islow IDCT, as libjpeg-turbo's x86 SIMD kernels compute it
+ * The islow algorithm of libjpeg's jidctint.c (Loeffler-Ligtenberg-Moschytz, CONST_BITS 13, PASS1_BITS 2) in the 16-bit dataflow of
+ * jidctint-sse2 / -avx2, the IDCT cv2.imdecode runs.  On natural streams it equals the C code; they part where coefficients are far out
+ * of range (a damaged stream, a hostile encoder, 16-bit DQT):
+ *   - dequantisation keeps the low 16 bits of coef * q (pmullw);
+ *   - i0 +- i4, i7 + i3 and i5 + i1 wrap to 16 bits (paddw / psubw); the products and their sums are exact in 32 bits (pmaddwd);
+ *   - each pass's output saturates to int16 (packssdw), the result to [-128, 127] before 128 is added (packsswb);
+ *   - a block whose coefficients in rows 1..7 are all zero skips pass 1: the workspace rows are row 0 of the dequantised block shifted
+ *     left by PASS1_BITS in 16 bits (psllw), so they wrap instead of saturating.
+ * tests/jpeg_idct16.py states the same in numpy; tests/test_jpeg_extreme_cpu.py pins both against cv2. */
+static inline int jo_w16(int x) { return (int16_t)(uint16_t)(unsigned)x; }
+static inline int jo_sat16(int x) { return x < -32768 ? -32768 : x > 32767 ? 32767 : x; }
 
-static inline uint8_t jo_range_limit(int x) {
-  /* libjpeg range_limit table indexed with (x & RANGE_MASK), table centred on +128 */
-  int idx = x & 1023;
-  if (idx < 128) return (uint8_t)(idx + 128);
-  if (idx < 512) return 255;
-  if (idx < 896) return 0;
-  return (uint8_t)(idx - 896);
-}
-
+/* in[0..7]: int16 values; out: the descaled 32-bit results (the caller saturates).  No sum below leaves 32 bits for int16 inputs. */
 static void jo_idct_1d(const int in[8], int out[8], int shift) {
-  int z1, z2, z3, z4, z5, tmp0, tmp1, tmp2, tmp3, tmp10, tmp11, tmp12, tmp13;
-  z2 = in[2]; z3 = in[6];
-  z1 = (z2 + z3) * FIX_0_541196100;
-  tmp2 = z1 + z3 * (-FIX_1_847759065);
-  tmp3 = z1 + z2 * FIX_0_765366865;
-  z2 = in[0]; z3 = in[4];
-  tmp0 = (int)((unsigned)(z2 + z3) << CONST_BITS);
-  tmp1 = (int)((unsigned)(z2 - z3) << CONST_BITS);
-  tmp10 = tmp0 + tmp3; tmp13 = tmp0 - tmp3;
-  tmp11 = tmp1 + tmp2; tmp12 = tmp1 - tmp2;
-  tmp0 = in[7]; tmp1 = in[5]; tmp2 = in[3]; tmp3 = in[1];
-  z1 = tmp0 + tmp3; z2 = tmp1 + tmp2; z3 = tmp0 + tmp2; z4 = tmp1 + tmp3;
-  z5 = (z3 + z4) * FIX_1_175875602;
-  tmp0 *= FIX_0_298631336; tmp1 *= FIX_2_053119869;
-  tmp2 *= FIX_3_072711026; tmp3 *= FIX_1_501321110;
-  z1 *= -FIX_0_899976223; z2 *= -FIX_2_562915447;
-  z3 *= -FIX_1_961570560; z4 *= -FIX_0_390180644;
-  z3 += z5; z4 += z5;
-  tmp0 += z1 + z3; tmp1 += z2 + z4; tmp2 += z2 + z3; tmp3 += z1 + z4;
-  out[0] = DESCALE(tmp10 + tmp3, shift); out[7] = DESCALE(tmp10 - tmp3, shift);
-  out[1] = DESCALE(tmp11 + tmp2, shift); out[6] = DESCALE(tmp11 - tmp2, shift);
-  out[2] = DESCALE(tmp12 + tmp1, shift); out[5] = DESCALE(tmp12 - tmp1, shift);
-  out[3] = DESCALE(tmp13 + tmp0, shift); out[4] = DESCALE(tmp13 - tmp0, shift);
+  const int tmp3 = in[2] * 10703 + in[6] * 4433, tmp2 = in[2] * 4433 - in[6] * 10704;
+  const int tmp0 = jo_w16(in[0] + in[4]) * 8192, tmp1 = jo_w16(in[0] - in[4]) * 8192;
+  const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  const int z3 = jo_w16(in[7] + in[3]), z4 = jo_w16(in[5] + in[1]);
+  const int Z3 = z3 * -6436 + z4 * 9633, Z4 = z3 * 9633 + z4 * 6437;
+  const int o0 = in[7] * -4927 + in[1] * -7373 + Z3, o3 = in[7] * -7373 + in[1] * 4926 + Z4;
+  const int o1 = in[5] * -4176 + in[3] * -20995 + Z4, o2 = in[5] * -20995 + in[3] * 4177 + Z3;
+  const int r = 1 << (shift - 1);
+  out[0] = (t10 + o3 + r) >> shift; out[7] = (t10 - o3 + r) >> shift;
+  out[1] = (t11 + o2 + r) >> shift; out[6] = (t11 - o2 + r) >> shift;
+  out[2] = (t12 + o1 + r) >> shift; out[5] = (t12 - o1 + r) >> shift;
+  out[3] = (t13 + o0 + r) >> shift; out[4] = (t13 - o0 + r) >> shift;
 }
 
 static void jo_idct_block(const int16_t *coef, const uint16_t *q, uint8_t *out, int stride) {
-  int ws[64];
+  int ws[64], skip = 1;
+  for (int i = 8; i < 64; i++) skip &= coef[i] == 0;
   for (int x = 0; x < 8; x++) {               /* pass 1: columns */
     int in[8], o[8];
-    for (int y = 0; y < 8; y++) in[y] = coef[y * 8 + x] * (int)q[y * 8 + x];
-    jo_idct_1d(in, o, CONST_BITS - PASS1_BITS);
-    for (int y = 0; y < 8; y++) ws[y * 8 + x] = o[y];
+    for (int y = 0; y < 8; y++) in[y] = jo_w16(coef[y * 8 + x] * (int)q[y * 8 + x]);
+    jo_idct_1d(in, o, 11);
+    for (int y = 0; y < 8; y++) ws[y * 8 + x] = skip ? jo_w16(in[0] * 4) : jo_sat16(o[y]);
   }
   for (int y = 0; y < 8; y++) {               /* pass 2: rows */
     int o[8];
-    jo_idct_1d(ws + y * 8, o, CONST_BITS + PASS1_BITS + 3);
-    for (int x = 0; x < 8; x++) out[y * stride + x] = jo_range_limit(o[x]);
+    jo_idct_1d(ws + y * 8, o, 18);
+    for (int x = 0; x < 8; x++) out[y * stride + x] = (uint8_t)((o[x] < -128 ? -128 : o[x] > 127 ? 127 : o[x]) + 128);
   }
 }
 

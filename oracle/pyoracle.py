@@ -114,6 +114,12 @@ def jpeg_coeffs(buf):
     return [o for o in outs if o is not None]
 
 
+def jpeg_overrun():
+    """Whether the last JPEG entropy decode of the oracle (jpeg_decode, jpeg_coeffs) consumed padding bits behind a marker or the end of
+    the data in some unit: that unit ran out of data, which the GPU decoder reports as status 1."""
+    return bool(lib().jpeg_oracle_overrun())
+
+
 # ------------------------------------------------------------------------------------------- resample
 def _fd(t):
     if isinstance(t, FilterDesc):

@@ -12,17 +12,18 @@ from oracle import pyoracle as po
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
-_lib = None
+_libs = {}
 
 
-def lib():
-    global _lib
-    if _lib is None:
+def lib(defines=()):
+    """the library; `defines` (e.g. ("JO_BAD_CODE_BITS=16",)) builds a variant with planted mistakes for the tests that must catch them"""
+    defines = tuple(defines)
+    if defines not in _libs:
         out = os.path.join(tempfile.mkdtemp(prefix="jpeg_cmyk_oracle_"), "libjpegcmykoracle.so")
-        subprocess.run(["gcc", "-O2", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unused-function", "-shared",
-                        "-I" + os.path.join(_ROOT, "oracle"), os.path.join(_HERE, "jpeg_cmyk_oracle.c"), "-o", out], check=True)
-        _lib = C.CDLL(out)
-    return _lib
+        subprocess.run(["gcc", "-O2", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unused-function", "-shared"] + ["-D" + d for d in defines] +
+                       ["-I" + os.path.join(_ROOT, "oracle"), os.path.join(_HERE, "jpeg_cmyk_oracle.c"), "-o", out], check=True)
+        _libs[defines] = C.CDLL(out)
+    return _libs[defines]
 
 
 def _p(a):
@@ -48,21 +49,26 @@ def mcu_order(buf):
                      for c in range(info["ncomp"]) for v in range(vs[c]) for h in range(hs[c])])
 
 
-def _decode(buf, fancy, gray):
+def _decode(buf, fancy, gray, defines=()):
     b = np.frombuffer(bytes(buf), np.uint8)
     i = po.jpeg_info(buf)
     out = np.empty((i["height"], i["width"]) if gray else (i["height"], i["width"], 3), np.uint8)
-    rc = lib().cmyk_oracle_decode(_p(b), C.c_size_t(b.size), _p(out), int(bool(fancy)), int(bool(gray)))
+    rc = lib(defines).cmyk_oracle_decode(_p(b), C.c_size_t(b.size), _p(out), int(bool(fancy)), int(bool(gray)))
     if rc != 0:
         raise ValueError(f"cmyk_oracle_decode rc={rc}")
     return out
 
 
-def decode(buf, fancy=True):
+def decode(buf, fancy=True, defines=()):
     """[H, W, 3] RGB u8 as cv2.imdecode(..., IMREAD_COLOR)[..., ::-1] returns it."""
-    return _decode(buf, fancy, False)
+    return _decode(buf, fancy, False, defines)
 
 
-def decode_gray(buf, fancy=True):
+def decode_gray(buf, fancy=True, defines=()):
     """[H, W] u8 as cv2.imdecode(..., IMREAD_GRAYSCALE) returns it (Y plane, rgb_gray for RGB frames, CMYK -> gray for 4 components)."""
-    return _decode(buf, fancy, True)
+    return _decode(buf, fancy, True, defines)
+
+
+def overrun(defines=()):
+    """whether the last decode consumed padding behind a marker in some unit (oracle/jpeg_oracle.c jpeg_oracle_overrun)"""
+    return bool(lib(defines).jpeg_oracle_overrun())
