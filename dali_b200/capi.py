@@ -46,6 +46,8 @@ EXPORTS = [
     "dalib200SpectrogramMelSupported", "dalib200SpectrogramMelLaunch",
     "dalib200JpegDistortPlanCreate", "dalib200JpegDistortPlanDestroy", "dalib200JpegDistortPlanSetup", "dalib200JpegDistortLaunch",
     "dalib200JpegDistortDebugGetCoefficients",
+    "dalib200AudioGetInfo", "dalib200AudioPlanCreate", "dalib200AudioPlanDestroy", "dalib200AudioPlanSetup", "dalib200AudioPlanGetOutputShape",
+    "dalib200AudioLaunch", "dalib200AudioStatusAsync", "dalib200AudioStatusFetch",
 ]
 
 
@@ -122,6 +124,15 @@ class MfccArgs(C.Structure):
 
 class NormalizeArgs(C.Structure):
     _fields_ = [("mode", C.c_int32), ("ddof", C.c_int32), ("scale", C.c_float), ("shift", C.c_float), ("epsilon", C.c_float)]
+
+
+class AudioInfo(C.Structure):
+    _fields_ = [("format", C.c_int32), ("sample_rate", C.c_int32), ("channels", C.c_int32), ("bits", C.c_int32), ("is_float", C.c_int32),
+                ("length", C.c_int64)]
+
+
+class AudioParams(C.Structure):
+    _fields_ = [("downmix", C.c_int32), ("out_rate", C.c_float), ("quality", C.c_float), ("dtype", C.c_int32)]
 
 
 class DaliB200Error(RuntimeError):

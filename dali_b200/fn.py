@@ -144,6 +144,7 @@ def _install():
     # deprecated aliases kept by the reference (mixed_decoder.cc:40-50)
     if hasattr(this, "decoders"):
         this.image_decoder = this.decoders.image
+        this.audio_decoder = this.decoders.audio
 
 
 

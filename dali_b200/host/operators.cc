@@ -245,6 +245,97 @@ class ImageDecoderMixed : public ImageDecoderBase {
 };
 DALI_REGISTER_OPERATOR(decoders__Image, ImageDecoderMixed, Mixed);
 
+// =============================================================================================== decoders.audio
+// dali/operators/decoder/audio/audio_decoder_op.cc (a CPU operator over libsndfile there): a mixed operator here, decoding on the GPU.
+// Both outputs live on the GPU, so `sample_rate` is not usable as another operator's argument input (DESIGN section 2, deviations).
+DALI_SCHEMA(decoders__Audio)
+    .DocStr("Decodes WAV and FLAC audio on the GPU (FLAC: frame search, entropy decode and prediction in CUDA), with an optional "
+            "downmix to mono and resampling.  Outputs (audio, sample_rate).")
+    .NumInput(1).NumOutput(2)
+    .AddOptionalArg("sample_rate", "Target sampling rate; 0 keeps the file's rate.", 0.0f, true)
+    .AddOptionalArg("downmix", "Average all channels into one (audio of shape [T], layout \"T\").", false)
+    .AddOptionalArg("dtype", "Output type: FLOAT (default), INT16 or INT32.", DALI_FLOAT)
+    .AddOptionalArg("quality", "Resampling quality, 0 (lowest) .. 100 (highest), as AudioResample.", 50.0f);
+
+class AudioDecoderMixed : public Operator<MixedBackend> {
+ public:
+  explicit AudioDecoderMixed(const OpSpec &spec) : Operator<MixedBackend>(spec) {
+    dtype_ = spec.GetArgument<DALIDataType>("dtype");
+    DALI_ENFORCE(dtype_ == DALI_FLOAT || dtype_ == DALI_INT16 || dtype_ == DALI_INT32, "decoders.audio: dtype must be FLOAT, INT16 or INT32");
+    downmix_ = spec.GetArgument<bool>("downmix");
+    resample_ = spec.ArgumentDefined("sample_rate");
+    DALI_ENFORCE(dtype_ == DALI_FLOAT || !(downmix_ || resample_),
+                 "decoders.audio: integer output (INT16 / INT32) is not available with `downmix` or `sample_rate`");
+    quality_ = spec.GetArgument<float>("quality");
+    DALI_ENFORCE(quality_ >= 0 && quality_ <= 100, "``quality`` out of range: ", quality_, "\nValid range is [0..100].");
+    CheckStatus(dalib200AudioPlanCreate(&plan_, max_batch_size_), "decoders.audio");
+  }
+  ~AudioDecoderMixed() override { dalib200AudioPlanDestroy(plan_); }
+
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<CPUBackend>(0);
+    const int n = in.num_samples();
+    DALI_ENFORCE(in.type() == DALI_UINT8, "decoders.audio expects encoded streams as 1-D uint8 tensors");
+    std::vector<const uint8_t *> ptrs(n);
+    std::vector<size_t> lens(n);
+    std::vector<dalib200AudioParams> prm(n);
+    const int dt = dtype_ == DALI_FLOAT ? DALIB200_FLOAT : dtype_ == DALI_INT16 ? DALIB200_INT16 : DALIB200_INT32;
+    for (int i = 0; i < n; i++) {
+      ptrs[i] = in.tensor<uint8_t>(i);
+      lens[i] = static_cast<size_t>(in.shape().tensor_size(i));
+      prm[i].downmix = downmix_ ? 1 : 0;
+      prm[i].out_rate = resample_ ? spec_.GetArgument<float>("sample_rate", &ws, i) : 0.0f;
+      DALI_ENFORCE(prm[i].out_rate >= 0, "decoders.audio: sample ", i, ": the sample rate must not be negative");
+      prm[i].quality = quality_;
+      prm[i].dtype = dt;
+    }
+    CheckStatus(dalib200AudioPlanSetup(plan_, n, ptrs.data(), lens.data(), prm.data()), "decoders.audio");
+    out.resize(2);
+    out[0].type = dtype_;
+    out[0].shape.resize(n, downmix_ ? 1 : 2);
+    out[1].type = DALI_FLOAT;
+    out[1].shape.resize(n, 0);
+    for (int i = 0; i < n; i++) {
+      int64_t sh[2];
+      int32_t nd;
+      float rate;
+      CheckStatus(dalib200AudioPlanGetOutputShape(plan_, i, sh, &nd, &rate), "decoders.audio");
+      if (downmix_) out[0].shape.set_tensor_shape(i, { sh[0] });
+      else out[0].shape.set_tensor_shape(i, { sh[0], sh[1] });
+    }
+    return true;
+  }
+  void RunImpl(Workspace &ws) override {
+    auto &audio = ws.Output<GPUBackend>(0);
+    auto &rate = ws.Output<GPUBackend>(1);
+    audio.SetLayout(downmix_ ? "T" : "TC");
+    const int n = audio.num_samples();
+    std::vector<void *> op(n), rp(n);
+    for (int i = 0; i < n; i++) { op[i] = audio.raw_mutable_tensor(i); rp[i] = rate.raw_mutable_tensor(i); }
+    CheckStatus(dalib200AudioLaunch(plan_, op.data(), rp.data(), ws.stream()), "decoders.audio");
+    CheckStatus(dalib200AudioStatusAsync(plan_, ws.stream()), "decoders.audio");
+    launched_ = n;
+  }
+  void CheckCompletion() override {
+    if (launched_ <= 0) return;
+    const int n = launched_;
+    launched_ = 0;
+    std::vector<int32_t> st(n);
+    CheckStatus(dalib200AudioStatusFetch(plan_, st.data(), n), "decoders.audio");
+    for (int i = 0; i < n; i++)
+      if (st[i] != 0) throw DALIException(make_string("Failed to decode sample #", i, ": the FLAC frame chain is broken or a frame is corrupt"));
+  }
+
+ private:
+  dalib200AudioPlan *plan_ = nullptr;
+  DALIDataType dtype_ = DALI_FLOAT;
+  bool downmix_ = false, resample_ = false;
+  float quality_ = 50;
+  int launched_ = 0;
+};
+DALI_REGISTER_OPERATOR(decoders__Audio, AudioDecoderMixed, Mixed);
+
 #define DALIB200_DECODER_ARGS(schema)                                                                                         \
   schema.AddOptionalArg("output_type", "Colour space of the output image.", DALI_RGB)                                          \
       .AddOptionalArg("dtype", "Output data type.", DALI_UINT8)                                                                \

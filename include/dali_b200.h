@@ -25,7 +25,7 @@ extern "C" {
 typedef struct CUstream_st *dalib200Stream_t;   /* == cudaStream_t */
 
 /* Data type ids equal the reference's DALIDataType (include/dali/core/dali_data_type.h:44-57). */
-enum { DALIB200_UINT8 = 0, DALIB200_INT16 = 5, DALIB200_FLOAT16 = 8, DALIB200_FLOAT = 9 };
+enum { DALIB200_UINT8 = 0, DALIB200_INT16 = 5, DALIB200_INT32 = 6, DALIB200_FLOAT16 = 8, DALIB200_FLOAT = 9 };
 /* Image types equal DALIImageType (include/dali/core/common.h:156-162). */
 enum { DALIB200_RGB = 0, DALIB200_BGR = 1, DALIB200_GRAY = 2, DALIB200_YCbCr = 3 };
 /* Resampling filters equal kernels::ResamplingFilterType (dali/kernels/imgproc/resample/params.h:27-34). */
@@ -448,6 +448,43 @@ int dalib200WindowCopySetup(dalib200GenericPlan *plan, int n, const dalib200Wind
 int dalib200PadSetup(dalib200GenericPlan *plan, int n, int ndim, int elem_size, const int64_t *in_shapes,
                      const int64_t *out_shapes, const void *fill_bytes);
 int dalib200GenericLaunch(dalib200GenericPlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Audio decode (fn.decoders.audio).  WAV (PCM 8 / 16 / 24 / 32-bit, IEEE float 32, WAVE_FORMAT_EXTENSIBLE with either) and native FLAC
+ * (8 / 16 / 24 bits per sample, optional ID3v2 tag in front), detected from the bytes.  The host parses the container and STREAMINFO
+ * only; the FLAC frames are found, checked (CRC-8, CRC-16, frame chain) and decoded on the device.  Samples read as libsndfile's
+ * sf_readf_float / short / int give them; an optional downmix to mono and a resampling behind it (the AudioResample kernel).
+ * Replaces: the reference's CPU AudioDecoder (dali/operators/decoder/audio/audio_decoder_op.cc, libsndfile). */
+typedef struct dalib200AudioPlan dalib200AudioPlan;
+enum { DALIB200_AUDIO_WAV = 1, DALIB200_AUDIO_FLAC = 2 };
+typedef struct {
+  int32_t format;               /* DALIB200_AUDIO_WAV | DALIB200_AUDIO_FLAC */
+  int32_t sample_rate, channels;
+  int32_t bits;                 /* bits per sample (WAV: of the container) */
+  int32_t is_float;             /* IEEE float WAV */
+  int64_t length;               /* samples per channel */
+} dalib200AudioInfo;
+/* per-sample decode arguments: out_rate 0 keeps the file's rate; quality 0..100 as AudioResample (one value for the batch's resampled
+ * samples); dtype DALIB200_FLOAT | INT16 | INT32 (integer output: no downmix, no resampling, integer sources) */
+typedef struct { int32_t downmix; float out_rate; float quality; int32_t dtype; } dalib200AudioParams;
+
+/* header-only parse of one stream; DALIB200_ERROR_UNSUPPORTED / BAD_DATA as at plan set-up */
+int dalib200AudioGetInfo(const uint8_t *data, size_t len, dalib200AudioInfo *info);
+int dalib200AudioPlanCreate(dalib200AudioPlan **plan, int max_batch);
+int dalib200AudioPlanDestroy(dalib200AudioPlan *plan);
+/* Parses n streams (host pointers, BORROWED until dalib200AudioLaunch returns) and plans the batch.  A refused stream fails the call
+ * with its code and a message naming the sample. */
+int dalib200AudioPlanSetup(dalib200AudioPlan *plan, int n, const uint8_t *const *streams, const size_t *lengths,
+                           const dalib200AudioParams *params);
+/* shape of sample i's audio output: shape[0] = T, shape[1] = C; *ndim = 1 with downmix ([T]), 2 otherwise ([T, C]);
+ * *rate: the sample_rate output (the target rate when resampling, else the file's) */
+int dalib200AudioPlanGetOutputShape(const dalib200AudioPlan *plan, int sample, int64_t *shape, int32_t *ndim, float *rate);
+/* out_ptrs[i]: device buffer of the shape above in the sample's dtype; rate_ptrs[i]: device float scalar */
+int dalib200AudioLaunch(dalib200AudioPlan *plan, void *const *out_ptrs, void *const *rate_ptrs, dalib200Stream_t stream);
+/* per-sample status of the last launch (0 ok, 1 = the FLAC frame chain is broken or a frame is corrupt): ...Async enqueues the copy,
+ * ...Fetch reads it after the caller synchronised the stream */
+int dalib200AudioStatusAsync(dalib200AudioPlan *plan, dalib200Stream_t stream);
+int dalib200AudioStatusFetch(const dalib200AudioPlan *plan, int32_t *status_out, int n);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,7 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM and lossless JPEG kernels (and U2 / U3, which feed the last) are
+// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM, lossless JPEG and audio decode kernels (and U2 / U3, which feed the
+// lossless JPEG stage) are
 // EXECUTED on the host -- their bodies are single
 // host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h, bitmap_core.h), so a
 // launch is a loop over blocks and threads around
@@ -29,6 +30,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <vector>
 #include "../../include/dali_b200.h"
 #include "../../dali_b200/csrc/resample3d_core.h"
 #include "../../dali_b200/csrc/jpeg_prog_core.h"
@@ -38,6 +40,7 @@
 #include "../../dali_b200/csrc/bitmap_core.h"
 #include "../../dali_b200/csrc/jpeg_recon.h"
 #include "../../dali_b200/csrc/ljpeg_core.h"
+#include "../../dali_b200/csrc/audio_decode_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -145,7 +148,7 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[21];
+static long g_emulated[27];
 long emul_launch_count(int which) { return g_emulated[which]; }
 void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
@@ -460,6 +463,63 @@ static void run_ljpeg_color(void **args) {
   }
 }
 
+// audio_decode.cu: every pass over its whole index space in REVERSE order (the sync pass's atomic add is a plain one here, so the
+// candidates land in reverse byte order), with the descriptor searches the kernels make.
+static void run_flac_sync(void **args) {
+  const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
+  auto add = [](uint32_t *p, uint32_t v) { const uint32_t o = *p; *p = o + v; return o; };
+  for (int64_t g = a.flac_bytes - 1; g >= 0; g--) {
+    const int f = audio_find(a.flac, a.nf, g, &FlacDesc::first_byte);
+    flac_sync_at(a.flac[f], f, a.raw, g - a.flac[f].first_byte, a.fend, a.cand, a.ccount, add);
+  }
+}
+static void run_flac_frame(void **args) {
+  const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
+  for (int64_t k = a.cand_slots - 1; k >= 0; k--) {
+    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::cand_base);
+    flac_candidate(a.flac[f], f, a.raw, k - a.flac[f].cand_base, a.cand, a.ccount, a.fend);
+  }
+}
+static void run_flac_chain(void **args) {
+  const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
+  for (int f = a.nf - 1; f >= 0; f--)
+    if (!flac_chain(a.flac[f], f, a.raw, a.fend, a.ccount, a.frames, a.nframes)) a.status[a.flac[f].sample] = 1;
+}
+static void run_flac_decode(void **args) {
+  const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
+  for (int64_t k = a.frame_slots - 1; k >= 0; k--) {
+    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::frame_base);
+    if (!flac_decode(a.flac[f], f, a.raw, k - a.flac[f].frame_base, a.frames, a.nframes, a.pcm)) a.status[a.flac[f].sample] = 1;
+  }
+}
+static void run_audio_convert(void **args) {
+  const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
+  for (int i = a.n - 1; i >= 0; i--) *a.descs[i].rate_out = a.descs[i].rate;
+  for (int64_t e = a.total_elems - 1; e >= 0; e--) {
+    const AudioDesc &d = a.descs[audio_find(a.descs, a.n, e, &AudioDesc::first_elem)];
+    audio_convert(d, a.raw, a.pcm, e - d.first_elem, [](float x, float y) { return x * y; }, [](float x, float y) { return x + y; });
+  }
+}
+// audio_resample_kernel (audio_tail.cu) is not a host/device function: its launches are recorded, not run.  For each sample of the last
+// launch the stub keeps the descriptor's lengths and channels and a copy of its input, so that a test can check what decoders.audio hands
+// to the resampler.  The layout restates audio_tail.cu's ArDesc.
+struct EmulArDesc { const float *in; float *out; int64_t n_in, n_out, first_item; double scale; int32_t channels; };
+static std::vector<std::vector<float>> g_res_in;
+static std::vector<EmulArDesc> g_res_desc;
+static void run_audio_resample_record(void **args) {
+  const EmulArDesc *d = *static_cast<const EmulArDesc **>(args[0]);
+  const int n = *static_cast<int *>(args[1]);
+  g_res_desc.assign(d, d + n);
+  g_res_in.assign(n, {});
+  for (int i = 0; i < n; i++) g_res_in[i].assign(d[i].in, d[i].in + d[i].n_in * d[i].channels);
+}
+int emul_resample_count(void) { return (int)g_res_desc.size(); }
+// info: { n_in, n_out, channels }; copies the input (n_in * channels floats) to dst when dst is not NULL
+void emul_resample_sample(int i, int64_t *info, float *dst) {
+  info[0] = g_res_desc[i].n_in; info[1] = g_res_desc[i].n_out; info[2] = g_res_desc[i].channels;
+  if (dst) memcpy(dst, g_res_in[i].data(), g_res_in[i].size() * sizeof(float));
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *stream) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -487,6 +547,12 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_ljpeg_write = !strcmp(name, "_ZN8dalib20018ljpeg_write_kernelENS_11LjpegLaunchE");
   const bool is_ljpeg_recon = !strcmp(name, "_ZN8dalib20018ljpeg_recon_kernelEPKNS_10LjpegImageEPKNS_9LjpegBandEPs");
   const bool is_ljpeg_color = !strcmp(name, "_ZN8dalib20018ljpeg_color_kernelEPKNS_10LjpegImageEilPKs");
+  const bool is_flac_sync = !strcmp(name, "_ZN8dalib20016flac_sync_kernelENS_11AudioLaunchE");
+  const bool is_flac_frame = !strcmp(name, "_ZN8dalib20017flac_frame_kernelENS_11AudioLaunchEi");
+  const bool is_flac_chain = !strcmp(name, "_ZN8dalib20017flac_chain_kernelENS_11AudioLaunchE");
+  const bool is_flac_decode = !strcmp(name, "_ZN8dalib20018flac_decode_kernelENS_11AudioLaunchEi");
+  const bool is_audio_convert = !strcmp(name, "_ZN8dalib20020audio_convert_kernelENS_11AudioLaunchE");
+  const bool is_audio_resample = !strcmp(name, "_ZN8dalib20021audio_resample_kernelEPKNS_6ArDescEilNS_8ArWindowE");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -513,6 +579,12 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_ljpeg_write) { run_ljpeg_write(args); g_emulated[17]++; }
   else if (is_ljpeg_recon) { run_ljpeg_recon(grid, args); g_emulated[18]++; }
   else if (is_ljpeg_color) { run_ljpeg_color(args); g_emulated[19]++; }
+  else if (is_flac_sync) { run_flac_sync(args); g_emulated[21]++; }
+  else if (is_flac_frame) { run_flac_frame(args); g_emulated[22]++; }
+  else if (is_flac_chain) { run_flac_chain(args); g_emulated[23]++; }
+  else if (is_flac_decode) { run_flac_decode(args); g_emulated[24]++; }
+  else if (is_audio_convert) { run_audio_convert(args); g_emulated[25]++; }
+  else if (is_audio_resample) { run_audio_resample_record(args); g_emulated[26]++; }
   return 0;
 }
 }  // extern "C"

@@ -43,6 +43,14 @@ seeds += [bytearray(s) for n, s in bitmap_streams.corpus() if len(s) < 100000][:
 # table build and the split at the restart markers of ljpeg_plan.h
 import ljpeg_streams
 seeds += [bytearray(s) for n, s, _, _ in ljpeg_streams.corpus() if len(s) < 100000][::5]
+# WAV and FLAC streams (every format the corpus holds, the refused and the corrupt ones): the container parse, plan set-up and the
+# launch-side staging and descriptor build of decoders.audio (audio_decode_plan.h, dalib200AudioPlanSetup / dalib200AudioLaunch)
+import audio_streams
+audio_seeds = [bytearray(s) for _, s, _, _ in audio_streams.corpus() if len(s) < 60000] + \
+    [bytearray(s) for _, s, _, _ in audio_streams.refused()] + [bytearray(s) for _, s in audio_streams.corrupt()]
+audio_plan = C.c_void_p()
+assert L.dalib200AudioPlanCreate(C.byref(audio_plan), 4) == 0, L.dalib200GetLastError()
+ainfo = (C.c_int32 * 8)()
 info = (C.c_int32 * 32)()
 plan = C.c_void_p()
 assert L.dalib200JpegPlanCreate(C.byref(plan), 4) == 0, L.dalib200GetLastError()
@@ -95,4 +103,34 @@ for it in range(n):
             rc2 = L.dalib200JpegLaunch(plan, outs, None)
         rcs["launch", rc2] = rcs.get(("launch", rc2), 0) + 1
     rcs[rc] = rcs.get(rc, 0) + 1
+    # an audio batch: RIFF chunk sizes, fmt fields, ID3 sizes, metadata block headers and STREAMINFO fields mutated like the above
+    abatch = []
+    for b in range(int(rng.integers(1, 4))):
+        s = bytearray(audio_seeds[int(rng.integers(0, len(audio_seeds)))])
+        k = int(rng.integers(0, 4))
+        if k == 0:
+            for _ in range(rng.integers(1, 6)): s[rng.integers(0, min(len(s), 120))] = rng.integers(0, 256)
+        elif k == 1:
+            s = s[:rng.integers(0, len(s))]
+        elif k == 2:
+            p = rng.integers(0, len(s)); s[p:p] = bytes(rng.integers(0, 256, rng.integers(1, 9)).astype(np.uint8))
+        abatch.append(bytes(s) if len(s) else b"\0")
+    abufs = [(C.c_uint8 * len(s)).from_buffer_copy(s) for s in abatch]
+    aptrs = (C.c_void_p * len(abufs))(*[C.addressof(b) for b in abufs])
+    alens = (C.c_size_t * len(abufs))(*[len(s) for s in abatch])
+    aprm = (C.c_int32 * (4 * len(abufs)))()
+    for b in range(len(abufs)):
+        L.dalib200AudioGetInfo(abufs[b], C.c_size_t(len(abatch[b])), ainfo)
+        rate = float(rng.choice([0.0, 16000.0, 8000.5, -1.0]))
+        aprm[4 * b:4 * b + 4] = [int(rng.integers(0, 2)), C.c_int32.from_buffer(C.c_float(rate)).value, C.c_int32.from_buffer(C.c_float(50.0)).value,
+                                 int(rng.choice([9, 5, 6, 1]))]
+    rc = L.dalib200AudioPlanSetup(audio_plan, len(abufs), aptrs, alens, aprm)
+    if rc == 0:
+        shape, nd, r = (C.c_int64 * 2)(), C.c_int32(), C.c_float()
+        for b in range(len(abufs)):
+            L.dalib200AudioPlanGetOutputShape(audio_plan, b, shape, C.byref(nd), C.byref(r))
+        outs = (C.c_void_p * len(abufs))(*[0x10000 * (b + 1) for b in range(len(abufs))])       # never dereferenced on the host
+        rc2 = L.dalib200AudioLaunch(audio_plan, outs, outs, None)
+        rcs["audio launch", rc2] = rcs.get(("audio launch", rc2), 0) + 1
+    rcs["audio", rc] = rcs.get(("audio", rc), 0) + 1
 print("seed", sys.argv[2] if len(sys.argv) > 2 else 0, "iterations", n, "status histogram", rcs, "- no sanitizer report")

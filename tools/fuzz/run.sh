@@ -4,6 +4,7 @@
 # are built with -fsanitize=address and the handful of CUDA runtime calls the host side makes are replaced by a preloaded stub
 # (cuda_stub.c: events = no-ops, pinned / device allocations = malloc, so that ASAN's red zones surround them).
 # Inputs: valid baseline and progressive streams (4:2:0 / 4:4:4 / 4:2:2 / gray / CMYK / YCCK, restart intervals, EXIF orientations), PNG, TIFF, WebP, BMP and PNM streams with byte flips, truncation,
+# and WAV / FLAC streams through the audio decoder's container parse, plan set-up and launch-side staging (dalib200Audio*),
 # corrupted segment lengths, wrapping EXIF offsets, inserted / deleted bytes, markers sprinkled into the entropy data.
 # A finding is an ASAN report on stderr (non-zero exit).
 set -e
@@ -19,7 +20,9 @@ $NVCC $F -c "$ROOT/dali_b200/csrc/tiff.cu" -o "$OUT/tiff.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/webp.cu" -o "$OUT/webp.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/bitmap.cu" -o "$OUT/bitmap.o"
 $NVCC $F -c "$ROOT/dali_b200/csrc/ljpeg.cu" -o "$OUT/ljpeg.o"
-$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" "$OUT/bitmap.o" "$OUT/ljpeg.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
+$NVCC $F -c "$ROOT/dali_b200/csrc/audio_decode.cu" -o "$OUT/audio_decode.o"
+$NVCC $F -c "$ROOT/dali_b200/csrc/audio_tail.cu" -o "$OUT/audio_tail.o"
+$NVCC -shared -o "$OUT/libfuzz.so" "$OUT/jpeg.o" "$OUT/common.o" "$OUT/jpeg_prog.o" "$OUT/png.o" "$OUT/tiff.o" "$OUT/webp.o" "$OUT/bitmap.o" "$OUT/ljpeg.o" "$OUT/audio_decode.o" "$OUT/audio_tail.o" -gencode arch=compute_90a,code=sm_90a -lcudart -Xcompiler -fsanitize=address
 gcc -shared -fPIC -O1 -o "$OUT/cuda_stub.so" "$HERE/cuda_stub.c"
 # the progressive scan decoder itself (the body of prog_scan_kernel, compiled for the host by tools/emul) under ASAN + UBSAN on mutated
 # progressive streams: garbage Huffman codes, runs past the band, truncated scans, markers inside the data must stay inside the arena
