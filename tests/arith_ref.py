@@ -1,7 +1,8 @@
 """numpy statement of the arithmetic-expression rules (DESIGN.md section 2, "Arithmetic expressions and fn.cast").  The reference's
 source is not available here, so this file IS the statement for type promotion, result types, integer corner cases and ConvertSat;
 tests/test_arith_cpu.py pins it against numpy wherever numpy agrees, and the host build of the kernel bodies (tools/emul/arith_emul.cc)
-and the GPU (tests/test_gpu_arith.py) are checked against it bit for bit, the transcendentals within ULP bounds.
+and the GPU (tests/test_gpu_arith.py, tests/test_gpu_arith_shapes.py) are checked against it bit for bit, the transcendentals within
+ULP bounds.
 
 Types are DALIDataType ids.  Every node is computed in its own type: integers wrap, a BOOL result is "value != 0", FLOAT16 nodes are
 computed in float32 and rounded to binary16 (to nearest even) after every operator."""
@@ -244,6 +245,157 @@ def same_bits(got, want):
         both_nan = np.isnan(got) & np.isnan(want)
         return bool(np.all(both_nan | (got.view(np.dtype(f"u{got.itemsize}")) == want.view(np.dtype(f"u{want.itemsize}")))))
     return bool(np.array_equal(got, want))
+
+
+def _transcendental(op, ct):
+    return not op.startswith("cast_") and (op not in EXACT or (op == "pow" and ct in FLOATS))
+
+
+# CUDA C Programming Guide, "Mathematical Functions" appendix: maximum ULP errors (float / double), without fast math
+ULP32 = {"cbrt": 1, "exp": 2, "log": 1, "log2": 1, "log10": 2, "sin": 2, "cos": 2, "tan": 4, "asin": 2, "acos": 2, "atan": 2,
+         "sinh": 3, "cosh": 2, "tanh": 2, "asinh": 3, "acosh": 4, "atanh": 3, "pow": 4, "fpow": 4, "atan2": 3}
+ULP64 = {"cbrt": 1, "exp": 1, "log": 1, "log2": 1, "log10": 1, "sin": 2, "cos": 2, "tan": 2, "asin": 2, "acos": 2, "atan": 2,
+         "sinh": 2, "cosh": 1, "tanh": 1, "asinh": 2, "acosh": 2, "atanh": 2, "pow": 2, "fpow": 2, "atan2": 2}
+
+
+def check(op, got, xs, types, ulp=None):
+    """got is op applied to xs: bit for bit where the result is exact, else within the ULP bound of a float64 evaluation (ULP32 /
+    ULP64 by default, `ulp` when given; FLOAT16 within 1; FLOAT64 one more for the float64 reference's own rounding)."""
+    rt = result_type(op, types)
+    want = evaluate(op, xs, types)
+    assert got.dtype == want.dtype and got.shape == want.shape, (op, types, got.dtype, want.dtype, got.shape, want.shape)
+    ct = compute_type(op, types)
+    if not _transcendental(op, ct):
+        assert same_bits(got, want), (op, [NAMES[t] for t in types], np.argwhere(~((got == want) | (want != want)))[:4])
+        return
+    ys = [cvt(np.asarray(x, NP[t]), t, ct).astype(np.float64) for x, t in zip(xs, types)]
+    with np.errstate(all="ignore"):
+        ref = _float_op(op, ys, np.float64)
+    if rt == F16:
+        bound = 1.0
+    elif ulp is not None:
+        bound = ulp + (rt == F64)
+    else:
+        bound = ULP64[op] + 1 if rt == F64 else ULP32[op]
+    err = ulp_error(got, ref, rt)
+    assert np.all(err <= bound), (op, [NAMES[t] for t in types], float(np.max(err)), bound)
+
+
+# ---- expression trees: ("add", ("mul", 0, 1), 2) is add(mul(&0 &1) &2); a leaf k is input k
+def tree_desc(tree):
+    if isinstance(tree, int):
+        return f"&{tree}"
+    return f"{tree[0]}({' '.join(tree_desc(t) for t in tree[1:])})"
+
+
+def tree_type(tree, types):
+    return types[tree] if isinstance(tree, int) else result_type(tree[0], [tree_type(t, types) for t in tree[1:]])
+
+
+def tree_eval(tree, xs, types):
+    """(value, type) of the tree over the operand arrays xs, every node evaluated by evaluate() (numpy broadcasting)."""
+    if isinstance(tree, int):
+        return np.asarray(xs[tree], NP[types[tree]]), types[tree]
+    kids = [tree_eval(t, xs, types) for t in tree[1:]]
+    op = tree[0]
+    tt = [t for _, t in kids]
+    return evaluate(op, [v for v, _ in kids], tt), result_type(op, tt)
+
+
+def tree_check(tree, got, xs, types, ulp=None):
+    """got is the tree over xs: its operands evaluated exactly, the root held to check() (so a transcendental root is bounded)."""
+    if isinstance(tree, int):
+        assert same_bits(got, np.asarray(xs[tree], NP[types[tree]]))
+        return
+    kids = [tree_eval(t, xs, types) for t in tree[1:]]
+    check(tree[0], got, [v for v, _ in kids], [t for _, t in kids], ulp)
+
+
+def _rand(t, shape, rng):
+    return random_values(t, int(np.prod(shape, dtype=np.int64)), rng).reshape(shape)
+
+
+def _ones_at(shape, mask):
+    """shape with the axes in bit mask `mask` (bit a: axis a) set to 1"""
+    return tuple(1 if (mask >> a) & 1 else e for a, e in enumerate(shape))
+
+
+# sample volumes around the kernel's 4-element threads and 8192-element work items
+VOLUMES = (1, 3, 4, 5, 8191, 8192, 8193, 3 * 8192 + 5)
+
+
+def shape_cases(rng, big=False):
+    """[(name, tree, types, scalar flags, samples)]: expressions whose result depends on the operands' shapes rather than their types.
+    samples[i][k] is operand k of sample i (a 0-d array for a per-sample scalar).  Every operator is exact except the root of the
+    atan2 case.  big: the float cases also get a 1080p x 3 sample (the integer reference loops in Python)."""
+    cases = []
+    # ranks 0-6: a full operand, one with random unit axes, one of lower rank (the trailing half of the axes)
+    for r in range(7):
+        samples = []
+        for _ in range(3):
+            s = tuple(int(v) for v in rng.integers(1, 5 if r < 5 else 4, r))
+            samples.append([_rand(I16, s, rng), _rand(F32, _ones_at(s, int(rng.integers(0, 1 << r))), rng),
+                            _rand(U8, s[r - r // 2:], rng)])
+        cases.append((f"rank {r}", ("mul", ("add", 0, 1), 2), [I16, F32, U8], None, samples))
+    # operands of lower rank than the output, each broadcast along the leading axes
+    cases.append(("lower ranks", ("add", ("add", ("mul", 0, 1), 2), 3), [U16, I32, U8, I8], None,
+                  [[_rand(U16, (2, 3, 4, 5), rng), _rand(I32, (5,), rng), _rand(U8, (4, 1), rng), _rand(I8, (3, 1, 1), rng)],
+                   [_rand(U16, (1, 2, 7, 3), rng), _rand(I32, (1,), rng), _rand(U8, (7, 3), rng), _rand(I8, (2, 1, 3), rng)]]))
+    # two-way broadcasts: neither operand has the output's shape
+    hw = [(5, 7), (1, 9), (6, 1), (1, 1), (33, 130)]
+    cases.append(("(H, 1) + (1, W)", ("add", 0, 1), [F32, F32], None, [[_rand(F32, (h, 1), rng), _rand(F32, (1, w), rng)] for h, w in hw]))
+    cases.append(("(H, 1) - (1, W) u8", ("sub", 0, 1), [U8, U8], None, [[_rand(U8, (h, 1), rng), _rand(U8, (1, w), rng)] for h, w in hw]))
+    fhwc = [(3, 4, 5, 3), (1, 9, 2, 1), (2, 1, 1, 4), (4, 6, 7, 2)]
+    cases.append(("(F, 1, W, 1) * (1, H, 1, C)", ("mul", 0, 1), [F16, F16], None,
+                  [[_rand(F16, (f, 1, w, 1), rng), _rand(F16, (1, h, 1, c), rng)] for f, h, w, c in fhwc]))
+    # size-1 output axes
+    cases.append(("size-1 output axes", ("sub", 0, 1), [I32, I32], None,
+                  [[_rand(I32, (4, 1, 5), rng), _rand(I32, (4, 1, 1), rng)], [_rand(I32, (1, 1, 1), rng), _rand(I32, (1, 1, 1), rng)],
+                   [_rand(I32, (1, 1, 9), rng), _rand(I32, (1, 1, 9), rng)], [_rand(I32, (3, 1, 1), rng), _rand(I32, (1, 1, 1), rng)]]))
+    # every subset of broadcast axes at rank 4, one subset per sample: x broadcasts the subset, y its complement, z is full
+    full = (3, 2, 5, 4)
+    cases.append(("rank-4 broadcast subsets", ("sub", ("mul", 0, 1), 2), [F32, F32, F32], None,
+                  [[_rand(F32, _ones_at(full, m), rng), _rand(F32, _ones_at(full, 15 & ~m), rng), _rand(F32, full, rng)]
+                   for m in range(16)]))
+    # 16 tensor operands over 6 axes, each broadcasting a different subset: the whole stride table
+    masks = [0, 1, 2, 4, 8, 16, 32, 63, 5, 10, 20, 40, 21, 42, 7, 56]
+    ops = ("add", "mul", "bitxor", "sub")
+    tree = 0
+    for k in range(1, 16):
+        tree = (ops[k % 4], tree, k)
+    samples = []
+    for j, shape in enumerate([(3, 2, 4, 3, 2, 5), (2, 3, 2, 5, 3, 2)]):
+        samples.append([_rand(I32, _ones_at(shape, masks[(k + j) % 16]), rng) for k in range(16)])
+    cases.append(("16 operands, 6 axes", tree, [I32] * 16, None, samples))
+    # the same input broadcasts in some samples and not in others
+    cases.append(("per-sample operand shapes", ("add", ("mul", 0, 1), 2), [U8, U8, I16], None,
+                  [[_rand(U8, (4, 3), rng), _rand(U8, s1, rng), _rand(I16, s2, rng)]
+                   for s1, s2 in (((4, 3), (3,)), ((1, 3), (1,)), ((4, 1), (3,)), ((1, 1), (1,)))]))
+    # per-sample scalars (read on the host) between broadcast tensors, narrow and wide
+    cases.append(("scalars and broadcasts", ("min", ("mul", ("sub", 0, 2), 1), 3), [F32, I32, F32, F32], [0, 1, 0, 1],
+                  [[_rand(F32, (h, 4), rng), _rand(I32, (), rng), _rand(F32, (1, 4), rng), _rand(F32, (), rng)] for h in (5, 1, 3)]))
+    cases.append(("scalars and broadcasts, 64-bit", ("add", ("mul", 0, 1), 2), [U16, I64, U8], [0, 1, 0],
+                  [[_rand(U16, (h, 5), rng), _rand(I64, (), rng), _rand(U8, (5,), rng)] for h in (4, 1, 2)]))
+    # empty samples (an extent of 0 broadcast against 1) between non-empty ones
+    pairs = [((3, 4), (1, 4)), ((0, 4), (1, 4)), ((5, 1), (1, 0)), ((2, 3), (2, 1)), ((0, 1), (1, 0)), ((1, 1), (1, 1)), ((0, 0), (0, 1)),
+             ((7, 9), (7, 9))]
+    cases.append(("empty samples", ("add", 0, 1), [U8, F32], None, [[_rand(U8, a, rng), _rand(F32, b, rng)] for a, b in pairs]))
+    cases.append(("all 0-d", ("fdiv", ("add", 0, 1), 1), [F64, F64], None, [[_rand(F64, (), rng), _rand(F64, (), rng)] for _ in range(5)]))
+    cases.append(("every sample empty", ("add", 0, 1), [I16, I16], None,
+                  [[_rand(I16, a, rng), _rand(I16, b, rng)] for a, b in (((0, 3), (1, 3)), ((4, 0), (4, 1)), ((0, 0), (1, 1)))]))
+    # sample volumes around the 4-element threads and the work items, every element size, both value files, the FLOAT fast path
+    # and the generic path; a linear pair beside a broadcast third operand
+    for name, tree, types in (("u8", ("sub", ("add", 0, 1), 2), [U8] * 3), ("i16", ("sub", ("add", 0, 1), 2), [I16] * 3),
+                              ("f16", ("sub", ("add", 0, 1), 2), [F16] * 3), ("f32", ("sub", ("mul", 0, 1), 2), [F32] * 3),
+                              ("i32", ("sub", ("mul", 0, 1), 2), [I32] * 3), ("f64", ("sub", ("add", 0, 1), 2), [F64] * 3),
+                              ("i64", ("sub", ("mul", 0, 1), 2), [I64] * 3), ("bool", ("lt", ("add", 0, 2), 1), [U8] * 3),
+                              ("narrow", ("cast_int32", ("add", 0, ("mul", 1, 2))), [I32] * 3),
+                              ("wide", ("cast_int32", ("add", 0, ("mul", 1, 2))), [I32, I64, I32]),
+                              ("atan2", ("atan2", ("add", 0, 2), 1), [F32] * 3)):
+        vs = VOLUMES + ((1080 * 1920 * 3,) if big and types[0] in FLOATS else ())
+        cases.append((f"volumes {name}", tree, types, None,
+                      [[_rand(types[0], (v,), rng), _rand(types[1], (v,), rng), _rand(types[2], (1,), rng)] for v in vs]))
+    return cases
 
 
 def ulp_error(got, ref64, t):

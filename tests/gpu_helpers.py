@@ -17,6 +17,52 @@ def to_dev(arrs):
     return [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in arrs]
 
 
+SENTINEL = 0xA5
+
+
+def byte_positions(sizes, aligns, offsets=None, packed=False):
+    """Byte positions of buffers inside one allocation: back to back, each at its alignment, when packed; else each `offsets[k]`
+    bytes past a 256-byte boundary with 16 spare bytes behind it.  Returns (positions, allocation size)."""
+    pos, cur = [], 0
+    for k, (nb, al) in enumerate(zip(sizes, aligns)):
+        p = -(-cur // al) * al if packed else -(-cur // 256) * 256 + (offsets[k] if offsets else 0)
+        pos.append(p)
+        cur = p + nb + (0 if packed else 16)
+    return pos, cur + 256
+
+
+def upload_slices(arrays, offsets=None, packed=False):
+    """The arrays copied into one device allocation at byte_positions(); returns (the allocation, device pointer of each array)."""
+    arrays = [np.ascontiguousarray(a) for a in arrays]
+    pos, total = byte_positions([a.nbytes for a in arrays], [a.itemsize for a in arrays], offsets, packed)
+    host = np.zeros(total, np.uint8)
+    for a, p in zip(arrays, pos):
+        host[p:p + a.nbytes] = a.reshape(-1).view(np.uint8)
+    dev = _torch().from_numpy(host).cuda()
+    return dev, [dev.data_ptr() + p for p in pos]
+
+
+class SentinelSlices:
+    """Output buffers of the given byte sizes inside one device allocation filled with SENTINEL; read() returns their bytes and
+    asserts that every byte outside them still holds SENTINEL (an element written past its sample, or into a gap)."""
+
+    def __init__(self, sizes, itemsize, offsets=None, packed=False):
+        self.sizes = list(sizes)
+        self.pos, total = byte_positions(self.sizes, [itemsize] * len(self.sizes), offsets, packed)
+        self.dev = _torch().from_numpy(np.full(total, SENTINEL, np.uint8)).cuda()
+        self.ptrs = [self.dev.data_ptr() + p for p in self.pos]
+
+    def read(self, what=""):
+        _torch().cuda.synchronize()
+        got = self.dev.cpu().numpy()
+        inside = np.zeros(got.size, bool)
+        for p, nb in zip(self.pos, self.sizes):
+            inside[p:p + nb] = True
+        stray = np.flatnonzero(~inside)[got[~inside] != SENTINEL]
+        assert stray.size == 0, (what, "bytes written outside the outputs at", stray[:8])
+        return [got[p:p + nb].copy() for p, nb in zip(self.pos, self.sizes)]
+
+
 def cmn(imgs, anchors, crops, mirrors, mean, inv_std, out_dtype=np.float32, layout="CHW", out_channels=None, fill=None, plan=None):
     torch = _torch()
     n = len(imgs)

@@ -3,8 +3,10 @@
   * the Python graph building: the expression_desc strings, fusion and materialisation, constants, device rules and refusals;
   * the planner and the kernel bodies compiled for the host (tools/emul/arith_emul.cc): every operator over every type pair of the
     12 types on edge and random values, bit for bit against arith_ref.py (transcendentals within ULP bounds of a float64
-    evaluation), broadcasting, fn.cast against pointwise_ref's ConvertSat, the planner's limits and refusals, and mutated
-    descriptions under ASan + UBSan."""
+    evaluation), broadcasting, the shape edges of arith_ref.shape_cases (ranks 0-6, broadcast patterns up to 16 operands, empty and
+    0-d samples, volumes around the threads and work items) with operands and outputs at unaligned offsets and every output checked
+    for stray writes, fn.cast against pointwise_ref's ConvertSat, the planner's limits and refusals, and mutated descriptions under
+    ASan + UBSan."""
 import ctypes as C
 import os
 import shutil
@@ -181,11 +183,23 @@ def emul(tmp_path_factory):
     return C.CDLL(so)
 
 
-def run(lib, desc, xs, types, scalar=None, ints=(), reals=()):
-    """Evaluates desc over one sample per entry of xs (a list of per-sample input lists); returns (outputs, error)."""
+def _at(x, off):
+    """a copy of x starting `off` bytes past a 64-byte boundary"""
+    x = np.asarray(x)
+    buf = np.zeros(x.nbytes + off + 64, np.uint8)
+    start = (-buf.ctypes.data) % 64 + off
+    y = buf[start:start + x.nbytes].view(x.dtype).reshape(x.shape)
+    y[...] = x
+    return y
+
+
+def run(lib, desc, xs, types, scalar=None, ints=(), reals=(), out_offset=0):
+    """Evaluates desc over one sample per entry of xs (a list of per-sample input lists); returns (outputs, error).  Each output is
+    written `out_offset` bytes past a 64-byte boundary of a buffer filled with 0xA5, whose bytes around the output must stay so."""
     nin = len(types)
     n = len(xs)
-    arrs = [[np.ascontiguousarray(np.asarray(x, ar.NP[t])) for x, t in zip(sample, types)] for sample in xs]
+    arrs = [[np.asarray(x, ar.NP[t]) for x, t in zip(sample, types)] for sample in xs]
+    arrs = [[a if a.flags.c_contiguous else a.copy() for a in sample] for sample in arrs]
     ndims = (C.c_int32 * max(nin, 1))(*[arrs[0][k].ndim if not (scalar and scalar[k]) else 0 for k in range(nin)])
     shp = (C.c_int64 * (n * nin * 6 or 1))()
     for i in range(n):
@@ -202,29 +216,26 @@ def run(lib, desc, xs, types, scalar=None, ints=(), reals=()):
     args = (desc.encode(), nin, tv, sc, iv, len(ints), rv, len(reals), n, ndims, shp, ptrs)
     if lib.emul_arith(*args, None, osh, C.byref(ond), C.byref(ot), err, 1024):
         return None, err.value.decode()
-    outs = [np.zeros(tuple(osh[i * 6 + a] for a in range(ond.value)), ar.NP[ot.value]) for i in range(n)]
+    dt = np.dtype(ar.NP[ot.value])
+    outs, bufs, starts = [], [], []
+    for i in range(n):
+        shape = tuple(osh[i * 6 + a] for a in range(ond.value))
+        nbytes = int(np.prod(shape, dtype=np.int64)) * dt.itemsize
+        bufs.append(np.full(nbytes + out_offset + 128, 0xA5, np.uint8))
+        starts.append((-bufs[i].ctypes.data) % 64 + out_offset)
+        outs.append(bufs[i][starts[i]:starts[i] + nbytes].view(dt).reshape(shape))
     op = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
     assert lib.emul_arith(*args, op, osh, C.byref(ond), C.byref(ot), err, 1024) == 0
-    return outs, None
+    for i, (o, b, s) in enumerate(zip(outs, bufs, starts)):
+        assert np.all(b[:s] == 0xA5) and np.all(b[s + o.nbytes:] == 0xA5), ("written outside the output", desc, i)
+    return [o.copy() for o in outs], None
 
 
 ULP_HOST = 4          # glibc's float math functions against a float64 evaluation (FLOAT64: one more for the reference's own rounding)
 
 
 def _check(op, got, xs, types):
-    want = ar.evaluate(op, xs, types)
-    assert got.dtype == want.dtype and got.shape == want.shape, (op, types)
-    ct = ar.compute_type(op, types)
-    if op in ar.EXACT and not (op == "pow" and ct in ar.FLOATS):
-        assert ar.same_bits(got, want), (op, [ar.NAMES[t] for t in types])
-        return
-    ys = [ar.cvt(np.asarray(x, ar.NP[t]), t, ct).astype(np.float64) for x, t in zip(xs, types)]
-    with np.errstate(all="ignore"):
-        ref = ar._float_op(op, ys, np.float64)
-    rt = ar.result_type(op, types)
-    bound = 1 if rt == ar.F16 else ULP_HOST + (rt == ar.F64)
-    err = ar.ulp_error(got, ref, rt)
-    assert np.all(err <= bound), (op, [ar.NAMES[t] for t in types], float(np.max(err)))
+    ar.check(op, got, xs, types, ULP_HOST)
 
 
 def test_every_op_every_type_pair_bit_exact(emul):
@@ -286,6 +297,36 @@ def test_broadcasting_scalars_and_errors(emul):
     # shapes that do not broadcast: the sample and both shapes are named
     _, e = run(emul, "add(&0 &1)", [[np.zeros((4, 3)), np.zeros((4, 3))], [np.zeros((5, 3)), np.zeros((2, 3))]], [ar.F32, ar.F32])
     assert "sample 1" in e and "(5, 3)" in e and "(2, 3)" in e, e
+
+
+def test_shapes_broadcasts_empty_samples_and_boundaries(emul):
+    """arith_ref.shape_cases through the planner and the kernel bodies: ranks 0-6, lower-rank operands, two-way broadcasts, size-1
+    output axes, every subset of broadcast axes at rank 4, 16 operands filling the whole stride table, operand shapes that change
+    from sample to sample, per-sample scalars, empty and 0-d samples, and volumes around the 4-element threads and 8192-element work
+    items for every output element size, both value files, the FLOAT fast path and the generic one."""
+    for name, tree, types, scalar, samples in ar.shape_cases(np.random.default_rng(15)):
+        outs, e = run(emul, ar.tree_desc(tree), samples, types, scalar=scalar)
+        assert e is None, (name, e)
+        for i, s in enumerate(samples):
+            want_shape = np.broadcast_shapes(*[x.shape for k, x in enumerate(s) if not (scalar and scalar[k])])
+            assert outs[i].shape == want_shape, (name, i, outs[i].shape, want_shape)
+            ar.tree_check(tree, outs[i], s, types, ULP_HOST)
+
+
+def test_unaligned_operands_and_outputs(emul):
+    """Operands and outputs that break the vector alignment of their element size (the element-by-element branch), next to aligned
+    ones, for every element size; the broadcast operand stays aligned."""
+    rng = np.random.default_rng(16)
+    for name, tree, types, scalar, samples in ar.shape_cases(rng):
+        if not name.startswith("volumes"):
+            continue
+        out_size = np.dtype(ar.NP[ar.tree_type(tree, types)]).itemsize
+        for in_step, out_step in ((1, 0), (0, 1), (1, 2), (3, 3)):
+            moved = [[_at(x, in_step * x.itemsize) if k < 2 else x for k, x in enumerate(s)] for s in samples]
+            outs, e = run(emul, ar.tree_desc(tree), moved, types, scalar=scalar, out_offset=out_step * out_size)
+            assert e is None, (name, e)
+            for i, s in enumerate(samples):
+                ar.tree_check(tree, outs[i], s, types, ULP_HOST)
 
 
 @pytest.mark.parametrize("desc,msg", [

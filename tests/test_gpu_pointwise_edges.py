@@ -2,6 +2,10 @@
   * multiply_add_kernel (fn.brightness_contrast): sizes around the 8192-element work items and the 4-element quads, a batch whose
     grid loops, unaligned pointers (the scalar branch), exact halves, saturation, the default contrast_center, float output,
     sequences -- against the float32 form of tests/pointwise_ref.py;
+  * linear_transform_kernel (fn.hsv, fn.color_twist) and csc_kernel (fn.color_space_conversion): pixel counts around the quads and
+    the 16-pixel vector groups, inputs and outputs at every byte offset, 3000 packed samples with empty ones first and last, every
+    colour-space pair, outputs in an allocation filled with a sentinel whose bytes outside them must stay unchanged -- against the
+    oracle bit for bit and the float64 statements of tests/image_f64.py;
   * jpeg_post_kernel (orientation + ROI + output type + dtype): one plan holding every source kind, all EXIF orientations, ROIs
     touching each edge, 1-pixel windows and a 1x1 image, tiny samples between large ones -- against the u8 RGB / GRAY decode of the
     same streams, oriented and cut in numpy, then converted by tests/pointwise_ref.py;
@@ -134,7 +138,123 @@ def test_brightness_contrast_sequences_and_contrast_center():
         _assert_bc(np.asarray(c[i]), s, (1.1, 0.0, 0.6, 128.0), True, ("float", i))
 
 
-# ------------------------------------------------------------------------------------------------------------- decoder post pass
+# ------------------------------------------------------------------------------------------------------------- colour kernels
+PIXELS = (0, 1, 3, 4, 5, 15, 16, 17, 4095, 4096, 4097, 1080 * 1920)
+
+
+def _pointwise_launch(setup, ins, out_sizes, out_itemsize, in_offs=None, out_offs=None, packed=False, what=""):
+    """setup(plan) (LinearTransformSetup / ColorSpaceSetup) then PointwiseLaunch over the u8 inputs, laid out in one device
+    allocation (gpu_helpers.upload_slices), into outputs of out_sizes bytes in one allocation filled with the sentinel; returns the
+    outputs' bytes after checking that nothing outside them was written."""
+    import gpu_helpers as g
+    plan = capi.Plan("Pointwise", max(len(ins), 1))
+    setup(plan)
+    din, in_ptrs = g.upload_slices(ins, in_offs, packed)
+    out = g.SentinelSlices(out_sizes, out_itemsize, out_offs, packed)
+    capi.check(capi.lib().dalib200PointwiseLaunch(plan.handle, capi.ptr_array(in_ptrs), capi.ptr_array(out.ptrs), capi.stream_handle()))
+    return out.read(what)
+
+
+def _linear_transform(imgs, mats, offs, out_dtype, in_offs=None, out_offs=None, packed=False):
+    n = len(imgs)
+    samples = (capi.ColorSample * n)()
+    for i, im in enumerate(imgs):
+        samples[i].num_pixels = im.size // 3
+        samples[i].matrix[:] = [float(v) for v in np.asarray(mats[i], np.float32).reshape(9)]
+        samples[i].offset[:] = [float(v) for v in np.asarray(offs[i], np.float32).reshape(3)]
+    dt = np.dtype(out_dtype)
+    odt = capi.UINT8 if dt == np.uint8 else capi.FLOAT
+    got = _pointwise_launch(lambda plan: capi.check(capi.lib().dalib200LinearTransformSetup(plan.handle, n, samples, odt)), imgs,
+                            [im.size * dt.itemsize for im in imgs], dt.itemsize, in_offs, out_offs, packed, "linear transform")
+    return [b.view(dt).reshape(im.shape) for b, im in zip(got, imgs)]
+
+
+def _lt_args(rng, n):
+    """per-sample 3x3 matrices with negative entries and offsets whose three channels differ (colour twist makes them equal)"""
+    mats = [rng.uniform(-0.6, 1.4, (3, 3)).astype(np.float32) for _ in range(n)]
+    offs = [np.array([rng.uniform(-40, -5), rng.uniform(0, 30), rng.uniform(60, 120)], np.float32) for _ in range(n)]
+    return mats, offs
+
+
+def _assert_lt(got, imgs, mats, offs, out_dtype, what, f64=False):
+    import image_f64 as F
+    for i, (o, im, M, T) in enumerate(zip(got, imgs, mats, offs)):
+        want = po.linear_transform(im, M, T, out_dtype)
+        if not np.array_equal(o.view(np.uint8), want.view(np.uint8)):
+            bad = np.argwhere(o.view(np.uint8).reshape(want.shape[0], -1) != want.view(np.uint8).reshape(want.shape[0], -1))[0]
+            raise AssertionError(f"{what}: sample {i} of {im.shape[0]} pixels, first wrong byte at pixel {bad[0]}")
+        if f64 and im.size:
+            v, b = F.linear_transform(im, M.astype(np.float64), T.astype(np.float64))
+            (F.check_u8 if np.dtype(out_dtype) == np.uint8 else F.check)(o, v, b, (what, i))
+
+
+def test_linear_transform_sizes_and_alignments():
+    """Pixel counts around the 4-pixel quads and the 16-pixel vector groups of the linear transform (fn.hsv, fn.color_twist), u8 and
+    float output: first with every sample 256-byte aligned (the 48-byte vector branch where a group is whole), then with the inputs
+    at byte offsets 1..15 and the outputs at offsets that break the 16-byte alignment (u8: 1..15, float: 4, 8, 12) inside one
+    allocation each (the quad-by-quad branch).  Bit for bit against the oracle, and within the bound of the float64 statement."""
+    rng = np.random.default_rng(7)
+    imgs = [rng.integers(0, 256, (p, 3), dtype=np.uint8) for p in PIXELS]
+    mats, offs = _lt_args(rng, len(imgs))
+    for dt in (np.uint8, np.float32):
+        got = _linear_transform(imgs, mats, offs, dt)
+        _assert_lt(got, imgs, mats, offs, dt, ("aligned", np.dtype(dt).name), f64=True)
+        for shift in range(15):
+            in_offs = [1 + (k + shift) % 15 for k in range(len(imgs))]
+            out_offs = [1 + (3 * k + shift) % 15 if dt == np.uint8 else 4 * (1 + (k + shift) % 3) for k in range(len(imgs))]
+            got = _linear_transform(imgs, mats, offs, dt, in_offs, out_offs)
+            _assert_lt(got, imgs, mats, offs, dt, ("unaligned", np.dtype(dt).name, shift), f64=shift == 0)
+
+
+def _many_pixel_counts(rng):
+    """3000 pixel counts, every 97th and the first and the last 0: more quads than the grid's NumSMs x 32 CTAs of 256 quads cover on
+    an H100 (132 SMs), so that the CTAs take ranges of many samples"""
+    npx = rng.integers(0, 4000, 3000)
+    npx[::97] = 0
+    npx[-1] = 0
+    assert int(np.sum((npx + 3) // 4)) > 132 * 32 * 256
+    return npx
+
+
+def test_linear_transform_batch_of_many_packed_samples():
+    """3000 samples packed back to back with matrices and offsets of their own, u8 and float output."""
+    rng = np.random.default_rng(8)
+    imgs = [rng.integers(0, 256, (int(p), 3), dtype=np.uint8) for p in _many_pixel_counts(rng)]
+    mats, offs = _lt_args(rng, len(imgs))
+    for dt in (np.uint8, np.float32):
+        got = _linear_transform(imgs, mats, offs, dt, packed=True)
+        _assert_lt(got, imgs, mats, offs, dt, ("packed", np.dtype(dt).name))
+
+
+def test_color_space_conversion_every_pair_packed_and_unaligned():
+    """Every (input, output) pair of RGB / BGR / GRAY / YCbCr, GRAY in and GRAY out included, over the pixel counts above followed
+    by 3000 random ones, packed back to back (so at every byte alignment): bit for bit against the oracle, and the YCbCr
+    conversions within the bound of the float64 BT.601 statement."""
+    import image_f64 as F
+    rng = np.random.default_rng(9)
+    npx = np.concatenate([[0], PIXELS, _many_pixel_counts(rng)])
+    nch = {capi.RGB: 3, capi.BGR: 3, capi.GRAY: 1, capi.YCbCr: 3}
+    rgb = lambda x: x[..., ::-1]
+    f64 = {(capi.RGB, capi.YCbCr): F.rgb_to_ycbcr, (capi.BGR, capi.YCbCr): lambda x: F.rgb_to_ycbcr(rgb(x)),
+           (capi.YCbCr, capi.RGB): F.ycbcr_to_rgb, (capi.YCbCr, capi.BGR): lambda x: tuple(rgb(a) for a in F.ycbcr_to_rgb(x)),
+           (capi.YCbCr, capi.GRAY): F.ycbcr_to_gray, (capi.GRAY, capi.YCbCr): F.gray_to_ycbcr}
+    for it in (capi.RGB, capi.BGR, capi.GRAY, capi.YCbCr):
+        ic = nch[it]
+        imgs = [rng.integers(0, 256, (int(p), ic), dtype=np.uint8) for p in npx]
+        num = (C.c_int64 * len(npx))(*[int(p) for p in npx])
+        for ot in (capi.RGB, capi.BGR, capi.GRAY, capi.YCbCr):
+            oc = nch[ot]
+            got = _pointwise_launch(lambda plan: capi.check(capi.lib().dalib200ColorSpaceSetup(plan.handle, len(npx), num, it, ot)),
+                                    imgs, [int(p) * oc for p in npx], 1, packed=True, what=("csc", it, ot))
+            got = np.concatenate(got).reshape(-1, oc)
+            src = np.concatenate(imgs)
+            want = po.csc(src, it, ot)
+            bad = np.flatnonzero(np.any(got != want, axis=1))
+            if bad.size:
+                k = int(np.searchsorted(np.cumsum(npx), bad[0], side="right"))
+                raise AssertionError(f"csc {it} -> {ot}: sample {k} of {npx[k]} pixels wrong ({bad.size} pixels in all)")
+            if (it, ot) in f64:
+                F.check_u8(got, *f64[(it, ot)](src), ("csc", it, ot))
 def _jpg(img, *params):
     import cv2
     ok, enc = cv2.imencode(".jpg", img, [cv2.IMWRITE_JPEG_QUALITY, 90, *params])
