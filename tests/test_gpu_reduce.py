@@ -3,7 +3,7 @@ bound takes the depth of each sample's accumulation tree from dalib200ReducePlan
   * every operator and type; ranks 0-6 with axis subsets, negative axes, axis_names and keep_dims; unit and zero extents; shapes that
     differ per sample; each path on both sides of its threshold;
   * 256 x 1080p x 3 uint8 per-channel mean; 3000 tiny samples; one uint8 sample of more than 2^31 elements;
-  * a sample alone and inside a mixed batch, and a repeated run: bit-identical;
+  * a sample alone and inside a mixed batch, and a repeated run: bit-identical, and within the bound of the reference;
   * per-image standardisation (x - mean) / std_dev through pipeline_def against float64; 0-d outputs through DALIGenericIterator;
   * outputs written into one sentinel-filled allocation, checked for stray writes."""
 import ctypes as C
@@ -21,13 +21,7 @@ pytestmark = pytest.mark.gpu
 FN = ["min", "max", "sum", "mean", "mean_square", "rms", "std_dev", "variance"]
 
 
-def _data(shape, dt, rng):
-    dt = np.dtype(dt)
-    if dt.kind == "f":
-        return (rng.standard_normal(shape) * 10 + 3).astype(dt)
-    info = np.iinfo(dt)
-    lo, hi = (max(info.min, -(1 << 20)), 1 << 20) if dt.itemsize >= 4 else (info.min, info.max)
-    return rng.integers(lo, hi, shape, dtype=dt, endpoint=True)
+_data = rr.random_data
 
 
 def depths(op, xs, axes, keep_dims=False, dtype=None):
@@ -179,12 +173,20 @@ def test_per_channel_mean_of_256_1080p_images_and_determinism():
     # a float sample alone, inside a mixed batch and run twice: bit-identical
     f = [(rng.standard_normal((1080, 1920, 3)) * 50).astype(np.float32), (rng.standard_normal((300, 17, 3))).astype(np.float32)]
     mixed = [f[1], f[0], _data((5, 5, 3), np.float32, rng), f[0]]
-    build = lambda x: (fn.reductions.sum(x), fn.reductions.std_dev(x, fn.reductions.mean(x, axes=[0, 1], keep_dims=True), axes=[0, 1]))
+    def build(x):
+        m = fn.reductions.mean(x, axes=[0, 1], keep_dims=True)
+        return fn.reductions.sum(x), fn.reductions.std_dev(x, m, axes=[0, 1]), m
     alone, again = _run(build, [[f[0]], [f[0]]], batch_size=4)
     (inmix,) = _run(build, [mixed])
-    for k in range(2):
+    for k in range(3):
         a = alone[k][0][0]
         assert a.tobytes() == again[k][0][0].tobytes() == inmix[k][0][1].tobytes() == inmix[k][0][3].tobytes()
+    # and each of them within the bound of its accumulation tree (tests/test_gpu_reduce_exact.py pins them bit for bit)
+    s, sd, m = (alone[k][0][0] for k in range(3))
+    for op, got, axes, keep, mean in ((rr.SUM, s, None, False, None), (rr.MEAN, m, (0, 1), True, None), (rr.STD_DEV, sd, (0, 1), False, m)):
+        dep, _ = depths(op, [f[0]], axes, keep)
+        want, tol = rr.reference(op, f[0], axes, keep, mean=mean, depth=dep[0])
+        rr.check(got, np.asarray(want), tol, ("1080p", rr.NAMES[op]))
 
 
 def test_3000_tiny_samples():

@@ -4,7 +4,8 @@
   * the planner and the kernel bodies compiled for the host (tools/emul/reduce_emul.cc), every work item and every thread run in
     reverse order, against tests/reduce_ref.py: every operator and type, ranks 0-6 with every subset of axes at ranks 4 and 6,
     negative axes, both keep_dims, unit and zero extents, shapes that differ per sample, unaligned inputs and both sides of every path
-    threshold and of the chunk sizes (the path of each pass is read back);
+    threshold and of the chunk sizes (the path of each pass is read back); and on exact-sum inputs (reduce_ref.exact_data) byte for
+    byte against reduce_ref.exact_reference;
   * random cases under ASan + UBSan."""
 import ctypes as C
 import itertools
@@ -19,6 +20,7 @@ import pytest
 from dali_b200 import backend
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import reduce_host as rh  # noqa: E402
 import reduce_ref as rr  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -93,80 +95,29 @@ def test_refusals_name_the_problem():
     assert "at most 6 dimensions" in e, e
 
 
-# ---- the host build of the planner and the kernel bodies
+# ---- the host build of the planner and the kernel bodies (tests/reduce_host.py)
 @pytest.fixture(scope="module")
 def emul(tmp_path_factory):
-    if shutil.which("g++") is None:
+    lib = rh.build(tmp_path_factory.mktemp("reduce"))
+    if lib is None:
         pytest.skip("needs g++")
-    so = str(tmp_path_factory.mktemp("reduce") / "reduce_emul.so")
-    r = subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-shared", "-fPIC", SRC, "-o", so], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return C.CDLL(so)
+    return lib
 
 
-def _placed(x, off, keep):
-    """x's bytes at element offset `off` past a 16-byte boundary of a fresh buffer (kept alive in `keep`)"""
-    buf = np.zeros(x.nbytes + 48, np.uint8)
-    base = (-buf.ctypes.data) % 16 + off * x.itemsize
-    buf[base:base + x.nbytes] = np.frombuffer(np.ascontiguousarray(x).tobytes(), np.uint8)
-    keep.append(buf)
-    return buf.ctypes.data + base
+run = rh.run
 
 
-def run(lib, op, xs, axes=None, keep_dims=False, dtype=None, ddof=0, means=None, off=0):
-    """-> (outputs, kinds [sample][pass], depths) or (None, message, None)"""
-    n, nd = len(xs), xs[0].ndim
-    ax = rr._axes(xs[0], axes) if nd else ()
-    mask = sum(1 << a for a in ax)
-    shp = (C.c_int64 * max(1, n * nd))(*[e for x in xs for e in x.shape])
-    ond = nd if keep_dims else nd - len(ax)
-    osh = (C.c_int64 * max(1, n * ond))()
-    ot = C.c_int32()
-    kinds = (C.c_int32 * (3 * n))()
-    depths = (C.c_int64 * n)()
-    err = C.create_string_buffer(512)
-    args = (op, rr.CODE[xs[0].dtype], -1 if dtype is None else dtype, n, nd, shp, mask, int(keep_dims), ddof)
-    if lib.emul_reduce(*args, None, None, None, osh, C.byref(ot), kinds, depths, err, 512):
-        return None, err.value.decode(), None
-    keep = []
-    ip = (C.c_void_p * n)(*[_placed(x, (off + 3 * i) % (16 // x.itemsize), keep) for i, x in enumerate(xs)])
-    mp = None if means is None else (C.c_void_p * n)(*[_placed(np.asarray(m, np.float32), 0, keep) for m in means])
-    ots = np.dtype(rr.TYPES[ot.value])
-    outs, optrs = [], []
-    for i in range(n):
-        shape = tuple(osh[i * ond + a] for a in range(ond))
-        nbytes = int(np.prod(shape, dtype=np.int64)) * ots.itemsize
-        buf = np.full(nbytes + 64, 0xA5, np.uint8)
-        base = (-buf.ctypes.data) % 16 + 16
-        outs.append((buf, base, shape))
-        optrs.append(buf.ctypes.data + base)
-    assert lib.emul_reduce(*args, ip, mp, (C.c_void_p * n)(*optrs), osh, C.byref(ot), kinds, depths, err, 512) == 0
-    res = []
-    for buf, base, shape in outs:
-        nbytes = int(np.prod(shape, dtype=np.int64)) * ots.itemsize
-        assert np.all(buf[:base] == 0xA5) and np.all(buf[base + nbytes:] == 0xA5), "a write outside the output"
-        res.append(np.frombuffer(buf[base:base + nbytes].tobytes(), ots).reshape(shape))
-    return res, [list(kinds[3 * i:3 * i + 3]) for i in range(n)], list(depths)
+_data = rr.random_data
 
 
-def _data(shape, dt, rng):
-    dt = np.dtype(dt)
-    if dt.kind == "f":
-        return (rng.standard_normal(shape) * 10 + 3).astype(dt)
-    info = np.iinfo(dt)
-    if dt.itemsize >= 4:                       # squares of 32- and 64-bit values would leave the range of FLOAT
-        return rng.integers(max(info.min, -(1 << 20)), 1 << 20, shape, dtype=dt, endpoint=True)
-    return rng.integers(info.min, info.max, shape, dtype=dt, endpoint=True)
-
-
-def check_all(lib, op, xs, axes=None, keep_dims=False, dtype=None, ddof=0, off=0, what=""):
+def check_all(lib, op, xs, axes=None, keep_dims=False, dtype=None, ddof=0, off=0, moff=0, what=""):
     means = None
     if op in (rr.STD_DEV, rr.VARIANCE):
         ax = rr._axes(xs[0], axes) if xs[0].ndim else ()
         means = [np.mean(x.astype(np.float64), axis=ax, keepdims=keep_dims).astype(np.float32) if x.size else
                  np.zeros([1 if a in ax else e for a, e in enumerate(x.shape)] if keep_dims else
                           [e for a, e in enumerate(x.shape) if a not in ax], np.float32) for x in xs]
-    got, kinds, depths = run(lib, op, xs, axes, keep_dims, dtype, ddof, means, off)
+    got, kinds, depths = run(lib, op, xs, axes, keep_dims, dtype, ddof, means, off, moff, off)
     assert got is not None, (what, kinds)
     for i, x in enumerate(xs):
         want, tol = rr.reference(op, x, (rr._axes(x, axes) if x.ndim else None), keep_dims, dtype, ddof,
@@ -289,9 +240,46 @@ def test_unaligned_inputs(emul):
     for t in (np.uint8, np.int16, np.float32, np.float64):
         xs = [_data((50, 123), t, rng), _data((2500, 3), t, rng)]
         for off in range(16 // np.dtype(t).itemsize):
-            for op in (rr.SUM, rr.MEAN_SQUARE, rr.MAX):
-                check_all(emul, op, xs, (1,), off=off, what=("offset", t, off))
-                check_all(emul, op, xs, (0,), off=off, what=("offset", t, off))
+            for op in (rr.SUM, rr.MEAN_SQUARE, rr.MAX, rr.STD_DEV, rr.VARIANCE):
+                check_all(emul, op, xs, (1,), off=off, moff=off % 4, what=("offset", t, off))
+                check_all(emul, op, xs, (0,), off=off, moff=off % 4, what=("offset", t, off))
+
+
+def run_exact(lib, op, xs, cs, axes, keep_dims, off=0, what="", **kw):
+    """one batch of exact_data through the host build against exact_reference, byte for byte; returns the kinds"""
+    means = [rr.exact_mean(c, x, axes, keep_dims) for x, c in zip(xs, cs)] if op in (rr.STD_DEV, rr.VARIANCE) else None
+    got, kinds, _ = run(lib, op, xs, axes, keep_dims, means=means, off=off, moff=off, ooff=off, **kw)
+    assert got is not None, (what, kinds)
+    for i, x in enumerate(xs):
+        want = rr.exact_reference(op, x, axes, keep_dims, mean=None if means is None else means[i], **kw)
+        rr.same_bytes(got[i], want, (what, rr.NAMES[op], kw, x.dtype, x.shape, axes, off))
+    return kinds
+
+
+def test_exact_sums_bit_for_bit(emul):
+    """float sums, means, std_dev and variance on inputs whose every partial sum is exact: the one right result, byte for byte"""
+    rng = np.random.default_rng(8)
+    for what, types, ops, shapes, ch, axes, keep in rr.exact_cases(rng):
+        for t in types:
+            xs, cs = rr.exact_batch(rng, t, shapes, ch, axes)
+            for op in ops:
+                for kw in rr.VARIANTS.get(op, [{}]):
+                    run_exact(emul, op, xs, cs, axes, keep, off=int(rng.integers(0, 16)), what=what, **kw)
+
+
+def test_exact_sums_see_a_mixed_up_channel(emul):
+    """the exact data centres each channel on its own value: a channel's statistics moved to its neighbour are wrong by whole steps"""
+    rng = np.random.default_rng(9)
+    for t in (np.uint8, np.float32):
+        xs, cs = rr.exact_batch(rng, t, [(2500, 3), (700, 5)], 1, (0,))
+        for op in (rr.SUM, rr.MEAN, rr.STD_DEV):
+            means = [rr.exact_mean(c, x, (0,)) for x, c in zip(xs, cs)] if op == rr.STD_DEV else None
+            got, _, _ = run(emul, op, xs, (0,), means=means)
+            for i, x in enumerate(xs):
+                want = rr.exact_reference(op, x, (0,), mean=None if means is None else means[i])
+                rr.same_bytes(got[i], want)
+                rolled = np.roll(want, 1)
+                assert not np.any(rolled == want), (op, t, want)
 
 
 def test_random_cases_under_sanitizers(tmp_path):
