@@ -30,6 +30,7 @@
 // units of no JPEG image, and ljpeg.cu decodes their clean streams on a stream forked behind U3.
 #include "common.cuh"
 #include "jpeg_recon.h"
+#include "jpeg_idct_core.h"
 #include <algorithm>
 #include <cstring>
 #include <map>
@@ -996,31 +997,8 @@ __global__ void __launch_bounds__(256) truncation_fixup_kernel(HuffCtx cx) {
 }
 
 // ============================================================================================
-// I1: dequantisation + islow IDCT (libjpeg jidctint: CONST_BITS 13, PASS1_BITS 2).  One thread per 8x8 block.
-// The arithmetic is that of libjpeg-turbo's x86 SIMD kernels (jidctint-sse2 / -avx2), which cv2.imdecode and the reference's CPU decoder
-// run; it equals the C jidctint on natural streams and parts from it where coefficients are far out of range (damaged or hostile
-// streams, 16-bit DQT): dequantised words and the sums i0 +- i4, i7 + i3, i5 + i1 wrap to 16 bits, the multiply-adds are exact in 32
-// bits, each pass saturates its output to int16 and the result to [-128, 127].  Restated in oracle/jpeg_oracle.c and tests/jpeg_idct16.py.
-__device__ __forceinline__ int wrap16(int x) { return (int)(int16_t)x; }
-
-// One 1-D pass over int16 inputs: the descaled 32-bit results (no sum leaves 32 bits for int16 inputs); the caller saturates.
-template <int SHIFT>
-__device__ __forceinline__ void idct8(int i0, int i1, int i2, int i3, int i4, int i5, int i6, int i7, int *o) {
-  const int tmp3 = i2 * 10703 + i6 * 4433, tmp2 = i2 * 4433 - i6 * 10704;
-  const int tmp0 = wrap16(i0 + i4) * 8192, tmp1 = wrap16(i0 - i4) * 8192;
-  const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
-  const int z3 = wrap16(i7 + i3), z4 = wrap16(i5 + i1);
-  const int Z3 = z3 * -6436 + z4 * 9633, Z4 = z3 * 9633 + z4 * 6437;
-  const int o0 = i7 * -4927 + i1 * -7373 + Z3, o3 = i7 * -7373 + i1 * 4926 + Z4;
-  const int o1 = i5 * -4176 + i3 * -20995 + Z4, o2 = i5 * -20995 + i3 * 4177 + Z3;
-  const int r = 1 << (SHIFT - 1);
-  o[0] = (t10 + o3 + r) >> SHIFT; o[7] = (t10 - o3 + r) >> SHIFT;
-  o[1] = (t11 + o2 + r) >> SHIFT; o[6] = (t11 - o2 + r) >> SHIFT;
-  o[2] = (t12 + o1 + r) >> SHIFT; o[5] = (t12 - o1 + r) >> SHIFT;
-  o[3] = (t13 + o0 + r) >> SHIFT; o[4] = (t13 - o0 + r) >> SHIFT;
-}
-
-__device__ __forceinline__ uint32_t pixel(int x) { return (uint32_t)(min(max(x, -128), 127) + 128); }     // packsswb, + 128
+// I1: dequantisation + islow IDCT (libjpeg jidctint: CONST_BITS 13, PASS1_BITS 2).  One thread per 8x8 block.  The arithmetic, and
+// its relation to libjpeg-turbo's SIMD kernels, is in jpeg_idct_core.h.
 
 __device__ __forceinline__ int find_by_prefix(const int64_t *first, int n, int64_t v) {
   int lo = 0, hi = n - 1;
@@ -1036,48 +1014,19 @@ __device__ __forceinline__ int find_by_prefix(const int64_t *first, int n, int64
 __device__ __forceinline__ void idct_block(const int16_t *__restrict__ coef_arena, const int16_t *__restrict__ dc_arena, int64_t gb,
                                            const uint16_t *__restrict__ q, uint2 *rows) {
   const int4 *src = reinterpret_cast<const int4 *>(coef_arena + gb * 64);
-  int ws[64];
-  {
-    int in[64];
-    const uint4 *q4 = reinterpret_cast<const uint4 *>(q);      // 8 x u16 per row in ONE 16-byte load (the table is 16-byte aligned)
-    uint32_t q00 = 0, ac_rows = 0;
+  const uint4 *q4 = reinterpret_cast<const uint4 *>(q);      // 8 x u16 per row in ONE 16-byte load (the table is 16-byte aligned)
+  int w[32];
+  uint32_t qw[32], rw[16];
 #pragma unroll
-    for (int r = 0; r < 8; r++) {
-      const int4 v = __ldg(src + r);
-      const uint4 qv = __ldg(q4 + r);
-      const int w[4] = { v.x, v.y, v.z, v.w };
-      const uint32_t qw[4] = { qv.x, qv.y, qv.z, qv.w };
-      if (r == 0) q00 = qv.x & 0xFFFFu;
-      else ac_rows |= (uint32_t)(v.x | v.y | v.z | v.w);
-#pragma unroll
-      for (int k = 0; k < 4; k++) {
-        in[r * 8 + 2 * k] = wrap16(w[k] * (int)(qw[k] & 0xFFFFu));                     // the low 16 bits of coef * q (pmullw)
-        in[r * 8 + 2 * k + 1] = wrap16((w[k] >> 16) * (int)(qw[k] >> 16));
-      }
-    }
-    in[0] = wrap16((int)__ldg(dc_arena + gb) * (int)q00);  // DC lives in the compact array (after prediction)
-    // coefficients of rows 1..7 all zero: the SIMD kernels skip pass 1 and shift row 0 left by PASS1_BITS in 16 bits, which wraps
-    // where the full pass (whose outputs are then exactly in[x] << 2) saturates.  wrap16(in[x] << 2) is a multiple of 4, so feeding the
-    // full pass a quarter of it yields the wrapped value unsaturated.
-    if (ac_rows == 0) {
-#pragma unroll
-      for (int x = 0; x < 8; x++) in[x] = wrap16(in[x] * 4) >> 2;
-    }
-#pragma unroll
-    for (int x = 0; x < 8; x++) {       // pass 1: columns
-      int o[8];
-      idct8<11>(in[x], in[8 + x], in[16 + x], in[24 + x], in[32 + x], in[40 + x], in[48 + x], in[56 + x], o);
-#pragma unroll
-      for (int y = 0; y < 8; y++) ws[y * 8 + x] = min(max(o[y], -32768), 32767);       // packssdw
-    }
+  for (int r = 0; r < 8; r++) {
+    const int4 v = __ldg(src + r);
+    const uint4 qv = __ldg(q4 + r);
+    w[4 * r] = v.x; w[4 * r + 1] = v.y; w[4 * r + 2] = v.z; w[4 * r + 3] = v.w;
+    qw[4 * r] = qv.x; qw[4 * r + 1] = qv.y; qw[4 * r + 2] = qv.z; qw[4 * r + 3] = qv.w;
   }
+  idct_block_words(w, qw, __ldg(dc_arena + gb), rw);
 #pragma unroll
-  for (int y = 0; y < 8; y++) {         // pass 2: rows
-    int o[8];
-    idct8<18>(ws[y * 8], ws[y * 8 + 1], ws[y * 8 + 2], ws[y * 8 + 3], ws[y * 8 + 4], ws[y * 8 + 5], ws[y * 8 + 6], ws[y * 8 + 7], o);
-    rows[y].x = pixel(o[0]) | (pixel(o[1]) << 8) | (pixel(o[2]) << 16) | (pixel(o[3]) << 24);
-    rows[y].y = pixel(o[4]) | (pixel(o[5]) << 8) | (pixel(o[6]) << 16) | (pixel(o[7]) << 24);
-  }
+  for (int y = 0; y < 8; y++) rows[y] = make_uint2(rw[2 * y], rw[2 * y + 1]);
 }
 
 // Work list: the blocks of the MCUs [mcu_x0, +mcu_nx) x [mcu_y0, +mcu_ny) of every image (all MCUs unless a region of interest
@@ -1313,14 +1262,6 @@ __device__ __forceinline__ void color_row8(const JpegImage &im, const uint8_t *_
   }
 }
 
-// four ints -> four saturated bytes of one word (byte 0 = p0): two cvt.pack.sat instead of eight min/max and three merges
-__device__ __forceinline__ uint32_t pack4_sat_u8(int p0, int p1, int p2, int p3) {
-  uint32_t hi, w;
-  asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, %3;" : "=r"(hi) : "r"(p3), "r"(p2), "r"(0));
-  asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, %3;" : "=r"(w) : "r"(p1), "r"(p0), "r"(hi));
-  return w;
-}
-
 // items: per image height * ceil(width / kColorSeg); images not eligible for this path (or decoded by idct_color_420) own zero items
 __global__ void __launch_bounds__(128, 10) color_fast_kernel(const JpegImage *__restrict__ images, const int64_t *__restrict__ first_item,
                                                          int nimages, int64_t total_items, const uint8_t *__restrict__ planes) {
@@ -1360,20 +1301,12 @@ __global__ void __launch_bounds__(128, 10) color_fast_kernel(const JpegImage *__
 // The IDCT of band m leaves its last luma and chroma rows in carry row m & 1 as well, where band m + 1 finds them while the IDCT of
 // band m + 1 is already overwriting the band rows.  A segment that does not start at the top first transforms the band above it.  The
 // horizontal halo is the edge column of the chroma blocks of the MCUs left and right of the strip.
-// the 16 upsampled chroma samples of luma columns 2 * i0 .. 2 * i0 + 15 from the near / far chroma tile rows; c = tile byte of column i0
-__device__ __forceinline__ void fancy_row16(const uint8_t *near, const uint8_t *far, int c, int i0, int dw, int *v) {
-  const uint2 a = *reinterpret_cast<const uint2 *>(near + c), b = *reinterpret_cast<const uint2 *>(far + c);
-  int cs[10];
-  cs[0] = 3 * near[c - 1] + far[c - 1];                    // read, but unused, at the image's left / right edge
-  cs[9] = 3 * near[c + 8] + far[c + 8];
-#pragma unroll
-  for (int k = 0; k < 8; k++) cs[1 + k] = 3 * (int)(((k < 4 ? a.x : a.y) >> (8 * (k & 3))) & 0xFFu) + (int)(((k < 4 ? b.x : b.y) >> (8 * (k & 3))) & 0xFFu);
-#pragma unroll
-  for (int k = 0; k < 8; k++) {
-    v[2 * k] = fancy_h2v2_even(cs[k], cs[1 + k], i0 + k);
-    v[2 * k + 1] = fancy_h2v2_odd(cs[1 + k], cs[2 + k], i0 + k, dw);
-  }
-}
+//
+// Warps 0-2 transform the luma and chroma blocks of the strip, one block per thread.  Warp 3 transforms the (up to) 4 halo blocks, of
+// which one column each is needed, with 8 lanes per block (halo_pass1 / halo_pass2): a whole block per thread there would cost warp 3
+// as many instructions as each of the others for 4 % of the work.  The colour unit (color_unit16) has no image-edge case: the thread
+// that transforms the chroma block of the image's first or last chroma column also stores a copy of that column beside it.
+static_assert(kFusedThreads == 128 && 6 * kFusedMcus <= 96, "idct_color_420: warps 0-2 take the strip's blocks, warp 3 the halo");
 
 // items: per image fused_geo().nstrips * nseg, strips of one segment consecutive; one CTA per item
 __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegImage *__restrict__ images, const int64_t *__restrict__ first_item,
@@ -1381,6 +1314,7 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
                                                                 const int16_t *__restrict__ dc_arena, const QuantSet *__restrict__ quants) {
   __shared__ __align__(16) uint8_t s_y[18][16 * kFusedMcus];      // rows 0, 1: carry rows; 2 + r: luma row 16m + r of band m
   __shared__ __align__(16) uint8_t s_c[2][10][kFusedCPitch];      // Cb, Cr; rows 0, 1: carry rows; 2 + r: chroma row 8m + r
+  __shared__ int s_hws[4][8][9];                                  // pass-1 workspace of the halo blocks (row y, column x)
   __shared__ int s_img;
   if (threadIdx.x == 0) s_img = find_by_prefix(first_item, nimages, blockIdx.x);
   __syncthreads();
@@ -1395,6 +1329,7 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
   // this thread's block in every band: the luma blocks in tile order (the lanes of a warp store consecutive 8-byte runs of one row),
   // then Cb, Cr, then the chroma blocks of the MCUs left / right of the strip, of which only the edge column is kept
   const int j = threadIdx.x;
+  const bool halo = j >= 96;
   int mx = 0, comp = 0, bx = 0, by = 0, col = 0;                  // col: tile byte of the block's column 0 (halo: of the kept column)
   bool active = true;
   if (j < 4 * nt) {
@@ -1405,8 +1340,8 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
     comp = 1 + (j - 4 * nt) / nt;
     const int u = (j - 4 * nt) % nt;
     mx = mxa + u; col = 8 + 8 * u;
-  } else if (j < 6 * nt + 4) {
-    const int h = j - 6 * nt;
+  } else if (halo) {
+    const int h = (j - 96) >> 3;
     comp = 1 + (h & 1);
     if (h < 2) { mx = mxa - 1; active = mxa > 0; col = 7; }
     else { mx = mxa + nt; active = mx < im.mcux; col = 8 + 8 * nt; }
@@ -1419,24 +1354,61 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
   const int64_t blk0 = im.coef_off / 64;
   const int wx0 = im.win_x0, wx1 = im.win_x0 + im.win_w, wy0 = im.win_y0, wy1 = im.win_y0 + im.win_h;
   const int dw = (im.width + 1) >> 1, dh = (im.height + 1) >> 1;
-  const bool bgr = im.out_type == DALIB200_BGR;
+  const ColorK ck = color_k(im.out_type == DALIB200_BGR);
+  const int s0 = im.out_type == DALIB200_BGR ? 0 : 1;             // chroma of channel 0: Cr for RGB, Cb for BGR
+  const int edge = dw - 1 - 8 * mx;                               // chroma block: column of the image's last chroma column if < 8
   for (int m = b_lo > 0 ? b_lo - 1 : b_lo; m < b_hi; m++) {
-    if (active) {
+    if (halo) {
+      // lane x: pass 1 on column x of block hb; then lane y: pass 2 on row y, the kept column only
+      const int x = j & 7, hb = (j >> 3) & 3;
+      int in[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+      uint32_t ac = 0;
+      if (active) {
+        const int64_t gb = blk0 + ((int64_t)m * im.mcux + mx) * im.bpm + b;
+#pragma unroll
+        for (int y = 0; y < 8; y++) {
+          const int c = __ldg(coef_arena + gb * 64 + 8 * y + x);
+          in[y] = wrap16(c * (int)__ldg(q + 8 * y + x));
+          if (y) ac |= (uint32_t)c;
+        }
+        if (x == 0) in[0] = wrap16((int)__ldg(dc_arena + gb) * (int)__ldg(q));
+      }
+      ac |= __shfl_xor_sync(0xFFFFFFFFu, ac, 1);
+      ac |= __shfl_xor_sync(0xFFFFFFFFu, ac, 2);
+      ac |= __shfl_xor_sync(0xFFFFFFFFu, ac, 4);
+      int wsc[8];
+      halo_pass1(in, ac == 0, wsc);
+#pragma unroll
+      for (int y = 0; y < 8; y++) s_hws[hb][y][x] = wsc[y];
+      __syncwarp();
+      int wsr[8];
+#pragma unroll
+      for (int k = 0; k < 8; k++) wsr[k] = s_hws[hb][x][k];
+      const uint8_t v = (uint8_t)halo_pass2(wsr, col == 7);
+      if (active) {
+        s_c[comp - 1][2 + x][col] = v;
+        if (x == 7) s_c[comp - 1][m & 1][col] = v;
+      }
+    } else if (active) {
       uint2 rows[8];
       idct_block(coef_arena, dc_arena, blk0 + ((int64_t)m * im.mcux + mx) * im.bpm + b, q, rows);
       if (comp == 0) {
 #pragma unroll
         for (int y = 0; y < 8; y++) *reinterpret_cast<uint2 *>(&s_y[2 + 8 * by + y][col]) = rows[y];
         if (by == 1) *reinterpret_cast<uint2 *>(&s_y[m & 1][col]) = rows[7];
-      } else if (j < 6 * nt) {
+      } else {
 #pragma unroll
         for (int y = 0; y < 8; y++) *reinterpret_cast<uint2 *>(&s_c[comp - 1][2 + y][col]) = rows[y];
         *reinterpret_cast<uint2 *>(&s_c[comp - 1][m & 1][col]) = rows[7];
-      } else {
-        const bool left = col == 7;                           // left neighbour: its column 7; right neighbour: its column 0
+        if (mx == 0 || edge < 8) {      // libjpeg: the missing neighbour of the first / last chroma column is the column itself
 #pragma unroll
-        for (int y = 0; y < 8; y++) s_c[comp - 1][2 + y][col] = (uint8_t)(left ? rows[y].y >> 24 : rows[y].x);
-        s_c[comp - 1][m & 1][col] = (uint8_t)(left ? rows[7].y >> 24 : rows[7].x);
+          for (int y = 0; y < 9; y++) {
+            uint8_t *t = s_c[comp - 1][y < 8 ? 2 + y : m & 1];
+            const uint2 rv = rows[y < 8 ? y : 7];
+            if (mx == 0) t[col - 1] = (uint8_t)rv.x;
+            if (edge < 8) t[col + edge + 1] = (uint8_t)((edge < 4 ? rv.x : rv.y) >> (8 * (edge & 3)));
+          }
+        }
       }
     }
     __syncthreads();
@@ -1450,26 +1422,9 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
         const int ly = y - 16 * m, cn = (y >> 1) - 8 * m, cf = fancy_far_row(y, dh) - 8 * m;
         const uint4 yv = *reinterpret_cast<const uint4 *>(&s_y[ly < 0 ? carry : 2 + ly][16 * u]);
         const int rn = cn < 0 ? carry : 2 + cn, rf = cf < 0 ? carry : 2 + cf;
-        int cb[16], cr[16];
-        fancy_row16(s_c[0][rn], s_c[0][rf], 8 + 8 * u, 8 * (mxa + u), dw, cb);
-        fancy_row16(s_c[1][rn], s_c[1][rf], 8 + 8 * u, 8 * (mxa + u), dw, cr);
         const uint32_t yw[4] = { yv.x, yv.y, yv.z, yv.w };
         uint32_t w[12];
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          int px[24];
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            const int yy = (int)((yw[2 * h + (k >> 2)] >> (8 * (k & 3))) & 0xFFu);
-            const int cbm = cb[8 * h + k] - 128, crm = cr[8 * h + k] - 128;
-            const int rr = yy + ((91881 * crm + 32768) >> 16);    // jdcolor.c, SCALEBITS 16; saturated by the pack (range_limit)
-            const int gg = yy + ((-22554 * cbm + 32768 - 46802 * crm) >> 16);
-            const int bb = yy + ((116130 * cbm + 32768) >> 16);
-            px[3 * k] = bgr ? bb : rr; px[3 * k + 1] = gg; px[3 * k + 2] = bgr ? rr : bb;
-          }
-#pragma unroll
-          for (int t = 0; t < 6; t++) w[6 * h + t] = pack4_sat_u8(px[4 * t], px[4 * t + 1], px[4 * t + 2], px[4 * t + 3]);
-        }
+        color_unit16(yw, s_c[s0][rn], s_c[s0][rf], s_c[1 - s0][rn], s_c[1 - s0][rf], 8 + 8 * u, ck, w);
         uint8_t *o = im.out + ((int64_t)(y - wy0) * im.win_w + (x0 - wx0)) * 3;     // clipped to the window below
         if (x0 >= wx0 && x0 + 16 <= wx1 && (reinterpret_cast<uintptr_t>(o) & 15) == 0) {
           uint4 *o16 = reinterpret_cast<uint4 *>(o);
