@@ -11,12 +11,6 @@
 
 namespace dalib200 {
 
-__device__ __forceinline__ int find_arith(const ArithSample *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 constexpr int kArithThreads = 256;
 
 // kWide = prog.wide: programs without 64-bit values keep a 32-bit value file (fewer registers per thread)
@@ -28,7 +22,7 @@ __global__ void __launch_bounds__(kArithThreads) arith_kernel(const ArithProgram
     reinterpret_cast<uint32_t *>(&p)[k] = reinterpret_cast<const uint32_t *>(&prog)[k];
   __syncthreads();
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const ArithSample &d = samples[find_arith(samples, n, item)];
+    const ArithSample &d = samples[last_at_most(samples, 0, n - 1, item, [](const ArithSample &s) { return s.first_item; })];
     const int64_t e0 = (item - d.first_item) * kArithItem, e1 = min(d.n, e0 + kArithItem);
     for (int64_t base = e0; base < e1; base += (int64_t)kArithEpt * blockDim.x)
       arith_elements<kWide>(p, d, base, e1, threadIdx.x);

@@ -18,12 +18,7 @@
 #include <string.h>
 #include <math.h>
 #include <type_traits>
-
-#ifdef __CUDACC__
-#define ARITH_HD __host__ __device__ __forceinline__
-#else
-#define ARITH_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -69,9 +64,9 @@ struct ArithSample {
   int32_t ndim;
 };
 
-ARITH_HD bool arith_is_float(int t) { return t == kAF16 || t == kAF32 || t == kAF64; }
-ARITH_HD bool arith_is_signed(int t) { return t >= kAI8 && t <= kAI64; }
-ARITH_HD int arith_bits(int t) {
+DB_HD bool arith_is_float(int t) { return t == kAF16 || t == kAF32 || t == kAF64; }
+DB_HD bool arith_is_signed(int t) { return t >= kAI8 && t <= kAI64; }
+DB_HD int arith_bits(int t) {
   switch (t) {
     case kAU8: case kAI8: return 8;
     case kAU16: case kAI16: case kAF16: return 16;
@@ -80,23 +75,23 @@ ARITH_HD int arith_bits(int t) {
     default: return 64;
   }
 }
-ARITH_HD int arith_size(int t) { return t == kABool ? 1 : arith_bits(t) / 8; }
+DB_HD int arith_size(int t) { return t == kABool ? 1 : arith_bits(t) / 8; }
 
-ARITH_HD float arith_f(uint64_t v) { float f; uint32_t b = (uint32_t)v; memcpy(&f, &b, 4); return f; }
-ARITH_HD uint64_t arith_uf(float f) { uint32_t b; memcpy(&b, &f, 4); return b; }
-ARITH_HD double arith_d(uint64_t v) { double d; memcpy(&d, &v, 8); return d; }
-ARITH_HD uint64_t arith_ud(double d) { uint64_t b; memcpy(&b, &d, 8); return b; }
+DB_HD float arith_f(uint64_t v) { float f; uint32_t b = (uint32_t)v; memcpy(&f, &b, 4); return f; }
+DB_HD uint64_t arith_uf(float f) { uint32_t b; memcpy(&b, &f, 4); return b; }
+DB_HD double arith_d(uint64_t v) { double d; memcpy(&d, &v, 8); return d; }
+DB_HD uint64_t arith_ud(double d) { uint64_t b; memcpy(&b, &d, 8); return b; }
 
 #ifdef __CUDA_ARCH__
-ARITH_HD float arith_fadd(float a, float b) { return __fadd_rn(a, b); }
-ARITH_HD float arith_fmul(float a, float b) { return __fmul_rn(a, b); }
+DB_HD float arith_fadd(float a, float b) { return __fadd_rn(a, b); }
+DB_HD float arith_fmul(float a, float b) { return __fmul_rn(a, b); }
 #else
-ARITH_HD float arith_fadd(float a, float b) { return a + b; }
-ARITH_HD float arith_fmul(float a, float b) { return a * b; }
+DB_HD float arith_fadd(float a, float b) { return a + b; }
+DB_HD float arith_fmul(float a, float b) { return a * b; }
 #endif
 
 // float32 -> the nearest binary16 value (ties to even, overflow to infinity), as a float32
-ARITH_HD float arith_half_rne(float f) {
+DB_HD float arith_half_rne(float f) {
   uint32_t b = (uint32_t)arith_uf(f);
   const uint32_t s = b & 0x80000000u, a = b & 0x7FFFFFFFu;
   if (a >= 0x7F800000u) return f;                                   // inf, NaN
@@ -111,7 +106,7 @@ ARITH_HD float arith_half_rne(float f) {
 }
 
 // float32 -> binary16 as the CPU backend converts (ConvertSat<float16>): clamped to +-65504, then to nearest, ties away from zero
-ARITH_HD float arith_half_sat(float f) {
+DB_HD float arith_half_sat(float f) {
   if (f != f) return f;
   f = f > 65504.0f ? 65504.0f : f < -65504.0f ? -65504.0f : f;
   const uint32_t b = (uint32_t)arith_uf(f), s = b & 0x80000000u, a = b & 0x7FFFFFFFu;
@@ -123,7 +118,7 @@ ARITH_HD float arith_half_sat(float f) {
 }
 
 // an integer of type t from its 64-bit two's complement bits: truncated to the width and re-extended
-ARITH_HD uint64_t arith_wrap(uint64_t x, int t) {
+DB_HD uint64_t arith_wrap(uint64_t x, int t) {
   switch (t) {
     case kAU8: return (uint8_t)x;
     case kAU16: return (uint16_t)x;
@@ -136,11 +131,11 @@ ARITH_HD uint64_t arith_wrap(uint64_t x, int t) {
   }
 }
 
-ARITH_HD double arith_int_to_d(uint64_t v, int t) { return arith_is_signed(t) ? (double)(int64_t)v : (double)v; }
-ARITH_HD float arith_int_to_f(uint64_t v, int t) { return arith_is_signed(t) ? (float)(int64_t)v : (float)v; }
+DB_HD double arith_int_to_d(uint64_t v, int t) { return arith_is_signed(t) ? (double)(int64_t)v : (double)v; }
+DB_HD float arith_int_to_f(uint64_t v, int t) { return arith_is_signed(t) ? (float)(int64_t)v : (float)v; }
 
 // value conversion of a type promotion (integer widening or re-interpretation, integer -> float, float -> wider float)
-ARITH_HD uint64_t arith_cvt(uint64_t v, int from, int to) {
+DB_HD uint64_t arith_cvt(uint64_t v, int from, int to) {
   if (!arith_is_float(to)) return arith_wrap(v, to);
   if (to == kAF64) return arith_ud(arith_is_float(from) ? (from == kAF64 ? arith_d(v) : (double)arith_f(v)) : arith_int_to_d(v, from));
   if (arith_is_float(from)) return from == kAF64 ? arith_uf((float)arith_d(v)) : v;
@@ -150,7 +145,7 @@ ARITH_HD uint64_t arith_cvt(uint64_t v, int from, int to) {
 
 // ConvertSat<to>(from): floats round half away from zero and saturate (NaN -> 0); integers saturate; BOOL is "!= 0";
 // -> FLOAT16 goes through float32 and is clamped to +-65504 (ties away); FLOAT64 -> FLOAT rounds to nearest
-ARITH_HD uint64_t arith_cast(uint64_t v, int from, int to) {
+DB_HD uint64_t arith_cast(uint64_t v, int from, int to) {
   if (to == kABool) return arith_is_float(from) ? (from == kAF64 ? arith_d(v) != 0 : arith_f(v) != 0) : v != 0;
   if (arith_is_float(to)) {
     if (to == kAF64) return arith_cvt(v, from, to);
@@ -182,7 +177,7 @@ ARITH_HD uint64_t arith_cast(uint64_t v, int from, int to) {
 }
 
 template <typename F>
-ARITH_HD F arith_fop(int op, F a, F b, F c) {
+DB_HD F arith_fop(int op, F a, F b, F c) {
   switch (op) {
     case kOpPlus: return a;
     case kOpMinus: return -a;
@@ -223,7 +218,7 @@ ARITH_HD F arith_fop(int op, F a, F b, F c) {
 
 // float32: the float math library functions (no promotion to double); + - * through the non-contracting intrinsics
 template <>
-ARITH_HD float arith_fop<float>(int op, float a, float b, float c) {
+DB_HD float arith_fop<float>(int op, float a, float b, float c) {
   switch (op) {
     case kOpPlus: return a;
     case kOpMinus: return -a;
@@ -263,7 +258,7 @@ ARITH_HD float arith_fop<float>(int op, float a, float b, float c) {
 }
 
 template <typename F>
-ARITH_HD bool arith_fcmp(int op, F a, F b) {
+DB_HD bool arith_fcmp(int op, F a, F b) {
   switch (op) {
     case kOpEq: return a == b;
     case kOpNeq: return a != b;
@@ -275,7 +270,7 @@ ARITH_HD bool arith_fcmp(int op, F a, F b) {
 }
 
 template <typename U>
-ARITH_HD U arith_upow(U b, U e, bool sgn) {
+DB_HD U arith_upow(U b, U e, bool sgn) {
   typedef typename std::make_signed<U>::type S;
   if (sgn && (S)e < 0) {
     if ((S)b == 1) return 1;
@@ -290,7 +285,7 @@ ARITH_HD U arith_upow(U b, U e, bool sgn) {
 // an integer / BOOL operator in I (int64_t / uint64_t, or int32_t / uint32_t when no operand is wider than 32 bits: the result
 // wraps to the same value); the result's bits are zero-extended, arith_wrap gives them their type
 template <typename I>
-ARITH_HD uint64_t arith_iop(int op, I a, I b, I c) {
+DB_HD uint64_t arith_iop(int op, I a, I b, I c) {
   typedef typename std::make_unsigned<I>::type U;
   const bool sgn = I(-1) < I(0);
   const U ua = (U)a, ub = (U)b;
@@ -319,12 +314,12 @@ ARITH_HD uint64_t arith_iop(int op, I a, I b, I c) {
   }
 }
 
-ARITH_HD bool arith_is_cmp(int op) { return op >= kOpEq && op <= kOpGeq; }
+DB_HD bool arith_is_cmp(int op) { return op >= kOpEq && op <= kOpGeq; }
 
 // one operator instruction (not LOAD / SCALAR) on register values.  kWide = false: the program holds no 64-bit value (ArithProgram::
 // wide), so integers are computed in 32 bits and the FLOAT64 code is left out.
 template <bool kWide>
-ARITH_HD uint64_t arith_apply(const ArithInstr &I, uint64_t a, uint64_t b, uint64_t c) {
+DB_HD uint64_t arith_apply(const ArithInstr &I, uint64_t a, uint64_t b, uint64_t c) {
   const int ct = I.ct, rt = I.rt;
   if (I.op == kOpCvt) return arith_cvt(a, ct, rt);
   if (I.op == kOpCast) return arith_cast(a, ct, rt);
@@ -345,7 +340,7 @@ ARITH_HD uint64_t arith_apply(const ArithInstr &I, uint64_t a, uint64_t b, uint6
 }
 
 // the storage form of one element of type t from its raw bits (the low arith_size(t) bytes of raw)
-ARITH_HD uint64_t arith_from_bits(uint64_t raw, int t) {
+DB_HD uint64_t arith_from_bits(uint64_t raw, int t) {
   switch (t) {
     case kAU8: case kABool: return (uint8_t)raw;
     case kAU16: return (uint16_t)raw;
@@ -365,7 +360,7 @@ ARITH_HD uint64_t arith_from_bits(uint64_t raw, int t) {
 }
 
 // the raw bits of a storage value of type t (a FLOAT16 value is a float32 that is exactly a binary16 value)
-ARITH_HD uint64_t arith_to_bits(uint64_t v, int t) {
+DB_HD uint64_t arith_to_bits(uint64_t v, int t) {
   if (t != kAF16) return v;
   const uint32_t b = (uint32_t)v, s = (b >> 16) & 0x8000u, a = b & 0x7FFFFFFFu;
   if (a >= 0x7F800000u) return s | 0x7C00u | (a > 0x7F800000u ? 0x200u | ((a >> 13) & 0x3FFu) : 0u);
@@ -373,7 +368,7 @@ ARITH_HD uint64_t arith_to_bits(uint64_t v, int t) {
   return s | (uint32_t)(arith_f(a) * 16777216.0f);
 }
 
-ARITH_HD uint64_t arith_load(const void *p, int64_t k, int t) {
+DB_HD uint64_t arith_load(const void *p, int64_t k, int t) {
   const uint8_t *q = static_cast<const uint8_t *>(p) + k * arith_size(t);
   switch (arith_size(t)) {
     case 1: return arith_from_bits(*q, t);
@@ -383,7 +378,7 @@ ARITH_HD uint64_t arith_load(const void *p, int64_t k, int t) {
   }
 }
 
-ARITH_HD void arith_store(void *p, int64_t k, int t, uint64_t v) {
+DB_HD void arith_store(void *p, int64_t k, int t, uint64_t v) {
   uint8_t *q = static_cast<uint8_t *>(p) + k * arith_size(t);
   const uint64_t b = arith_to_bits(v, t);
   switch (arith_size(t)) {
@@ -395,7 +390,7 @@ ARITH_HD void arith_store(void *p, int64_t k, int t, uint64_t v) {
 }
 
 // element index inside operand j of output element e
-ARITH_HD int64_t arith_index(const ArithSample &d, int j, int64_t e) {
+DB_HD int64_t arith_index(const ArithSample &d, int j, int64_t e) {
   if ((d.linear >> j) & 1u) return e;
   int64_t idx = 0;
   for (int a = d.ndim - 1; a >= 0; a--) {
@@ -415,10 +410,10 @@ ARITH_HD int64_t arith_index(const ArithSample &d, int j, int64_t e) {
 // kArithEpt consecutive elements of type t starting at element e of p: one access of kArithEpt * size bytes (16 bytes for 4-byte
 // types, two of 16 for 8-byte ones) when p + e is aligned to it, else element by element
 struct alignas(16) ArithVec { uint64_t w[kArithEpt * 8 / 8]; };   // kArithEpt * 8 bytes: room for kArithEpt 8-byte elements
-ARITH_HD bool arith_vec_ok(const void *p, int64_t e, int sz) {
+DB_HD bool arith_vec_ok(const void *p, int64_t e, int sz) {
   return ((uintptr_t)(static_cast<const uint8_t *>(p) + e * sz) & (uintptr_t)(kArithEpt * sz - 1)) == 0;
 }
-ARITH_HD void arith_load_run(const void *p, int64_t e, int t, uint64_t (&v)[kArithEpt]) {
+DB_HD void arith_load_run(const void *p, int64_t e, int t, uint64_t (&v)[kArithEpt]) {
   const int sz = arith_size(t);
   const uint8_t *q = static_cast<const uint8_t *>(p) + e * sz;
   ArithVec u;
@@ -440,7 +435,7 @@ ARITH_HD void arith_load_run(const void *p, int64_t e, int t, uint64_t (&v)[kAri
     v[k] = arith_from_bits(raw, t);
   }
 }
-ARITH_HD void arith_store_run(void *p, int64_t e, int t, const uint64_t (&v)[kArithEpt]) {
+DB_HD void arith_store_run(void *p, int64_t e, int t, const uint64_t (&v)[kArithEpt]) {
   const int sz = arith_size(t);
   uint8_t *q = static_cast<uint8_t *>(p) + e * sz;
   ArithVec u;
@@ -470,7 +465,7 @@ ARITH_HD void arith_store_run(void *p, int64_t e, int t, const uint64_t (&v)[kAr
 // switches below dispatch on the instruction's register field, which is uniform across the block), so it stays in registers.
 #define ARITH_REGS(X) X(0) X(1) X(2) X(3) X(4) X(5) X(6) X(7)
 template <typename R>
-ARITH_HD void arith_get(const R (&r)[kArithMaxRegs][kArithEpt], int j, R (&v)[kArithEpt]) {
+DB_HD void arith_get(const R (&r)[kArithMaxRegs][kArithEpt], int j, R (&v)[kArithEpt]) {
   switch (j) {
 #define ARITH_GET(J) case J: ARITH_UNROLL for (int k = 0; k < kArithEpt; k++) v[k] = r[J][k]; break;
     ARITH_REGS(ARITH_GET)
@@ -479,7 +474,7 @@ ARITH_HD void arith_get(const R (&r)[kArithMaxRegs][kArithEpt], int j, R (&v)[kA
   }
 }
 template <typename R>
-ARITH_HD void arith_set(R (&r)[kArithMaxRegs][kArithEpt], int j, const R (&v)[kArithEpt]) {
+DB_HD void arith_set(R (&r)[kArithMaxRegs][kArithEpt], int j, const R (&v)[kArithEpt]) {
   switch (j) {
 #define ARITH_SET(J) case J: ARITH_UNROLL for (int k = 0; k < kArithEpt; k++) r[J][k] = v[k]; break;
     ARITH_REGS(ARITH_SET)
@@ -491,14 +486,14 @@ ARITH_HD void arith_set(R (&r)[kArithMaxRegs][kArithEpt], int j, const R (&v)[kA
 
 // a register value of type t held in R (uint32_t: the low word of the storage form) -> the storage form
 template <typename R>
-ARITH_HD uint64_t arith_widen(R x, int t) {
+DB_HD uint64_t arith_widen(R x, int t) {
   return sizeof(R) == 8 || !arith_is_signed(t) ? (uint64_t)x : (uint64_t)(int64_t)(int32_t)(uint32_t)x;
 }
 
 // The common FLOAT operators and integer -> FLOAT conversions over a thread's kArithEpt values, dispatched once for all of them; the
 // same arithmetic as arith_apply.  Returns false for every other instruction.
 template <typename R>
-ARITH_HD bool arith_apply_f32(const ArithInstr &I, const R (&a)[kArithEpt], const R (&b)[kArithEpt], const R (&c)[kArithEpt],
+DB_HD bool arith_apply_f32(const ArithInstr &I, const R (&a)[kArithEpt], const R (&b)[kArithEpt], const R (&c)[kArithEpt],
                               R (&v)[kArithEpt]) {
   if (I.rt != kAF32) return false;
   if (I.op == kOpCvt || I.op == kOpCast) {
@@ -530,7 +525,7 @@ ARITH_HD bool arith_apply_f32(const ArithInstr &I, const R (&a)[kArithEpt], cons
 // operands with the output's shape are read and the output written with one vector access per thread and instruction, and every
 // instruction is decoded once per kArithEpt elements.  kWide must be p.wide: without 64-bit values the value file is 32 bits wide.
 template <bool kWide>
-ARITH_HD void arith_elements(const ArithProgram &p, const ArithSample &d, int64_t base, int64_t end, int tid) {
+DB_HD void arith_elements(const ArithProgram &p, const ArithSample &d, int64_t base, int64_t end, int tid) {
   typedef typename std::conditional<kWide, uint64_t, uint32_t>::type R;
   const int64_t e0 = base + (int64_t)tid * kArithEpt;
   if (e0 >= end) return;

@@ -39,15 +39,6 @@ struct SpecParams {
   int pre_border;          // DALIB200_BORDER_* of the fused pre-emphasis
 };
 
-__device__ __forceinline__ int find_spec_sample(const SpecDesc *d, int n, int64_t g) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_group <= g) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 __device__ __forceinline__ int64_t reflect101(int64_t i, int64_t n) {
   if (n < 2) return n - 1;
   for (;;) {
@@ -108,7 +99,7 @@ __global__ void __launch_bounds__(256) spectrogram_kernel(const SpecDesc *__rest
   for (int i = threadIdx.x; i < (N >> 1); i += blockDim.x) tw[i] = twiddle[i];
   __syncthreads();
   for (int64_t grp = blockIdx.x; grp < total_groups; grp += gridDim.x) {
-    const int s = find_spec_sample(descs, n, grp);
+    const int s = last_at_most(descs, 0, n - 1, grp, [](const SpecDesc &d) { return d.first_group; });
     const SpecDesc &d = descs[s];
     const int64_t w0 = (grp - d.first_group) * F;
     const int nf = (int)min((int64_t)F, d.nwin - w0);
@@ -210,7 +201,7 @@ __global__ void __launch_bounds__(256) spectrogram_dft_kernel(const SpecDesc *__
   float *fr = reinterpret_cast<float *>(dbuf + N);     // [F][N]
   for (int i = threadIdx.x; i < N; i += blockDim.x) tw[i] = twiddle_full[i];
   for (int64_t grp = blockIdx.x; grp < total_groups; grp += gridDim.x) {
-    const int s = find_spec_sample(descs, n, grp);
+    const int s = last_at_most(descs, 0, n - 1, grp, [](const SpecDesc &d) { return d.first_group; });
     const SpecDesc &d = descs[s];
     const int64_t w0 = (grp - d.first_group) * F;
     const int nf = (int)min((int64_t)F, d.nwin - w0);
@@ -248,15 +239,6 @@ struct MelDesc {
   int64_t nwin;
   int64_t first_item;      // first (filter, 128-column chunk) work item
 };
-
-__device__ __forceinline__ int find_mel_sample(const MelDesc *d, int n, int64_t g) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_item <= g) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
 
 // ---------------------------------------------------------------------------------------------
 // nfft = 1024: the FFT lives in REGISTERS.  One warp transforms one pair of frames (frame 2p = real part, 2p + 1 = imaginary part)
@@ -329,7 +311,7 @@ __global__ void __launch_bounds__(kF1024Warps * 32, 2) spectrogram1024_kernel(co
   }
   __syncthreads();
   for (int64_t grp = blockIdx.x; grp < total_groups; grp += gridDim.x) {
-    const int s = find_spec_sample(descs, n, grp);
+    const int s = last_at_most(descs, 0, n - 1, grp, [](const SpecDesc &d) { return d.first_group; });
     const SpecDesc &d = descs[s];
     const int64_t w0 = (grp - d.first_group) * (2 * kF1024Warps) + 2 * warp;
     if (w0 >= d.nwin) continue;
@@ -448,7 +430,7 @@ __global__ void __launch_bounds__(128) mel_kernel(const MelDesc *__restrict__ de
                                                   const int32_t *__restrict__ ends, const float *__restrict__ w_up,
                                                   const float *__restrict__ w_down) {
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_mel_sample(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const MelDesc &d) { return d.first_item; });
     const MelDesc &d = descs[s];
     const int64_t li = item - d.first_item;
     const int64_t chunks = (d.nwin + 127) / 128;
@@ -492,7 +474,7 @@ __global__ void __launch_bounds__(256) mel_mma_kernel(const MelDesc *__restrict_
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gid = lane >> 2, tig = lane & 3;
   const int mblocks = (nfilter + kMmM - 1) / kMmM;
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_mel_sample(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const MelDesc &d) { return d.first_item; });
     const MelDesc &d = descs[s];
     const int64_t li = item - d.first_item;
     const int mb = (int)(li % mblocks);

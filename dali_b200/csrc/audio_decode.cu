@@ -24,7 +24,7 @@ namespace dalib200 {
 __global__ void __launch_bounds__(256) flac_sync_kernel(AudioLaunch a) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < a.flac_bytes; g += step) {
-    const int f = audio_find(a.flac, a.nf, g, &FlacDesc::first_byte);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, g, [](const FlacDesc &d) { return d.first_byte; });
     flac_sync_at(a.flac[f], f, a.raw, g - a.flac[f].first_byte, a.fend, a.cand, a.ccount,
                  [](uint32_t *p, uint32_t v) { return atomicAdd(p, v); });
   }
@@ -33,7 +33,7 @@ __global__ void __launch_bounds__(256) flac_sync_kernel(AudioLaunch a) {
 __global__ void __launch_bounds__(32) flac_frame_kernel(AudioLaunch a, int lanes) {
   if ((int)threadIdx.x >= lanes) return;
   for (int64_t k = (int64_t)blockIdx.x * lanes + threadIdx.x; k < a.cand_slots; k += (int64_t)gridDim.x * lanes) {
-    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::cand_base);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, k, [](const FlacDesc &d) { return d.cand_base; });
     flac_candidate(a.flac[f], f, a.raw, k - a.flac[f].cand_base, a.cand, a.ccount, a.fend);
   }
 }
@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(128) flac_chain_kernel(AudioLaunch a) {
 __global__ void __launch_bounds__(32) flac_decode_kernel(AudioLaunch a, int lanes) {
   if ((int)threadIdx.x >= lanes) return;
   for (int64_t k = (int64_t)blockIdx.x * lanes + threadIdx.x; k < a.frame_slots; k += (int64_t)gridDim.x * lanes) {
-    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::frame_base);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, k, [](const FlacDesc &d) { return d.frame_base; });
     if (!flac_decode(a.flac[f], f, a.raw, k - a.flac[f].frame_base, a.frames, a.nframes, a.pcm)) a.status[a.flac[f].sample] = 1;
   }
 }
@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(256) audio_convert_kernel(AudioLaunch a) {
   if (g0 < a.n) *a.descs[g0].rate_out = a.descs[g0].rate;
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = g0; e < a.total_elems; e += step) {
-    const AudioDesc &d = a.descs[audio_find(a.descs, a.n, e, &AudioDesc::first_elem)];
+    const AudioDesc &d = a.descs[last_at_most(a.descs, 0, a.n - 1, e, [](const AudioDesc &p) { return p.first_elem; })];
     audio_convert(d, a.raw, a.pcm, e - d.first_elem, [](float x, float y) { return mul_rn(x, y); }, [](float x, float y) { return add_rn(x, y); });
   }
 }

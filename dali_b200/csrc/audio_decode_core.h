@@ -10,12 +10,7 @@
 #include <stdint.h>
 #include <cstring>
 #include "../../include/dali_b200.h"
-
-#if defined(__CUDACC__)
-#define AUDIO_HD __host__ __device__ __forceinline__
-#else
-#define AUDIO_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -63,14 +58,6 @@ struct AudioLaunch {
   int n, nf;
 };
 
-// The descriptor whose index range [d[i].*first, d[i + 1].*first) holds v: d is sorted by `first`.
-template <typename D>
-AUDIO_HD int audio_find(const D *d, int n, int64_t v, int64_t D::*first) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (d[mid].*first <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 struct FlacHeader {
   int32_t blocksize, assign, variable, len;   // assign: 0..7 independent, 8 left/side, 9 right/side, 10 mid/side; len: header bytes
   uint64_t number;                            // frame number (fixed block size) or first sample number (variable)
@@ -78,17 +65,17 @@ struct FlacHeader {
 
 // Frames the stream may hold: every frame but the last has at least STREAMINFO's minimum block size, and every frame at least 9 + C bytes
 // (a 6-byte header, C subframes of at least 9 bits each, the CRC-16), so that a STREAMINFO total alone cannot raise the cap.
-AUDIO_HD int64_t flac_frame_cap(int64_t length, int32_t min_block, int64_t raw_len, int32_t channels) {
+DB_HD int64_t flac_frame_cap(int64_t length, int32_t min_block, int64_t raw_len, int32_t channels) {
   const int64_t by_length = (length + min_block - 1) / min_block + 1, by_bytes = raw_len / (8 + channels) + 1;
   return by_length < by_bytes ? by_length : by_bytes;
 }
 // Candidate headers the parser follows: twice the frames plus a margin for false syncs; more fails the sample.
-AUDIO_HD int64_t flac_cand_cap(int64_t frame_cap) { return 2 * frame_cap + 64; }
+DB_HD int64_t flac_cand_cap(int64_t frame_cap) { return 2 * frame_cap + 64; }
 // Longest frame of `block` samples followed: the header, per channel an LPC-32 subframe header and 5 bytes per sample (a 31-bit escape
 // code with its partition overhead stays below that), the CRC-16.  Longer frames are corrupt here.
-AUDIO_HD int64_t flac_frame_bound(int32_t channels, int32_t block) { return 18 + (int64_t)channels * (160 + 5 * (int64_t)block); }
+DB_HD int64_t flac_frame_bound(int32_t channels, int32_t block) { return 18 + (int64_t)channels * (160 + 5 * (int64_t)block); }
 
-AUDIO_HD uint32_t flac_crc8(const uint8_t *p, int n) {       // x^8 + x^2 + x + 1
+DB_HD uint32_t flac_crc8(const uint8_t *p, int n) {       // x^8 + x^2 + x + 1
   uint32_t c = 0;
   for (int i = 0; i < n; i++) {
     c ^= p[i];
@@ -97,7 +84,7 @@ AUDIO_HD uint32_t flac_crc8(const uint8_t *p, int n) {       // x^8 + x^2 + x + 
   return c;
 }
 
-AUDIO_HD uint32_t flac_crc16(const uint8_t *p, int64_t n) {  // x^16 + x^15 + x^2 + 1
+DB_HD uint32_t flac_crc16(const uint8_t *p, int64_t n) {  // x^16 + x^15 + x^2 + 1
   uint32_t c = 0;
   for (int64_t i = 0; i < n; i++) {
     c ^= (uint32_t)p[i] << 8;
@@ -108,7 +95,7 @@ AUDIO_HD uint32_t flac_crc16(const uint8_t *p, int64_t n) {  // x^16 + x^15 + x^
 
 // Parses the frame header at p (avail bytes readable) and checks it against STREAMINFO: channel count, bits per sample and sample rate
 // where the header gives them, block size at most STREAMINFO's maximum.  False for anything else.
-AUDIO_HD bool flac_header(const uint8_t *p, int64_t avail, const FlacDesc &d, FlacHeader *h) {
+DB_HD bool flac_header(const uint8_t *p, int64_t avail, const FlacDesc &d, FlacHeader *h) {
   if (avail < 6 || p[0] != 0xFF || (p[1] & 0xFE) != 0xF8) return false;
   const int bs_code = p[2] >> 4, rate_code = p[2] & 15, ch = p[3] >> 4, ss = (p[3] >> 1) & 7;
   if (bs_code == 0 || rate_code == 15 || ch > 10 || ss == 3 || (p[3] & 1)) return false;
@@ -173,8 +160,8 @@ struct FlacBits {
   int64_t pos, end;              // next byte to load, end of the readable bytes
   uint64_t cache;                // left-aligned; the bits below the `n` valid ones are 0
   int n;
-  AUDIO_HD void init(const uint8_t *q, int64_t start, int64_t e) { p = q; pos = start; end = e; cache = 0; n = 0; }
-  AUDIO_HD void refill() {
+  DB_HD void init(const uint8_t *q, int64_t start, int64_t e) { p = q; pos = start; end = e; cache = 0; n = 0; }
+  DB_HD void refill() {
     while (n <= 56) {
       const uint64_t b = pos < end ? p[pos] : 0u;
       cache |= b << (56 - n);
@@ -182,9 +169,9 @@ struct FlacBits {
       pos++;
     }
   }
-  AUDIO_HD int64_t tell() const { return pos * 8 - n; }
-  AUDIO_HD bool past_end() const { return tell() > end * 8; }
-  AUDIO_HD uint32_t get(int k) {                             // k <= 32
+  DB_HD int64_t tell() const { return pos * 8 - n; }
+  DB_HD bool past_end() const { return tell() > end * 8; }
+  DB_HD uint32_t get(int k) {                             // k <= 32
     refill();
     if (k == 0) return 0;
     const uint32_t v = (uint32_t)(cache >> (64 - k));
@@ -192,13 +179,13 @@ struct FlacBits {
     n -= k;
     return v;
   }
-  AUDIO_HD int32_t sget(int k) {                             // k <= 32 bits, two's complement
+  DB_HD int32_t sget(int k) {                             // k <= 32 bits, two's complement
     if (k == 0) return 0;
     const uint32_t v = get(k);
     return (int32_t)(v << (32 - k)) >> (32 - k);
   }
   // number of 0 bits before the next 1 (consumed), or -1 past the end
-  AUDIO_HD int64_t unary() {
+  DB_HD int64_t unary() {
     int64_t q = 0;
     for (;;) {
       refill();
@@ -222,7 +209,7 @@ struct FlacBits {
 
 // Subframe samples go to out[t * stride] (write mode).  Returns false on a reserved code, a bad parameter or data past the end.
 template <bool kWrite>
-AUDIO_HD bool flac_subframe(FlacBits &br, int bs, int sb, int32_t *out, int stride) {
+DB_HD bool flac_subframe(FlacBits &br, int bs, int sb, int32_t *out, int stride) {
   if (br.get(1)) return false;                               // the zero bit in front of the subframe type
   const uint32_t type = br.get(6);
   int wasted = 0;
@@ -326,7 +313,7 @@ AUDIO_HD bool flac_subframe(FlacBits &br, int bs, int sb, int32_t *out, int stri
 // checks the zero padding and the CRC-16 and returns the frame's length in bytes, 0 when it is not a valid frame.  Decode mode writes
 // the decorrelated samples to pcm[t * channels + c] and returns the length, or 0 on an error.
 template <bool kWrite>
-AUDIO_HD int64_t flac_frame(const uint8_t *p, int64_t avail, const FlacDesc &d, const FlacHeader &h, int32_t *pcm) {
+DB_HD int64_t flac_frame(const uint8_t *p, int64_t avail, const FlacDesc &d, const FlacHeader &h, int32_t *pcm) {
   FlacBits br;
   br.init(p, h.len, avail);
   const int C = d.channels, bs = h.blocksize;
@@ -357,7 +344,7 @@ AUDIO_HD int64_t flac_frame(const uint8_t *p, int64_t avail, const FlacDesc &d, 
 }
 
 // ---- audio_convert: one output element
-AUDIO_HD int32_t wav_sample(const uint8_t *q, int bits) {  // q: the sample's bytes, little-endian
+DB_HD int32_t wav_sample(const uint8_t *q, int bits) {  // q: the sample's bytes, little-endian
   if (bits == 8) return (int32_t)q[0] - 128;
   if (bits == 16) return (int32_t)(int16_t)(uint16_t)(q[0] | q[1] << 8);
   if (bits == 24) return (int32_t)((uint32_t)q[0] << 8 | (uint32_t)q[1] << 16 | (uint32_t)q[2] << 24) >> 8;
@@ -367,7 +354,7 @@ AUDIO_HD int32_t wav_sample(const uint8_t *q, int bits) {  // q: the sample's by
 // the source sample (t, c) as libsndfile's float read gives it: x / 2^(b-1) (exact for b <= 24; 32-bit: RN(float(x)) * 2^-31), a float
 // WAV sample as stored.  mul: the host / device multiplication without contraction.
 template <typename Mul>
-AUDIO_HD float audio_float(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t t, int c, Mul mul) {
+DB_HD float audio_float(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t t, int c, Mul mul) {
   const int64_t i = t * a.channels + c;
   if (a.format == 2) return mul((float)pcm[a.pcm_off + i], 1.0f / (float)(1u << (a.bits - 1)));
   const uint8_t *q = raw + a.raw_off + i * (a.bits >> 3);
@@ -381,7 +368,7 @@ AUDIO_HD float audio_float(const AudioDesc &a, const uint8_t *raw, const int32_t
 }
 
 // the integer read: x shifted to 16 / 32 bits (left to widen, arithmetic right to narrow)
-AUDIO_HD int32_t audio_int(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t t, int c, int out_bits) {
+DB_HD int32_t audio_int(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t t, int c, int out_bits) {
   const int64_t i = t * a.channels + c;
   const int32_t x = a.format == 2 ? pcm[a.pcm_off + i] : wav_sample(raw + a.raw_off + i * (a.bits >> 3), a.bits);
   const int s = out_bits - a.bits;
@@ -390,7 +377,7 @@ AUDIO_HD int32_t audio_int(const AudioDesc &a, const uint8_t *raw, const int32_t
 
 // Element le of sample a's output.  Downmix: w = 1 / C, sum = x0 * w, then sum = sum + xc * w, every product and sum rounded on its own.
 template <typename Mul, typename Add>
-AUDIO_HD void audio_convert(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t le, Mul mul, Add add) {
+DB_HD void audio_convert(const AudioDesc &a, const uint8_t *raw, const int32_t *pcm, int64_t le, Mul mul, Add add) {
   const float w = a.weight;
   const int64_t t = le / a.out_channels;
   const int c = (int)(le - t * a.out_channels);
@@ -411,7 +398,7 @@ AUDIO_HD void audio_convert(const AudioDesc &a, const uint8_t *raw, const int32_
 // flac_sync: byte pos of stream f.  Clears its end record and keeps the offset as a candidate when a header that agrees with STREAMINFO
 // starts there.  add: atomic add returning the old value.
 template <typename Add>
-AUDIO_HD void flac_sync_at(const FlacDesc &d, int f, const uint8_t *raw, int64_t pos, uint32_t *fend, uint32_t *cand, uint32_t *ccount, Add add) {
+DB_HD void flac_sync_at(const FlacDesc &d, int f, const uint8_t *raw, int64_t pos, uint32_t *fend, uint32_t *cand, uint32_t *ccount, Add add) {
   fend[d.first_byte + pos] = 0;
   const uint8_t *p = raw + d.raw_off + pos;
   if (pos + 1 >= d.raw_len || p[0] != 0xFF || (p[1] & 0xFE) != 0xF8) return;
@@ -422,7 +409,7 @@ AUDIO_HD void flac_sync_at(const FlacDesc &d, int f, const uint8_t *raw, int64_t
 }
 
 // flac_frame (parse): candidate k of stream f.  Records the frame's length at its offset when it parses to a valid CRC-16.
-AUDIO_HD void flac_candidate(const FlacDesc &d, int f, const uint8_t *raw, int64_t k, const uint32_t *cand, const uint32_t *ccount,
+DB_HD void flac_candidate(const FlacDesc &d, int f, const uint8_t *raw, int64_t k, const uint32_t *cand, const uint32_t *ccount,
                              uint32_t *fend) {
   if (k >= (int64_t)ccount[f] || k >= d.cand_cap) return;
   const int64_t pos = cand[d.cand_base + k];
@@ -437,7 +424,7 @@ AUDIO_HD void flac_candidate(const FlacDesc &d, int f, const uint8_t *raw, int64
 // flac_chain: stream f from the first byte of its audio region, each frame's end to the next start.  Keeps the frames of the chain and
 // returns false when it breaks: too many candidates, a gap, a frame number or sample number out of sequence, a change of blocking
 // strategy, more samples than STREAMINFO's total, fewer, or another frame behind the last.
-AUDIO_HD bool flac_chain(const FlacDesc &d, int f, const uint8_t *raw, const uint32_t *fend, const uint32_t *ccount, FlacFrame *frames,
+DB_HD bool flac_chain(const FlacDesc &d, int f, const uint8_t *raw, const uint32_t *fend, const uint32_t *ccount, FlacFrame *frames,
                          uint32_t *nframes) {
   nframes[f] = 0;
   if (ccount[f] > (uint32_t)d.cand_cap) return false;
@@ -465,7 +452,7 @@ AUDIO_HD bool flac_chain(const FlacDesc &d, int f, const uint8_t *raw, const uin
 }
 
 // flac_frame (decode): frame slot k of stream f, into the stream's [T][C] samples
-AUDIO_HD bool flac_decode(const FlacDesc &d, int f, const uint8_t *raw, int64_t k, const FlacFrame *frames, const uint32_t *nframes,
+DB_HD bool flac_decode(const FlacDesc &d, int f, const uint8_t *raw, int64_t k, const FlacFrame *frames, const uint32_t *nframes,
                           int32_t *pcm) {
   if (k >= (int64_t)nframes[f]) return true;
   const FlacFrame fr = frames[d.frame_base + k];

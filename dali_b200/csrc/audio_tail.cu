@@ -43,12 +43,6 @@ struct SigDesc {
   int64_t first_item;
 };
 
-__device__ __forceinline__ int find_sig(const SigDesc *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 // ---- AudioResample
 struct ArDesc {
   const float *in; float *out;
@@ -73,9 +67,7 @@ __global__ void __launch_bounds__(256) audio_resample_kernel(const ArDesc *__res
   __shared__ float s_pos[kArBlocksPerCta][kArBlock];
   __shared__ long long s_blk[kArBlocksPerCta];
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (descs[mid].first_item <= item) lo = mid; else hi = mid - 1; }
-    const ArDesc &d = descs[lo];
+    const ArDesc &d = descs[last_at_most(descs, 0, n - 1, item, [](const ArDesc &a) { return a.first_item; })];
     const int64_t out0 = (item - d.first_item) * (kArBlock * kArBlocksPerCta);
     const float fscale = (float)d.scale;
     // ---- the float source position of every output of the group: one thread replays one block of 256 (resampling_cpu.cc:131-136)
@@ -154,9 +146,7 @@ constexpr int kPeItem = 4096;
 template <typename T>
 __global__ void __launch_bounds__(256) preemphasis_kernel(const PeDesc *__restrict__ descs, int n, int64_t total_items, int border) {
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (descs[mid].first_item <= item) lo = mid; else hi = mid - 1; }
-    const PeDesc &d = descs[lo];
+    const PeDesc &d = descs[last_at_most(descs, 0, n - 1, item, [](const PeDesc &p) { return p.first_item; })];
     const T *x = static_cast<const T *>(d.in);
     const int64_t e0 = (item - d.first_item) * kPeItem, e1 = min(d.n, e0 + kPeItem);
     for (int64_t e = e0 + threadIdx.x; e < e1; e += blockDim.x) d.out[e] = preemph_at(x, e, d.n, d.coeff, border);
@@ -172,17 +162,11 @@ struct NsDesc {
   int32_t window, interval;
 };
 
-__device__ __forceinline__ int find_ns(const NsDesc *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 // thread = one reset interval of one sample (moving_mean_square.cc:55-77)
 __global__ void __launch_bounds__(128) nonsilent_mms_kernel(const NsDesc *__restrict__ descs, int n, int64_t total_items) {
   const int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (item >= total_items) return;
-  const NsDesc &d = descs[find_ns(descs, n, item)];
+  const NsDesc &d = descs[last_at_most(descs, 0, n - 1, item, [](const NsDesc &p) { return p.first_item; })];
   const int64_t out0 = (item - d.first_item) * d.interval, out1 = min(d.n, out0 + d.interval);
   const float mean_factor = 1.0f / (float)d.window;
   int64_t win_begin = out0 - d.window + 1;
@@ -239,7 +223,7 @@ constexpr int kDbItem = 4096;       // elements per work item
 __global__ void __launch_bounds__(256) todb_max_kernel(const SigDesc *__restrict__ descs, int n, int64_t total_items, uint32_t *__restrict__ smax) {
   __shared__ float wmax[8];
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_sig(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const SigDesc &d) { return d.first_item; });
     const SigDesc &d = descs[s];
     const int64_t e0 = (item - d.first_item) * kDbItem, e1 = min(d.n, e0 + kDbItem);
     float m = 0.0f;                                    // s_ref starts at 0: only values above it count
@@ -258,7 +242,7 @@ __global__ void __launch_bounds__(256) todb_max_kernel(const SigDesc *__restrict
 __global__ void __launch_bounds__(256) todb_kernel(const SigDesc *__restrict__ descs, int n, int64_t total_items, float mul_log2, float s_ref,
                                                    float min_ratio, const uint32_t *__restrict__ smax) {
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_sig(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const SigDesc &d) { return d.first_item; });
     const SigDesc &d = descs[s];
     float ref = s_ref;
     if (smax) { ref = __uint_as_float(smax[s]); if (ref == 0.0f) ref = 1.0f; }
@@ -277,7 +261,7 @@ __global__ void __launch_bounds__(128) mfcc_kernel(const SigDesc *__restrict__ d
   for (int i = threadIdx.x; i < ndct * nfeat; i += blockDim.x) s_tab[i] = table[i];
   __syncthreads();
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_sig(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const SigDesc &d) { return d.first_item; });
     const SigDesc &d = descs[s];
     const int64_t t = (item - d.first_item) * blockDim.x + threadIdx.x;
     if (t >= d.cols) continue;
@@ -314,7 +298,7 @@ __global__ void __launch_bounds__(256) normalize_kernel(const SigDesc *__restric
                                                         float shift, float eps, int ddof) {
   __shared__ float sh[8];
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_sig(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const SigDesc &d) { return d.first_item; });
     const SigDesc &d = descs[s];
     const int64_t g = item - d.first_item;               // group inside the sample
     int64_t cnt, stride, base;

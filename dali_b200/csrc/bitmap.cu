@@ -26,9 +26,7 @@ __global__ void __launch_bounds__(256) bitmap_color_kernel(const BitmapImage *__
                                                            const uint8_t *__restrict__ raw, const uint8_t *__restrict__ scratch) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_grp <= e) lo = mid; else hi = mid - 1; }
-    const BitmapImage &im = images[lo];
+    const BitmapImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const BitmapImage &m) { return m.first_grp; })];
     bitmap_group(im, im.unpack == kBitmapDirect ? raw + im.raw_off : scratch + im.plane_off, e - im.first_grp);
   }
 }

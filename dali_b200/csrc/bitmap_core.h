@@ -12,12 +12,7 @@
 #define DALI_B200_CSRC_BITMAP_CORE_H_
 #include <stdint.h>
 #include <vector_types.h>
-
-#if defined(__CUDACC__)
-#define BITMAP_HD __host__ __device__ __forceinline__
-#else
-#define BITMAP_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -60,7 +55,7 @@ struct BitmapImage {
 // OpenCV's PxM ReadNumber: skips whitespace and '#' comments (up to '\n' or '\r'), reads decimal digits (at most `maxdigits`, 0 = no
 // limit) and consumes the byte behind them.  Any other byte in front of the number, a value above INT_MAX or the end of the data is an
 // error (returns false).
-BITMAP_HD bool pnm_read_number(const uint8_t *s, uint32_t n, uint32_t &pos, int maxdigits, int32_t &val) {
+DB_HD bool pnm_read_number(const uint8_t *s, uint32_t n, uint32_t &pos, int maxdigits, int32_t &val) {
   auto space = [](int c) { return c == ' ' || (c >= '\t' && c <= '\r'); };
   auto digit = [](int c) { return c >= '0' && c <= '9'; };
   if (pos >= n) return false;
@@ -91,7 +86,7 @@ BITMAP_HD bool pnm_read_number(const uint8_t *s, uint32_t n, uint32_t &pos, int 
 }
 
 // cv2's FillUniColor: `count` pixels of palette index v from (x, y) on, wrapping at the end of each row, stopping behind the last row
-BITMAP_HD void bitmap_fill(uint8_t *plane, int64_t W, int64_t H, int64_t &x, int64_t &y, int64_t count, uint8_t v) {
+DB_HD void bitmap_fill(uint8_t *plane, int64_t W, int64_t H, int64_t &x, int64_t &y, int64_t count, uint8_t v) {
   do {
     const int64_t end = x + count < W ? x + count : W;
     count -= end - x;
@@ -104,7 +99,7 @@ BITMAP_HD void bitmap_fill(uint8_t *plane, int64_t W, int64_t H, int64_t &x, int
 // end-of-line, delta or end-of-bitmap code skips take index 0; a delta (dx, dy) skips dx + dy * W pixels in RLE8 and dx in RLE4 (whose
 // dy byte is read and ignored), and RLE4's end-of-bitmap ends the image only on its last row (elsewhere it acts as end-of-line).  A run
 // past the end of its row, or data that ends before the last row is complete, is an error.
-BITMAP_HD int bitmap_rle(const BitmapImage &im, const uint8_t *s, uint8_t *plane) {
+DB_HD int bitmap_rle(const BitmapImage &im, const uint8_t *s, uint8_t *plane) {
   const int64_t W = im.width, H = im.height;
   const uint32_t n = im.raw_len;
   const bool rle8 = im.unpack == kBitmapRle8;
@@ -154,7 +149,7 @@ BITMAP_HD int bitmap_rle(const BitmapImage &im, const uint8_t *s, uint8_t *plane
 
 // ASCII P1 / P2 / P3 as cv2's PxMDecoder reads them, into a plane of `ascii_channels` bytes per pixel: P1 one digit per pixel (index 1
 // for a non-zero digit: black), P2 / P3 samples clamped to maxval, then v * 255 / maxval for maxval < 256 or v >> 8 above.
-BITMAP_HD int bitmap_ascii(const BitmapImage &im, const uint8_t *s, uint8_t *plane) {
+DB_HD int bitmap_ascii(const BitmapImage &im, const uint8_t *s, uint8_t *plane) {
   const int64_t count = (int64_t)im.width * im.height * im.ascii_channels;
   uint32_t pos = 0;
   for (int64_t i = 0; i < count; i++) {
@@ -169,12 +164,12 @@ BITMAP_HD int bitmap_ascii(const BitmapImage &im, const uint8_t *s, uint8_t *pla
 
 // bitmap_unpack_kernel's body: the plane of one RLE or ASCII image.  Returns 0, or 1 for data cv2 refuses.  Reads stay inside the
 // image's raw_len staged bytes, writes inside its plane (width * height * ascii_channels bytes; RLE: width * height).
-BITMAP_HD int bitmap_unpack(const BitmapImage &im, const uint8_t *raw, uint8_t *plane) {
+DB_HD int bitmap_unpack(const BitmapImage &im, const uint8_t *raw, uint8_t *plane) {
   return im.unpack == kBitmapAscii ? bitmap_ascii(im, raw, plane) : bitmap_rle(im, raw, plane);
 }
 
 // R, G, B of image pixel (x, y) from the source raster `src`
-BITMAP_HD void bitmap_rgb(const BitmapImage &im, const uint8_t *src, int x, int y, uint32_t &r, uint32_t &g, uint32_t &b) {
+DB_HD void bitmap_rgb(const BitmapImage &im, const uint8_t *src, int x, int y, uint32_t &r, uint32_t &g, uint32_t &b) {
   const uint8_t *row = src + (int64_t)(im.bottom_up ? im.height - 1 - y : y) * im.stride;
   if (im.layout == kBitmapIndexed) {
     const uint32_t i = im.bits == 8 ? row[x] : im.bits == 4 ? (row[x >> 1] >> (x & 1 ? 0 : 4)) & 15 : (row[x >> 3] >> (7 - (x & 7))) & 1;
@@ -198,7 +193,7 @@ BITMAP_HD void bitmap_rgb(const BitmapImage &im, const uint8_t *src, int x, int 
 // pixel: (1868 B + 9617 G + 4899 R + 8192) >> 14 (cv2's BGR -> gray in both decoders), except for gray_float images, which cv2 reads
 // through its bitfield-mask path: the float32 sum (0.299 R + 0.587 G) + 0.114 B, each product and sum rounded once, truncated.
 constexpr int kBitmapGroup = 16;
-BITMAP_HD uint32_t bitmap_gray(const BitmapImage &im, uint32_t r, uint32_t g, uint32_t b) {
+DB_HD uint32_t bitmap_gray(const BitmapImage &im, uint32_t r, uint32_t g, uint32_t b) {
   if (!im.gray_float) return (b * 1868u + g * 9617u + r * 4899u + 8192u) >> 14;
 #if defined(__CUDA_ARCH__)
   return (uint32_t)__fadd_rn(__fadd_rn(__fmul_rn(0.299f, (float)r), __fmul_rn(0.587f, (float)g)), __fmul_rn(0.114f, (float)b));
@@ -206,7 +201,7 @@ BITMAP_HD uint32_t bitmap_gray(const BitmapImage &im, uint32_t r, uint32_t g, ui
   return (uint32_t)((0.299f * (float)r + 0.587f * (float)g) + 0.114f * (float)b);   // built with -ffp-contract=off
 #endif
 }
-BITMAP_HD void bitmap_group(const BitmapImage &im, const uint8_t *src, int64_t g) {
+DB_HD void bitmap_group(const BitmapImage &im, const uint8_t *src, int64_t g) {
   const int64_t p0 = g * kBitmapGroup, npx = (int64_t)im.win_w * im.win_h;
   const int cnt = npx - p0 < kBitmapGroup ? (int)(npx - p0) : kBitmapGroup;
   int ly = (int)(p0 / im.win_w), lx = (int)(p0 - (int64_t)ly * im.win_w);

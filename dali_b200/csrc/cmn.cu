@@ -33,23 +33,6 @@ struct CmnDesc {
   float mean[4], inv_std[4], fill[4];
 };
 
-__device__ __forceinline__ int find_sample_units(const CmnDesc *d, int n, int64_t u) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_unit <= u) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-__device__ __forceinline__ int find_sample_elems(const CmnDesc *d, int n, int64_t e) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_elem <= e) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 template <typename Out>
 __device__ __forceinline__ void store4(Out *p, Out a, Out b, Out c, Out d);
 template <>
@@ -174,7 +157,7 @@ __global__ void __launch_bounds__(256) cmn_hwc2chw_kernel(const CmnDesc *__restr
   const int64_t per_cta = ((total_units + gridDim.x - 1) / gridDim.x + 2 * wpc - 1) / (2 * wpc) * (2 * wpc);
   const int64_t u0 = (int64_t)blockIdx.x * per_cta, u1 = min(total_units, u0 + per_cta);
   if (u0 >= u1) return;
-  if (threadIdx.x == 0) s_first = find_sample_units(descs, n, u0);
+  if (threadIdx.x == 0) s_first = last_at_most(descs, 0, n - 1, u0, [](const CmnDesc &d) { return d.first_unit; });
   __syncthreads();
   int s = s_first;
   for (int64_t unit = u0 + (threadIdx.x >> 5); unit < u1; unit += 2 * wpc) {
@@ -199,7 +182,7 @@ template <typename Out>
 __global__ void __launch_bounds__(256) cmn_generic_kernel(const CmnDesc *__restrict__ descs, int n, int64_t total_elems,
                                                           int out_c, int chw) {
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total_elems; e += (int64_t)gridDim.x * blockDim.x) {
-    const int s = find_sample_elems(descs, n, e);
+    const int s = last_at_most(descs, 0, n - 1, e, [](const CmnDesc &d) { return d.first_elem; });
     const CmnDesc &d = descs[s];
     if (d.fast) continue;
     int64_t i = e - d.first_elem;

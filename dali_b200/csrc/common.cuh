@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 #include "../../include/dali_b200.h"
+#include "host_device.h"
 
 namespace dalib200 {
 

@@ -26,16 +26,10 @@ struct GenDesc {
 
 constexpr int kGenItem = 8192;                  // output elements per work item
 
-__device__ __forceinline__ int find_gen(const GenDesc *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 template <typename Out>
 __global__ void __launch_bounds__(256) multiply_add_kernel(const GenDesc *__restrict__ descs, int n, int64_t total_items) {
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_gen(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const GenDesc &d) { return d.first_item; });
     const GenDesc &d = descs[s];
     const int64_t e0 = (item - d.first_item) * kGenItem, e1 = min(d.n, e0 + kGenItem);
     Out *out = static_cast<Out *>(d.out);
@@ -79,12 +73,6 @@ struct PadDesc {
   int32_t nouter;
 };
 
-__device__ __forceinline__ int find_pad(const PadDesc *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 // input row of output row r, or -1 when r lies in the padding of an outer axis
 __device__ __forceinline__ int64_t pad_in_row(const PadDesc &d, int64_t r) {
   int64_t in_r = 0, mul = 1;
@@ -100,7 +88,7 @@ template <typename T>
 __global__ void __launch_bounds__(256) pad_kernel(const PadDesc *__restrict__ descs, int n, int64_t total_items, T fill) {
   constexpr int V = 16 / sizeof(T);
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const PadDesc &d = descs[find_pad(descs, n, item)];
+    const PadDesc &d = descs[last_at_most(descs, 0, n - 1, item, [](const PadDesc &p) { return p.first_item; })];
     const int64_t b0 = (item - d.first_item) * kPadItemBytes, b1 = min(d.out_bytes, b0 + kPadItemBytes);
     const T *in = reinterpret_cast<const T *>(d.in);
     T *out = reinterpret_cast<T *>(d.out);
@@ -126,7 +114,7 @@ __global__ void __launch_bounds__(256) pad_kernel(const PadDesc *__restrict__ de
 
 __global__ void __launch_bounds__(256) window_copy_kernel(const GenDesc *__restrict__ descs, int n, int64_t total_items) {
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const int s = find_gen(descs, n, item);
+    const int s = last_at_most(descs, 0, n - 1, item, [](const GenDesc &d) { return d.first_item; });
     const GenDesc &d = descs[s];
     const int64_t e0 = (item - d.first_item) * kGenItem, e1 = min(d.n, e0 + kGenItem);
     uint8_t *out = static_cast<uint8_t *>(d.out);

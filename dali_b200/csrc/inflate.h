@@ -10,12 +10,7 @@
 #ifndef DALI_B200_CSRC_INFLATE_H_
 #define DALI_B200_CSRC_INFLATE_H_
 #include <stdint.h>
-
-#if defined(__CUDACC__)
-#define INFL_HD __host__ __device__ __forceinline__
-#else
-#define INFL_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -32,12 +27,12 @@ struct InflateBits {
   int64_t used, avail;         // bits consumed / bits of data in all ranges
 };
 template <class R>
-INFL_HD void ibits_init(InflateBits<R> &b, const uint8_t *raw, const R *ranges, int k, int kend) {
+DB_HD void ibits_init(InflateBits<R> &b, const uint8_t *raw, const R *ranges, int k, int kend) {
   b.raw = raw; b.ranges = ranges; b.k = k; b.kend = kend; b.pos = 0; b.acc = 0; b.nbits = 0; b.used = 0; b.avail = 0;
   for (int i = k; i < kend; i++) b.avail += 8 * (int64_t)ranges[i].len;
 }
 template <class R>
-INFL_HD void ibits_fill(InflateBits<R> &b) {
+DB_HD void ibits_fill(InflateBits<R> &b) {
   while (b.nbits <= 56) {
     while (b.k < b.kend && b.pos >= b.ranges[b.k].len) { b.k++; b.pos = 0; }
     uint32_t v = 0;
@@ -47,17 +42,17 @@ INFL_HD void ibits_fill(InflateBits<R> &b) {
   }
 }
 template <class R>
-INFL_HD uint32_t ibits_get(InflateBits<R> &b, int n) {        // n <= 32
+DB_HD uint32_t ibits_get(InflateBits<R> &b, int n) {        // n <= 32
   if (b.nbits < n) ibits_fill(b);
   const uint32_t v = n ? (uint32_t)(b.acc & ((1ull << n) - 1)) : 0u;
   b.acc >>= n; b.nbits -= n; b.used += n;
   return v;
 }
 template <class R>
-INFL_HD bool ibits_dry(const InflateBits<R> &b) { return b.used > b.avail; }
+DB_HD bool ibits_dry(const InflateBits<R> &b) { return b.used > b.avail; }
 
 // zlib header (RFC 1950): deflate, window <= 32 KiB, check bits, no preset dictionary
-INFL_HD bool zlib_header_ok(uint32_t cmf, uint32_t flg) {
+DB_HD bool zlib_header_ok(uint32_t cmf, uint32_t flg) {
   return (cmf & 15) == 8 && (cmf >> 4) <= 7 && ((cmf << 8) | flg) % 31 == 0 && !(flg & 0x20);
 }
 
@@ -72,7 +67,7 @@ struct InflateHuff {
 // builds the code from `n` code lengths; returns false for an over-subscribed set, or an incomplete one that is not a single code
 // of length 1 or that may not be incomplete at all (zlib inflate_table: a single length-1 code is accepted for the literal / length
 // and distance codes, never for the code-length code; a code without any symbol is left empty)
-INFL_HD bool inflate_build(InflateHuff &h, const uint8_t *len, int n, bool allow_incomplete) {
+DB_HD bool inflate_build(InflateHuff &h, const uint8_t *len, int n, bool allow_incomplete) {
   for (int l = 0; l < 16; l++) h.count[l] = 0;
   for (int s = 0; s < n; s++) h.count[len[s]]++;
   for (int i = 0; i < (1 << kInflLutBits); i++) h.lut[i] = 0;
@@ -107,7 +102,7 @@ INFL_HD bool inflate_build(InflateHuff &h, const uint8_t *len, int n, bool allow
 
 // next symbol, -1 = no such code
 template <class R>
-INFL_HD int inflate_decode(InflateBits<R> &b, const InflateHuff &h) {
+DB_HD int inflate_decode(InflateBits<R> &b, const InflateHuff &h) {
   if (b.nbits < 16) ibits_fill(b);
   const uint16_t e = h.lut[b.acc & ((1u << kInflLutBits) - 1)];
   if (e) { const int l = e >> 9; b.acc >>= l; b.nbits -= l; b.used += l; return e & 511; }
@@ -127,7 +122,7 @@ struct InflateWork { InflateHuff lit, dist, cl; uint8_t lens[288 + 32]; };     /
 // Returns 0, or 1 for a malformed or short stream.  Reads stay inside the ranges; writes stay inside [dst, dst + total).  The end of
 // the output follows libpng (kStopWhenFull = false) or libtiff (true), as the head of this file describes.
 template <bool kStopWhenFull, class R>
-INFL_HD int inflate_zlib(InflateBits<R> &b, uint8_t *dst, int64_t total, InflateWork &w) {
+DB_HD int inflate_zlib(InflateBits<R> &b, uint8_t *dst, int64_t total, InflateWork &w) {
   int64_t out = 0;                                        // bytes produced, surplus included
   bool drain = false;
   uint32_t s1 = 1, s2 = 0, nmod = 0;                      // Adler-32

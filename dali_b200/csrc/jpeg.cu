@@ -89,15 +89,6 @@ __constant__ uint8_t c_zigzag[64] = {
 
 // ============================================================================================
 // U1..U3: byte un-stuffing
-__device__ __forceinline__ int find_unit_by_chunk(const JpegUnit *u, int n, uint32_t chunk) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (u[mid].first_chunk <= chunk) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // a byte is dropped when it is the 0x00 that follows a 0xFF.  Word-at-a-time: bit 8k+7.. of the result marks byte k of
 // `w` as dropped; `prev` is the byte in front of the word (0 at the start of a unit).
 __device__ __forceinline__ uint32_t dropped_mask(uint32_t w, uint32_t prev) {
@@ -151,7 +142,7 @@ __global__ void __launch_bounds__(256) unstuff_count_kernel(const uint8_t *__res
   const uint32_t per = (nchunks + gridDim.x - 1) / gridDim.x;
   const uint32_t ch0 = blockIdx.x * per, ch1 = min(nchunks, ch0 + per);
   if (ch0 >= ch1) return;
-  if (threadIdx.x == 0) s_ui = find_unit_by_chunk(units, nunits, ch0);
+  if (threadIdx.x == 0) s_ui = last_at_most(units, 0, nunits - 1, ch0, [](const JpegUnit &u) { return u.first_chunk; });
   __syncthreads();
   int ui = s_ui;
   for (uint32_t chunk = ch0; chunk < ch1; chunk++) {
@@ -206,7 +197,7 @@ __global__ void __launch_bounds__(256) unstuff_scatter_kernel(const uint8_t *__r
   const uint32_t per = (nchunks + gridDim.x - 1) / gridDim.x;
   const uint32_t ch0 = blockIdx.x * per, ch1 = min(nchunks, ch0 + per);
   if (ch0 >= ch1) return;
-  if (threadIdx.x == 0) s_ui = find_unit_by_chunk(units, nunits, ch0);
+  if (threadIdx.x == 0) s_ui = last_at_most(units, 0, nunits - 1, ch0, [](const JpegUnit &u) { return u.first_chunk; });
   __syncthreads();
   int ui = s_ui;
   for (uint32_t chunk = ch0; chunk < ch1; chunk++) {
@@ -471,15 +462,6 @@ __device__ __forceinline__ void decode_span(Win &win, const Lut &lut, const Huff
   }
 }
 
-__device__ __forceinline__ int find_unit_by_subseq(const JpegUnit *u, int ub, int ue, int j) {
-  int lo = ub, hi = ue - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (u[mid].first_subseq <= j) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 struct HuffCtx {
   const JpegImage *images; int nimages;
   const int32_t *block_image;           // sync block -> image
@@ -560,7 +542,7 @@ __device__ __forceinline__ SubGeom sync_block_prologue(const HuffCtx &cx, const 
   sg.g = (int64_t)im.subseq_begin + j;
   const uint8_t *ptr = nullptr;
   if (sg.valid) {
-    sg.ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : find_unit_by_subseq(cx.units, im.unit_begin, im.unit_end, j);
+    sg.ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : last_at_most(cx.units, im.unit_begin, im.unit_end - 1, j, [](const JpegUnit &u) { return u.first_subseq; });
     const JpegUnit &u = cx.units[sg.ui];
     sg.clean_bits = cx.unit_clean_len[sg.ui] * 8u;
     sg.nsub_eff = (sg.clean_bits + (1u << cx.log2_sub) - 1) >> cx.log2_sub;
@@ -678,7 +660,7 @@ __device__ __forceinline__ void walk_chain(const HuffCtx &cx, const uint4 rec, i
   const JpegImage &im = cx.images[img_i];
   int64_t g = rec.z;
   const int j = (int)(g - im.subseq_begin);
-  const int ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : find_unit_by_subseq(cx.units, im.unit_begin, im.unit_end, j);
+  const int ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : last_at_most(cx.units, im.unit_begin, im.unit_end - 1, j, [](const JpegUnit &u) { return u.first_subseq; });
   const JpegUnit &u = cx.units[ui];
   const uint32_t clean_bits = cx.unit_clean_len[ui] * 8u;
   const uint32_t nsub_eff = (clean_bits + (1u << cx.log2_sub) - 1) >> cx.log2_sub;
@@ -828,7 +810,7 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
     sg.ui = 0; sg.jl = 0; sg.nsub_eff = 0; sg.clean_bits = 0;
     sg.g = (int64_t)im.subseq_begin + j;
     if (sg.valid) {
-      sg.ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : find_unit_by_subseq(cx.units, im.unit_begin, im.unit_end, j);
+      sg.ui = im.unit_end - im.unit_begin == 1 ? im.unit_begin : last_at_most(cx.units, im.unit_begin, im.unit_end - 1, j, [](const JpegUnit &u) { return u.first_subseq; });
       const JpegUnit &u = cx.units[sg.ui];
       sg.clean_bits = cx.unit_clean_len[sg.ui] * 8u;
       sg.nsub_eff = (sg.clean_bits + (1u << cx.log2_sub) - 1) >> cx.log2_sub;
@@ -1000,15 +982,6 @@ __global__ void __launch_bounds__(256) truncation_fixup_kernel(HuffCtx cx) {
 // I1: dequantisation + islow IDCT (libjpeg jidctint: CONST_BITS 13, PASS1_BITS 2).  One thread per 8x8 block.  The arithmetic, and
 // its relation to libjpeg-turbo's SIMD kernels, is in jpeg_idct_core.h.
 
-__device__ __forceinline__ int find_by_prefix(const int64_t *first, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (first[mid] <= v) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // Dequantises and transforms block `gb` (index in MCU order over the arenas) with quantisation table q; rows[y] = the 8 output samples
 // of row y, byte k = column k.
 __device__ __forceinline__ void idct_block(const int16_t *__restrict__ coef_arena, const int16_t *__restrict__ dc_arena, int64_t gb,
@@ -1040,7 +1013,7 @@ __global__ void __launch_bounds__(128) idct_kernel(const JpegImage *__restrict__
   const int64_t per_cta = ((total_work + gridDim.x - 1) / gridDim.x + 127) / 128 * 128;
   const int64_t b0 = (int64_t)blockIdx.x * per_cta, b1 = min(total_work, b0 + per_cta);
   if (b0 >= b1) return;
-  if (threadIdx.x == 0) s_first = find_by_prefix(first_work, nimages, b0);
+  if (threadIdx.x == 0) s_first = last_at_most(first_work, 0, nimages - 1, b0);
   __syncthreads();
   int ii = s_first;
   for (int64_t wb = b0 + threadIdx.x; wb < b1; wb += blockDim.x) {
@@ -1101,11 +1074,10 @@ __device__ __forceinline__ int clamp255(int v) { return min(max(v, 0), 255); }
 __global__ void __launch_bounds__(256) color_kernel(const JpegImage *__restrict__ images, const int64_t *__restrict__ first_quad,
                                                     int nimages, int64_t total_quads, const uint8_t *__restrict__ planes) {
   for (int64_t gq = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; gq < total_quads; gq += (int64_t)gridDim.x * blockDim.x) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (first_quad[mid] <= gq) lo = mid; else hi = mid - 1; }
-    const JpegImage &im = images[lo];
+    const int i = last_at_most(first_quad, 0, nimages - 1, gq);
+    const JpegImage &im = images[i];
     if (im.fast_color) continue;
-    const int64_t q = gq - first_quad[lo];
+    const int64_t q = gq - first_quad[i];
     const int qpr = (im.win_w + 3) >> 2;
     const uint32_t qy = (uint32_t)q / (uint32_t)qpr;
     const int y = im.win_y0 + (int)qy, x0 = im.win_x0 + ((int)((uint32_t)q - qy * (uint32_t)qpr) << 2);
@@ -1271,7 +1243,7 @@ __global__ void __launch_bounds__(128, 10) color_fast_kernel(const JpegImage *__
   const int64_t per_cta = (total_items + gridDim.x - 1) / gridDim.x;
   const int64_t it0 = (int64_t)blockIdx.x * per_cta, it1 = min(total_items, it0 + per_cta);
   if (it0 >= it1) return;
-  if (threadIdx.x == 0) s_first = find_by_prefix(first_item, nimages, it0);
+  if (threadIdx.x == 0) s_first = last_at_most(first_item, 0, nimages - 1, it0);
   __syncthreads();
   int lo = s_first;
   for (int64_t item = it0; item < it1; item++) {
@@ -1316,7 +1288,7 @@ __global__ void __launch_bounds__(kFusedThreads, 5) idct_color_420(const JpegIma
   __shared__ __align__(16) uint8_t s_c[2][10][kFusedCPitch];      // Cb, Cr; rows 0, 1: carry rows; 2 + r: chroma row 8m + r
   __shared__ int s_hws[4][8][9];                                  // pass-1 workspace of the halo blocks (row y, column x)
   __shared__ int s_img;
-  if (threadIdx.x == 0) s_img = find_by_prefix(first_item, nimages, blockIdx.x);
+  if (threadIdx.x == 0) s_img = last_at_most(first_item, 0, nimages - 1, (int64_t)blockIdx.x);
   __syncthreads();
   const int ii = s_img;
   const JpegImage &im = images[ii];
@@ -1471,9 +1443,7 @@ __global__ void __launch_bounds__(256) jpeg_post_kernel(const JpegPost *__restri
   const int64_t p0 = (int64_t)blockIdx.x * per_cta, p1 = min(total_px, p0 + per_cta);
   if (p0 >= p1) return;
   if (threadIdx.x == 0) {
-    int lo = 0, hi = n - 1;
-    while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (posts[mid].first_px <= p0) lo = mid; else hi = mid - 1; }
-    s_first = lo;
+    s_first = last_at_most(posts, 0, n - 1, p0, [](const JpegPost &p) { return p.first_px; });
   }
   __syncthreads();
   int ii = s_first;

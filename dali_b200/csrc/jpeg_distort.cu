@@ -21,11 +21,7 @@ __global__ void __launch_bounds__(kJdThreads) jpeg_distort_fdct_kernel(const JdI
                                                                      int16_t *dc) {
   __shared__ JdStrip t;
   __shared__ int s_img;
-  if (threadIdx.x == 0) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (first_strip[mid] <= (int64_t)blockIdx.x) lo = mid; else hi = mid - 1; }
-    s_img = lo;
-  }
+  if (threadIdx.x == 0) s_img = last_at_most(first_strip, 0, nimages - 1, (int64_t)blockIdx.x);
   __syncthreads();
   const JdImage &im = images[s_img];
   int my, mx0, nt;

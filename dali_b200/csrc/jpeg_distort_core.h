@@ -18,12 +18,7 @@
 #define DALI_B200_CSRC_JPEG_DISTORT_CORE_H_
 #include <stdint.h>
 #include "jpeg_recon.h"
-
-#if defined(__CUDACC__)
-#define JD_HD __host__ __device__ __forceinline__
-#else
-#define JD_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -46,21 +41,21 @@ struct JdStrip {
   int32_t dc[kJdMcus][4];                    // quantised DC of the real luma blocks (for the dummy blocks)
 };
 
-JD_HD void jd_rgb_ycc(int r, int g, int b, int &y, int &cb, int &cr) {
+DB_HD void jd_rgb_ycc(int r, int g, int b, int &y, int &cb, int &cr) {
   y = (19595 * r + 38470 * g + 7471 * b + 32768) >> 16;
   cb = (-11059 * r - 21709 * g + 32768 * b + (128 << 16) + 32767) >> 16;
   cr = (32768 * r - 27439 * g - 5329 * b + (128 << 16) + 32767) >> 16;
 }
 
 // strip li of image im: MCU row my, first MCU column mx0, nt MCU columns
-JD_HD void jd_strip(const JdImage &im, int64_t li, int &my, int &mx0, int &nt) {
+DB_HD void jd_strip(const JdImage &im, int64_t li, int &my, int &mx0, int &nt) {
   my = (int)(li / im.strips_x);
   mx0 = (int)(li - (int64_t)my * im.strips_x) * kJdMcus;
   nt = im.mcux - mx0 < kJdMcus ? im.mcux - mx0 : kJdMcus;
 }
 
 // 2x2 pixel quad e (row-major over 8 x 8 nt quads) of the strip: its four luma samples and one chroma sample of each component
-JD_HD void jd_convert_quad(const JdImage &im, int my, int mx0, int nt, int e, JdStrip &t) {
+DB_HD void jd_convert_quad(const JdImage &im, int my, int mx0, int nt, int e, JdStrip &t) {
   const int W = im.width, H = im.height, qw = 8 * nt;
   const int qy = e / qw, qx = e - qy * qw;
   const int x0 = 16 * mx0 + 2 * qx, y0 = 16 * my + 2 * qy;
@@ -92,7 +87,7 @@ JD_HD void jd_convert_quad(const JdImage &im, int my, int mx0, int nt, int e, Jd
 }
 
 // jpeg_fdct_islow + quantize of the 8 x 8 samples at src (row pitch `pitch`, 8-byte aligned rows); out: 64 coefficients, natural order
-JD_HD void jd_fdct_quant(const uint8_t *src, int pitch, const uint16_t *q, int *out) {
+DB_HD void jd_fdct_quant(const uint8_t *src, int pitch, const uint16_t *q, int *out) {
   int d[64];
 #pragma unroll
   for (int r = 0; r < 8; r++) {              // pass 1: rows
@@ -150,7 +145,7 @@ JD_HD void jd_fdct_quant(const uint8_t *src, int pitch, const uint16_t *q, int *
   }
 }
 
-JD_HD void jd_store_block(int16_t *dst, const int *c) {
+DB_HD void jd_store_block(int16_t *dst, const int *c) {
 #if defined(__CUDA_ARCH__)
   uint4 *d4 = reinterpret_cast<uint4 *>(dst);
 #pragma unroll
@@ -166,7 +161,7 @@ JD_HD void jd_store_block(int16_t *dst, const int *c) {
 
 // Block j (MCU j / 6 of the strip, block j % 6 of the MCU) of the strip.  pass 0 transforms the real blocks and records the luma DCs
 // in t.dc; pass 1 (after every pass-0 block of the strip) writes the dummy blocks from them.
-JD_HD void jd_block(const JdImage &im, const QuantSet &qs, int my, int mx0, int j, int pass, JdStrip &t, int16_t *coef, int16_t *dc) {
+DB_HD void jd_block(const JdImage &im, const QuantSet &qs, int my, int mx0, int j, int pass, JdStrip &t, int16_t *coef, int16_t *dc) {
   const int m = j / 6, b = j - 6 * m;
   const int64_t gb = im.blk0 + ((int64_t)my * im.mcux + mx0 + m) * 6 + b;
   const int wb = (im.width + 7) >> 3, hb = (im.height + 7) >> 3;      // real luma block columns / rows

@@ -10,21 +10,20 @@
 #ifndef DALI_B200_CSRC_JPEG_IDCT_CORE_H_
 #define DALI_B200_CSRC_JPEG_IDCT_CORE_H_
 #include <stdint.h>
+#include "host_device.h"
 
 #if defined(__CUDACC__)
-#define JPEG_IDCT_HD __host__ __device__ __forceinline__
 #define JPEG_IDCT_UNROLL _Pragma("unroll")
 #else
-#define JPEG_IDCT_HD inline
 #define JPEG_IDCT_UNROLL
 #endif
 
 namespace dalib200 {
 
-JPEG_IDCT_HD int wrap16(int x) { return (int)(int16_t)x; }
+DB_HD int wrap16(int x) { return (int)(int16_t)x; }
 
 // __byte_perm: byte k of the result is byte (s >> 4k) & 7 of the pair {b:a} (a = bytes 0..3)
-JPEG_IDCT_HD uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
+DB_HD uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
 #if defined(__CUDA_ARCH__)
   return __byte_perm(a, b, s);
 #else
@@ -36,7 +35,7 @@ JPEG_IDCT_HD uint32_t prmt(uint32_t a, uint32_t b, uint32_t s) {
 }
 
 // four ints -> four saturated bytes of one word (byte 0 = p0): two cvt.pack.sat instead of eight min/max and three merges
-JPEG_IDCT_HD uint32_t pack4_sat_u8(int p0, int p1, int p2, int p3) {
+DB_HD uint32_t pack4_sat_u8(int p0, int p1, int p2, int p3) {
 #if defined(__CUDA_ARCH__)
   uint32_t hi, w;
   asm("cvt.pack.sat.u8.s32.b32 %0, %1, %2, %3;" : "=r"(hi) : "r"(p3), "r"(p2), "r"(0));
@@ -50,14 +49,14 @@ JPEG_IDCT_HD uint32_t pack4_sat_u8(int p0, int p1, int p2, int p3) {
 #endif
 }
 
-JPEG_IDCT_HD int sat16(int x) { return x < -32768 ? -32768 : x > 32767 ? 32767 : x; }     // packssdw
+DB_HD int sat16(int x) { return x < -32768 ? -32768 : x > 32767 ? 32767 : x; }     // packssdw
 
 // One 1-D pass over int16 inputs: the descaled 32-bit results; the caller saturates.  No sum leaves 32 bits for int16 inputs:
 // |t1x| <= 2^28 + 32768 * (10703 + 4433), |o_k| <= 32768 * (20995 + 4177 + 6436 + 9633), and with pass 2's rounding constant 2^17 the
 // largest sum is 2 115 960 832 < 2^31 (tests/test_jpeg_idct_core_cpu.py).  That leaves no room to fold pass 2's + 128 into the
 // rounding constant (128 << 18 would take the sum past 2^31), so the output packs to signed bytes and flips their sign bits.
 template <int SHIFT>
-JPEG_IDCT_HD void idct8(int i0, int i1, int i2, int i3, int i4, int i5, int i6, int i7, int *o) {
+DB_HD void idct8(int i0, int i1, int i2, int i3, int i4, int i5, int i6, int i7, int *o) {
   const int tmp3 = i2 * 10703 + i6 * 4433, tmp2 = i2 * 4433 - i6 * 10704;
   const int tmp0 = wrap16(i0 + i4) * 8192, tmp1 = wrap16(i0 - i4) * 8192;
   const int r = 1 << (SHIFT - 1);
@@ -73,7 +72,7 @@ JPEG_IDCT_HD void idct8(int i0, int i1, int i2, int i3, int i4, int i5, int i6, 
 }
 
 // packsswb + 128 of four pass-2 outputs: four bytes saturated to [-128, 127], each + 128 (= its sign bit flipped)
-JPEG_IDCT_HD uint32_t pack4_pixels(int p0, int p1, int p2, int p3) {
+DB_HD uint32_t pack4_pixels(int p0, int p1, int p2, int p3) {
 #if defined(__CUDA_ARCH__)
   uint32_t hi, w;
   asm("cvt.pack.sat.s8.s32.b32 %0, %1, %2, %3;" : "=r"(hi) : "r"(p3), "r"(p2), "r"(0));
@@ -87,17 +86,17 @@ JPEG_IDCT_HD uint32_t pack4_pixels(int p0, int p1, int p2, int p3) {
 // Dequantised coefficient: the low 16 bits of coef * q (pmullw).  For a word w holding two coefficients and a word qw holding their
 // two table entries, the low half is wrap16(w * qw) (the high halves only add multiples of 2^16) and the high half is
 // wrap16((w >> 16) * (qw >> 16)).
-JPEG_IDCT_HD int dequant_lo(int w, uint32_t qw) { return wrap16(w * (int)qw); }
-JPEG_IDCT_HD int dequant_hi(int w, uint32_t qw) { return wrap16((w >> 16) * (int)(qw >> 16)); }
+DB_HD int dequant_lo(int w, uint32_t qw) { return wrap16(w * (int)qw); }
+DB_HD int dequant_hi(int w, uint32_t qw) { return wrap16((w >> 16) * (int)(qw >> 16)); }
 
 // The coefficients of rows 1..7 all zero (rows0only): the SIMD kernels skip pass 1 and shift row 0 left by PASS1_BITS in 16 bits,
 // which wraps where the full pass (whose outputs are then exactly in[x] << 2) saturates.  wrap16(in[x] << 2) is a multiple of 4, so
 // feeding the full pass a quarter of it yields the wrapped value unsaturated.
-JPEG_IDCT_HD int row0_only(int v) { return wrap16(v * 4) >> 2; }
+DB_HD int row0_only(int v) { return wrap16(v * 4) >> 2; }
 
 // A whole block: w = its 32 coefficient words (row r = words 4r .. 4r + 3, natural order, the arena's DC slot ignored), qw = the
 // table's 32 words, dc = the block's absolute DC.  rows[2y], rows[2y + 1] = output row y, byte k = column k.
-JPEG_IDCT_HD void idct_block_words(const int *w, const uint32_t *qw, int dc, uint32_t *rows) {
+DB_HD void idct_block_words(const int *w, const uint32_t *qw, int dc, uint32_t *rows) {
   int ws[64];
   {
     int in[64];
@@ -132,7 +131,7 @@ JPEG_IDCT_UNROLL
 // pass 1 on column x (halo_pass1: in[y] = dequantised coefficient (y, x), the DC included; ws[y] = workspace (y, x)), lane y then
 // runs pass 2 on row y for the one output it needs (halo_pass2: ws = workspace row y; returns the sample of column 7 if last, else
 // of column 0).  rows0only is the whole block's, as in idct_block_words.
-JPEG_IDCT_HD void halo_pass1(int *in, bool rows0only, int *ws) {
+DB_HD void halo_pass1(int *in, bool rows0only, int *ws) {
   if (rows0only) in[0] = row0_only(in[0]);
   int o[8];
   idct8<11>(in[0], in[1], in[2], in[3], in[4], in[5], in[6], in[7], o);
@@ -140,7 +139,7 @@ JPEG_IDCT_UNROLL
   for (int y = 0; y < 8; y++) ws[y] = sat16(o[y]);
 }
 
-JPEG_IDCT_HD uint32_t halo_pass2(const int *ws, bool last) {
+DB_HD uint32_t halo_pass2(const int *ws, bool last) {
   int o[8];
   idct8<18>(ws[0], ws[1], ws[2], ws[3], ws[4], ws[5], ws[6], ws[7], o);
   const int v = last ? o[7] : o[0];
@@ -167,7 +166,7 @@ struct ColorK {
   int ca, cb, cg, ca16, cb16, cg16;
 };
 
-JPEG_IDCT_HD ColorK color_k(bool bgr) {
+DB_HD ColorK color_k(bool bgr) {
   const int kr = 91881, kb = 116130, kgb = -22554, kgr = -46802;       // R: Cr, B: Cb, G: Cb and Cr
   ColorK k;
   k.a = bgr ? kb : kr; k.b = bgr ? kr : kb;
@@ -179,7 +178,7 @@ JPEG_IDCT_HD ColorK color_k(bool bgr) {
 
 // the upsampled chroma of the unit in 16-bit lanes, each lane 16 times the sample plus 4 bits below it: u[q] holds the samples of
 // pixels 8 (q >> 2) + (q & 3) (low lane) and 4 more (high lane); near / far: the tile rows, c: the byte of chroma column i0 (8-aligned)
-JPEG_IDCT_HD void fancy_unit16(const uint8_t *near, const uint8_t *far, int c, uint32_t *u) {
+DB_HD void fancy_unit16(const uint8_t *near, const uint8_t *far, int c, uint32_t *u) {
   const uint64_t nw = *reinterpret_cast<const uint64_t *>(near + c), fw = *reinterpret_cast<const uint64_t *>(far + c);
   const uint32_t n0 = (uint32_t)nw, n1 = (uint32_t)(nw >> 32), f0 = (uint32_t)fw, f1 = (uint32_t)(fw >> 32);
   const uint32_t csl = 3u * near[c - 1] + far[c - 1], csr = 3u * near[c + 8] + far[c + 8];
@@ -197,7 +196,7 @@ JPEG_IDCT_HD void fancy_unit16(const uint8_t *near, const uint8_t *far, int c, u
 
 // yw: the unit's 16 luma samples (byte k of yw[k >> 2] = pixel k); s0n / s0f, s2n / s2f: near / far tile rows of the chroma of
 // channel 0 and 2 (ColorK); out: 48 bytes, 3 per pixel
-JPEG_IDCT_HD void color_unit16(const uint32_t *yw, const uint8_t *s0n, const uint8_t *s0f, const uint8_t *s2n, const uint8_t *s2f, int c,
+DB_HD void color_unit16(const uint32_t *yw, const uint8_t *s0n, const uint8_t *s0f, const uint8_t *s2n, const uint8_t *s2f, int c,
                                const ColorK &k, uint32_t *out) {
   uint32_t u0[8], u2[8];
   fancy_unit16(s0n, s0f, c, u0);

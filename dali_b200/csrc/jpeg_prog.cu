@@ -28,10 +28,9 @@ __global__ void __launch_bounds__(256) prog_dc_kernel(const ProgImage *__restric
                                                       int32_t *status) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (first_blk[mid] <= e) lo = mid; else hi = mid - 1; }
-    prog_dc_difference(images[lo], coef, dc, e - first_blk[lo]);
-    if (e == first_blk[lo] && images[lo].incomplete) status[images[lo].sample] = 1;
+    const int i = last_at_most(first_blk, 0, nimages - 1, e);
+    prog_dc_difference(images[i], coef, dc, e - first_blk[i]);
+    if (e == first_blk[i] && images[i].incomplete) status[images[i].sample] = 1;
   }
 }
 

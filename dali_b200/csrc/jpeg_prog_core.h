@@ -13,12 +13,7 @@
 #ifndef DALI_B200_CSRC_JPEG_PROG_CORE_H_
 #define DALI_B200_CSRC_JPEG_PROG_CORE_H_
 #include <stdint.h>
-
-#if defined(__CUDACC__)
-#define PG_HD __host__ __device__ __forceinline__
-#else
-#define PG_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -61,7 +56,7 @@ static const uint8_t h_prog_natural[64] = {
    0,  1,  8, 16,  9,  2,  3, 10, 17, 24, 32, 25, 18, 11,  4,  5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13,  6,  7, 14, 21, 28,
   35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
 // zig-zag index -> natural index; a run past 63 (corrupt data) lands on 63, as on the guard entries of libjpeg's jpeg_natural_order
-PG_HD int prog_natural(int k) {
+DB_HD int prog_natural(int k) {
   if (k > 63) k = 63;
 #if defined(__CUDA_ARCH__)
   return d_prog_natural[k];
@@ -78,7 +73,7 @@ struct ProgBits {
   int nbits, pad;
   bool dry;                    // padding has been CONSUMED (the window is filled ahead of use: merely touching the end is not an error)
 };
-PG_HD void pb_fill(ProgBits &b) {
+DB_HD void pb_fill(ProgBits &b) {
   while (b.nbits <= 24) {
     uint32_t v = 0;
     bool real = false;
@@ -93,18 +88,18 @@ PG_HD void pb_fill(ProgBits &b) {
     b.nbits += 8;
   }
 }
-PG_HD void pb_drop(ProgBits &b, int n) {
+DB_HD void pb_drop(ProgBits &b, int n) {
   b.acc <<= n; b.nbits -= n;
   if (b.nbits < b.pad) { b.dry = true; b.pad = b.nbits > 0 ? b.nbits : 0; }
 }
-PG_HD int pb_get(ProgBits &b, int n) {                      // 0 <= n <= 16
+DB_HD int pb_get(ProgBits &b, int n) {                      // 0 <= n <= 16
   if (n == 0) return 0;
   if (b.nbits < n) pb_fill(b);
   const int v = (int)(b.acc >> (32 - n));
   pb_drop(b, n);
   return v;
 }
-PG_HD int pb_huff(ProgBits &b, const ProgHuff &h) {         // jdhuff.c HUFF_DECODE + jpeg_huff_decode
+DB_HD int pb_huff(ProgBits &b, const ProgHuff &h) {         // jdhuff.c HUFF_DECODE + jpeg_huff_decode
   if (b.nbits < 17) pb_fill(b);
   const uint32_t e = h.look[b.acc >> 24];
   if (e) { pb_drop(b, (int)(e >> 8)); return (int)(e & 255u); }
@@ -115,10 +110,10 @@ PG_HD int pb_huff(ProgBits &b, const ProgHuff &h) {         // jdhuff.c HUFF_DEC
   if (l > 16) return 0;                                     // garbage: libjpeg warns and uses symbol 0
   return h.vals[(code + h.valoffset[l]) & 255];
 }
-PG_HD int pb_extend(int v, int s) { return v < (1 << (s - 1)) ? v - (1 << s) + 1 : v; }      // HUFF_EXTEND, s >= 1
+DB_HD int pb_extend(int v, int s) { return v < (1 << (s - 1)) ? v - (1 << s) + 1 : v; }      // HUFF_EXTEND, s >= 1
 
 // jdphuff.c process_restart: drop the partial byte, step over the RSTn marker, reset the predictors
-PG_HD void pb_restart(ProgBits &b) {
+DB_HD void pb_restart(ProgBits &b) {
   b.acc = 0; b.nbits = 0; b.pad = 0; b.dry = false;
   while (b.p + 1 < b.end) {
     if (b.p[0] == 0xFF && b.p[1] >= 0xD0 && b.p[1] <= 0xD7) { b.p += 2; return; }
@@ -128,14 +123,14 @@ PG_HD void pb_restart(ProgBits &b) {
 }
 
 // arena block of block (bx, by) of component c in a single-component scan / of block k of MCU m in an interleaved scan
-PG_HD int64_t prog_block_single(const ProgImage &im, int c, int bx, int by) {
+DB_HD int64_t prog_block_single(const ProgImage &im, int c, int bx, int by) {
   const int mx = bx / im.hs[c], my = by / im.vs[c];
   return ((int64_t)my * im.mcux + mx) * im.bpm + im.blk0[c] + (by % im.vs[c]) * im.hs[c] + (bx % im.hs[c]);
 }
 
 // Decodes one scan into the image's coefficient blocks (natural order inside a block; slot 0 holds the ABSOLUTE DC value while the
 // scans run).  Returns 0, or 1 when the data ran out before the scan was complete (the remaining blocks keep what they had).
-PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuff *huff, const uint8_t *raw, int16_t *coef_arena) {
+DB_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuff *huff, const uint8_t *raw, int16_t *coef_arena) {
   ProgBits b;
   b.p = raw + im.raw_off + s.data_off; b.end = b.p + s.data_len; b.acc = 0; b.nbits = 0; b.pad = 0; b.dry = false;
   int16_t *coef = coef_arena + im.coef_off;
@@ -275,7 +270,7 @@ PG_HD int prog_decode_scan(const ProgScan &s, const ProgImage &im, const ProgHuf
 // After the last wave: slot 0 of every block holds the absolute DC.  The IDCT stage takes the DC from the decoder's compact per-block
 // array, in which dc_scan_kernel (jpeg.cu) accumulates differences component by component in MCU order; this writes the difference
 // of block `blk` (index inside the image) to its predecessor in exactly that order, so that the shared stage can stay as it is.
-PG_HD void prog_dc_difference(const ProgImage &im, const int16_t *coef_arena, int16_t *dc_arena, int64_t blk) {
+DB_HD void prog_dc_difference(const ProgImage &im, const int16_t *coef_arena, int16_t *dc_arena, int64_t blk) {
   const int64_t m = blk / im.bpm;
   const int b = (int)(blk - m * im.bpm);
   int c = 0;

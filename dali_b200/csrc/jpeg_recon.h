@@ -7,12 +7,10 @@
 #define DALI_B200_CSRC_JPEG_RECON_H_
 #include <stdint.h>
 #include "../../include/dali_b200.h"
+#include "host_device.h"
 
 #if defined(__CUDACC__)
 #include <cuda_runtime.h>
-#define JPEG_RECON_HD __host__ __device__ inline
-#else
-#define JPEG_RECON_HD inline
 #endif
 
 namespace dalib200 {
@@ -22,7 +20,7 @@ constexpr int kMaxBlocksPerMcu = 10;
 struct QuantSet { uint16_t q[4][64]; };       // natural order
 
 // GRAY of an RGB-coded JPEG pixel (libjpeg-turbo rgb_gray_convert): the baseline path's Adobe-0 / R-G-B images and lossless RGB.
-JPEG_RECON_HD int RgbJpegGray(int r, int g, int b) { return (r * 19595 + g * 38470 + b * 7471 + 32768) >> 16; }
+DB_HD int RgbJpegGray(int r, int g, int b) { return (r * 19595 + g * 38470 + b * 7471 + 32768) >> 16; }
 
 // Colour space of the decoded components (libjpeg default_decompress_parms).  Decided once per image by the plan; the kernels read
 // nothing else to pick the conversion.
@@ -83,7 +81,7 @@ constexpr int kFusedThreads = 128;                 // >= 6 * kFusedMcus + 4 bloc
 constexpr int kFusedCPitch = 8 * kFusedMcus + 16;  // chroma tile: byte 8 + (i - 8 * first MCU column) holds chroma column i
 
 struct FusedGeo { int mx0, mx_end, nstrips, m0, nbands, nseg, seg_len; };
-JPEG_RECON_HD FusedGeo fused_geo(const JpegImage &im) {
+DB_HD FusedGeo fused_geo(const JpegImage &im) {
   FusedGeo g;
   const int wx1 = im.win_x0 + im.win_w, wy1 = im.win_y0 + im.win_h, last = im.mcuy - 1;
   g.mx0 = im.win_x0 >> 4; g.mx_end = ((wx1 - 1) >> 4) + 1;                  // MCU columns that hold window pixels

@@ -19,16 +19,10 @@ namespace dalib200 {
 
 constexpr int kLjpegRecThreads = 512;
 
-__device__ __forceinline__ int ljpeg_find_unit(const LjpegUnit *u, int n, int64_t g) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (u[mid].first_sub <= g) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 __global__ void __launch_bounds__(256) ljpeg_sync_kernel(LjpegLaunch a) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < a.total_sub; g += step) {
-    const LjpegUnit &u = a.d_units[ljpeg_find_unit(a.d_units, a.nunits, g)];
+    const LjpegUnit &u = a.d_units[last_at_most(a.d_units, 0, a.nunits - 1, g, [](const LjpegUnit &p) { return p.first_sub; })];
     ljpeg_walk(a.d_images[u.image], u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec,
                [](uint64_t *p, uint64_t v) { return (uint64_t)atomicMax(reinterpret_cast<unsigned long long *>(p), (unsigned long long)v); });
   }
@@ -66,7 +60,7 @@ __global__ void __launch_bounds__(256) ljpeg_scan_kernel(LjpegLaunch a) {
 __global__ void __launch_bounds__(256) ljpeg_write_kernel(LjpegLaunch a) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < a.total_sub; g += step) {
-    const LjpegUnit &u = a.d_units[ljpeg_find_unit(a.d_units, a.nunits, g)];
+    const LjpegUnit &u = a.d_units[last_at_most(a.d_units, 0, a.nunits - 1, g, [](const LjpegUnit &p) { return p.first_sub; })];
     const LjpegImage &im = a.d_images[u.image];
     if (ljpeg_write(im, u, g, a.d_clean, a.d_unit_clean_len, a.d_tables, a.d_rec, a.d_first[g], a.d_diff)) a.d_status[im.sample] = 1;
   }
@@ -110,9 +104,8 @@ __global__ void __launch_bounds__(256) ljpeg_color_kernel(const LjpegImage *__re
                                                           const int16_t *__restrict__ diff) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-    ljpeg_pixel(images[lo], diff, e - images[lo].first_px, [](int r, int g, int b) { return RgbJpegGray(r, g, b); });
+    const int i = last_at_most(images, 0, nimages - 1, e, [](const LjpegImage &im) { return im.first_px; });
+    ljpeg_pixel(images[i], diff, e - images[i].first_px, [](int r, int g, int b) { return RgbJpegGray(r, g, b); });
   }
 }
 

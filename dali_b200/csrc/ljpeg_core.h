@@ -9,12 +9,7 @@
 #ifndef DALI_B200_CSRC_LJPEG_CORE_H_
 #define DALI_B200_CSRC_LJPEG_CORE_H_
 #include <stdint.h>
-
-#if defined(__CUDACC__)
-#define LJPEG_HD __host__ __device__ __forceinline__
-#else
-#define LJPEG_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -79,13 +74,13 @@ struct LjpegLaunch {
 // [63:45] priority = distance of the chain that wrote it from the chain's origin (see ljpeg_walk)
 constexpr uint64_t kLjpegStateMask = (1ull << 34) - 1;
 constexpr uint32_t kLjpegMaxChain = (1u << 19) - 1;
-LJPEG_HD uint64_t ljpeg_pack(uint32_t pos, int phase, uint32_t cnt, uint32_t prio) {
+DB_HD uint64_t ljpeg_pack(uint32_t pos, int phase, uint32_t cnt, uint32_t prio) {
   return (uint64_t)pos | ((uint64_t)(uint32_t)phase << 32) | ((uint64_t)(cnt & 2047u) << 34) | ((uint64_t)prio << 45);
 }
-LJPEG_HD uint32_t ljpeg_count(uint64_t r) { return (uint32_t)(r >> 34) & 2047u; }
+DB_HD uint32_t ljpeg_count(uint64_t r) { return (uint32_t)(r >> 34) & 2047u; }
 
 // 32 bits of the clean stream at bit `pos`.  The clean stream is word-swapped (jpeg.cu unstuff_scatter): a 32-bit load is big-endian.
-LJPEG_HD uint32_t ljpeg_peek(const uint32_t *w, uint32_t pos) {
+DB_HD uint32_t ljpeg_peek(const uint32_t *w, uint32_t pos) {
   const uint32_t i = pos >> 5, s = pos & 31u;
   const uint64_t v = ((uint64_t)w[i] << 32) | w[i + 1];
   return (uint32_t)((v << s) >> 32);
@@ -94,7 +89,7 @@ LJPEG_HD uint32_t ljpeg_peek(const uint32_t *w, uint32_t pos) {
 // Decodes the symbol at the top of `hi`: returns the bits it takes (code + extra bits) and its difference in `diff`.  A code that no
 // table entry matches takes 16 bits with difference 0 and sets `bad` (a speculative decode meets those all the time; only the write
 // pass reports them).  Category 16 is 32768 with no extra bits (T.81 H.1.2.2), stored as the int16 -32768 (the same modulo 2^16).
-LJPEG_HD uint32_t ljpeg_symbol(const LjpegTable &t, uint32_t hi, int32_t &diff, bool &bad) {
+DB_HD uint32_t ljpeg_symbol(const LjpegTable &t, uint32_t hi, int32_t &diff, bool &bad) {
   uint32_t e = t.lut[hi >> (32 - kLjpegLutBits)];
   if (e == 0) {
     const int32_t code16 = (int32_t)(hi >> 16);
@@ -113,7 +108,7 @@ LJPEG_HD uint32_t ljpeg_symbol(const LjpegTable &t, uint32_t hi, int32_t &diff, 
 
 // Decodes the symbols that START before bit `end` from (pos, phase): advances them and counts the symbols.  No output: the
 // synchronisation passes only need the state.
-LJPEG_HD void ljpeg_span(const uint32_t *w, const LjpegTable *const *tab, int ncomp, uint32_t &pos, int &phase, uint32_t end,
+DB_HD void ljpeg_span(const uint32_t *w, const LjpegTable *const *tab, int ncomp, uint32_t &pos, int &phase, uint32_t end,
                          uint32_t &cnt) {
   bool bad = false;
   while (pos < end) {
@@ -126,7 +121,7 @@ LJPEG_HD void ljpeg_span(const uint32_t *w, const LjpegTable *const *tab, int nc
 
 // Geometry of one subsequence.
 struct LjpegSub { const uint32_t *w; uint32_t jl, nsub_eff, clean_bits; };
-LJPEG_HD LjpegSub ljpeg_sub(const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len) {
+DB_HD LjpegSub ljpeg_sub(const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len) {
   LjpegSub s;
   s.w = reinterpret_cast<const uint32_t *>(clean + u.clean_off);
   s.jl = (uint32_t)(g - u.first_sub);
@@ -145,7 +140,7 @@ LJPEG_HD LjpegSub ljpeg_sub(const LjpegUnit &u, int64_t g, const uint8_t *clean,
 // written by a chain that entered the subsequence in its true state, whatever the order in which the threads run.  `atomic_max`
 // returns the old value.
 template <class AtomicMax>
-LJPEG_HD void ljpeg_walk(const LjpegImage &im, const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len,
+DB_HD void ljpeg_walk(const LjpegImage &im, const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len,
                          const LjpegTable *tables, uint64_t *rec, AtomicMax atomic_max) {
   const LjpegSub s = ljpeg_sub(u, g, clean, unit_clean_len);
   if (s.jl >= s.nsub_eff) return;
@@ -168,7 +163,7 @@ LJPEG_HD void ljpeg_walk(const LjpegImage &im, const LjpegUnit &u, int64_t g, co
 // L3, one thread per subsequence: decodes it from its true entry state and writes the differences of its symbols (first symbol index
 // `first`, the exclusive scan of the counts) into the arena.  Symbols at or past the unit's sample count are the pad bits behind the
 // data.  Returns true when a code of the unit's data matches no table entry.
-LJPEG_HD bool ljpeg_write(const LjpegImage &im, const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len,
+DB_HD bool ljpeg_write(const LjpegImage &im, const LjpegUnit &u, int64_t g, const uint8_t *clean, const uint32_t *unit_clean_len,
                           const LjpegTable *tables, const uint64_t *rec, uint32_t first, int16_t *diff) {
   const LjpegSub s = ljpeg_sub(u, g, clean, unit_clean_len);
   if (s.jl >= s.nsub_eff) return false;
@@ -194,7 +189,7 @@ LJPEG_HD bool ljpeg_write(const LjpegImage &im, const LjpegUnit &u, int64_t g, c
 // L4 step: the prediction of sample (x, y) of a component (T.81 H.1.2.1; libjpeg-turbo jdpred.c).  The first line of the scan and of
 // every restart band is predicted by 2^(P - Pt - 1) at x = 0 and by Ra behind it; the first column of every other line by Rb.  Ra, Rb
 // and Rc are reconstructed values in [0, 65535]; the caller adds the difference modulo 2^16.
-LJPEG_HD int32_t ljpeg_predict(int pred, bool first_line, int x, int32_t init, int32_t Ra, int32_t Rb, int32_t Rc) {
+DB_HD int32_t ljpeg_predict(int pred, bool first_line, int x, int32_t init, int32_t Ra, int32_t Rb, int32_t Rc) {
   if (first_line) return x == 0 ? init : Ra;
   if (x == 0) return Rb;
   switch (pred) {
@@ -212,7 +207,7 @@ LJPEG_HD int32_t ljpeg_predict(int pred, bool first_line, int x, int32_t init, i
 // component: GRAY, or the sample replicated for RGB / BGR.  Three components: R, G, B as stored; GRAY by `gray` (the baseline path's
 // rule for an RGB JPEG).
 template <class Gray>
-LJPEG_HD void ljpeg_pixel(const LjpegImage &im, const int16_t *diff, int64_t e, Gray gray) {
+DB_HD void ljpeg_pixel(const LjpegImage &im, const int16_t *diff, int64_t e, Gray gray) {
   const int lx = (int)(e % im.win_w), ly = (int)(e / im.win_w);
   const int64_t s = ((int64_t)(im.win_y0 + ly) * im.width + im.win_x0 + lx) * im.ncomp;
   const int sh = im.pt;

@@ -8,16 +8,10 @@
 
 namespace dalib200 {
 
-__device__ __forceinline__ int find_perm(const PermDesc *d, int n, int64_t v) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { int mid = (lo + hi + 1) >> 1; if (d[mid].first_item <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 __global__ void __launch_bounds__(kPermThreads) permute_kernel(const PermDesc *__restrict__ descs, int n, int64_t total_items) {
   __shared__ __align__(16) uint8_t sm[kPermSmemBytes];
   for (int64_t item = blockIdx.x; item < total_items; item += gridDim.x) {
-    const PermDesc &d = descs[find_perm(descs, n, item)];
+    const PermDesc &d = descs[last_at_most(descs, 0, n - 1, item, [](const PermDesc &p) { return p.first_item; })];
     const int64_t local = item - d.first_item;
     if (d.path == kPermPathRow) {
       const PermRowItem it = perm_row_item(d, local);

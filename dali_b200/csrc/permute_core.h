@@ -17,12 +17,7 @@
 #define DALI_B200_CSRC_PERMUTE_CORE_H_
 
 #include <stdint.h>
-
-#ifdef __CUDACC__
-#define PERM_HD __host__ __device__ __forceinline__
-#else
-#define PERM_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -54,7 +49,7 @@ struct PermDesc {
 };
 
 // the byte offsets of outer index `o` on both sides
-PERM_HD void perm_outer(const PermDesc &d, int64_t o, int64_t *io, int64_t *oo) {
+DB_HD void perm_outer(const PermDesc &d, int64_t o, int64_t *io, int64_t *oo) {
   int64_t a = 0, b = 0;
   for (int k = d.nouter - 1; k >= 0; k--) {
     const int64_t q = o / d.ext[k], idx = o - q * d.ext[k];
@@ -65,12 +60,12 @@ PERM_HD void perm_outer(const PermDesc &d, int64_t o, int64_t *io, int64_t *oo) 
 
 // ---------------------------------------------------------------------------------------------------------------- spans
 template <typename W>
-PERM_HD void perm_words(uint8_t *dst, const uint8_t *src, int64_t nwords, int tid, int nt) {
+DB_HD void perm_words(uint8_t *dst, const uint8_t *src, int64_t nwords, int tid, int nt) {
   for (int64_t i = tid; i < nwords; i += nt) reinterpret_cast<W *>(dst)[i] = reinterpret_cast<const W *>(src)[i];
 }
 
 // a contiguous span, in the widest words that both addresses and the length allow
-PERM_HD void perm_span(uint8_t *dst, const uint8_t *src, int64_t bytes, int tid, int nt) {
+DB_HD void perm_span(uint8_t *dst, const uint8_t *src, int64_t bytes, int tid, int nt) {
   const uint64_t a = (uint64_t)(uintptr_t)dst | (uint64_t)(uintptr_t)src | (uint64_t)bytes;
   if ((a & 15) == 0) perm_words<PermV16>(dst, src, bytes >> 4, tid, nt);
   else if ((a & 7) == 0) perm_words<PermV8>(dst, src, bytes >> 3, tid, nt);
@@ -85,7 +80,7 @@ struct PermTile {
   int32_t cx, cy;                       // units of this tile along X and Y (edge tiles are partial)
 };
 
-PERM_HD PermTile perm_tile_at(const PermDesc &d, int64_t local) {
+DB_HD PermTile perm_tile_at(const PermDesc &d, int64_t local) {
   const int64_t tx = local % d.ntx;
   local /= d.ntx;
   const int64_t ty = local % d.nty, o = local / d.nty;
@@ -100,12 +95,12 @@ PERM_HD PermTile perm_tile_at(const PermDesc &d, int64_t local) {
   return t;
 }
 
-PERM_HD int32_t perm_smem_at(const PermDesc &d, int32_t x, int32_t y, int32_t b, int32_t k) {
+DB_HD int32_t perm_smem_at(const PermDesc &d, int32_t x, int32_t y, int32_t b, int32_t k) {
   return d.out_major ? x * d.pitch + (y * k + b) * d.ps : y * d.pitch + (x * k + b) * d.ps;
 }
 
 template <typename T>
-PERM_HD void perm_tile_load(const PermDesc &d, const PermTile &t, uint8_t *sm, int tid, int nt) {
+DB_HD void perm_tile_load(const PermDesc &d, const PermTile &t, uint8_t *sm, int tid, int nt) {
   const int32_t k = (int32_t)(d.r / d.ps);
   if (!d.out_major && d.pitch == t.cx * d.r && (t.cy == 1 || d.istr_y == d.pitch) && (t.cx == 1 || d.istr_x == d.r)) {
     perm_span(sm, t.in, (int64_t)t.cy * d.pitch, tid, nt);
@@ -120,7 +115,7 @@ PERM_HD void perm_tile_load(const PermDesc &d, const PermTile &t, uint8_t *sm, i
 }
 
 template <typename T>
-PERM_HD void perm_tile_store(const PermDesc &d, const PermTile &t, const uint8_t *sm, int tid, int nt) {
+DB_HD void perm_tile_store(const PermDesc &d, const PermTile &t, const uint8_t *sm, int tid, int nt) {
   const int32_t k = (int32_t)(d.r / d.ps);
   if (d.out_major && d.pitch == t.cy * d.r && (t.cx == 1 || d.ostr_x == d.pitch) && (t.cy == 1 || d.ostr_y == d.r)) {
     perm_span(t.out, sm, (int64_t)t.cx * d.pitch, tid, nt);
@@ -140,7 +135,7 @@ struct PermRowItem {
   int32_t nrows;
 };
 
-PERM_HD PermRowItem perm_row_item(const PermDesc &d, int64_t local) {
+DB_HD PermRowItem perm_row_item(const PermDesc &d, int64_t local) {
   PermRowItem it;
   if (d.segs > 1) {
     it.row0 = local / d.segs;
@@ -156,12 +151,12 @@ PERM_HD PermRowItem perm_row_item(const PermDesc &d, int64_t local) {
 }
 
 // phase 1: the byte offsets of the item's rows, kept in shared memory (at most kPermTileBytes / kPermRowBytes rows)
-PERM_HD void perm_rows_prepare(const PermDesc &d, const PermRowItem &it, int64_t *sm, int tid, int nt) {
+DB_HD void perm_rows_prepare(const PermDesc &d, const PermRowItem &it, int64_t *sm, int tid, int nt) {
   for (int32_t j = tid; j < it.nrows; j += nt) perm_outer(d, it.row0 + j, &sm[2 * j], &sm[2 * j + 1]);
 }
 
 template <typename W>
-PERM_HD void perm_rows_copy_w(const PermDesc &d, const PermRowItem &it, const int64_t *sm, int tid, int nt) {
+DB_HD void perm_rows_copy_w(const PermDesc &d, const PermRowItem &it, const int64_t *sm, int tid, int nt) {
   const int64_t len = it.b1 - it.b0;
   // every row starts at the same offset modulo sizeof(W) on both sides (d.w divides the strides and in - out)
   int64_t h = (int64_t)((0 - (uint64_t)(uintptr_t)(d.out + it.b0)) & (sizeof(W) - 1));
@@ -181,7 +176,7 @@ PERM_HD void perm_rows_copy_w(const PermDesc &d, const PermRowItem &it, const in
   }
 }
 
-PERM_HD void perm_rows_copy(const PermDesc &d, const PermRowItem &it, const int64_t *sm, int tid, int nt) {
+DB_HD void perm_rows_copy(const PermDesc &d, const PermRowItem &it, const int64_t *sm, int tid, int nt) {
   switch (d.w) {
     case 16: perm_rows_copy_w<PermV16>(d, it, sm, tid, nt); break;
     case 8: perm_rows_copy_w<PermV8>(d, it, sm, tid, nt); break;
@@ -192,7 +187,7 @@ PERM_HD void perm_rows_copy(const PermDesc &d, const PermRowItem &it, const int6
 }
 
 // phase 1 / phase 2 of a TILE item, dispatched on the piece size
-PERM_HD void perm_tile_phase(const PermDesc &d, const PermTile &t, uint8_t *sm, int tid, int nt, bool store) {
+DB_HD void perm_tile_phase(const PermDesc &d, const PermTile &t, uint8_t *sm, int tid, int nt, bool store) {
   switch (d.ps) {
     case 16: store ? perm_tile_store<PermV16>(d, t, sm, tid, nt) : perm_tile_load<PermV16>(d, t, sm, tid, nt); break;
     case 8: store ? perm_tile_store<PermV8>(d, t, sm, tid, nt) : perm_tile_load<PermV8>(d, t, sm, tid, nt); break;

@@ -38,9 +38,7 @@ __global__ void __launch_bounds__(256) png_color_kernel(const PngImage *__restri
                                                         const uint8_t *__restrict__ scan) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-    const PngImage &im = images[lo];
+    const PngImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const PngImage &m) { return m.first_px; })];
     const int64_t lp = e - im.first_px;
     const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
     png_pixel(im, scan + im.scan_off, lx, ly);

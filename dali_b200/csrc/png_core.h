@@ -16,12 +16,7 @@
 #define DALI_B200_CSRC_PNG_CORE_H_
 #include <stdint.h>
 #include "inflate.h"
-
-#if defined(__CUDACC__)
-#define PNG_HD __host__ __device__ __forceinline__
-#else
-#define PNG_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -51,7 +46,7 @@ struct PngImage {
 };
 
 // Adam7: pass p starts at (x0, y0) and steps (dx, dy); a non-interlaced image is one pass (0, 0, 1, 1)
-PNG_HD void png_pass_geom(int interlace, int p, int &x0, int &y0, int &dx, int &dy) {
+DB_HD void png_pass_geom(int interlace, int p, int &x0, int &y0, int &dx, int &dy) {
   if (!interlace) { x0 = y0 = 0; dx = dy = 1; return; }
   switch (p) {
     case 0: x0 = 0; y0 = 0; dx = 8; dy = 8; break;
@@ -65,7 +60,7 @@ PNG_HD void png_pass_geom(int interlace, int p, int &x0, int &y0, int &dx, int &
 }
 
 // Adam7 pass of pixel (x, y): the 8 x 8 pattern of the PNG specification (8.2), decided on (y & 7, x & 7)
-PNG_HD int png_adam7_pass(int x, int y) {
+DB_HD int png_adam7_pass(int x, int y) {
   const int xm = x & 7, ym = y & 7;
   if (ym & 1) return 6;
   if (xm & 1) return 5;
@@ -78,13 +73,13 @@ PNG_HD int png_adam7_pass(int x, int y) {
 
 // CRC-32 (ISO 3309, as PNG uses it) over an IDAT chunk's type and data, against the value stored behind them.  `table`: the 256
 // entries of the reflected polynomial 0xEDB88320, indexed by the low byte.
-PNG_HD bool png_chunk_crc_ok(const uint8_t *type, uint32_t len, const uint32_t *table) {
+DB_HD bool png_chunk_crc_ok(const uint8_t *type, uint32_t len, const uint32_t *table) {
   uint32_t c = 0xFFFFFFFFu;
   for (uint32_t i = 0; i < len + 4; i++) c = table[(c ^ type[i]) & 255] ^ (c >> 8);
   const uint8_t *e = type + 4 + len;
   return (c ^ 0xFFFFFFFFu) == (((uint32_t)e[0] << 24) | ((uint32_t)e[1] << 16) | ((uint32_t)e[2] << 8) | e[3]);
 }
-PNG_HD uint32_t png_crc_table_entry(uint32_t i) {
+DB_HD uint32_t png_crc_table_entry(uint32_t i) {
   uint32_t c = i;
   for (int k = 0; k < 8; k++) c = c & 1 ? 0xEDB88320u ^ (c >> 1) : c >> 1;
   return c;
@@ -102,7 +97,7 @@ PNG_HD uint32_t png_crc_table_entry(uint32_t i) {
 //     bad Adler-32 trailer met before that is an error;
 //   * once a byte beyond the image (a surplus) would be produced, libpng only drains the rest of the stream: malformed data or a bad
 //     trailer there is a warning, so the rest is decoded without output ("draining") and only its end is required.
-PNG_HD int png_inflate(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
+DB_HD int png_inflate(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
   InflateBits<PngChunk> b;
   ibits_init(b, raw + im.raw_off, chunks, im.chunk_begin, im.chunk_end);
   ibits_get(b, 16);                                       // CMF / FLG, checked by the planner
@@ -110,7 +105,7 @@ PNG_HD int png_inflate(const PngImage &im, const PngChunk *chunks, const uint8_t
 }
 
 // png_inflate, then the unfilter in place.  Returns 0, or 1 for a malformed stream or filter byte.
-PNG_HD int png_inflate_unfilter(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
+DB_HD int png_inflate_unfilter(const PngImage &im, const PngChunk *chunks, const uint8_t *raw, uint8_t *scan, InflateWork &w) {
   if (png_inflate(im, chunks, raw, scan, w)) return 1;
   // unfilter in place, pass by pass (filter types 0..4 of the PNG specification, 9.2); bpp = bytes of a whole pixel, at least 1
   const int bpp = (im.spp * im.depth + 7) >> 3;
@@ -160,7 +155,7 @@ PNG_HD int png_inflate_unfilter(const PngImage &im, const PngChunk *chunks, cons
 //   * 16-bit samples keep their high byte; alpha is dropped;
 //   * GRAY of a colour or palette pixel: (9797 R + 19234 G + 3737 B) >> 15 on 8-bit values, and on 16-bit samples
 //     ((9797 R + 19234 G + 3737 B + 16384) >> 15) >> 8.
-PNG_HD void png_pixel(const PngImage &im, const uint8_t *scan, int lx, int ly) {
+DB_HD void png_pixel(const PngImage &im, const uint8_t *scan, int lx, int ly) {
   const int x = im.win_x0 + lx, y = im.win_y0 + ly;
   int p = 0, px = x, py = y;
   if (im.interlace) {

@@ -31,15 +31,6 @@ struct PwDesc {
   float m[9], t[3];
 };
 
-__device__ __forceinline__ int find_pw_sample(const PwDesc *d, int n, int64_t q) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_quad <= q) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 template <int NB>
 __device__ __forceinline__ void load_bytes(const uint8_t *p, int n, uint8_t *b) {
   if (n == NB && (reinterpret_cast<uintptr_t>(p) & 3) == 0) {
@@ -110,7 +101,7 @@ __global__ void __launch_bounds__(256) linear_transform_kernel(const PwDesc *__r
   const int64_t per_cta = ((total_quads + gridDim.x - 1) / gridDim.x + 1023) / 1024 * 1024;
   const int64_t q0 = (int64_t)blockIdx.x * per_cta, q1 = min(total_quads, q0 + per_cta);
   if (q0 >= q1) return;
-  if (threadIdx.x == 0) s_first = find_pw_sample(descs, n, q0);
+  if (threadIdx.x == 0) s_first = last_at_most(descs, 0, n - 1, q0, [](const PwDesc &d) { return d.first_quad; });
   __syncthreads();
   int s = s_first;
   for (int64_t gq = q0 + 4 * threadIdx.x; gq < q1; gq += 4 * blockDim.x) {
@@ -168,7 +159,7 @@ __global__ void __launch_bounds__(256) csc_kernel(const PwDesc *__restrict__ des
   const int64_t per_cta = ((total_quads + gridDim.x - 1) / gridDim.x + 255) / 256 * 256;
   const int64_t q0 = (int64_t)blockIdx.x * per_cta, q1 = min(total_quads, q0 + per_cta);
   if (q0 >= q1) return;
-  if (threadIdx.x == 0) s_first = find_pw_sample(descs, n, q0);
+  if (threadIdx.x == 0) s_first = last_at_most(descs, 0, n - 1, q0, [](const PwDesc &d) { return d.first_quad; });
   __syncthreads();
   int s = s_first;
   for (int64_t gq = q0 + threadIdx.x; gq < q1; gq += blockDim.x) {

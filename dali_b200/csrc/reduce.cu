@@ -8,15 +8,6 @@
 
 namespace dalib200 {
 
-__device__ __forceinline__ int find_red(const RedPass *d, int n, int64_t v, bool combine) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if ((combine ? d[mid].cfirst : d[mid].first_item) <= v) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 template <typename T, typename A, int E>
 __global__ void __launch_bounds__(kRedThreads) reduce_pass_kernel(const RedPass *__restrict__ descs, int n, int64_t total, RedFinal f) {
   __shared__ __align__(16) uint8_t smem[kRedSmemBytes];
@@ -24,7 +15,7 @@ __global__ void __launch_bounds__(kRedThreads) reduce_pass_kernel(const RedPass 
   A *sm2 = reinterpret_cast<A *>(smem + kRedThreads * 16 * 8);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int64_t item = blockIdx.x; item < total; item += gridDim.x) {
-    const RedPass &d = descs[find_red(descs, n, item, false)];
+    const RedPass &d = descs[last_at_most(descs, 0, n - 1, item, [](const RedPass &p) { return p.first_item; })];
     const int64_t local = item - d.first_item;
     if (d.path == kRedPathColumns) {
       red_columns<T, A, E>(d, f, local, tid);
@@ -50,7 +41,7 @@ __global__ void __launch_bounds__(kRedThreads) reduce_pass_kernel(const RedPass 
 template <typename A, int E>
 __global__ void __launch_bounds__(kRedThreads) reduce_combine_kernel(const RedPass *__restrict__ descs, int n, int64_t total, RedFinal f) {
   for (int64_t item = blockIdx.x; item < total; item += gridDim.x) {
-    const RedPass &d = descs[find_red(descs, n, item, true)];
+    const RedPass &d = descs[last_at_most(descs, 0, n - 1, item, [](const RedPass &p) { return p.cfirst; })];
     red_combine<A, E>(d, f, item - d.cfirst, threadIdx.x);
   }
 }

@@ -19,12 +19,7 @@
 #include <stdint.h>
 #include <string.h>
 #include <math.h>
-
-#ifdef __CUDACC__
-#define RED_HD __host__ __device__ __forceinline__
-#else
-#define RED_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -59,34 +54,34 @@ struct RedPass {
 struct RedFinal { int32_t op, out_type, ddof, pad; };
 
 // ---- conversions
-RED_HD float red_f32_of(uint32_t b) {
+DB_HD float red_f32_of(uint32_t b) {
 #ifdef __CUDA_ARCH__
   return __uint_as_float(b);
 #else
   float f; memcpy(&f, &b, 4); return f;
 #endif
 }
-RED_HD double red_f64_of(uint64_t b) {
+DB_HD double red_f64_of(uint64_t b) {
 #ifdef __CUDA_ARCH__
   return __longlong_as_double((long long)b);
 #else
   double f; memcpy(&f, &b, 8); return f;
 #endif
 }
-RED_HD uint64_t red_bits_f64(double x) {
+DB_HD uint64_t red_bits_f64(double x) {
 #ifdef __CUDA_ARCH__
   return (uint64_t)__double_as_longlong(x);
 #else
   uint64_t b; memcpy(&b, &x, 8); return b;
 #endif
 }
-RED_HD float red_h2f(uint16_t h) {
+DB_HD float red_h2f(uint16_t h) {
   const uint32_t s = (uint32_t)(h & 0x8000u) << 16, e = (h >> 10) & 31u, m = h & 1023u;
   if (e == 0) { const float f = (float)m * 5.9604644775390625e-8f; return s ? -f : f; }   // zero and subnormals: m * 2^-24
   return red_f32_of(s | (e == 31 ? 0x7F800000u | (m << 13) : ((e + 112u) << 23) | (m << 13)));
 }
 // double -> half, round to nearest even (numpy's astype(float16)); a float converts through it exactly
-RED_HD uint16_t red_d2h(double x) {
+DB_HD uint16_t red_d2h(double x) {
   const uint64_t b = red_bits_f64(x), a = b & 0x7FFFFFFFFFFFFFFFull;
   const uint16_t s = (uint16_t)((b >> 48) & 0x8000u);
   if (a > 0x7FF0000000000000ull) return s | 0x7E00u;
@@ -102,29 +97,29 @@ RED_HD uint16_t red_d2h(double x) {
   return e >= -14 ? (uint16_t)(s | (((uint32_t)(e + 14) << 10) + (uint32_t)q)) : (uint16_t)(s | (uint32_t)q);
 }
 
-template <typename T> struct RedVal { typedef T type; RED_HD static T get(T v) { return v; } };
-template <> struct RedVal<RedHalf> { typedef float type; RED_HD static float get(RedHalf v) { return red_h2f(v.bits); } };
+template <typename T> struct RedVal { typedef T type; DB_HD static T get(T v) { return v; } };
+template <> struct RedVal<RedHalf> { typedef float type; DB_HD static float get(RedHalf v) { return red_h2f(v.bits); } };
 
-template <typename A> RED_HD A red_inf();
-template <> RED_HD float red_inf<float>() { return red_f32_of(0x7F800000u); }
-template <> RED_HD double red_inf<double>() { return red_f64_of(0x7FF0000000000000ull); }
-template <> RED_HD int64_t red_inf<int64_t>() { return INT64_MAX; }
-template <> RED_HD uint64_t red_inf<uint64_t>() { return UINT64_MAX; }
-template <typename A> RED_HD A red_ninf();
-template <> RED_HD float red_ninf<float>() { return red_f32_of(0xFF800000u); }
-template <> RED_HD double red_ninf<double>() { return red_f64_of(0xFFF0000000000000ull); }
-template <> RED_HD int64_t red_ninf<int64_t>() { return INT64_MIN; }
-template <> RED_HD uint64_t red_ninf<uint64_t>() { return 0; }
+template <typename A> DB_HD A red_inf();
+template <> DB_HD float red_inf<float>() { return red_f32_of(0x7F800000u); }
+template <> DB_HD double red_inf<double>() { return red_f64_of(0x7FF0000000000000ull); }
+template <> DB_HD int64_t red_inf<int64_t>() { return INT64_MAX; }
+template <> DB_HD uint64_t red_inf<uint64_t>() { return UINT64_MAX; }
+template <typename A> DB_HD A red_ninf();
+template <> DB_HD float red_ninf<float>() { return red_f32_of(0xFF800000u); }
+template <> DB_HD double red_ninf<double>() { return red_f64_of(0xFFF0000000000000ull); }
+template <> DB_HD int64_t red_ninf<int64_t>() { return INT64_MIN; }
+template <> DB_HD uint64_t red_ninf<uint64_t>() { return 0; }
 
-template <int E, typename A> RED_HD A red_ident() { return E == kElemMin ? red_inf<A>() : E == kElemMax ? red_ninf<A>() : (A)0; }
+template <int E, typename A> DB_HD A red_ident() { return E == kElemMin ? red_inf<A>() : E == kElemMax ? red_ninf<A>() : (A)0; }
 // min / max propagate a NaN as np.min / np.max do; sums wrap for integers
-template <int E, typename A> RED_HD A red_comb(A a, A x) {
+template <int E, typename A> DB_HD A red_comb(A a, A x) {
   if (E == kElemMin) return (x < a || x != x) ? x : a;
   if (E == kElemMax) return (x > a || x != x) ? x : a;
   if ((A)0.5 == (A)0) return (A)((uint64_t)a + (uint64_t)x);    // integers wrap modulo 2^64
   return a + x;
 }
-template <int E, typename A, typename T> RED_HD A red_elem(T v, A m) {
+template <int E, typename A, typename T> DB_HD A red_elem(T v, A m) {
   const A x = (A)RedVal<T>::get(v);
   if (E == kElemSq) return x * x;
   if (E == kElemSqDev) { const A d = x - m; return d * d; }
@@ -132,7 +127,7 @@ template <int E, typename A, typename T> RED_HD A red_elem(T v, A m) {
 }
 
 // ---- the final value of one output, stored in the output type
-template <typename V> RED_HD void red_put(uint8_t *out, int32_t type, int64_t q, V v) {
+template <typename V> DB_HD void red_put(uint8_t *out, int32_t type, int64_t q, V v) {
   switch (type) {
     case kRedU8: reinterpret_cast<uint8_t *>(out)[q] = (uint8_t)v; break;
     case kRedU16: reinterpret_cast<uint16_t *>(out)[q] = (uint16_t)v; break;
@@ -148,7 +143,7 @@ template <typename V> RED_HD void red_put(uint8_t *out, int32_t type, int64_t q,
   }
 }
 // integer accumulators hold exact sums: the mean family divides them in double, one rounding to the output type follows
-template <typename A> RED_HD void red_final(const RedFinal &f, int64_t count, uint8_t *out, int64_t q, A acc) {
+template <typename A> DB_HD void red_final(const RedFinal &f, int64_t count, uint8_t *out, int64_t q, A acc) {
   const bool integral = (A)0.5 == (A)0;
   switch (f.op) {
     case kRedMin: case kRedMax: case kRedSum: red_put(out, f.out_type, q, acc); return;
@@ -172,14 +167,14 @@ template <typename A> RED_HD void red_final(const RedFinal &f, int64_t count, ui
   }
 }
 // output q of pass d holds acc: a partial of chunk ch, an intermediate of the next pass, or the sample's result
-template <typename A> RED_HD void red_store(const RedPass &d, const RedFinal &f, int64_t ch, int64_t q, A acc) {
+template <typename A> DB_HD void red_store(const RedPass &d, const RedFinal &f, int64_t ch, int64_t q, A acc) {
   if (d.nchunks > 1) { reinterpret_cast<A *>(d.part)[ch * d.O * d.I + q] = acc; return; }
   if (!d.last) { reinterpret_cast<A *>(d.out)[q] = acc; return; }
   red_final(f, d.count, d.out, q, acc);
 }
 
 // the mean of output (o, i) (first pass of std_dev / variance)
-RED_HD int64_t red_mean_index(const RedPass &d, int64_t o, int64_t i) {
+DB_HD int64_t red_mean_index(const RedPass &d, int64_t o, int64_t i) {
   int64_t idx = i;
   for (int g = 0; g < d.ngroups; g++) {
     const int64_t nx = o / d.gext[g];
@@ -191,7 +186,7 @@ RED_HD int64_t red_mean_index(const RedPass &d, int64_t o, int64_t i) {
 
 // ---- COLUMNS: thread tid of item `local` folds the rows of one chunk for one output
 template <typename T, typename A, int E>
-RED_HD void red_columns(const RedPass &d, const RedFinal &f, int64_t local, int tid) {
+DB_HD void red_columns(const RedPass &d, const RedFinal &f, int64_t local, int tid) {
   const int64_t tile = local / d.nchunks, ch = local - tile * d.nchunks, q = tile * kRedThreads + tid;
   if (q >= d.O * d.I) return;
   const int64_t o = q / d.I, i = q - o * d.I, r0 = ch * d.rc, r1 = r0 + d.rc < d.R ? r0 + d.rc : d.R;
@@ -204,7 +199,7 @@ RED_HD void red_columns(const RedPass &d, const RedFinal &f, int64_t local, int 
 
 // ---- INNER
 struct RedRun { int64_t o, ch, len, head; const uint8_t *base; };   // base: 16-byte aligned, `head` elements before the run
-template <typename T> RED_HD RedRun red_run(const RedPass &d, int64_t local) {
+template <typename T> DB_HD RedRun red_run(const RedPass &d, int64_t local) {
   RedRun u;
   u.o = local / d.nchunks; u.ch = local - u.o * d.nchunks;
   const int64_t r0 = u.ch * d.rc, r1 = r0 + d.rc < d.R ? r0 + d.rc : d.R;
@@ -216,7 +211,7 @@ template <typename T> RED_HD RedRun red_run(const RedPass &d, int64_t local) {
 }
 // phase 1: thread tid < d.active folds 16-byte words tid, tid + active, ...; its V partials go to sm[tid * V + j]
 template <typename T, typename A, int E>
-RED_HD void red_inner_fold(const RedPass &d, const RedRun &u, A *sm, int tid) {
+DB_HD void red_inner_fold(const RedPass &d, const RedRun &u, A *sm, int tid) {
   constexpr int V = 16 / (int)sizeof(T);
   if (tid >= d.active) return;
   A acc[V], m[V];
@@ -251,7 +246,7 @@ RED_HD void red_inner_fold(const RedPass &d, const RedRun &u, A *sm, int tid) {
 }
 // phase 2: thread q < I * S (S = 256 / I slices per i) folds the partials of i = q / S at slice s = q % S into sm2[q]
 template <typename T, typename A, int E>
-RED_HD void red_inner_slices(const RedPass &d, const RedRun &u, const A *sm, A *sm2, int q) {
+DB_HD void red_inner_slices(const RedPass &d, const RedRun &u, const A *sm, A *sm2, int q) {
   constexpr int V = 16 / (int)sizeof(T);
   const int I = (int)d.I, S = kRedThreads / I;
   if (q >= I * S) return;
@@ -261,21 +256,21 @@ RED_HD void red_inner_slices(const RedPass &d, const RedRun &u, const A *sm, A *
   sm2[q] = acc;
 }
 // phase 3, lane `lane` of the warp that finishes i: its share of the slices of i (a butterfly over the 32 lanes follows)
-template <typename A, int E> RED_HD A red_inner_lane(const RedPass &d, const A *sm2, int i, int lane) {
+template <typename A, int E> DB_HD A red_inner_lane(const RedPass &d, const A *sm2, int i, int lane) {
   const int S = kRedThreads / (int)d.I;
   A acc = red_ident<E, A>();
   for (int s = lane; s < S; s += 32) acc = red_comb<E, A>(acc, sm2[i * S + s]);
   return acc;
 }
 // the butterfly stated on 32 values (the device runs it with shuffles: v[l] += v[l + off] for off = 16, 8, 4, 2, 1); v[0] is the result
-template <typename A, int E> RED_HD A red_tree32(A *v) {
+template <typename A, int E> DB_HD A red_tree32(A *v) {
   for (int off = 16; off > 0; off >>= 1)
     for (int l = 0; l < off; l++) v[l] = red_comb<E, A>(v[l], v[l + off]);
   return v[0];
 }
 
 // ---- the combine launch: the chunk partials of one output, in chunk order
-template <typename A, int E> RED_HD void red_combine(const RedPass &d, const RedFinal &f, int64_t local, int tid) {
+template <typename A, int E> DB_HD void red_combine(const RedPass &d, const RedFinal &f, int64_t local, int tid) {
   const int64_t oi = d.O * d.I, q = local * kRedThreads + tid;
   if (q >= oi) return;
   const A *p = reinterpret_cast<const A *>(d.part) + q;

@@ -60,14 +60,6 @@ struct RsDesc {
 
 // ---------------------------------------------------------------------------------------------
 // device
-__device__ __forceinline__ int find_tile_sample(const RsDesc *d, int n, int64_t t) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_tile <= t) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
 
 template <typename T> __device__ __forceinline__ float ld_as_float(const T *p);
 template <> __device__ __forceinline__ float ld_as_float<uint8_t>(const uint8_t *p) { return (float)__ldg(p); }
@@ -222,7 +214,7 @@ __global__ void __launch_bounds__(256) resample_fused_kernel(const RsDesc *__res
                                                              int n, int64_t total_tiles) {
   extern __shared__ __align__(16) float tmp[];
   for (int64_t tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-    const int s = find_tile_sample(descs, n, tile);
+    const int s = last_at_most(descs, 0, n - 1, tile, [](const RsDesc &d) { return d.first_tile; });
     const RsDesc &d = descs[s];
     if (d.use_stream) continue;
     const int64_t tl = tile - d.first_tile;

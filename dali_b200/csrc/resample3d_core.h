@@ -9,12 +9,10 @@
 #ifndef DALI_B200_CSRC_RESAMPLE3D_CORE_H_
 #define DALI_B200_CSRC_RESAMPLE3D_CORE_H_
 #include <stdint.h>
+#include "host_device.h"
 
-#if defined(__CUDACC__)
-#define R3_HD __host__ __device__ __forceinline__
-#else
+#if !defined(__CUDACC__)
 #include <math.h>
-#define R3_HD inline
 #endif
 
 namespace dalib200 {
@@ -38,23 +36,23 @@ struct R3Pass {
 };
 
 #if defined(__CUDA_ARCH__)
-R3_HD float r3_mul(float a, float b) { return __fmul_rn(a, b); }
-R3_HD float r3_add(float a, float b) { return __fadd_rn(a, b); }
-R3_HD uint8_t r3_u8_away(float v) { return sat_u8_half_away(v); }
-R3_HD uint8_t r3_u8_even(float v) { return sat_u8_half_even(v); }
+DB_HD float r3_mul(float a, float b) { return __fmul_rn(a, b); }
+DB_HD float r3_add(float a, float b) { return __fadd_rn(a, b); }
+DB_HD uint8_t r3_u8_away(float v) { return sat_u8_half_away(v); }
+DB_HD uint8_t r3_u8_even(float v) { return sat_u8_half_even(v); }
 #else
 // host build: compile with -ffp-contract=off (no FMA contraction), default rounding mode
-R3_HD float r3_mul(float a, float b) { return a * b; }
-R3_HD float r3_add(float a, float b) { return a + b; }
-R3_HD uint8_t r3_u8_away(float v) { float r = roundf(v); return (uint8_t)(r <= 0.0f ? 0 : r >= 255.0f ? 255 : (int)r); }
-R3_HD uint8_t r3_u8_even(float v) { float r = nearbyintf(v); return (uint8_t)(r <= 0.0f ? 0 : r >= 255.0f ? 255 : (int)r); }
+DB_HD float r3_mul(float a, float b) { return a * b; }
+DB_HD float r3_add(float a, float b) { return a + b; }
+DB_HD uint8_t r3_u8_away(float v) { float r = roundf(v); return (uint8_t)(r <= 0.0f ? 0 : r >= 255.0f ? 255 : (int)r); }
+DB_HD uint8_t r3_u8_even(float v) { float r = nearbyintf(v); return (uint8_t)(r <= 0.0f ? 0 : r >= 255.0f ? 255 : (int)r); }
 #endif
 
-R3_HD float r3_load(const R3Pass &p, int64_t i) {
+DB_HD float r3_load(const R3Pass &p, int64_t i) {
   return p.in_u8 ? (float)static_cast<const uint8_t *>(p.in)[i] : static_cast<const float *>(p.in)[i];
 }
 
-R3_HD void r3_element(const R3Pass &p, const int32_t *tab, int64_t e) {
+DB_HD void r3_element(const R3Pass &p, const int32_t *tab, int64_t e) {
   // a pass has fewer than 2^31 output elements (the planner checks): 32-bit index arithmetic (a 64-bit division costs ~100 instructions)
   const uint32_t C = (uint32_t)p.C, X = (uint32_t)p.osz[0], Y = (uint32_t)p.osz[1];
   uint32_t t = (uint32_t)e;

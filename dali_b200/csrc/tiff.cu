@@ -35,9 +35,7 @@ __global__ void __launch_bounds__(256) tiff_color_kernel(const TiffImage *__rest
                                                          const TiffSeg *__restrict__ segs, const uint8_t *__restrict__ dec) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-    const TiffImage &im = images[lo];
+    const TiffImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const TiffImage &m) { return m.first_px; })];
     const int64_t lp = e - im.first_px;
     const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
     tiff_pixel(im, segs, dec, lx, ly);

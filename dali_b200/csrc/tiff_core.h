@@ -12,12 +12,7 @@
 #define DALI_B200_CSRC_TIFF_CORE_H_
 #include <stdint.h>
 #include "inflate.h"
-
-#if defined(__CUDACC__)
-#define TIFF_HD __host__ __device__ __forceinline__
-#else
-#define TIFF_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -61,7 +56,7 @@ struct TiffImage {
 // the first byte of the next one.  So the table is only the output offset where each code's string starts, `start` (kTiffLzwStarts
 // entries), and strings are copied out of the segment's own output.  Errors, as libtiff's: a first code that is not Clear, a code past
 // the next free one, a literal expected after Clear, a full table, EOI or the end of the data before the segment is complete.
-TIFF_HD int tiff_lzw(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t total, uint32_t *start) {
+DB_HD int tiff_lzw(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t total, uint32_t *start) {
   uint64_t acc = 0;
   int nb = 0;
   uint32_t pos = 0, out = 0;
@@ -96,7 +91,7 @@ TIFF_HD int tiff_lzw(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t tota
 }
 
 // PackBits (libtiff PackBitsDecode): a run longer than the rest of the segment is clipped, data ending early is an error
-TIFF_HD int tiff_packbits(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t total) {
+DB_HD int tiff_packbits(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t total) {
   uint32_t pos = 0, out = 0;
   while (pos < n && out < total) {
     int c = (int8_t)src[pos++];
@@ -118,7 +113,7 @@ TIFF_HD int tiff_packbits(const uint8_t *src, uint32_t n, uint8_t *dst, uint32_t
 // Decodes segment `s` into `dst` (s.rows * im.row_bytes bytes) and undoes the horizontal predictor row by row.  Returns 0, or 1 for a
 // malformed or short segment.  Reads stay inside the segment's bytes; writes inside [dst, dst + size).  `slot`: kTiffSlotBytes of
 // working memory (4-byte aligned).
-TIFF_HD int tiff_decode_segment(const TiffImage &im, const TiffSeg &s, const uint8_t *raw, uint8_t *dst, void *slot) {
+DB_HD int tiff_decode_segment(const TiffImage &im, const TiffSeg &s, const uint8_t *raw, uint8_t *dst, void *slot) {
   const uint8_t *src = raw + im.raw_off + s.off;
   const uint32_t total = s.rows * im.row_bytes;
   int rc = 0;
@@ -154,7 +149,7 @@ TIFF_HD int tiff_decode_segment(const TiffImage &im, const TiffSeg &s, const uin
 }
 
 // sample c of pixel (x, y), as stored (1 to 16 bits)
-TIFF_HD uint32_t tiff_sample(const TiffImage &im, const TiffSeg *segs, const uint8_t *dec, int x, int y, int c) {
+DB_HD uint32_t tiff_sample(const TiffImage &im, const TiffSeg *segs, const uint8_t *dec, int x, int y, int c) {
   const int plane = im.planar == 2 ? c : 0, sx = x / im.seg_w, sy = y / im.seg_h;
   const TiffSeg &s = segs[im.seg_begin + plane * im.segs_per_plane + sy * im.segs_across + sx];
   const int64_t bit = (int64_t)(x - sx * im.seg_w) * (im.planar == 2 ? 1 : im.spp) * im.bps + (im.planar == 2 ? 0 : c * im.bps);
@@ -172,7 +167,7 @@ TIFF_HD uint32_t tiff_sample(const TiffImage &im, const TiffSeg *segs, const uin
 //     no MinIsWhite inversion; unassociated alpha premultiplies, (c * a + 127) / 255 on the 8-bit values;
 //   * palette: the ColorMap scaled to 8 bits by the planner;
 //   * GRAY of a colour pixel: (1868 B + 9617 G + 4899 R + 8192) >> 14 (OpenCV's BGRA -> gray, the CMYK JPEG path's rule).
-TIFF_HD void tiff_pixel(const TiffImage &im, const TiffSeg *segs, const uint8_t *dec, int lx, int ly) {
+DB_HD void tiff_pixel(const TiffImage &im, const TiffSeg *segs, const uint8_t *dec, int lx, int ly) {
   const int x = im.win_x0 + lx, y = im.win_y0 + ly;
   uint32_t r, g, b;
   if (im.photometric == kTiffPalette) {

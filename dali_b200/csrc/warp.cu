@@ -31,15 +31,6 @@ struct WarpDesc {
   float m[6];
 };
 
-__device__ __forceinline__ int find_warp_sample(const WarpDesc *d, int n, int64_t t) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    int mid = (lo + hi + 1) >> 1;
-    if (d[mid].first_tile <= t) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 template <bool CLAMP>
 __device__ __forceinline__ float warp_fetch(const uint8_t *__restrict__ in, int H, int W, int C, int x, int y, int c, float border) {
   if ((unsigned)x < (unsigned)W && (unsigned)y < (unsigned)H) return (float)__ldg(in + ((int64_t)y * W + x) * C + c);
@@ -123,7 +114,7 @@ __global__ void __launch_bounds__(256) warp_affine_kernel(const WarpDesc *__rest
   const int64_t per_cta = (total_tiles + gridDim.x - 1) / gridDim.x;
   const int64_t t0 = (int64_t)blockIdx.x * per_cta, t1 = min(total_tiles, t0 + per_cta);
   if (t0 >= t1) return;
-  if (threadIdx.x == 0) s_first = find_warp_sample(descs, n, t0);
+  if (threadIdx.x == 0) s_first = last_at_most(descs, 0, n - 1, t0, [](const WarpDesc &d) { return d.first_tile; });
   __syncthreads();
   int s = s_first;
   for (int64_t tile = t0; tile < t1; tile++) {
@@ -227,7 +218,7 @@ __global__ void __launch_bounds__(256, 2) warp_affine_band_kernel(const WarpDesc
   const int64_t i0 = (int64_t)blockIdx.x * per_cta, i1 = min(total_items, i0 + per_cta);
   if (i0 >= i1) return;
   if (tid == 0) {
-    s_first = find_warp_sample(descs, n, i0);
+    s_first = last_at_most(descs, 0, n - 1, i0, [](const WarpDesc &d) { return d.first_tile; });
     mbar_init(&bars[0], 1); mbar_init(&bars[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }

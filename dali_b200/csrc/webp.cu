@@ -56,9 +56,7 @@ __global__ void __launch_bounds__(kWebpWaveThreads) webp_wave_kernel(const WebpI
 __global__ void __launch_bounds__(256) webp_color_kernel(const WebpImage *__restrict__ images, int nimages, int64_t total, uint8_t *scratch) {
   const int64_t step = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += step) {
-    int lo = 0, hi = nimages - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-    const WebpImage &im = images[lo];
+    const WebpImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const WebpImage &m) { return m.first_px; })];
     const int64_t lp = e - im.first_px;
     const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
     webp_pixel(im, scratch, lx, ly);

@@ -18,12 +18,7 @@
 #ifndef DALI_B200_CSRC_WEBP_CORE_H_
 #define DALI_B200_CSRC_WEBP_CORE_H_
 #include <stdint.h>
-
-#if defined(__CUDACC__)
-#define WEBP_HD __host__ __device__ __forceinline__
-#else
-#define WEBP_HD inline
-#endif
+#include "host_device.h"
 
 namespace dalib200 {
 
@@ -65,7 +60,7 @@ struct WebpImage {
 };
 
 // the padded planes of an image: Y (16 mb_w x 16 mb_h), then U and V (8 mb_w x 8 mb_h each)
-WEBP_HD uint8_t *webp_plane(const WebpImage &im, uint8_t *scratch, int c) {
+DB_HD uint8_t *webp_plane(const WebpImage &im, uint8_t *scratch, int c) {
   uint8_t *y = scratch + im.plane_off;
   const int64_t ny = (int64_t)im.mb_w * im.mb_h * 256;
   return c == 0 ? y : y + ny + (c - 1) * (ny >> 2);
@@ -122,23 +117,23 @@ struct WebpBits {
   int bits, eof;
 };
 
-WEBP_HD void webp_bits_load(WebpBits &b) {
+DB_HD void webp_bits_load(WebpBits &b) {
   if (b.buf < b.end) { b.bits += 8; b.value = (b.value << 8) | *b.buf++; }
   else if (!b.eof) { b.value <<= 8; b.bits += 8; b.eof = 1; }
   else { b.bits = 0; }
 }
-WEBP_HD void webp_bits_init(WebpBits &b, const uint8_t *p, uint32_t n) {
+DB_HD void webp_bits_init(WebpBits &b, const uint8_t *p, uint32_t n) {
   b.buf = p; b.end = p + n; b.value = 0; b.range = 254; b.bits = -8; b.eof = 0;
   webp_bits_load(b);
 }
-WEBP_HD int webp_log2_floor(uint32_t v) {
+DB_HD int webp_log2_floor(uint32_t v) {
 #if defined(__CUDA_ARCH__)
   return 31 - __clz(v);
 #else
   return 31 - __builtin_clz(v);
 #endif
 }
-WEBP_HD int webp_bit(WebpBits &b, int prob) {
+DB_HD int webp_bit(WebpBits &b, int prob) {
   uint32_t range = b.range;
   if (b.bits < 0) webp_bits_load(b);
   const int pos = b.bits;
@@ -154,7 +149,7 @@ WEBP_HD int webp_bit(WebpBits &b, int prob) {
   return bit;
 }
 // VP8GetSigned: the sign bit at probability 1/2, always one bit of shift (the range never is 255 here)
-WEBP_HD int webp_signed(WebpBits &b, int v) {
+DB_HD int webp_signed(WebpBits &b, int v) {
   if (b.bits < 0) webp_bits_load(b);
   const int pos = b.bits;
   const uint32_t split = b.range >> 1;
@@ -166,19 +161,19 @@ WEBP_HD int webp_signed(WebpBits &b, int v) {
   b.value -= ((split + 1) & (uint32_t)mask) << pos;
   return (v ^ mask) - mask;
 }
-WEBP_HD uint32_t webp_value(WebpBits &b, int nbits) {
+DB_HD uint32_t webp_value(WebpBits &b, int nbits) {
   uint32_t v = 0;
   while (nbits-- > 0) v |= (uint32_t)webp_bit(b, 0x80) << nbits;
   return v;
 }
-WEBP_HD int webp_signed_value(WebpBits &b, int nbits) {
+DB_HD int webp_signed_value(WebpBits &b, int nbits) {
   const int v = (int)webp_value(b, nbits);
   return webp_bit(b, 0x80) ? -v : v;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Entropy decode (libwebp GetCoeffsFast / GetLargeValue).  `bp`: the probabilities of one block type, [band][ctx][11].
-WEBP_HD int webp_large_value(WebpBits &b, const uint8_t *p) {
+DB_HD int webp_large_value(WebpBits &b, const uint8_t *p) {
   int v;
   if (!webp_bit(b, p[3])) {
     v = !webp_bit(b, p[4]) ? 2 : 3 + webp_bit(b, p[5]);
@@ -196,7 +191,7 @@ WEBP_HD int webp_large_value(WebpBits &b, const uint8_t *p) {
   return v;
 }
 // Tokens of one block from coefficient n on into out[16] (zeroed by the caller).  Returns the index behind the last token.
-WEBP_HD int webp_coeffs(WebpBits &b, const uint8_t *bp, int ctx, int dq0, int dq1, int n, int16_t *out) {
+DB_HD int webp_coeffs(WebpBits &b, const uint8_t *bp, int ctx, int dq0, int dq1, int n, int16_t *out) {
   const uint8_t *p = bp + (WEBP_T(webp_bands)[n] * 3 + ctx) * 11;
   for (; n < 16; ++n) {
     if (!webp_bit(b, p[0])) return n;
@@ -214,7 +209,7 @@ WEBP_HD int webp_coeffs(WebpBits &b, const uint8_t *bp, int ctx, int dq0, int dq
 }
 
 // libwebp TransformWHT: the 16 luma DCs of a 16x16 macroblock from its Y2 block, into coefficient 0 of each 4x4 block
-WEBP_HD void webp_wht(const int16_t *in, int16_t *out) {
+DB_HD void webp_wht(const int16_t *in, int16_t *out) {
   int tmp[16];
   for (int i = 0; i < 4; ++i) {
     const int a0 = in[0 + i] + in[12 + i], a1 = in[4 + i] + in[8 + i];
@@ -231,7 +226,7 @@ WEBP_HD void webp_wht(const int16_t *in, int16_t *out) {
   }
 }
 
-WEBP_HD void webp_bits_restore(WebpBits &b, const WebpBitState &s, const uint8_t *base) {
+DB_HD void webp_bits_restore(WebpBits &b, const WebpBitState &s, const uint8_t *base) {
   b.buf = base + s.pos; b.end = base + s.end; b.value = s.value; b.range = s.range; b.bits = s.bits; b.eof = s.eof;
 }
 
@@ -239,7 +234,7 @@ WEBP_HD void webp_bits_restore(WebpBits &b, const WebpBitState &s, const uint8_t
 // macroblock records and the dequantised coefficients (384 per macroblock, zero-filled; not written for a skipped macroblock).
 // `top`: mb_w words of per-column context (bits 0-15: the four 4x4 modes of the bottom row, 16-23: non-zero flags, 24: Y2 non-zero).
 // Returns 0, or 1 when a partition ran out of data (libwebp: "Premature end-of-partition0" / "Premature end-of-file").
-WEBP_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int16_t *coef, uint32_t *top) {
+DB_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int16_t *coef, uint32_t *top) {
   const uint8_t *base = raw + im.raw_off;
   WebpBits br;
   webp_bits_restore(br, im.br0, base);
@@ -360,12 +355,12 @@ WEBP_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, i
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Reconstruction (libwebp ReconstructRow): prediction from the unfiltered neighbours, then the inverse DCT added block by block.
-WEBP_HD uint8_t webp_clip8(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
-WEBP_HD int webp_mul1(int a) { return ((a * 20091) >> 16) + a; }
-WEBP_HD int webp_mul2(int a) { return (a * 35468) >> 16; }
+DB_HD uint8_t webp_clip8(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v); }
+DB_HD int webp_mul1(int a) { return ((a * 20091) >> 16) + a; }
+DB_HD int webp_mul2(int a) { return (a * 35468) >> 16; }
 
 // libwebp TransformOne: adds the inverse DCT of `in` to the 4x4 block at dst
-WEBP_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride) {
+DB_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride) {
   int C[16];
   int *tmp = C;
   for (int i = 0; i < 4; ++i) {
@@ -387,11 +382,11 @@ WEBP_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride) {
   }
 }
 
-WEBP_HD uint8_t webp_avg3(int a, int b, int c) { return (uint8_t)((a + 2 * b + c + 2) >> 2); }
-WEBP_HD uint8_t webp_avg2(int a, int b) { return (uint8_t)((a + b + 1) >> 1); }
+DB_HD uint8_t webp_avg3(int a, int b, int c) { return (uint8_t)((a + 2 * b + c + 2) >> 2); }
+DB_HD uint8_t webp_avg2(int a, int b) { return (uint8_t)((a + b + 1) >> 1); }
 
 // libwebp's 4x4 predictors.  T[0]: top-left, T[1..8]: the 8 samples above (4 above, 4 above-right), L[0..3]: left.
-WEBP_HD void webp_pred4(int mode, const uint8_t *T, const uint8_t *L, uint8_t *d /* 4x4, stride 4 */) {
+DB_HD void webp_pred4(int mode, const uint8_t *T, const uint8_t *L, uint8_t *d /* 4x4, stride 4 */) {
   const int X = T[0], A = T[1], B = T[2], C = T[3], D = T[4], E = T[5], F = T[6], G = T[7], H = T[8];
   const int I = L[0], J = L[1], K = L[2], Lq = L[3];
 #define DST(x, y) d[(x) + (y) * 4]
@@ -485,7 +480,7 @@ WEBP_HD void webp_pred4(int mode, const uint8_t *T, const uint8_t *L, uint8_t *d
 
 // 16x16 or 8x8 prediction into dst (libwebp's VP8PredLuma16 / VP8PredChroma8 after CheckMode: DC without top and / or left samples).
 // top[0]: top-left, top[1..n]: above; left[0..n-1].
-WEBP_HD void webp_pred_block(int mode, int n, int mbx, int mby, const uint8_t *top, const uint8_t *left, uint8_t *dst, int stride) {
+DB_HD void webp_pred_block(int mode, int n, int mbx, int mby, const uint8_t *top, const uint8_t *left, uint8_t *dst, int stride) {
   const int sh = n == 16 ? 4 : 3;
   int dc = 0;
   if (mode == kWebpDC) {
@@ -514,7 +509,7 @@ WEBP_HD void webp_pred_block(int mode, int n, int mbx, int mby, const uint8_t *t
 
 // Reconstructs macroblock (mbx, mby) into the padded planes.  Reads the unfiltered left, top and top-right macroblocks: the caller
 // orders the macroblocks so that (mbx - 1, mby), (mbx, mby - 1) and (mbx + 1, mby - 1) are complete.
-WEBP_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t *coef, uint8_t *scratch, int mbx, int mby) {
+DB_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t *coef, uint8_t *scratch, int mbx, int mby) {
   const int64_t m = (int64_t)mby * im.mb_w + mbx;
   const WebpMb mb = mbs[m];
   const int16_t *c = coef + m * 384;
@@ -567,18 +562,18 @@ WEBP_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t
 
 // ---------------------------------------------------------------------------------------------------------------------------------
 // Loop filter (libwebp DoFilter and the dsp/dec.c filters), in place on the padded planes
-WEBP_HD int webp_sclip1(int v) { return v < -128 ? -128 : v > 127 ? 127 : v; }
-WEBP_HD int webp_sclip2(int v) { return v < -16 ? -16 : v > 15 ? 15 : v; }
-WEBP_HD int webp_abs(int v) { return v < 0 ? -v : v; }
+DB_HD int webp_sclip1(int v) { return v < -128 ? -128 : v > 127 ? 127 : v; }
+DB_HD int webp_sclip2(int v) { return v < -16 ? -16 : v > 15 ? 15 : v; }
+DB_HD int webp_abs(int v) { return v < 0 ? -v : v; }
 
-WEBP_HD void webp_do_filter2(uint8_t *p, int step) {
+DB_HD void webp_do_filter2(uint8_t *p, int step) {
   const int p1 = p[-2 * step], p0 = p[-step], q0 = p[0], q1 = p[step];
   const int a = 3 * (q0 - p0) + webp_sclip1(p1 - q1);
   const int a1 = webp_sclip2((a + 4) >> 3), a2 = webp_sclip2((a + 3) >> 3);
   p[-step] = webp_clip8(p0 + a2);
   p[0] = webp_clip8(q0 - a1);
 }
-WEBP_HD void webp_do_filter4(uint8_t *p, int step) {
+DB_HD void webp_do_filter4(uint8_t *p, int step) {
   const int p1 = p[-2 * step], p0 = p[-step], q0 = p[0], q1 = p[step];
   const int a = 3 * (q0 - p0);
   const int a1 = webp_sclip2((a + 4) >> 3), a2 = webp_sclip2((a + 3) >> 3);
@@ -588,7 +583,7 @@ WEBP_HD void webp_do_filter4(uint8_t *p, int step) {
   p[0] = webp_clip8(q0 - a1);
   p[step] = webp_clip8(q1 - a3);
 }
-WEBP_HD void webp_do_filter6(uint8_t *p, int step) {
+DB_HD void webp_do_filter6(uint8_t *p, int step) {
   const int p2 = p[-3 * step], p1 = p[-2 * step], p0 = p[-step], q0 = p[0], q1 = p[step], q2 = p[2 * step];
   const int a = webp_sclip1(3 * (q0 - p0) + webp_sclip1(p1 - q1));
   const int a1 = (27 * a + 63) >> 7, a2 = (18 * a + 63) >> 7, a3 = (9 * a + 63) >> 7;
@@ -599,15 +594,15 @@ WEBP_HD void webp_do_filter6(uint8_t *p, int step) {
   p[step] = webp_clip8(q1 - a2);
   p[2 * step] = webp_clip8(q2 - a3);
 }
-WEBP_HD bool webp_hev(const uint8_t *p, int step, int thresh) {
+DB_HD bool webp_hev(const uint8_t *p, int step, int thresh) {
   const int p1 = p[-2 * step], p0 = p[-step], q0 = p[0], q1 = p[step];
   return webp_abs(p1 - p0) > thresh || webp_abs(q1 - q0) > thresh;
 }
-WEBP_HD bool webp_needs_filter(const uint8_t *p, int step, int t) {
+DB_HD bool webp_needs_filter(const uint8_t *p, int step, int t) {
   const int p1 = p[-2 * step], p0 = p[-step], q0 = p[0], q1 = p[step];
   return 4 * webp_abs(p0 - q0) + webp_abs(p1 - q1) <= t;
 }
-WEBP_HD bool webp_needs_filter2(const uint8_t *p, int step, int t, int it) {
+DB_HD bool webp_needs_filter2(const uint8_t *p, int step, int t, int it) {
   const int p3 = p[-4 * step], p2 = p[-3 * step], p1 = p[-2 * step], p0 = p[-step];
   const int q0 = p[0], q1 = p[step], q2 = p[2 * step], q3 = p[3 * step];
   if (4 * webp_abs(p0 - q0) + webp_abs(p1 - q1) > t) return false;
@@ -615,13 +610,13 @@ WEBP_HD bool webp_needs_filter2(const uint8_t *p, int step, int t, int it) {
          webp_abs(q2 - q1) <= it && webp_abs(q1 - q0) <= it;
 }
 // simple filter across one edge of `size` pixels: hstride steps across the edge, vstride along it
-WEBP_HD void webp_simple_edge(uint8_t *p, int hstride, int vstride, int thresh) {
+DB_HD void webp_simple_edge(uint8_t *p, int hstride, int vstride, int thresh) {
   const int t2 = 2 * thresh + 1;
   for (int i = 0; i < 16; ++i, p += vstride)
     if (webp_needs_filter(p, hstride, t2)) webp_do_filter2(p, hstride);
 }
 // normal filter: 6-tap on macroblock edges (mb_edge), 4-tap on inner edges
-WEBP_HD void webp_normal_edge(uint8_t *p, int hstride, int vstride, int size, int thresh, int ithresh, int hev_thresh, bool mb_edge) {
+DB_HD void webp_normal_edge(uint8_t *p, int hstride, int vstride, int size, int thresh, int ithresh, int hev_thresh, bool mb_edge) {
   const int t2 = 2 * thresh + 1;
   for (int i = 0; i < size; ++i, p += vstride) {
     if (!webp_needs_filter2(p, hstride, t2, ithresh)) continue;
@@ -633,7 +628,7 @@ WEBP_HD void webp_normal_edge(uint8_t *p, int hstride, int vstride, int size, in
 
 // Filters macroblock (mbx, mby) in place.  The caller orders the macroblocks so that (mbx - 1, mby) and (mbx + 1, mby - 1) -- whose
 // left edge wrote pixels this top edge reads -- are complete; two macroblocks on one diagonal mbx + 2 mby touch disjoint pixels.
-WEBP_HD void webp_filter_mb(const WebpImage &im, const WebpMb *mbs, uint8_t *scratch, int mbx, int mby) {
+DB_HD void webp_filter_mb(const WebpImage &im, const WebpMb *mbs, uint8_t *scratch, int mbx, int mby) {
   if (im.filter_type == 0) return;
   const WebpMb mb = mbs[(int64_t)mby * im.mb_w + mbx];
   const int limit = im.f_limit[mb.segment][mb.i4];
@@ -677,10 +672,10 @@ WEBP_HD void webp_filter_mb(const WebpImage &im, const WebpMb *mbs, uint8_t *scr
 // One output pixel of the window (lx, ly): libwebp's fancy upsampling (UpsampleRgbLinePair, restated per pixel) and VP8YUVToR/G/B.
 // Row r takes its chroma from the "near" chroma row with weight 3 and the "far" one with weight 1: row 0 and, for an even height, the
 // last row use one chroma row for both.  Column 0 and, for an even width, the last column use one chroma column.
-WEBP_HD int webp_mult_hi(int v, int coeff) { return (v * coeff) >> 8; }
-WEBP_HD int webp_clip_yuv(int v) { return (v & ~16383) == 0 ? (v >> 6) : v < 0 ? 0 : 255; }
+DB_HD int webp_mult_hi(int v, int coeff) { return (v * coeff) >> 8; }
+DB_HD int webp_clip_yuv(int v) { return (v & ~16383) == 0 ? (v >> 6) : v < 0 ? 0 : 255; }
 
-WEBP_HD void webp_pixel(const WebpImage &im, uint8_t *scratch, int lx, int ly) {
+DB_HD void webp_pixel(const WebpImage &im, uint8_t *scratch, int lx, int ly) {
   const int x = im.win_x0 + lx, r = im.win_y0 + ly;
   const int W = im.width, H = im.height;
   const int ys = 16 * im.mb_w, cs = 8 * im.mb_w;

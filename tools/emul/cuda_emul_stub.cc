@@ -193,10 +193,9 @@ static void run_prog_dc(Dim3 g, Dim3 b, void **args) {
   for (unsigned bx = 0; bx < g.x; bx++)
     for (unsigned tx = 0; tx < b.x; tx++)
       for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
-        int lo = 0, hi = nimages - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (first_blk[mid] <= e) lo = mid; else hi = mid - 1; }
-        prog_dc_difference(images[lo], coef, dc, e - first_blk[lo]);
-        if (e == first_blk[lo] && images[lo].incomplete) status[images[lo].sample] = 1;
+        const int i = last_at_most(first_blk, 0, nimages - 1, e);
+        prog_dc_difference(images[i], coef, dc, e - first_blk[i]);
+        if (e == first_blk[i] && images[i].incomplete) status[images[i].sample] = 1;
       }
 }
 
@@ -236,9 +235,7 @@ static void run_png_color(Dim3 g, Dim3 b, void **args) {
   for (unsigned bx = 0; bx < g.x; bx++)
     for (unsigned tx = 0; tx < b.x; tx++)
       for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
-        int lo = 0, hi = nimages - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-        const PngImage &im = images[lo];
+        const PngImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const PngImage &m) { return m.first_px; })];
         const int64_t lp = e - im.first_px;
         const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
         png_pixel(im, scan + im.scan_off, lx, ly);
@@ -274,9 +271,7 @@ static void run_tiff_color(Dim3 g, Dim3 b, void **args) {
   for (unsigned bx = 0; bx < g.x; bx++)
     for (unsigned tx = 0; tx < b.x; tx++)
       for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
-        int lo = 0, hi = nimages - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-        const TiffImage &im = images[lo];
+        const TiffImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const TiffImage &m) { return m.first_px; })];
         const int64_t lp = e - im.first_px;
         const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
         tiff_pixel(im, segs, dec, lx, ly);
@@ -329,9 +324,7 @@ static void run_webp_color(Dim3 g, Dim3 b, void **args) {
   for (unsigned bx = 0; bx < g.x; bx++)
     for (unsigned tx = 0; tx < b.x; tx++)
       for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
-        int lo = 0, hi = nimages - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_px <= e) lo = mid; else hi = mid - 1; }
-        const WebpImage &im = images[lo];
+        const WebpImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const WebpImage &m) { return m.first_px; })];
         const int64_t lp = e - im.first_px;
         const int ly = (int)(lp / im.win_w), lx = (int)(lp - (int64_t)ly * im.win_w);
         webp_pixel(im, scratch, lx, ly);
@@ -363,9 +356,7 @@ static void run_bitmap_color(Dim3 g, Dim3 b, void **args) {
   for (unsigned bx = 0; bx < g.x; bx++)
     for (unsigned tx = 0; tx < b.x; tx++)
       for (int64_t e = (int64_t)bx * b.x + tx; e < total; e += step) {
-        int lo = 0, hi = nimages - 1;
-        while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (images[mid].first_grp <= e) lo = mid; else hi = mid - 1; }
-        const BitmapImage &im = images[lo];
+        const BitmapImage &im = images[last_at_most(images, 0, nimages - 1, e, [](const BitmapImage &m) { return m.first_grp; })];
         bitmap_group(im, im.unpack == kBitmapDirect ? raw + im.raw_off : scratch + im.plane_off, e - im.first_grp);
       }
 }
@@ -471,14 +462,14 @@ static void run_flac_sync(void **args) {
   const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
   auto add = [](uint32_t *p, uint32_t v) { const uint32_t o = *p; *p = o + v; return o; };
   for (int64_t g = a.flac_bytes - 1; g >= 0; g--) {
-    const int f = audio_find(a.flac, a.nf, g, &FlacDesc::first_byte);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, g, [](const FlacDesc &d) { return d.first_byte; });
     flac_sync_at(a.flac[f], f, a.raw, g - a.flac[f].first_byte, a.fend, a.cand, a.ccount, add);
   }
 }
 static void run_flac_frame(void **args) {
   const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
   for (int64_t k = a.cand_slots - 1; k >= 0; k--) {
-    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::cand_base);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, k, [](const FlacDesc &d) { return d.cand_base; });
     flac_candidate(a.flac[f], f, a.raw, k - a.flac[f].cand_base, a.cand, a.ccount, a.fend);
   }
 }
@@ -490,7 +481,7 @@ static void run_flac_chain(void **args) {
 static void run_flac_decode(void **args) {
   const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
   for (int64_t k = a.frame_slots - 1; k >= 0; k--) {
-    const int f = audio_find(a.flac, a.nf, k, &FlacDesc::frame_base);
+    const int f = last_at_most(a.flac, 0, a.nf - 1, k, [](const FlacDesc &d) { return d.frame_base; });
     if (!flac_decode(a.flac[f], f, a.raw, k - a.flac[f].frame_base, a.frames, a.nframes, a.pcm)) a.status[a.flac[f].sample] = 1;
   }
 }
@@ -498,7 +489,7 @@ static void run_audio_convert(void **args) {
   const AudioLaunch &a = *static_cast<const AudioLaunch *>(args[0]);
   for (int i = a.n - 1; i >= 0; i--) *a.descs[i].rate_out = a.descs[i].rate;
   for (int64_t e = a.total_elems - 1; e >= 0; e--) {
-    const AudioDesc &d = a.descs[audio_find(a.descs, a.n, e, &AudioDesc::first_elem)];
+    const AudioDesc &d = a.descs[last_at_most(a.descs, 0, a.n - 1, e, [](const AudioDesc &p) { return p.first_elem; })];
     audio_convert(d, a.raw, a.pcm, e - d.first_elem, [](float x, float y) { return x * y; }, [](float x, float y) { return x + y; });
   }
 }
@@ -562,11 +553,6 @@ static std::vector<std::string> red_template_args(const std::string &name) {
   a.push_back(cur);
   return a;
 }
-static int red_find(const RedPass *d, int n, int64_t v, bool combine) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((combine ? d[mid].cfirst : d[mid].first_item) <= v) lo = mid; else hi = mid - 1; }
-  return lo;
-}
 static void run_reduce(const std::string &name, void **args, bool combine) {
   const RedPass *descs = *static_cast<const RedPass **>(args[0]);
   const int n = *static_cast<int *>(args[1]);
@@ -583,7 +569,7 @@ static void run_reduce(const std::string &name, void **args, bool combine) {
     constexpr int E = decltype(el)::value;
     A *sm = reinterpret_cast<A *>(smem), *sm2 = reinterpret_cast<A *>(smem + kRedThreads * 16 * 8);
     for (int64_t item = total - 1; item >= 0; item--) {
-      const RedPass &d = descs[red_find(descs, n, item, combine)];
+      const RedPass &d = descs[last_at_most(descs, 0, n - 1, item, [&](const RedPass &p) { return combine ? p.cfirst : p.first_item; })];
       if (combine) {
         for (int tx = kRedThreads - 1; tx >= 0; tx--) red_combine<A, E>(d, f, item - d.cfirst, tx);
         continue;
