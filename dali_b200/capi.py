@@ -52,6 +52,7 @@ EXPORTS = [
     "dalib200PermutePlanCreate", "dalib200PermutePlanDestroy", "dalib200TransposeSetup", "dalib200JoinSetup", "dalib200PermuteLaunch",
     "dalib200PermutePlanGetPaths",
     "dalib200ReducePlanCreate", "dalib200ReducePlanDestroy", "dalib200ReduceSetup", "dalib200ReduceLaunch", "dalib200ReducePlanGetPaths",
+    "dalib200EqualizePlanCreate", "dalib200EqualizePlanDestroy", "dalib200EqualizeSetup", "dalib200EqualizeLaunch",
 ]
 
 

@@ -7,6 +7,7 @@
 #include <string>
 #include "dali.h"
 #include "../../include/dali_b200.h"
+#include "../csrc/equalize_plan.h"
 
 using namespace dali;  // NOLINT
 
@@ -244,6 +245,20 @@ int dalihTestReduce(int op, int in_type, int n, int ndim, const int64_t *in_shap
   *out_ndim = ond;
   *out_type = t;
   snprintf(out_layout, cap, "%s", a.layout.c_str());
+  API_END
+}
+
+// Test hook (CPU): fn.experimental.equalize's type, layout and shape rules without a device -- the plan set-up the operator makes.
+// resolved: the layout the planner reads the input with (cap bytes; the output keeps the input's own layout).
+int dalihTestEqualize(int in_type, int n, int ndim, const int64_t *in_shapes, const char *layout, char *resolved, int cap) {
+  API_BEGIN
+  dalib200EqualizePlan *plan = nullptr;
+  PermuteSetupOrThrow(dalib200EqualizePlanCreate(&plan, std::max(n, 1)));
+  const int rc = dalib200EqualizeSetup(plan, in_type, n, ndim, in_shapes, layout);
+  dalib200EqualizePlanDestroy(plan);
+  PermuteSetupOrThrow(rc);
+  std::string err;
+  snprintf(resolved, cap, "%s", dalib200::kEqLayouts[dalib200::EqResolveLayout(layout, ndim, &err)]);
   API_END
 }
 

@@ -2584,6 +2584,55 @@ DALI_REGISTER_OPERATOR(reductions__RMS, ReduceGPU, GPU);
 DALI_REGISTER_OPERATOR(reductions__StdDev, ReduceGPU, GPU);
 DALI_REGISTER_OPERATOR(reductions__Variance, ReduceGPU, GPU);
 
+// =============================================================================================== experimental.Equalize
+// dali/operators/image/color/equalize (the reference's documented behaviour, DESIGN.md section 2): every channel of every frame of
+// every uint8 sample is mapped through the table cv2.equalizeHist builds from its histogram, by the two kernels of csrc/equalize.cu.
+DALI_SCHEMA(experimental__Equalize)
+    .DocStr("Performs grayscale/per-channel histogram equalization of uint8 images (HW, HWC, CHW and their sequences FHW, FHWC, FCHW).")
+    .NumInput(1).NumOutput(1).AllowSequences();
+
+class EqualizeGPU : public Operator<GPUBackend> {
+ public:
+  explicit EqualizeGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
+  ~EqualizeGPU() override { dalib200EqualizePlanDestroy(plan_); }
+
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    const int n = in.num_samples(), nd = in.shape().sample_dim();
+    std::vector<int64_t> is((size_t)n * nd);
+    for (int i = 0; i < n; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
+    if (n > cap_) {
+      dalib200EqualizePlanDestroy(plan_);
+      plan_ = nullptr;
+      cap_ = std::max(n, max_batch_size_);
+      CheckStatus(dalib200EqualizePlanCreate(&plan_, cap_), "experimental.Equalize");
+    }
+    if (dalib200EqualizeSetup(plan_, static_cast<int>(in.type()), n, nd, is.data(), in.GetLayout().str().c_str()))
+      throw DALIException(dalib200GetLastError());
+    out.resize(1);
+    out[0].type = DALI_UINT8;
+    out[0].shape = in.shape();
+    return true;
+  }
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(in.GetLayout());
+    const int n = out.num_samples();
+    std::vector<const void *> ip(n);
+    std::vector<void *> op(n);
+    for (int i = 0; i < n; i++) {
+      ip[i] = in.raw_tensor(i);
+      op[i] = out.raw_mutable_tensor(i);
+    }
+    CheckStatus(dalib200EqualizeLaunch(plan_, ip.data(), op.data(), ws.stream()), "experimental.Equalize");
+  }
+  dalib200EqualizePlan *plan_ = nullptr;
+  int cap_ = 0;
+};
+DALI_REGISTER_OPERATOR(experimental__Equalize, EqualizeGPU, GPU);
+
 // =============================================================================================== Rotate
 // dali/operators/image/remap/rotate.cc + rotate_params.h: a WarpAffine whose matrix is
 // translation(in / 2) * rotation2D(-a) * translation(-out / 2) with a = deg2rad(-angle) (counter-clockwise for a top-left origin)

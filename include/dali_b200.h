@@ -530,6 +530,22 @@ int dalib200ReduceLaunch(dalib200ReducePlan *plan, const void *const *in_ptrs, c
 int dalib200ReducePlanGetPaths(const dalib200ReducePlan *plan, int32_t *kinds, int32_t *depths, int cap);
 
 /* ------------------------------------------------------------------------------------------------
+ * fn.experimental.equalize (the reference's experimental.Equalize): per-channel histogram equalization of UINT8 images and sequences.
+ * Every (sample, frame, channel) plane is mapped through the table cv2.equalizeHist builds from that plane's histogram (DESIGN.md
+ * section 2).  Two launches per batch, plus zeroing the histogram scratch: the histogram of every plane, then the tables and the
+ * mapping (DESIGN.md section 5).  The histograms are integer, so the output is exact and the same alone or in any batch.
+ *   in_type       DALIDataType code of the data: UINT8 only
+ *   in_shapes     n x ndim; the output has the input's shape
+ *   layout        HW, HWC, CHW, FHW, FHWC or FCHW; "" or NULL: HW, HWC or FHWC by rank (2, 3, 4)
+ * At most 16 channels, and at most 2^31 - 1 pixels in one plane.  A type, layout or shape that does not fit fails with
+ * DALIB200_ERROR_INVALID_ARGUMENT and a message naming the sample.  Launch: in_ptrs, out_ptrs: n device buffers, any byte offset. */
+typedef struct dalib200EqualizePlan dalib200EqualizePlan;
+int dalib200EqualizePlanCreate(dalib200EqualizePlan **plan, int max_samples);
+int dalib200EqualizePlanDestroy(dalib200EqualizePlan *plan);
+int dalib200EqualizeSetup(dalib200EqualizePlan *plan, int in_type, int n, int ndim, const int64_t *in_shapes, const char *layout);
+int dalib200EqualizeLaunch(dalib200EqualizePlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Audio decode (fn.decoders.audio).  WAV (PCM 8 / 16 / 24 / 32-bit, IEEE float 32, WAVE_FORMAT_EXTENSIBLE with either) and native FLAC
  * (8 / 16 / 24 bits per sample, optional ID3v2 tag in front), detected from the bytes.  The host parses the container and STREAMINFO
  * only; the FLAC frames are found, checked (CRC-8, CRC-16, frame chain) and decoded on the device.  Samples read as libsndfile's

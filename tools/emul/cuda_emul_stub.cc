@@ -1,6 +1,6 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM, lossless JPEG, audio decode, arithmetic-expression and reduction kernels (and U2 / U3, which feed the
+// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM, lossless JPEG, audio decode, arithmetic-expression, reduction and equalize kernels (and U2 / U3, which feed the
 // lossless JPEG stage) are
 // EXECUTED on the host -- their bodies are single
 // host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h, bitmap_core.h, arith_core.h ...), so a
@@ -43,6 +43,7 @@
 #include "../../dali_b200/csrc/audio_decode_core.h"
 #include "../../dali_b200/csrc/arith_plan.h"
 #include "../../dali_b200/csrc/reduce_plan.h"
+#include "../../dali_b200/csrc/equalize_core.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -150,7 +151,7 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[30];
+static long g_emulated[32];
 long emul_launch_count(int which) { return g_emulated[which]; }
 void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
@@ -592,6 +593,30 @@ static void run_reduce(const std::string &name, void **args, bool combine) {
   red_dispatch(tc, acc, e, body);
 }
 
+// equalize.cu: the work items of the launch run in REVERSE order, the threads of each block in reverse order; the apply kernel's
+// per-plane warp scan runs lane by lane (eq_lut_plane)
+static void run_equalize(void **args, bool apply) {
+  const EqSample *descs = *static_cast<const EqSample **>(args[0]);
+  const int n = *static_cast<int *>(args[1]);
+  const int64_t total = *static_cast<int64_t *>(args[2]);
+  uint32_t *hist = *static_cast<uint32_t **>(args[3]);
+  static uint32_t sh[kEqSmemWords];
+  static uint8_t lut[kEqMaxChannels * 256];
+  for (int64_t item = total - 1; item >= 0; item--) {
+    const EqSample &d = descs[last_at_most(descs, 0, n - 1, item, [](const EqSample &e) { return e.first_item; })];
+    const int64_t local = item - d.first_item;
+    if (apply) {
+      const int64_t frame = eq_item(d, local).frame;
+      for (int c = d.C - 1; c >= 0; c--) eq_lut_plane(hist + d.hist_off + (frame * d.C + c) * 256, d.plane, lut + c * 256);
+      for (int t = kEqThreads - 1; t >= 0; t--) eq_apply_thread(d, local, lut, t);
+      continue;
+    }
+    memset(sh, 0, sizeof(sh));
+    for (int t = kEqThreads - 1; t >= 0; t--) eq_hist_thread(d, local, sh + ((t >> 5) % d.nsub) * d.C * 256, t);
+    for (int t = kEqThreads - 1; t >= 0; t--) eq_hist_flush(d, local, sh, hist, t);
+  }
+}
+
 cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **args, size_t, void *stream) {
   // the library is usually loaded with RTLD_LOCAL (ctypes): identify the kernel by the name of the host stub `func` points at
   Dl_info di;
@@ -630,6 +655,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const std::string kname = kernel_name(name);
   const bool is_reduce_pass = !kname.compare(0, 29, "dalib200::reduce_pass_kernel<");
   const bool is_reduce_combine = !kname.compare(0, 32, "dalib200::reduce_combine_kernel<");
+  const bool is_eq_hist = !strcmp(name, "_ZN8dalib20020equalize_hist_kernelEPKNS_8EqSampleEilPj");
+  const bool is_eq_apply = !strcmp(name, "_ZN8dalib20021equalize_apply_kernelEPKNS_8EqSampleEilPKj");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -665,6 +692,8 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   else if (is_arith) { run_arith(grid, block, args, is_arith_wide); g_emulated[27]++; }
   else if (is_reduce_pass) { run_reduce(kname, args, false); g_emulated[28]++; }
   else if (is_reduce_combine) { run_reduce(kname, args, true); g_emulated[29]++; }
+  else if (is_eq_hist) { run_equalize(args, false); g_emulated[30]++; }
+  else if (is_eq_apply) { run_equalize(args, true); g_emulated[31]++; }
   return 0;
 }
 }  // extern "C"

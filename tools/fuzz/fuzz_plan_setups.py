@@ -15,6 +15,7 @@ rng = np.random.default_rng(int(sys.argv[1]) if len(sys.argv) > 1 else 0)
 jd_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 1])
 pe_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 2])
 red_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 3])
+eq_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 4])
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
 L = capi.lib()
 MILD = float(os.environ.get("FUZZ_BAD_SCALE", "1"))      # < 1: fewer adversarial values per call -> more set-ups reach their deep paths
@@ -67,6 +68,8 @@ def note(name, rc):
 plans = {k: plan(k, 8) for k in ("Resample", "Resample3D", "Cmn", "Warp", "Pointwise", "Spectrogram", "Mel", "Signal", "Generic", "JpegDistort")}
 red_plan = C.c_void_p()
 capi.check(L.dalib200ReducePlanCreate(C.byref(red_plan), 8))
+eq_plan = C.c_void_p()
+capi.check(L.dalib200EqualizePlanCreate(C.byref(eq_plan), 8))
 for it in range(N):
     n = int(rng.integers(0, 9)) if rng.random() < 0.9 else int(rng.choice([9, 100, -1]))
     m = max(n, 1) if n < 64 else 8
@@ -289,5 +292,18 @@ for it in range(N):
     if rc == 0 and all(0 <= e < 2 ** 20 for e in ext) and np.prod([max(e, 1) for e in ext], dtype=np.float64) < 2 ** 26:
         launch("reduce", L.dalib200ReduceLaunch, red_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x5000000000), fake_ptrs(m, 0x7000000000), None)
         L.dalib200ReducePlanGetPaths(red_plan, (C.c_int32 * (3 * m))(), (C.c_int32 * m)(), m)
+    rng = main_rng
+    # ---- equalize: a generator of its own.  Zero, negative and 2^31-sized extents, more channels than the limit, layouts of the wrong
+    # rank or unknown, invalid type codes
+    rng, main_rng = eq_rng, rng
+    lay = [b"", b"HW", b"HWC", b"CHW", b"FHW", b"FHWC", b"FCHW", b"NHWC", b"HWCC"][int(rng.integers(0, 9))]
+    nd = small(0, 6) if rng.random() < 0.1 * MILD or not lay else len(lay)
+    nd_alloc = nd if 0 < nd <= 8 else 1
+    ext = [int(rng.choice([0, 1, -1, 17, 2 ** 31, 2 ** 31 - 1, 2 ** 40])) if rng.random() < 0.08 * MILD else int(rng.integers(1, 40))
+           for _ in range(m * nd_alloc)]
+    rc = L.dalib200EqualizeSetup(eq_plan, code([0, 0, 1, 9, 11]), n, nd, (C.c_int64 * len(ext))(*ext), lay)
+    note("equalize", rc)
+    if rc == 0 and all(0 <= e < 2 ** 20 for e in ext) and np.prod([max(e, 1) for e in ext], dtype=np.float64) < 2 ** 26:
+        launch("equalize", L.dalib200EqualizeLaunch, eq_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
     rng = main_rng
 print("seed", sys.argv[1] if len(sys.argv) > 1 else 0, "iterations", N, "- no sanitizer report;", {f"{k[0]}:{k[1]}": v for k, v in sorted(hist.items())})
