@@ -32,34 +32,58 @@ static void CheckStatus(int rc, const char *what) {
   if (rc != DALIB200_SUCCESS) throw DALIException(make_string(what, ": ", dalib200GetLastError()));
 }
 
-// frames of a (F)HWC batch flattened into independent 2-D samples (SequenceOperator, sequence_operator.h:57-110)
-struct FrameList {
-  int first_spatial = 0;                       // index of H in the sample shape
-  std::vector<int> sample_of_frame;            // frame -> sample
-  std::vector<int64_t> frame_offset_elems;     // element offset of the frame inside its sample
-  std::vector<int> h, w, c;
-  int num_frames() const { return static_cast<int>(h.size()); }
-};
-
-static FrameList ExpandFrames(const TensorListShape &shape, const TensorLayout &layout, const char *op) {
-  FrameList f;
-  const int nd = shape.sample_dim();
-  std::string l = layout.str();
-  if (l.empty()) l = nd == 3 ? "HWC" : nd == 4 ? "FHWC" : "";
-  DALI_ENFORCE(l == "HWC" || l == "FHWC", op, ": the GPU path supports HWC and FHWC inputs, got layout \"", l, "\" (", nd, "-D)");
-  DALI_ENFORCE(static_cast<int>(l.size()) == nd, op, ": layout \"", l, "\" does not match a ", nd, "-D input");
-  f.first_spatial = l == "HWC" ? 0 : 1;
-  for (int i = 0; i < shape.num_samples(); i++) {
-    const int64_t *s = shape.tensor_shape_span(i);
-    const int64_t frames = f.first_spatial ? s[0] : 1;
-    const int64_t H = s[f.first_spatial], W = s[f.first_spatial + 1], C = s[f.first_spatial + 2];
-    for (int64_t k = 0; k < frames; k++) {
-      f.sample_of_frame.push_back(i);
-      f.frame_offset_elems.push_back(k * H * W * C);
-      f.h.push_back(static_cast<int>(H)); f.w.push_back(static_cast<int>(W)); f.c.push_back(static_cast<int>(C));
-    }
+// A C-ABI plan owned by one operator: destroyed with it, and created again at a larger capacity when a batch needs more than it holds.
+// A plan never holds fewer items than min_cap (the operator's max_batch_size), so that a plan created on demand does not grow again
+// for every larger batch.
+template <typename Plan, int (*Create)(Plan **, int), int (*Destroy)(Plan *)>
+class OwnedPlan {
+ public:
+  explicit OwnedPlan(int min_cap) : min_cap_(min_cap) {}
+  OwnedPlan(const OwnedPlan &) = delete;
+  OwnedPlan &operator=(const OwnedPlan &) = delete;
+  ~OwnedPlan() { if (plan_) Destroy(plan_); }
+  void Ensure(int need, const char *what) {
+    if (need <= cap_) return;
+    if (plan_) Destroy(plan_);
+    plan_ = nullptr;
+    cap_ = 0;
+    const int cap = std::max(need, min_cap_);
+    CheckStatus(Create(&plan_, cap), what);
+    cap_ = cap;
   }
-  return f;
+  Plan *get() const { return plan_; }
+  int capacity() const { return cap_; }
+ private:
+  Plan *plan_ = nullptr;
+  int cap_ = 0, min_cap_;
+};
+#define DALIB200_PLAN(Kind) OwnedPlan<dalib200##Kind##Plan, dalib200##Kind##PlanCreate, dalib200##Kind##PlanDestroy>
+
+template <typename TL>
+static std::vector<const void *> InPtrs(const TL &tl) {
+  std::vector<const void *> p(tl.num_samples());
+  for (int i = 0; i < tl.num_samples(); i++) p[i] = tl.raw_tensor(i);
+  return p;
+}
+template <typename TL>
+static std::vector<void *> OutPtrs(TL &tl) {
+  std::vector<void *> p(tl.num_samples());
+  for (int i = 0; i < tl.num_samples(); i++) p[i] = tl.raw_mutable_tensor(i);
+  return p;
+}
+
+// The output frames of a sample lie back to back: frame k of sample sample_of_frame[k] starts where the previous frame of that
+// sample ends.  frame_bytes(k) is the size of output frame k.
+template <typename FrameBytes>
+static std::vector<void *> PackFrames(TensorList<GPUBackend> &out, const std::vector<int> &sample_of_frame, FrameBytes frame_bytes) {
+  std::vector<void *> p(sample_of_frame.size());
+  std::vector<int64_t> filled(out.num_samples(), 0);         // bytes of each sample taken by its earlier frames
+  for (size_t k = 0; k < p.size(); k++) {
+    const int s = sample_of_frame[k];
+    p[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + filled[s];
+    filled[s] += frame_bytes(k);
+  }
+  return p;
 }
 
 // Resize takes every layout of the reference's schema (resize.cc:28-29): the dimensions in front of the spatial ones collapse into
@@ -76,16 +100,58 @@ static void ParseResizeLayout(const std::string &l, int *spatial_ndim, int *firs
   *first_spatial = static_cast<int>(d == std::string::npos ? l.find('H') : d);
 }
 
-static FrameList ExpandFramesAnyLayout(const TensorListShape &shape, const TensorLayout &layout, const char *op) {
-  FrameList f;
+// A batch of 2-D images flattened into independent frames (SequenceOperator, sequence_operator.h:57-110), and where each frame's
+// output goes: the operator's setup sets out_hw, the output extents of the frames of each sample.
+struct FrameList {
+  int first_spatial = 0;                       // index of H in the sample shape
+  std::vector<int> sample_of_frame;            // frame -> sample
+  std::vector<int64_t> frame_offset_elems;     // element offset of the frame inside its sample
+  std::vector<int> h, w, c;
+  std::vector<std::pair<int, int>> out_hw;     // sample -> output (height, width) of its frames
+  int num_frames() const { return static_cast<int>(h.size()); }
+
+  std::vector<const void *> InputPtrs(const TensorList<GPUBackend> &in) const {
+    std::vector<const void *> p(num_frames());
+    for (int k = 0; k < num_frames(); k++)
+      p[k] = static_cast<const uint8_t *>(in.raw_tensor(sample_of_frame[k])) + frame_offset_elems[k] * TypeSize(in.type());
+    return p;
+  }
+  // output frames of out_hw x c elements of elem_size bytes
+  std::vector<void *> OutputPtrs(TensorList<GPUBackend> &out, size_t elem_size) const {
+    return PackFrames(out, sample_of_frame, [&](size_t k) {
+      const auto &hw = out_hw[sample_of_frame[k]];
+      return static_cast<int64_t>(hw.first) * hw.second * c[k] * elem_size;
+    });
+  }
+  // the input shapes with H and W replaced by out_hw
+  TensorListShape OutputShape(const TensorListShape &in) const {
+    TensorListShape o(in.num_samples(), in.sample_dim());
+    TensorShape sh;
+    for (int i = 0; i < in.num_samples(); i++) {
+      sh.assign(in.tensor_shape_span(i), in.tensor_shape_span(i) + in.sample_dim());
+      sh[first_spatial] = out_hw[i].first; sh[first_spatial + 1] = out_hw[i].second;
+      o.set_tensor_shape(i, sh);
+    }
+    return o;
+  }
+  // an input without a layout is HWC or FHWC
+  TensorLayout OutputLayout(const TensorLayout &in) const { return in.empty() ? TensorLayout(first_spatial ? "FHWC" : "HWC") : in; }
+};
+
+// Fills f with the frames of a batch in one of the 2-D layouts of Resize's schema or, for hwc_only, of an HWC or FHWC batch.
+static void ExpandFrames(FrameList &f, const TensorListShape &shape, const TensorLayout &layout, const char *op, bool hwc_only) {
   const int nd = shape.sample_dim();
   std::string l = layout.str();
   if (l.empty()) l = nd == 3 ? "HWC" : nd == 4 ? "FHWC" : "";
+  if (hwc_only)
+    DALI_ENFORCE(l == "HWC" || l == "FHWC", op, ": the GPU path supports HWC and FHWC inputs, got layout \"", l, "\" (", nd, "-D)");
   int sd = 2, fs = 0;
   ParseResizeLayout(l, &sd, &fs);
   DALI_ENFORCE(sd == 2, op, ": a 2-D layout is expected here, got \"", l, "\"");
   DALI_ENFORCE(static_cast<int>(l.size()) == nd, op, ": layout \"", l, "\" does not match a ", nd, "-D input");
   f.first_spatial = fs;
+  f.sample_of_frame.clear(); f.frame_offset_elems.clear(); f.h.clear(); f.w.clear(); f.c.clear();
+  f.out_hw.assign(shape.num_samples(), {0, 0});
   for (int i = 0; i < shape.num_samples(); i++) {
     const int64_t *s = shape.tensor_shape_span(i);
     int64_t frames = 1, C = 1;
@@ -98,15 +164,6 @@ static FrameList ExpandFramesAnyLayout(const TensorListShape &shape, const Tenso
       f.h.push_back(static_cast<int>(H)); f.w.push_back(static_cast<int>(W)); f.c.push_back(static_cast<int>(C));
     }
   }
-  return f;
-}
-
-template <typename TL>
-static std::vector<const void *> FramePtrs(const TL &tl, const FrameList &f, size_t elem_size) {
-  std::vector<const void *> p(f.num_frames());
-  for (int k = 0; k < f.num_frames(); k++)
-    p[k] = static_cast<const uint8_t *>(tl.raw_tensor(f.sample_of_frame[k])) + f.frame_offset_elems[k] * elem_size;
-  return p;
 }
 
 // =============================================================================================== decoders.image
@@ -146,17 +203,17 @@ class ImageDecoderBase : public Operator<MixedBackend>, public PlanarProducer {
   void EnableDeferredRun() override { deferred_ = true; }
   void SelectPlanar(const std::vector<uint8_t> &want, std::vector<uint8_t> &granted) override {
     granted.assign(want.size(), 0);
-    CheckStatus(dalib200JpegPlanSetPlanesOnly(plan_, want.data(), granted.data()), name_);
+    CheckStatus(dalib200JpegPlanSetPlanesOnly(plan_.get(), want.data(), granted.data()), name_);
   }
   void RunDeferred(cudaStream_t stream) override {
-    CheckStatus(dalib200JpegUpload(plan_, stream), name_);
-    CheckStatus(dalib200JpegLaunch(plan_, optr_.data(), stream), name_);
-    CheckStatus(dalib200JpegStatusAsync(plan_, stream), name_);
+    CheckStatus(dalib200JpegUpload(plan_.get(), stream), name_);
+    CheckStatus(dalib200JpegLaunch(plan_.get(), optr_.data(), stream), name_);
+    CheckStatus(dalib200JpegStatusAsync(plan_.get(), stream), name_);
     launched_ = static_cast<int>(optr_.size());
   }
   void GetPlanarSource(int sample, PlanarSource *out) override {
     dalib200PlanarImage pi;
-    CheckStatus(dalib200JpegPlanGetPlanes(plan_, sample, &pi), name_);
+    CheckStatus(dalib200JpegPlanGetPlanes(plan_.get(), sample, &pi), name_);
     out->y = pi.y; out->cb = pi.cb; out->cr = pi.cr; out->pitch_y = pi.pitch_y; out->pitch_c = pi.pitch_c;
     out->width = pi.width; out->height = pi.height;
     out->crop_x = rois_[sample].use_roi ? rois_[sample].x0 : 0;
@@ -171,9 +228,8 @@ class ImageDecoderBase : public Operator<MixedBackend>, public PlanarProducer {
     prm_.dtype = dt == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT;
     prm_.fancy_upsampling = spec.GetArgument<bool>("jpeg_fancy_upsampling");
     prm_.adjust_orientation = spec.GetArgument<bool>("adjust_orientation");
-    CheckStatus(dalib200JpegPlanCreate(&plan_, max_batch_size_), name_);
+    plan_.Ensure(max_batch_size_, name_);
   }
-  ~ImageDecoderBase() override { dalib200JpegPlanDestroy(plan_); }
 
  protected:
   // fills rois_[i] (use_roi = 0: whole image) for an image whose ORIENTED size is H x W
@@ -198,14 +254,14 @@ class ImageDecoderBase : public Operator<MixedBackend>, public PlanarProducer {
         SampleRoi(rois_[i], ws, i, H, W);
       }
     }
-    CheckStatus(dalib200JpegPlanSetSourceStable(plan_, in.stable() ? 1 : 0), name_);
-    CheckStatus(dalib200JpegPlanSetupEx(plan_, n, ptrs.data(), lens.data(), &prm_, HasRoi() ? rois_.data() : nullptr), name_);
+    CheckStatus(dalib200JpegPlanSetSourceStable(plan_.get(), in.stable() ? 1 : 0), name_);
+    CheckStatus(dalib200JpegPlanSetupEx(plan_.get(), n, ptrs.data(), lens.data(), &prm_, HasRoi() ? rois_.data() : nullptr), name_);
     out.resize(1);
     out[0].type = out_type_;
     out[0].shape.resize(n, 3);
     for (int i = 0; i < n; i++) {
       int32_t hwc[3];
-      CheckStatus(dalib200JpegPlanGetOutputShape(plan_, i, hwc), name_);
+      CheckStatus(dalib200JpegPlanGetOutputShape(plan_.get(), i, hwc), name_);
       out[0].shape.set_tensor_shape(i, { hwc[0], hwc[1], hwc[2] });
     }
     return true;
@@ -223,7 +279,7 @@ class ImageDecoderBase : public Operator<MixedBackend>, public PlanarProducer {
     std::vector<int32_t> st(launched_);
     const int n = launched_;
     launched_ = 0;
-    CheckStatus(dalib200JpegStatusFetch(plan_, st.data(), n), name_);
+    CheckStatus(dalib200JpegStatusFetch(plan_.get(), st.data(), n), name_);
     for (int i = 0; i < n; i++)
       if (st[i] != 0)       // image_decoder.h:826-831: "Failed to decode sample #i"
         throw DALIException(make_string("Failed to decode sample #", i, ": the entropy-coded data ends early or is corrupt"));
@@ -232,7 +288,7 @@ class ImageDecoderBase : public Operator<MixedBackend>, public PlanarProducer {
   bool deferred_ = false;
   std::vector<void *> optr_;
 
-  dalib200JpegPlan *plan_ = nullptr;
+  DALIB200_PLAN(Jpeg) plan_{max_batch_size_};
   dalib200JpegParams prm_{};
   DALIDataType out_type_ = DALI_UINT8;
   std::vector<dalib200JpegRoi> rois_;
@@ -268,9 +324,8 @@ class AudioDecoderMixed : public Operator<MixedBackend> {
                  "decoders.audio: integer output (INT16 / INT32) is not available with `downmix` or `sample_rate`");
     quality_ = spec.GetArgument<float>("quality");
     DALI_ENFORCE(quality_ >= 0 && quality_ <= 100, "``quality`` out of range: ", quality_, "\nValid range is [0..100].");
-    CheckStatus(dalib200AudioPlanCreate(&plan_, max_batch_size_), "decoders.audio");
+    plan_.Ensure(max_batch_size_, "decoders.audio");
   }
-  ~AudioDecoderMixed() override { dalib200AudioPlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
@@ -290,7 +345,7 @@ class AudioDecoderMixed : public Operator<MixedBackend> {
       prm[i].quality = quality_;
       prm[i].dtype = dt;
     }
-    CheckStatus(dalib200AudioPlanSetup(plan_, n, ptrs.data(), lens.data(), prm.data()), "decoders.audio");
+    CheckStatus(dalib200AudioPlanSetup(plan_.get(), n, ptrs.data(), lens.data(), prm.data()), "decoders.audio");
     out.resize(2);
     out[0].type = dtype_;
     out[0].shape.resize(n, downmix_ ? 1 : 2);
@@ -300,7 +355,7 @@ class AudioDecoderMixed : public Operator<MixedBackend> {
       int64_t sh[2];
       int32_t nd;
       float rate;
-      CheckStatus(dalib200AudioPlanGetOutputShape(plan_, i, sh, &nd, &rate), "decoders.audio");
+      CheckStatus(dalib200AudioPlanGetOutputShape(plan_.get(), i, sh, &nd, &rate), "decoders.audio");
       if (downmix_) out[0].shape.set_tensor_shape(i, { sh[0] });
       else out[0].shape.set_tensor_shape(i, { sh[0], sh[1] });
     }
@@ -310,25 +365,23 @@ class AudioDecoderMixed : public Operator<MixedBackend> {
     auto &audio = ws.Output<GPUBackend>(0);
     auto &rate = ws.Output<GPUBackend>(1);
     audio.SetLayout(downmix_ ? "T" : "TC");
-    const int n = audio.num_samples();
-    std::vector<void *> op(n), rp(n);
-    for (int i = 0; i < n; i++) { op[i] = audio.raw_mutable_tensor(i); rp[i] = rate.raw_mutable_tensor(i); }
-    CheckStatus(dalib200AudioLaunch(plan_, op.data(), rp.data(), ws.stream()), "decoders.audio");
-    CheckStatus(dalib200AudioStatusAsync(plan_, ws.stream()), "decoders.audio");
-    launched_ = n;
+    const auto op = OutPtrs(audio), rp = OutPtrs(rate);
+    CheckStatus(dalib200AudioLaunch(plan_.get(), op.data(), rp.data(), ws.stream()), "decoders.audio");
+    CheckStatus(dalib200AudioStatusAsync(plan_.get(), ws.stream()), "decoders.audio");
+    launched_ = audio.num_samples();
   }
   void CheckCompletion() override {
     if (launched_ <= 0) return;
     const int n = launched_;
     launched_ = 0;
     std::vector<int32_t> st(n);
-    CheckStatus(dalib200AudioStatusFetch(plan_, st.data(), n), "decoders.audio");
+    CheckStatus(dalib200AudioStatusFetch(plan_.get(), st.data(), n), "decoders.audio");
     for (int i = 0; i < n; i++)
       if (st[i] != 0) throw DALIException(make_string("Failed to decode sample #", i, ": the FLAC frame chain is broken or a frame is corrupt"));
   }
 
  private:
-  dalib200AudioPlan *plan_ = nullptr;
+  DALIB200_PLAN(Audio) plan_{max_batch_size_};
   DALIDataType dtype_ = DALI_FLOAT;
   bool downmix_ = false, resample_ = false;
   float quality_ = 50;
@@ -700,16 +753,35 @@ static int Interp2Filter(int interp) {      // resampling_attr.cc:60-74
   }
 }
 
+// The min / mag filters of sample i (resampling_attr.cc:76-133), from the filter arguments of Resize and RandomResizedCrop.
+struct ResizeFilterArgs {
+  bool has_interp, has_min, has_mag, antialias;
+  explicit ResizeFilterArgs(const OpSpec &spec)
+      : has_interp(spec.ArgumentDefined("interp_type")), has_min(spec.ArgumentDefined("min_filter")),
+        has_mag(spec.ArgumentDefined("mag_filter")), antialias(spec.GetArgument<bool>("antialias")) {}
+  void Get(const OpSpec &spec, const Workspace &ws, int i, dalib200FilterDesc &min_filter, dalib200FilterDesc &mag_filter) const {
+    const int interp = spec.GetArgument<int>("interp_type", &ws, i);
+    int minf = DALIB200_FILTER_TRIANGULAR, magf = DALIB200_FILTER_LINEAR;
+    auto conv = [](int t, bool aa) {
+      if (aa && t == DALI_INTERP_LINEAR) t = DALI_INTERP_TRIANGULAR; else if (!aa && t == DALI_INTERP_TRIANGULAR) t = DALI_INTERP_LINEAR;
+      return Interp2Filter(t);
+    };
+    if (has_min) minf = conv(spec.GetArgument<int>("min_filter", &ws, i), antialias); else if (has_interp) minf = conv(interp, antialias);
+    if (has_mag) magf = conv(spec.GetArgument<int>("mag_filter", &ws, i), false); else if (has_interp) magf = conv(interp, false);
+    min_filter = { minf, antialias ? 1 : 0, 0.0f };
+    mag_filter = { magf, 0, 0.0f };
+  }
+};
+
 class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
  public:
   void AttachProducer(PlanarProducer *p) override {
     producer_ = p;
-    CheckStatus(dalib200ResamplePlanCreate(&plan_planar_, plan_cap_), "Resize");
-    planar_cap_ = plan_cap_;
+    plan_planar_.Ensure(plan_.capacity(), "Resize");
   }
   // hook of ResizeCropMirror: crop window and mirror applied to the per-sample parameters
   virtual void AdjustSampleParams(resize_detail::Params &, const Workspace &, int) {}
-  explicit ResizeGPU(const OpSpec &spec, const char *name = "Resize") : Operator<GPUBackend>(spec) {
+  explicit ResizeGPU(const OpSpec &spec, const char *name = "Resize") : Operator<GPUBackend>(spec), filters_(spec) {
     using resize_detail::Mode;
     has_shorter_ = spec.ArgumentDefined("resize_shorter"); has_longer_ = spec.ArgumentDefined("resize_longer");
     has_x_ = spec.ArgumentDefined("resize_x"); has_y_ = spec.ArgumentDefined("resize_y");
@@ -735,17 +807,44 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
       else if (m == "not_larger") mode_ = Mode::NotLarger; else if (m == "not_smaller") mode_ = Mode::NotSmaller;
       else DALI_FAIL(make_string("Invalid resize mode: \"", m, "\""));
     }
-    antialias_ = spec.GetArgument<bool>("antialias");
-    CheckStatus(dalib200ResamplePlanCreate(&plan_, max_batch_size_ * 64), "Resize");
-    plan_cap_ = max_batch_size_ * 64;
-  }
-  ~ResizeGPU() override {
-    dalib200ResamplePlanDestroy(plan_);
-    if (plan_planar_) dalib200ResamplePlanDestroy(plan_planar_);
-    if (plan3_) dalib200Resample3DPlanDestroy(plan3_);
+    plan_.Ensure(max_batch_size_ * 64, "Resize");
   }
 
  protected:
+  // ResizeAttr (resize_attr.cc:102-255) for sd = 2 (images) or 3 (volumes) spatial dimensions of in_size (shape order): the output
+  // size and input ROI of sample i from the size request, the ROI and max_size (read once per batch by MaxSize)
+  resize_detail::Params SampleParams(const Workspace &ws, int i, int sd, const float *in_size, bool empty_input,
+                                     const std::vector<float> &max_size) const {
+    float req[3] = {0, 0, 0};
+    if (has_x_ || has_y_ || has_z_) {          // `resize_z` alone on 2-D data: both extents unspecified (resize_attr.cc:214-245)
+      if (has_z_ && sd == 3) req[0] = spec_.GetArgument<float>("resize_z", &ws, i);
+      if (has_y_) req[sd - 2] = spec_.GetArgument<float>("resize_y", &ws, i);
+      if (has_x_) req[sd - 1] = spec_.GetArgument<float>("resize_x", &ws, i);
+    } else if (has_shorter_ || has_longer_) {
+      std::fill(req, req + sd, spec_.GetArgument<float>(has_shorter_ ? "resize_shorter" : "resize_longer", &ws, i));
+    } else {
+      auto v = spec_.GetFloatVecArgument("size", &ws, i, sd);
+      std::copy(v.begin(), v.begin() + sd, req);
+    }
+    float lo[3] = {0, 0, 0}, hi[3] = {0, 0, 0};
+    std::copy(in_size, in_size + sd, hi);
+    if (has_roi_) {          // resize_attr.cc:125-160
+      auto rs = spec_.GetFloatVecArgument("roi_start", &ws, i, sd), re = spec_.GetFloatVecArgument("roi_end", &ws, i, sd);
+      for (int d = 0; d < sd; d++) if (in_size[d] > 0) {
+        double l = rs[d], h = re[d];
+        if (roi_relative_) { l *= in_size[d]; h *= in_size[d]; }
+        if (std::fabs(h - l) < 1e-3f) { float off = l <= h ? 0.5f * 1e-3f : -0.5f * 1e-3f; l -= off; h += off; }
+        lo[d] = static_cast<float>(l); hi[d] = static_cast<float>(h);
+      }
+    }
+    resize_detail::Params p;
+    resize_detail::CalculateSampleParams(p, req, lo, hi, subpixel_scale_, empty_input, mode_, has_max_ ? max_size.data() : nullptr, sd);
+    return p;
+  }
+  std::vector<float> MaxSize(const Workspace &ws, int sd) const {
+    return has_max_ ? spec_.GetFloatVecArgument("max_size", &ws, 0, sd) : std::vector<float>();
+  }
+
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     const int n = in.num_samples();
@@ -756,67 +855,29 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     volumes_ = in.GetLayout().str().find('D') != std::string::npos;
     DALI_ENFORCE(!volumes_ || plain_resize_, "ResizeCropMirror: volumetric inputs are not supported by the GPU path");
     if (volumes_) return SetupVolumes(out, ws, out_type);
-    frames_ = ExpandFramesAnyLayout(in.shape(), in.GetLayout(), "Resize");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "Resize", false);
     const int nf = frames_.num_frames();
-    if (nf > plan_cap_) { dalib200ResamplePlanDestroy(plan_); plan_ = nullptr; plan_cap_ = nf; CheckStatus(dalib200ResamplePlanCreate(&plan_, nf), "Resize"); }
-    std::vector<float> max_size(2, std::nextafter(static_cast<float>(std::numeric_limits<int>::max()), 0.0f));
-    if (has_max_) max_size = spec_.GetFloatVecArgument("max_size", &ws, 0, 2);
-    const bool has_interp = spec_.ArgumentDefined("interp_type"), has_min = spec_.ArgumentDefined("min_filter"),
-               has_mag = spec_.ArgumentDefined("mag_filter");
+    plan_.Ensure(nf, "Resize");
+    const std::vector<float> max_size = MaxSize(ws, 2);
     samples_.assign(nf, dalib200ResampleSample());
-    out_hw_.assign(n, {0, 0});
     int fk = 0;
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
       const int fs = frames_.first_spatial;
-      const float in_h = static_cast<float>(s[fs]), in_w = static_cast<float>(s[fs + 1]);
-      float req[2] = {0, 0};     // (H, W) order
-      if (has_x_ || has_y_ || has_z_) {          // `resize_z` alone on 2-D data: both extents unspecified (resize_attr.cc:214-245)
-        if (has_y_) req[0] = spec_.GetArgument<float>("resize_y", &ws, i);
-        if (has_x_) req[1] = spec_.GetArgument<float>("resize_x", &ws, i);
-      } else if (has_shorter_ || has_longer_) {
-        req[0] = req[1] = spec_.GetArgument<float>(has_shorter_ ? "resize_shorter" : "resize_longer", &ws, i);
-      } else {
-        auto v = spec_.GetFloatVecArgument("size", &ws, i, 2);
-        req[0] = v[0]; req[1] = v[1];
-      }
-      float lo[2] = {0, 0}, hi[2] = {in_h, in_w};
-      if (has_roi_) {          // resize_attr.cc:125-160
-        auto rs = spec_.GetFloatVecArgument("roi_start", &ws, i, 2), re = spec_.GetFloatVecArgument("roi_end", &ws, i, 2);
-        const float isz[2] = {in_h, in_w};
-        for (int d = 0; d < 2; d++) if (isz[d] > 0) {
-          double l = rs[d], h = re[d];
-          if (roi_relative_) { l *= isz[d]; h *= isz[d]; }
-          if (std::fabs(h - l) < 1e-3f) { float off = l <= h ? 0.5f * 1e-3f : -0.5f * 1e-3f; l -= off; h += off; }
-          lo[d] = static_cast<float>(l); hi[d] = static_cast<float>(h);
-        }
-      }
-      resize_detail::Params p;
-      const bool empty_input = in.shape().tensor_size(i) == 0;
-      resize_detail::CalculateSampleParams(p, req, lo, hi, subpixel_scale_, empty_input, mode_, has_max_ ? max_size.data() : nullptr);
+      const float in_hw[2] = { static_cast<float>(s[fs]), static_cast<float>(s[fs + 1]) };
+      resize_detail::Params p = SampleParams(ws, i, 2, in_hw, in.shape().tensor_size(i) == 0, max_size);
       AdjustSampleParams(p, ws, i);
-      // filters (resampling_attr.cc:76-133)
-      int interp = spec_.GetArgument<int>("interp_type", &ws, i);
-      int minf = DALIB200_FILTER_TRIANGULAR, magf = DALIB200_FILTER_LINEAR;
-      auto conv = [](int t, bool aa) {
-        if (aa && t == DALI_INTERP_LINEAR) t = DALI_INTERP_TRIANGULAR; else if (!aa && t == DALI_INTERP_TRIANGULAR) t = DALI_INTERP_LINEAR;
-        return Interp2Filter(t);
-      };
-      if (has_min) minf = conv(spec_.GetArgument<int>("min_filter", &ws, i), antialias_); else if (has_interp) minf = conv(interp, antialias_);
-      if (has_mag) magf = conv(spec_.GetArgument<int>("mag_filter", &ws, i), false); else if (has_interp) magf = conv(interp, false);
-      out_hw_[i] = { p.dst[0], p.dst[1] };
-      int64_t frames = 1, chans = 1;            // leading dimensions are frames, trailing ones channels (CHW: C frames of one channel)
-      for (int d = 0; d < fs; d++) frames *= s[d];
-      for (int d = fs + 2; d < in.shape().sample_dim(); d++) chans *= s[d];
-      for (int64_t k = 0; k < frames; k++, fk++) {
+      dalib200FilterDesc minf, magf;
+      filters_.Get(spec_, ws, i, minf, magf);
+      frames_.out_hw[i] = { p.dst[0], p.dst[1] };
+      for (; fk < nf && frames_.sample_of_frame[fk] == i; fk++) {      // leading dimensions are frames, trailing ones channels
         auto &r = samples_[fk];
-        r.in_h = static_cast<int>(s[fs]); r.in_w = static_cast<int>(s[fs + 1]); r.channels = static_cast<int>(chans);
+        r.in_h = frames_.h[fk]; r.in_w = frames_.w[fk]; r.channels = frames_.c[fk];
         r.out_h = p.dst[0]; r.out_w = p.dst[1];
         for (int d = 0; d < 2; d++) {
           r.use_roi[d] = p.lo[d] != p.hi[d];            // GetResamplingParams: roi only when non-degenerate
           r.roi_start[d] = p.lo[d]; r.roi_end[d] = p.hi[d];
-          r.min_filter[d] = { minf, antialias_ ? 1 : 0, 0.0f };
-          r.mag_filter[d] = { magf, 0, 0.0f };
+          r.min_filter[d] = minf; r.mag_filter[d] = magf;
         }
       }
     }
@@ -824,14 +885,14 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     planar_.assign(nf, 0);
     rest_.clear();
     if (producer_ && frames_.first_spatial == 0 && nf == n && in.type() == DALI_UINT8 && out_type == DALI_UINT8) {
-      if (nf > planar_cap_) { dalib200ResamplePlanDestroy(plan_planar_); plan_planar_ = nullptr; planar_cap_ = nf; CheckStatus(dalib200ResamplePlanCreate(&plan_planar_, nf), "Resize"); }
+      plan_planar_.Ensure(nf, "Resize");
       std::vector<uint8_t> ok(nf, 0), granted;
-      CheckStatus(dalib200ResamplePlanSetupPlanar(plan_planar_, nf, samples_.data(), ok.data()), "Resize");
+      CheckStatus(dalib200ResamplePlanSetupPlanar(plan_planar_.get(), nf, samples_.data(), ok.data()), "Resize");
       producer_->SelectPlanar(ok, granted);
       if (ok != granted) {       // the resampler's item list must cover exactly the granted samples
         std::vector<dalib200ResampleSample> tmp(samples_);
         for (int i = 0; i < nf; i++) if (!granted[i]) tmp[i].channels = 1;      // 1-channel samples are never planar-eligible
-        CheckStatus(dalib200ResamplePlanSetupPlanar(plan_planar_, nf, tmp.data(), ok.data()), "Resize");
+        CheckStatus(dalib200ResamplePlanSetupPlanar(plan_planar_.get(), nf, tmp.data(), ok.data()), "Resize");
       }
       planar_ = granted;
     } else if (producer_) {
@@ -840,21 +901,16 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     }
     for (int k = 0; k < nf; k++) if (!planar_[k]) rest_.push_back(k);
     if (static_cast<int>(rest_.size()) == nf) {
-      CheckStatus(dalib200ResamplePlanSetup(plan_, nf, samples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
+      CheckStatus(dalib200ResamplePlanSetup(plan_.get(), nf, samples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
                                             out_type == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Resize");
     } else if (!rest_.empty()) {
       std::vector<dalib200ResampleSample> sub(rest_.size());
       for (size_t q = 0; q < rest_.size(); q++) sub[q] = samples_[rest_[q]];
-      CheckStatus(dalib200ResamplePlanSetup(plan_, static_cast<int>(sub.size()), sub.data(), DALIB200_UINT8, DALIB200_UINT8), "Resize");
+      CheckStatus(dalib200ResamplePlanSetup(plan_.get(), static_cast<int>(sub.size()), sub.data(), DALIB200_UINT8, DALIB200_UINT8), "Resize");
     }
     out.resize(1);
     out[0].type = out_type;
-    out[0].shape.resize(n, in.shape().sample_dim());
-    for (int i = 0; i < n; i++) {
-      TensorShape sh = in.shape().tensor_shape(i);
-      sh[frames_.first_spatial] = out_hw_[i].first; sh[frames_.first_spatial + 1] = out_hw_[i].second;
-      out[0].shape.set_tensor_shape(i, sh);
-    }
+    out[0].shape = frames_.OutputShape(in.shape());
     out_type_ = out_type;
     return true;
   }
@@ -863,16 +919,9 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     if (volumes_) { RunVolumes(ws); return; }
-    out.SetLayout(in.GetLayout().empty() ? TensorLayout(frames_.first_spatial ? "FHWC" : "HWC") : in.GetLayout());
-    auto ip = FramePtrs(in, frames_, TypeSize(in.type()));
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      const int64_t fr = static_cast<int64_t>(out_hw_[s].first) * out_hw_[s].second * frames_.c[k] * TypeSize(out_type_);
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += fr;
-    }
+    out.SetLayout(frames_.OutputLayout(in.GetLayout()));
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = frames_.OutputPtrs(out, TypeSize(out_type_));
     if (producer_) {
       producer_->RunDeferred(ws.stream());
       if (rest_.size() != op.size()) {
@@ -885,16 +934,16 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
           srcs[k].y = ps.y; srcs[k].cb = ps.cb; srcs[k].cr = ps.cr; srcs[k].pitch_y = ps.pitch_y; srcs[k].pitch_c = ps.pitch_c;
           srcs[k].width = ps.width; srcs[k].height = ps.height; srcs[k].crop_x = ps.crop_x; srcs[k].crop_y = ps.crop_y;
         }
-        CheckStatus(dalib200ResampleLaunchPlanar(plan_planar_, srcs.data(), op.data(), ws.stream()), "Resize");
+        CheckStatus(dalib200ResampleLaunchPlanar(plan_planar_.get(), srcs.data(), op.data(), ws.stream()), "Resize");
       }
     }
     if (rest_.size() == op.size()) {
-      CheckStatus(dalib200ResampleLaunch(plan_, ip.data(), op.data(), ws.stream()), "Resize");
+      CheckStatus(dalib200ResampleLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "Resize");
     } else if (!rest_.empty()) {
       std::vector<const void *> ip2(rest_.size());
       std::vector<void *> op2(rest_.size());
       for (size_t q = 0; q < rest_.size(); q++) { ip2[q] = ip[rest_[q]]; op2[q] = op[rest_[q]]; }
-      CheckStatus(dalib200ResampleLaunch(plan_, ip2.data(), op2.data(), ws.stream()), "Resize");
+      CheckStatus(dalib200ResampleLaunch(plan_.get(), ip2.data(), op2.data(), ws.stream()), "Resize");
     }
   }
 
@@ -909,48 +958,16 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     ParseResizeLayout(lay, &sd, &fs);
     DALI_ENFORCE(nd == static_cast<int>(lay.size()), "Resize: layout \"", lay, "\" does not match a ", nd, "-D input");
     if (producer_) { std::vector<uint8_t> none(n, 0), granted; producer_->SelectPlanar(none, granted); }
-    std::vector<float> max_size(3, std::nextafter(static_cast<float>(std::numeric_limits<int>::max()), 0.0f));
-    if (has_max_) max_size = spec_.GetFloatVecArgument("max_size", &ws, 0, 3);
-    const bool has_interp = spec_.ArgumentDefined("interp_type"), has_min = spec_.ArgumentDefined("min_filter"),
-               has_mag = spec_.ArgumentDefined("mag_filter");
+    const std::vector<float> max_size = MaxSize(ws, 3);
     vsamples_.clear();
     vol_sample_.clear(); vol_offset_.clear();
     out_dhw_.assign(n, {0, 0, 0});
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
       const float isz[3] = { static_cast<float>(s[fs]), static_cast<float>(s[fs + 1]), static_cast<float>(s[fs + 2]) };
-      float req[3] = {0, 0, 0};     // (D, H, W): the shape order of `size`
-      if (has_x_ || has_y_ || has_z_) {
-        if (has_z_) req[0] = spec_.GetArgument<float>("resize_z", &ws, i);
-        if (has_y_) req[1] = spec_.GetArgument<float>("resize_y", &ws, i);
-        if (has_x_) req[2] = spec_.GetArgument<float>("resize_x", &ws, i);
-      } else if (has_shorter_ || has_longer_) {
-        req[0] = req[1] = req[2] = spec_.GetArgument<float>(has_shorter_ ? "resize_shorter" : "resize_longer", &ws, i);
-      } else {
-        auto v = spec_.GetFloatVecArgument("size", &ws, i, 3);
-        req[0] = v[0]; req[1] = v[1]; req[2] = v[2];
-      }
-      float lo[3] = {0, 0, 0}, hi[3] = { isz[0], isz[1], isz[2] };
-      if (has_roi_) {          // resize_attr.cc:125-160
-        auto rs = spec_.GetFloatVecArgument("roi_start", &ws, i, 3), re = spec_.GetFloatVecArgument("roi_end", &ws, i, 3);
-        for (int d = 0; d < 3; d++) if (isz[d] > 0) {
-          double l = rs[d], h = re[d];
-          if (roi_relative_) { l *= isz[d]; h *= isz[d]; }
-          if (std::fabs(h - l) < 1e-3f) { float off = l <= h ? 0.5f * 1e-3f : -0.5f * 1e-3f; l -= off; h += off; }
-          lo[d] = static_cast<float>(l); hi[d] = static_cast<float>(h);
-        }
-      }
-      resize_detail::Params p;
-      const bool empty_input = in.shape().tensor_size(i) == 0;
-      resize_detail::CalculateSampleParams(p, req, lo, hi, subpixel_scale_, empty_input, mode_, has_max_ ? max_size.data() : nullptr, 3);
-      int interp = spec_.GetArgument<int>("interp_type", &ws, i);
-      int minf = DALIB200_FILTER_TRIANGULAR, magf = DALIB200_FILTER_LINEAR;
-      auto conv = [](int t, bool aa) {      // resampling_attr.cc:76-133
-        if (aa && t == DALI_INTERP_LINEAR) t = DALI_INTERP_TRIANGULAR; else if (!aa && t == DALI_INTERP_TRIANGULAR) t = DALI_INTERP_LINEAR;
-        return Interp2Filter(t);
-      };
-      if (has_min) minf = conv(spec_.GetArgument<int>("min_filter", &ws, i), antialias_); else if (has_interp) minf = conv(interp, antialias_);
-      if (has_mag) magf = conv(spec_.GetArgument<int>("mag_filter", &ws, i), false); else if (has_interp) magf = conv(interp, false);
+      const resize_detail::Params p = SampleParams(ws, i, 3, isz, in.shape().tensor_size(i) == 0, max_size);
+      dalib200FilterDesc minf, magf;
+      filters_.Get(spec_, ws, i, minf, magf);
       out_dhw_[i] = { p.dst[0], p.dst[1], p.dst[2] };
       int64_t frames = 1, chans = 1;            // leading dimensions are frames, trailing ones channels (CDHW: C volumes of one channel)
       for (int d = 0; d < fs; d++) frames *= s[d];
@@ -964,8 +981,7 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
           r.in_shape[d] = static_cast<int>(s[fs + d]); r.out_shape[d] = p.dst[d];
           r.use_roi[d] = p.lo[d] != p.hi[d];
           r.roi_start[d] = p.lo[d]; r.roi_end[d] = p.hi[d];
-          r.min_filter[d] = { minf, antialias_ ? 1 : 0, 0.0f };
-          r.mag_filter[d] = { magf, 0, 0.0f };
+          r.min_filter[d] = minf; r.mag_filter[d] = magf;
         }
         vsamples_.push_back(r);
         vol_sample_.push_back(i);
@@ -973,12 +989,8 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
       }
     }
     const int nv = static_cast<int>(vsamples_.size());
-    if (nv > plan3_cap_ || !plan3_) {
-      if (plan3_) dalib200Resample3DPlanDestroy(plan3_);
-      plan3_ = nullptr; plan3_cap_ = std::max(nv, max_batch_size_);
-      CheckStatus(dalib200Resample3DPlanCreate(&plan3_, plan3_cap_), "Resize");
-    }
-    CheckStatus(dalib200Resample3DPlanSetup(plan3_, nv, vsamples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
+    plan3_.Ensure(std::max(nv, 1), "Resize");      // created by the first batch of volumes, even one without frames
+    CheckStatus(dalib200Resample3DPlanSetup(plan3_.get(), nv, vsamples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
                                             out_type == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Resize");
     out.resize(1);
     out[0].type = out_type;
@@ -997,38 +1009,33 @@ class ResizeGPU : public Operator<GPUBackend>, public PlanarConsumer {
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(in.GetLayout());
     if (producer_) producer_->RunDeferred(ws.stream());
-    const size_t nv = vsamples_.size();
-    std::vector<const void *> ip(nv);
-    std::vector<void *> op(nv);
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (size_t k = 0; k < nv; k++) {
-      const int s = vol_sample_[k];
-      ip[k] = static_cast<const uint8_t *>(in.raw_tensor(s)) + vol_offset_[k] * TypeSize(in.type());
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(out_dhw_[s][0]) * out_dhw_[s][1] * out_dhw_[s][2] * vsamples_[k].channels * TypeSize(out_type_);
-    }
-    CheckStatus(dalib200Resample3DLaunch(plan3_, ip.data(), op.data(), ws.stream()), "Resize");
+    std::vector<const void *> ip(vsamples_.size());
+    for (size_t k = 0; k < ip.size(); k++)
+      ip[k] = static_cast<const uint8_t *>(in.raw_tensor(vol_sample_[k])) + vol_offset_[k] * TypeSize(in.type());
+    const auto op = PackFrames(out, vol_sample_, [&](size_t k) {
+      const auto &e = out_dhw_[vol_sample_[k]];
+      return static_cast<int64_t>(e[0]) * e[1] * e[2] * vsamples_[k].channels * TypeSize(out_type_);
+    });
+    CheckStatus(dalib200Resample3DLaunch(plan3_.get(), ip.data(), op.data(), ws.stream()), "Resize");
   }
 
  private:
-  dalib200Resample3DPlan *plan3_ = nullptr;
-  int plan3_cap_ = 0;
+  DALIB200_PLAN(Resample3D) plan3_{max_batch_size_};
   bool volumes_ = false, has_z_ = false, plain_resize_ = true;
   std::vector<dalib200Resample3DSample> vsamples_;
   std::vector<int> vol_sample_;
   std::vector<int64_t> vol_offset_;
   std::vector<std::array<int, 3>> out_dhw_;
-  dalib200ResamplePlan *plan_ = nullptr, *plan_planar_ = nullptr;
-  int plan_cap_ = 0, planar_cap_ = 0;
+  DALIB200_PLAN(Resample) plan_{max_batch_size_}, plan_planar_{max_batch_size_};
   PlanarProducer *producer_ = nullptr;
   std::vector<uint8_t> planar_;
   std::vector<int> rest_;
   bool has_shorter_ = false, has_longer_ = false, has_x_ = false, has_y_ = false, has_size_ = false, has_max_ = false, has_roi_ = false;
-  bool roi_relative_ = false, subpixel_scale_ = true, antialias_ = true;
+  bool roi_relative_ = false, subpixel_scale_ = true;
   resize_detail::Mode mode_ = resize_detail::Mode::Default;
+  ResizeFilterArgs filters_;
   FrameList frames_;
   std::vector<dalib200ResampleSample> samples_;
-  std::vector<std::pair<int, int>> out_hw_;
   DALIDataType out_type_ = DALI_UINT8;
 };
 DALI_REGISTER_OPERATOR(Resize, ResizeGPU, GPU);
@@ -1106,15 +1113,13 @@ DALI_SCHEMA(RandomResizedCrop)
 
 class RandomResizedCropGPU : public Operator<GPUBackend> {
  public:
-  explicit RandomResizedCropGPU(const OpSpec &spec) : Operator<GPUBackend>(spec), gens_(MakeCropGenerators(spec, max_batch_size_)) {
+  explicit RandomResizedCropGPU(const OpSpec &spec)
+      : Operator<GPUBackend>(spec), filters_(spec), gens_(MakeCropGenerators(spec, max_batch_size_)) {
     size_ = spec.GetRepeatedArgument<int>("size");
     if (size_.size() == 1) size_.push_back(size_[0]);
     DALI_ENFORCE(size_.size() == 2 && size_[0] > 0 && size_[1] > 0, "RandomResizedCrop: `size` must be one or two positive integers");
-    antialias_ = spec.GetArgument<bool>("antialias");
-    CheckStatus(dalib200ResamplePlanCreate(&plan_, max_batch_size_ * 64), "RandomResizedCrop");
-    plan_cap_ = max_batch_size_ * 64;
+    plan_.Ensure(max_batch_size_ * 64, "RandomResizedCrop");
   }
-  ~RandomResizedCropGPU() override { dalib200ResamplePlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
@@ -1124,11 +1129,9 @@ class RandomResizedCropGPU : public Operator<GPUBackend> {
     out_type_ = in.type();
     if (spec_.ArgumentDefined("dtype")) out_type_ = spec_.GetArgument<DALIDataType>("dtype");
     DALI_ENFORCE(out_type_ == in.type() || out_type_ == DALI_FLOAT, "RandomResizedCrop: output type must be the same as input or FLOAT");
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "RandomResizedCrop");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "RandomResizedCrop", true);
     const int nf = frames_.num_frames();
-    if (nf > plan_cap_) { dalib200ResamplePlanDestroy(plan_); plan_ = nullptr; plan_cap_ = nf; CheckStatus(dalib200ResamplePlanCreate(&plan_, nf), "RandomResizedCrop"); }
-    const bool has_interp = spec_.ArgumentDefined("interp_type"), has_min = spec_.ArgumentDefined("min_filter"),
-               has_mag = spec_.ArgumentDefined("mag_filter");
+    plan_.Ensure(nf, "RandomResizedCrop");
     samples_.assign(nf, dalib200ResampleSample());
     crops_.resize(n);
     int fk = 0;
@@ -1137,14 +1140,9 @@ class RandomResizedCropGPU : public Operator<GPUBackend> {
       const int fs = frames_.first_spatial;
       const int H = static_cast<int>(s[fs]), W = static_cast<int>(s[fs + 1]);
       crops_[i] = (*gens_)[i].Generate(H, W);
-      int interp = spec_.GetArgument<int>("interp_type", &ws, i);
-      int minf = DALIB200_FILTER_TRIANGULAR, magf = DALIB200_FILTER_LINEAR;
-      auto conv = [](int t, bool aa) {
-        if (aa && t == DALI_INTERP_LINEAR) t = DALI_INTERP_TRIANGULAR; else if (!aa && t == DALI_INTERP_TRIANGULAR) t = DALI_INTERP_LINEAR;
-        return Interp2Filter(t);
-      };
-      if (has_min) minf = conv(spec_.GetArgument<int>("min_filter", &ws, i), antialias_); else if (has_interp) minf = conv(interp, antialias_);
-      if (has_mag) magf = conv(spec_.GetArgument<int>("mag_filter", &ws, i), false); else if (has_interp) magf = conv(interp, false);
+      dalib200FilterDesc minf, magf;
+      filters_.Get(spec_, ws, i, minf, magf);
+      frames_.out_hw[i] = { size_[0], size_[1] };
       const int64_t frames = fs ? s[0] : 1;
       for (int64_t k = 0; k < frames; k++, fk++) {
         auto &r = samples_[fk];
@@ -1154,41 +1152,28 @@ class RandomResizedCropGPU : public Operator<GPUBackend> {
           r.use_roi[d] = 1;
           r.roi_start[d] = static_cast<float>(crops_[i].anchor[d]);
           r.roi_end[d] = static_cast<float>(crops_[i].anchor[d] + crops_[i].shape[d]);
-          r.min_filter[d] = { minf, antialias_ ? 1 : 0, 0.0f };
-          r.mag_filter[d] = { magf, 0, 0.0f };
+          r.min_filter[d] = minf; r.mag_filter[d] = magf;
         }
       }
     }
-    CheckStatus(dalib200ResamplePlanSetup(plan_, nf, samples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
+    CheckStatus(dalib200ResamplePlanSetup(plan_.get(), nf, samples_.data(), in.type() == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT,
                                           out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "RandomResizedCrop");
     out.resize(1);
     out[0].type = out_type_;
-    out[0].shape.resize(n, in.shape().sample_dim());
-    for (int i = 0; i < n; i++) {
-      TensorShape sh = in.shape().tensor_shape(i);
-      sh[frames_.first_spatial] = size_[0]; sh[frames_.first_spatial + 1] = size_[1];
-      out[0].shape.set_tensor_shape(i, sh);
-    }
+    out[0].shape = frames_.OutputShape(in.shape());
     return true;
   }
   void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout().empty() ? TensorLayout(frames_.first_spatial ? "FHWC" : "HWC") : in.GetLayout());
-    auto ip = FramePtrs(in, frames_, TypeSize(in.type()));
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(size_[0]) * size_[1] * frames_.c[k] * TypeSize(out_type_);
-    }
-    CheckStatus(dalib200ResampleLaunch(plan_, ip.data(), op.data(), ws.stream()), "RandomResizedCrop");
+    out.SetLayout(frames_.OutputLayout(in.GetLayout()));
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = frames_.OutputPtrs(out, TypeSize(out_type_));
+    CheckStatus(dalib200ResampleLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "RandomResizedCrop");
   }
  private:
-  dalib200ResamplePlan *plan_ = nullptr;
-  int plan_cap_ = 0;
-  bool antialias_ = true;
+  DALIB200_PLAN(Resample) plan_{max_batch_size_};
+  ResizeFilterArgs filters_;
   std::vector<int> size_;
   CropGenerators gens_;
   std::vector<CropWindow2D> crops_;
@@ -1240,17 +1225,15 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
     DALI_ENFORCE(!(has_crop && (spec.ArgumentDefined("crop_h") || spec.ArgumentDefined("crop_w"))),
                  "`crop` argument is not compatible with `crop_h`, `crop_w`, `crop_d`");
     DALI_ENFORCE(spec.ArgumentDefined("crop_h") == spec.ArgumentDefined("crop_w"), "`crop_h` and `crop_w` arguments must be provided together");
-    CheckStatus(dalib200CmnPlanCreate(&plan_, max_batch_size_ * 64), "CropMirrorNormalize");
-    plan_cap_ = max_batch_size_ * 64;
+    plan_.Ensure(max_batch_size_ * 64, "CropMirrorNormalize");
   }
-  ~CropMirrorNormalizeGPU() override { dalib200CmnPlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, "CropMirrorNormalize: the GPU path expects uint8 input");
     const int n = in.num_samples();
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "CropMirrorNormalize");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "CropMirrorNormalize", true);
     const bool seq = frames_.first_spatial == 1;
     std::string ol = out_layout_.empty() ? (seq ? "FHWC" : "HWC") : out_layout_;
     if (seq && (ol == "CHW" || ol == "HWC")) ol = "F" + ol;       // fn.crop_mirror_normalize(output_layout="CHW") on FHWC -> FCHW
@@ -1259,9 +1242,8 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
     chw_ = ol.find("CHW") != std::string::npos;
     resolved_layout_ = ol;
     const int nf = frames_.num_frames();
-    if (nf > plan_cap_) { dalib200CmnPlanDestroy(plan_); plan_ = nullptr; plan_cap_ = nf; CheckStatus(dalib200CmnPlanCreate(&plan_, nf), "CropMirrorNormalize"); }
+    plan_.Ensure(nf, "CropMirrorNormalize");
     samples_.assign(nf, dalib200CmnSample());
-    crop_hw_.assign(n, {0, 0});
     int out_c = 0, fk = 0;
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
@@ -1322,7 +1304,7 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
           c.fill[d] = fill_values_.empty() ? 0.0f : fill_values_.size() == 1 ? fill_values_[0] : (d < static_cast<int>(fill_values_.size()) ? fill_values_[d] : 0.0f);
         }
       }
-      crop_hw_[i] = { static_cast<int>(ch), static_cast<int>(cw) };
+      frames_.out_hw[i] = { static_cast<int>(ch), static_cast<int>(cw) };
     }
     if (n > 0) {
       for (int i = 0; i < n; i++) {
@@ -1332,7 +1314,7 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
       }
     }
     out_c_ = out_c;
-    CheckStatus(dalib200CmnPlanSetup(plan_, nf, samples_.data(), out_type_ == DALI_FLOAT ? DALIB200_FLOAT : DALIB200_FLOAT16,
+    CheckStatus(dalib200CmnPlanSetup(plan_.get(), nf, samples_.data(), out_type_ == DALI_FLOAT ? DALIB200_FLOAT : DALIB200_FLOAT16,
                                      chw_ ? DALIB200_LAYOUT_CHW : DALIB200_LAYOUT_HWC, std::max(out_c, 1)), "CropMirrorNormalize");
     out.resize(1);
     out[0].type = out_type_;
@@ -1340,8 +1322,9 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
     for (int i = 0; i < n; i++) {
       TensorShape sh;
       if (seq) sh.push_back(in.shape().tensor_shape_span(i)[0]);
-      if (chw_) { sh.push_back(out_c); sh.push_back(crop_hw_[i].first); sh.push_back(crop_hw_[i].second); }
-      else { sh.push_back(crop_hw_[i].first); sh.push_back(crop_hw_[i].second); sh.push_back(out_c); }
+      const auto &hw = frames_.out_hw[i];
+      if (chw_) { sh.push_back(out_c); sh.push_back(hw.first); sh.push_back(hw.second); }
+      else { sh.push_back(hw.first); sh.push_back(hw.second); sh.push_back(out_c); }
       out[0].shape.set_tensor_shape(i, sh);
     }
     return true;
@@ -1351,28 +1334,24 @@ class CropMirrorNormalizeGPU : public Operator<GPUBackend> {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(resolved_layout_);
-    auto ip = FramePtrs(in, frames_, 1);
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(crop_hw_[s].first) * crop_hw_[s].second * out_c_ * TypeSize(out_type_);
-    }
-    CheckStatus(dalib200CmnLaunch(plan_, ip.data(), op.data(), ws.stream()), "CropMirrorNormalize");
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = PackFrames(out, frames_.sample_of_frame, [&](size_t k) {       // out_hw x out_c_ (padded channels)
+      const auto &hw = frames_.out_hw[frames_.sample_of_frame[k]];
+      return static_cast<int64_t>(hw.first) * hw.second * out_c_ * TypeSize(out_type_);
+    });
+    CheckStatus(dalib200CmnLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "CropMirrorNormalize");
   }
 
  private:
-  dalib200CmnPlan *plan_ = nullptr;
-  int plan_cap_ = 0, out_c_ = 3;
+  DALIB200_PLAN(Cmn) plan_{max_batch_size_};
+  int out_c_ = 3;
   DALIDataType out_type_ = DALI_FLOAT;
   std::string out_layout_, oob_, resolved_layout_;
   bool pad_output_ = false, truncate_ = false, chw_ = true;
   float scale_ = 1, shift_ = 0;
   std::vector<float> fill_values_;
-  FrameList frames_;
+  FrameList frames_;        // out_hw: the crop windows
   std::vector<dalib200CmnSample> samples_;
-  std::vector<std::pair<int, int>> crop_hw_;
 };
 DALI_REGISTER_OPERATOR(CropMirrorNormalize, CropMirrorNormalizeGPU, GPU);
 
@@ -1397,10 +1376,8 @@ class WarpAffineGPU : public Operator<GPUBackend> {
     invert_ = !spec.GetArgument<bool>("inverse_map");
     use_fill_ = spec.ArgumentDefined("fill_value");
     if (use_fill_) fill_ = spec.GetArgument<float>("fill_value");
-    CheckStatus(dalib200WarpPlanCreate(&plan_, max_batch_size_ * 64), "WarpAffine");
-    plan_cap_ = max_batch_size_ * 64;
+    plan_.Ensure(max_batch_size_ * 64, "WarpAffine");
   }
-  ~WarpAffineGPU() override { dalib200WarpPlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
@@ -1410,11 +1387,10 @@ class WarpAffineGPU : public Operator<GPUBackend> {
     DALI_ENFORCE(out_type_ == DALI_UINT8 || out_type_ == DALI_FLOAT, "WarpAffine: output type must be UINT8 or FLOAT");
     DALI_ENFORCE(spec_.ArgumentDefined("matrix"), "`matrix` argument must be provided when transforms are not passed as a regular input.");
     const int n = in.num_samples();
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "WarpAffine");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "WarpAffine", true);
     const int nf = frames_.num_frames();
-    if (nf > plan_cap_) { dalib200WarpPlanDestroy(plan_); plan_ = nullptr; plan_cap_ = nf; CheckStatus(dalib200WarpPlanCreate(&plan_, nf), "WarpAffine"); }
+    plan_.Ensure(nf, "WarpAffine");
     samples_.assign(nf, dalib200WarpSample());
-    out_hw_.assign(n, {0, 0});
     int fk = 0;
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
@@ -1430,7 +1406,7 @@ class WarpAffineGPU : public Operator<GPUBackend> {
         DALI_ENFORCE(sz[0] > 0 && sz[1] > 0, "Output size must be positive");
         oh = std::max<int>(static_cast<int>(std::roundf(sz[0])), 1); ow = std::max<int>(static_cast<int>(std::roundf(sz[1])), 1);
       }
-      out_hw_[i] = { oh, ow };
+      frames_.out_hw[i] = { oh, ow };
       const int64_t frames = fs ? s[0] : 1;
       for (int64_t k = 0; k < frames; k++, fk++) {
         auto &w = samples_[fk];
@@ -1439,41 +1415,28 @@ class WarpAffineGPU : public Operator<GPUBackend> {
         std::copy(M, M + 6, w.matrix);
       }
     }
-    CheckStatus(dalib200WarpPlanSetup(plan_, nf, samples_.data(), interp_, use_fill_, fill_, out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT),
-                "WarpAffine");
+    CheckStatus(dalib200WarpPlanSetup(plan_.get(), nf, samples_.data(), interp_, use_fill_, fill_,
+                                      out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "WarpAffine");
     out.resize(1);
     out[0].type = out_type_;
-    out[0].shape.resize(n, in.shape().sample_dim());
-    for (int i = 0; i < n; i++) {
-      TensorShape sh = in.shape().tensor_shape(i);
-      sh[frames_.first_spatial] = out_hw_[i].first; sh[frames_.first_spatial + 1] = out_hw_[i].second;
-      out[0].shape.set_tensor_shape(i, sh);
-    }
+    out[0].shape = frames_.OutputShape(in.shape());
     return true;
   }
   void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout().empty() ? TensorLayout(frames_.first_spatial ? "FHWC" : "HWC") : in.GetLayout());
-    auto ip = FramePtrs(in, frames_, 1);
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(out_hw_[s].first) * out_hw_[s].second * frames_.c[k] * TypeSize(out_type_);
-    }
-    CheckStatus(dalib200WarpLaunch(plan_, ip.data(), op.data(), ws.stream()), "WarpAffine");
+    out.SetLayout(frames_.OutputLayout(in.GetLayout()));
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = frames_.OutputPtrs(out, TypeSize(out_type_));
+    CheckStatus(dalib200WarpLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "WarpAffine");
   }
  private:
-  dalib200WarpPlan *plan_ = nullptr;
-  int plan_cap_ = 0;
+  DALIB200_PLAN(Warp) plan_{max_batch_size_};
   bool interp_ = true, invert_ = false, use_fill_ = false;
   float fill_ = 0;
   DALIDataType out_type_ = DALI_UINT8;
   FrameList frames_;
   std::vector<dalib200WarpSample> samples_;
-  std::vector<std::pair<int, int>> out_hw_;
 };
 DALI_REGISTER_OPERATOR(WarpAffine, WarpAffineGPU, GPU);
 
@@ -1489,25 +1452,16 @@ DALI_SCHEMA(Hsv)
 class PointwiseBase : public Operator<GPUBackend> {
  public:
   explicit PointwiseBase(const OpSpec &spec, const char *name) : Operator<GPUBackend>(spec), name_(name) {
-    CheckStatus(dalib200PointwisePlanCreate(&plan_, max_batch_size_), name_);
-    plan_cap_ = max_batch_size_;
+    plan_.Ensure(max_batch_size_, name_);
   }
-  ~PointwiseBase() override { dalib200PointwisePlanDestroy(plan_); }
  protected:
-  void EnsureCap(int n) {
-    if (n > plan_cap_) { dalib200PointwisePlanDestroy(plan_); plan_ = nullptr; plan_cap_ = n; CheckStatus(dalib200PointwisePlanCreate(&plan_, n), name_); }
-  }
-  void Launch(Workspace &ws) {
+  void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(in.GetLayout());
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
-    CheckStatus(dalib200PointwiseLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
+    CheckStatus(dalib200PointwiseLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), name_);
   }
-  dalib200PointwisePlan *plan_ = nullptr;
-  int plan_cap_ = 0;
+  DALIB200_PLAN(Pointwise) plan_{max_batch_size_};
   const char *name_;
 };
 
@@ -1522,7 +1476,7 @@ class HsvGPU : public PointwiseBase {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, "Hsv: the GPU path expects uint8 input");
     const int n = in.num_samples();
-    EnsureCap(n);
+    plan_.Ensure(n, name_);
     std::vector<dalib200ColorSample> cs(n);
     for (int i = 0; i < n; i++) {
       const int nd = in.shape().sample_dim();
@@ -1532,12 +1486,11 @@ class HsvGPU : public PointwiseBase {
       dalib200ColorTwistMatrix(spec_.GetArgument<float>("hue", &ws, i), spec_.GetArgument<float>("saturation", &ws, i),
                                spec_.GetArgument<float>("value", &ws, i), 1.0f, 1.0f, 128.0f, cs[i].matrix, cs[i].offset);
     }
-    CheckStatus(dalib200LinearTransformSetup(plan_, n, cs.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Hsv");
+    CheckStatus(dalib200LinearTransformSetup(plan_.get(), n, cs.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Hsv");
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = out_type_;
     return true;
   }
-  void RunImpl(Workspace &ws) override { Launch(ws); }
  private:
   DALIDataType out_type_ = DALI_UINT8;
 };
@@ -1561,7 +1514,7 @@ class ColorSpaceConversionGPU : public PointwiseBase {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, "Color space conversion accept only uint8 tensors");    // color_space_conversion.h:49
     const int n = in.num_samples(), nd = in.shape().sample_dim();
-    EnsureCap(n);
+    plan_.Ensure(n, name_);
     const int ic = in_t_ == DALI_GRAY ? 1 : 3, oc = out_t_ == DALI_GRAY ? 1 : 3;
     std::vector<int64_t> npx(n);
     out.resize(1);
@@ -1574,10 +1527,9 @@ class ColorSpaceConversionGPU : public PointwiseBase {
       sh[nd - 1] = oc;
       out[0].shape.set_tensor_shape(i, sh);
     }
-    CheckStatus(dalib200ColorSpaceSetup(plan_, n, npx.data(), in_t_, out_t_), "ColorSpaceConversion");
+    CheckStatus(dalib200ColorSpaceSetup(plan_.get(), n, npx.data(), in_t_, out_t_), "ColorSpaceConversion");
     return true;
   }
-  void RunImpl(Workspace &ws) override { Launch(ws); }
  private:
   int in_t_ = 0, out_t_ = 0;
 };
@@ -1603,7 +1555,7 @@ class SpectrogramGPU : public Operator<GPUBackend>, public SpectrumProducer, pub
   // ---- SpectrumProducer
   void EnableDeferredRun() override { fuse_ = true; }
   bool Deferred() const override { return deferred_now_; }
-  void *SpectrogramPlan() override { return plan_; }
+  void *SpectrogramPlan() override { return plan_.get(); }
   const std::vector<const void *> &DeferredInputs() const override { return deferred_in_; }
 
   explicit SpectrogramGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {
@@ -1622,9 +1574,8 @@ class SpectrogramGPU : public Operator<GPUBackend>, public SpectrumProducer, pub
       window_ = spec.GetRepeatedArgument<float>("window_fn");
       DALI_ENFORCE(static_cast<int>(window_.size()) == args_.window_length, "Window function should match the specified `window_length`");
     }
-    CheckStatus(dalib200SpectrogramPlanCreate(&plan_, max_batch_size_), "Spectrogram");
+    plan_.Ensure(max_batch_size_, "Spectrogram");
   }
-  ~SpectrogramGPU() override { dalib200SpectrogramPlanDestroy(plan_); }
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
@@ -1638,13 +1589,13 @@ class SpectrogramGPU : public Operator<GPUBackend>, public SpectrumProducer, pub
         DALI_ENFORCE(s[d] == 1 || s[d] == vol, "Input data must be 1D or all but one dimensions must be degenerate (extent 1).");
       lens[i] = vol;
     }
-    CheckStatus(dalib200SpectrogramPlanSetup(plan_, &args_, window_.empty() ? nullptr : window_.data(), n, lens.data()), "Spectrogram");
+    CheckStatus(dalib200SpectrogramPlanSetup(plan_.get(), &args_, window_.empty() ? nullptr : window_.data(), n, lens.data()), "Spectrogram");
     out.resize(1);
     out[0].type = DALI_FLOAT;
     out[0].shape.resize(n, 2);
     const int nbin = args_.nfft / 2 + 1;
     for (int i = 0; i < n; i++) {
-      const int64_t nw = dalib200SpectrogramNumWindows(plan_, i);
+      const int64_t nw = dalib200SpectrogramNumWindows(plan_.get(), i);
       out[0].shape.set_tensor_shape(i, args_.layout_ft ? TensorShape{nbin, nw} : TensorShape{nw, nbin});
     }
     return true;
@@ -1653,25 +1604,24 @@ class SpectrogramGPU : public Operator<GPUBackend>, public SpectrumProducer, pub
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(layout_);
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
+    auto ip = InPtrs(in);
+    const auto op = OutPtrs(out);
     // fused with the PreemphasisFilter that produces the input: the framing reads its unfiltered input and filters it
     if (pre_ && pre_->Deferred()) {
       ip = pre_->DeferredInputs();
-      CheckStatus(dalib200SpectrogramPlanSetPreemphasis(plan_, pre_->Coefficients().data(), pre_->Border()), "Spectrogram");
+      CheckStatus(dalib200SpectrogramPlanSetPreemphasis(plan_.get(), pre_->Coefficients().data(), pre_->Border()), "Spectrogram");
     }
     // fused with the MelFilterBank that consumes this output: it launches STFT -> mel as one kernel and the spectrogram is never
     // written (the fused kernel exists for nfft = 1024, (f, t) layout)
     deferred_now_ = fuse_ && args_.nfft == 1024 && args_.layout_ft;
     if (deferred_now_) { deferred_in_ = ip; return; }
-    CheckStatus(dalib200SpectrogramLaunch(plan_, ip.data(), op.data(), ws.stream()), "Spectrogram");
+    CheckStatus(dalib200SpectrogramLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "Spectrogram");
   }
  private:
   bool fuse_ = false, deferred_now_ = false;
   std::vector<const void *> deferred_in_;
   PreemphasisProducer *pre_ = nullptr;
-  dalib200SpectrogramPlan *plan_ = nullptr;
+  DALIB200_PLAN(Spectrogram) plan_{max_batch_size_};
   dalib200SpectrogramArgs args_{};
   std::vector<float> window_;
   std::string layout_;
@@ -1700,11 +1650,10 @@ class MelFilterBankGPU : public Operator<GPUBackend>, public SpectrumConsumer {
     const std::string f = spec.GetArgument<std::string>("mel_formula");
     DALI_ENFORCE(f == "slaney" || f == "htk", "Unsupported mel_formula value \"", f, "\". Supported values are: \"slaney\", \"htk\"");
     args_.htk = f == "htk";
-    CheckStatus(dalib200MelPlanCreate(&plan_, max_batch_size_), "MelFilterBank");
+    plan_.Ensure(max_batch_size_, "MelFilterBank");
     // opt-in: the dense-GEMM tensor-core path (tolerance ~1e-6 instead of bit-exact banded sums)
-    if (const char *e = getenv("DALIB200_MEL_TENSOR_CORES")) CheckStatus(dalib200MelPlanSetTensorCores(plan_, atoi(e)), "MelFilterBank");
+    if (const char *e = getenv("DALIB200_MEL_TENSOR_CORES")) CheckStatus(dalib200MelPlanSetTensorCores(plan_.get(), atoi(e)), "MelFilterBank");
   }
-  ~MelFilterBankGPU() override { dalib200MelPlanDestroy(plan_); }
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
@@ -1719,7 +1668,7 @@ class MelFilterBankGPU : public Operator<GPUBackend>, public SpectrumConsumer {
       DALI_ENFORCE(in.shape().tensor_shape_span(i)[0] == nbin, "MelFilterBank: all spectrograms of a batch must have the same number of bins");
       nwin[i] = in.shape().tensor_shape_span(i)[1];
     }
-    CheckStatus(dalib200MelPlanSetup(plan_, &args_, nbin, n, nwin.data()), "MelFilterBank");
+    CheckStatus(dalib200MelPlanSetup(plan_.get(), &args_, nbin, n, nwin.data()), "MelFilterBank");
     out.resize(1);
     out[0].type = DALI_FLOAT;
     out[0].shape.resize(n, 2);
@@ -1730,14 +1679,13 @@ class MelFilterBankGPU : public Operator<GPUBackend>, public SpectrumConsumer {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout("ft");
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
+    const auto ip = InPtrs(in);
+    const auto op = OutPtrs(out);
     if (producer_ && producer_->Deferred()) {
       auto *sp = static_cast<dalib200SpectrogramPlan *>(producer_->SpectrogramPlan());
       const auto &sin = producer_->DeferredInputs();
-      if (dalib200SpectrogramMelSupported(sp, plan_)) {
-        CheckStatus(dalib200SpectrogramMelLaunch(sp, plan_, sin.data(), nullptr, op.data(), ws.stream()), "MelFilterBank");
+      if (dalib200SpectrogramMelSupported(sp, plan_.get())) {
+        CheckStatus(dalib200SpectrogramMelLaunch(sp, plan_.get(), sin.data(), nullptr, op.data(), ws.stream()), "MelFilterBank");
         return;
       }
       // not fusable after all (e.g. the tensor-core mel path was requested): materialise the spectrogram, then filter it
@@ -1745,11 +1693,11 @@ class MelFilterBankGPU : public Operator<GPUBackend>, public SpectrumConsumer {
       for (int i = 0; i < in.num_samples(); i++) sp_out[i] = const_cast<void *>(in.raw_tensor(i));
       CheckStatus(dalib200SpectrogramLaunch(sp, sin.data(), sp_out.data(), ws.stream()), "Spectrogram");
     }
-    CheckStatus(dalib200MelLaunch(plan_, ip.data(), op.data(), ws.stream()), "MelFilterBank");
+    CheckStatus(dalib200MelLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "MelFilterBank");
   }
  private:
   SpectrumProducer *producer_ = nullptr;
-  dalib200MelPlan *plan_ = nullptr;
+  DALIB200_PLAN(Mel) plan_{max_batch_size_};
   dalib200MelArgs args_{};
 };
 DALI_REGISTER_OPERATOR(MelFilterBank, MelFilterBankGPU, GPU);
@@ -1767,16 +1715,17 @@ DALI_SCHEMA(BrightnessContrast)
 class GenericOpBase : public Operator<GPUBackend> {
  public:
   explicit GenericOpBase(const OpSpec &spec, const char *name) : Operator<GPUBackend>(spec), name_(name) {
-    CheckStatus(dalib200GenericPlanCreate(&plan_, max_batch_size_ * 64), name_);
-    plan_cap_ = max_batch_size_ * 64;
+    plan_.Ensure(max_batch_size_ * 64, name_);
   }
-  ~GenericOpBase() override { dalib200GenericPlanDestroy(plan_); }
  protected:
-  void EnsureCap(int n) {
-    if (n > plan_cap_) { dalib200GenericPlanDestroy(plan_); plan_ = nullptr; plan_cap_ = n; CheckStatus(dalib200GenericPlanCreate(&plan_, n), name_); }
+  // one output sample per input sample
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(in.GetLayout());
+    CheckStatus(dalib200GenericLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), name_);
   }
-  dalib200GenericPlan *plan_ = nullptr;
-  int plan_cap_ = 0;
+  DALIB200_PLAN(Generic) plan_{max_batch_size_};
   const char *name_;
 };
 
@@ -1790,7 +1739,7 @@ class BrightnessContrastGPU : public GenericOpBase {
     out_type_ = spec_.ArgumentDefined("dtype") ? spec_.GetArgument<DALIDataType>("dtype") : DALI_UINT8;
     DALI_ENFORCE(out_type_ == DALI_UINT8 || out_type_ == DALI_FLOAT, "BrightnessContrast: the GPU path supports dtype UINT8 and FLOAT");
     const int n = in.num_samples();
-    EnsureCap(n);
+    plan_.Ensure(n, name_);
     std::vector<int64_t> vol(n);
     std::vector<float> mul(n), add(n);
     // brightness_contrast.h:84-103: FullRange<Out> = 255 (u8) or 1 (float); HalfRange<uint8_t> = 128
@@ -1807,19 +1756,10 @@ class BrightnessContrastGPU : public GenericOpBase {
       add[i] = t3 + t2;
       mul[i] = brightness * contrast;
     }
-    CheckStatus(dalib200MultiplyAddSetup(plan_, n, vol.data(), mul.data(), add.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), name_);
+    CheckStatus(dalib200MultiplyAddSetup(plan_.get(), n, vol.data(), mul.data(), add.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), name_);
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = out_type_;
     return true;
-  }
-  void RunImpl(Workspace &ws) override {
-    const auto &in = ws.Input<GPUBackend>(0);
-    auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout());
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
-    CheckStatus(dalib200GenericLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
   }
   DALIDataType out_type_ = DALI_UINT8;
 };
@@ -1846,7 +1786,7 @@ class ColorTwistGPU : public PointwiseBase {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, "ColorTwist: the GPU path expects uint8 input");
     const int n = in.num_samples();
-    EnsureCap(n);
+    plan_.Ensure(n, name_);
     std::vector<dalib200ColorSample> cs(n);
     for (int i = 0; i < n; i++) {
       const int nd = in.shape().sample_dim();
@@ -1857,12 +1797,11 @@ class ColorTwistGPU : public PointwiseBase {
                                spec_.GetArgument<float>("brightness", &ws, i), spec_.GetArgument<float>("contrast", &ws, i), 128.0f,
                                cs[i].matrix, cs[i].offset);
     }
-    CheckStatus(dalib200LinearTransformSetup(plan_, n, cs.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "ColorTwist");
+    CheckStatus(dalib200LinearTransformSetup(plan_.get(), n, cs.data(), out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "ColorTwist");
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = out_type_;
     return true;
   }
-  void RunImpl(Workspace &ws) override { Launch(ws); }
  private:
   DALIDataType out_type_ = DALI_UINT8;
 };
@@ -1879,12 +1818,11 @@ DALI_SCHEMA(JpegCompressionDistortion)
 class JpegCompressionDistortionGPU : public Operator<GPUBackend> {
  public:
   explicit JpegCompressionDistortionGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
-  ~JpegCompressionDistortionGPU() override { dalib200JpegDistortPlanDestroy(plan_); }
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, "JpegCompressionDistortion: the input must be uint8");
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "JpegCompressionDistortion");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "JpegCompressionDistortion", true);
     std::vector<dalib200JpegDistortSample> s;
     kept_.clear();
     for (int k = 0; k < frames_.num_frames(); k++) {
@@ -1897,12 +1835,8 @@ class JpegCompressionDistortionGPU : public Operator<GPUBackend> {
       kept_.push_back(k);
     }
     const int n = static_cast<int>(s.size());
-    if (n > plan_cap_) {
-      dalib200JpegDistortPlanDestroy(plan_); plan_ = nullptr;
-      plan_cap_ = std::max(n, max_batch_size_);
-      CheckStatus(dalib200JpegDistortPlanCreate(&plan_, plan_cap_), "JpegCompressionDistortion");
-    }
-    if (plan_) CheckStatus(dalib200JpegDistortPlanSetup(plan_, n, s.data()), "JpegCompressionDistortion");
+    plan_.Ensure(n, "JpegCompressionDistortion");          // no plan before the first batch with frames to compress
+    if (plan_.get()) CheckStatus(dalib200JpegDistortPlanSetup(plan_.get(), n, s.data()), "JpegCompressionDistortion");
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = DALI_UINT8;
     return true;
@@ -1912,7 +1846,7 @@ class JpegCompressionDistortionGPU : public Operator<GPUBackend> {
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(in.GetLayout());
     if (kept_.empty()) return;
-    const auto ip = FramePtrs(in, frames_, 1);
+    const auto ip = frames_.InputPtrs(in);
     std::vector<const void *> src(kept_.size());
     std::vector<void *> dst(kept_.size());
     for (size_t i = 0; i < kept_.size(); i++) {
@@ -1920,11 +1854,10 @@ class JpegCompressionDistortionGPU : public Operator<GPUBackend> {
       src[i] = ip[k];
       dst[i] = static_cast<uint8_t *>(out.raw_mutable_tensor(frames_.sample_of_frame[k])) + frames_.frame_offset_elems[k];
     }
-    CheckStatus(dalib200JpegDistortLaunch(plan_, src.data(), dst.data(), ws.stream()), "JpegCompressionDistortion");
+    CheckStatus(dalib200JpegDistortLaunch(plan_.get(), src.data(), dst.data(), ws.stream()), "JpegCompressionDistortion");
   }
  private:
-  dalib200JpegDistortPlan *plan_ = nullptr;
-  int plan_cap_ = 0;
+  DALIB200_PLAN(JpegDistort) plan_{max_batch_size_};
   FrameList frames_;
   std::vector<int> kept_;                    // frames with pixels, in plan order
 };
@@ -1942,11 +1875,10 @@ class WindowOpBase : public GenericOpBase {
     const auto &in = ws.Input<GPUBackend>(0);
     DALI_ENFORCE(in.type() == DALI_UINT8, name_, ": the GPU path expects uint8 input");
     const int n = in.num_samples();
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), name_);
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), name_, true);
     const int nf = frames_.num_frames();
-    EnsureCap(nf);
+    plan_.Ensure(nf, name_);
     samples_.assign(nf, dalib200WindowSample());
-    out_hw_.assign(n, {0, 0});
     int fk = 0;
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
@@ -1955,34 +1887,23 @@ class WindowOpBase : public GenericOpBase {
       w.in_h = static_cast<int>(s[fs]); w.in_w = static_cast<int>(s[fs + 1]); w.channels = static_cast<int>(s[fs + 2]);
       DALI_ENFORCE(w.channels >= 1, name_, ": empty channel dimension");
       SampleWindow(w, ws, i, w.in_h, w.in_w, w.channels);
-      out_hw_[i] = { w.out_h, w.out_w };
+      frames_.out_hw[i] = { w.out_h, w.out_w };
       const int64_t frames = fs ? s[0] : 1;
       for (int64_t k = 0; k < frames; k++) samples_[fk++] = w;
     }
-    CheckStatus(dalib200WindowCopySetup(plan_, nf, samples_.data()), name_);
+    CheckStatus(dalib200WindowCopySetup(plan_.get(), nf, samples_.data()), name_);
     out.resize(1);
     out[0].type = DALI_UINT8;
-    out[0].shape.resize(n, in.shape().sample_dim());
-    for (int i = 0; i < n; i++) {
-      TensorShape sh = in.shape().tensor_shape(i);
-      sh[frames_.first_spatial] = out_hw_[i].first; sh[frames_.first_spatial + 1] = out_hw_[i].second;
-      out[0].shape.set_tensor_shape(i, sh);
-    }
+    out[0].shape = frames_.OutputShape(in.shape());
     return true;
   }
   void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout().empty() ? TensorLayout(frames_.first_spatial ? "FHWC" : "HWC") : in.GetLayout());
-    auto ip = FramePtrs(in, frames_, 1);
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(out_hw_[s].first) * out_hw_[s].second * frames_.c[k];
-    }
-    CheckStatus(dalib200GenericLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
+    out.SetLayout(frames_.OutputLayout(in.GetLayout()));
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = frames_.OutputPtrs(out, 1);
+    CheckStatus(dalib200GenericLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), name_);
   }
   // out_of_bounds_policy handling shared by crop and slice (generic/slice/out_of_bounds_policy.h)
   void ApplyOob(dalib200WindowSample &w, const std::string &policy, const std::vector<float> &fill, int64_t ay, int64_t ax, int64_t h, int64_t wd) {
@@ -2006,7 +1927,6 @@ class WindowOpBase : public GenericOpBase {
   }
   FrameList frames_;
   std::vector<dalib200WindowSample> samples_;
-  std::vector<std::pair<int, int>> out_hw_;
 };
 
 DALI_SCHEMA(Flip)
@@ -2218,8 +2138,8 @@ class PadGPU : public GenericOpBase {
     std::vector<int64_t> is((size_t)n * nd), os((size_t)n * nd);
     for (int i = 0; i < n; i++) std::copy(in.shape().tensor_shape_span(i), in.shape().tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
     PadOutputShapes(a, n, nd, is.data(), shp, os.data());
-    EnsureCap(std::max(n, 1));
-    CheckStatus(dalib200PadSetup(plan_, n, nd, static_cast<int>(TypeSize(in.type())), is.data(), os.data(), &fill), name_);
+    plan_.Ensure(std::max(n, 1), name_);
+    CheckStatus(dalib200PadSetup(plan_.get(), n, nd, static_cast<int>(TypeSize(in.type())), is.data(), os.data(), &fill), name_);
     out.resize(1);
     out[0].type = in.type();
     out[0].shape.resize(n, nd);
@@ -2228,15 +2148,6 @@ class PadGPU : public GenericOpBase {
       out[0].shape.set_tensor_shape(i, sh);
     }
     return true;
-  }
-  void RunImpl(Workspace &ws) override {
-    const auto &in = ws.Input<GPUBackend>(0);
-    auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout());
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
-    CheckStatus(dalib200GenericLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
   }
 };
 DALI_REGISTER_OPERATOR(Pad, PadGPU, GPU);
@@ -2332,15 +2243,7 @@ JoinArgs JoinResolveArgs(const OpSpec &spec, bool stack, int ndim, const std::ve
 class PermuteOpBase : public Operator<GPUBackend> {
  public:
   explicit PermuteOpBase(const OpSpec &spec, const char *name) : Operator<GPUBackend>(spec), name_(name) {}
-  ~PermuteOpBase() override { dalib200PermutePlanDestroy(plan_); }
  protected:
-  void EnsureCap(int copies) {
-    if (copies <= cap_) return;
-    dalib200PermutePlanDestroy(plan_);
-    plan_ = nullptr;
-    cap_ = std::max(copies, max_batch_size_);
-    CheckStatus(dalib200PermutePlanCreate(&plan_, cap_), name_);
-  }
   void SetOutput(std::vector<OutputDesc> &out, DALIDataType type, int n, int ond, const std::vector<int64_t> &os) {
     out.resize(1);
     out[0].type = type;
@@ -2357,10 +2260,9 @@ class PermuteOpBase : public Operator<GPUBackend> {
       op[i] = out.raw_mutable_tensor(i);
       for (int k = 0; k < nin; k++) ip[(size_t)i * nin + k] = ws.Input<GPUBackend>(k).raw_tensor(i);
     }
-    CheckStatus(dalib200PermuteLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
+    CheckStatus(dalib200PermuteLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), name_);
   }
-  dalib200PermutePlan *plan_ = nullptr;
-  int cap_ = 0;
+  DALIB200_PLAN(Permute) plan_{max_batch_size_};
   const char *name_;
   TensorLayout layout_;
 };
@@ -2376,8 +2278,8 @@ class TransposeGPU : public PermuteOpBase {
     std::vector<int32_t> perm(a.perm.begin(), a.perm.end());
     std::vector<int64_t> is((size_t)n * nd), os((size_t)n * nd);
     for (int i = 0; i < n; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
-    EnsureCap(std::max(n, 1));
-    CheckStatus(dalib200TransposeSetup(plan_, n, nd, static_cast<int>(TypeSize(in.type())), is.data(), perm.data(), os.data()), name_);
+    plan_.Ensure(std::max(n, 1), name_);
+    CheckStatus(dalib200TransposeSetup(plan_.get(), n, nd, static_cast<int>(TypeSize(in.type())), is.data(), perm.data(), os.data()), name_);
     layout_ = a.layout;
     SetOutput(out, in.type(), n, nd, os);
     return true;
@@ -2410,8 +2312,8 @@ class JoinGPU : public PermuteOpBase {
         const int64_t *s = ws.Input<GPUBackend>(k).tensor_shape_span(i);
         std::copy(s, s + nd, is.begin() + ((size_t)i * nin + k) * nd);
       }
-    EnsureCap(std::max(n * nin, 1));
-    CheckStatus(dalib200JoinSetup(plan_, n, nin, nd, static_cast<int>(TypeSize(in0.type())), is.data(), a.axis, stack_, os.data()), name_);
+    plan_.Ensure(std::max(n * nin, 1), name_);
+    CheckStatus(dalib200JoinSetup(plan_.get(), n, nin, nd, static_cast<int>(TypeSize(in0.type())), is.data(), a.axis, stack_, os.data()), name_);
     layout_ = a.layout;
     SetOutput(out, in0.type(), n, ond, os);
     return true;
@@ -2521,7 +2423,6 @@ class ReduceGPU : public Operator<GPUBackend> {
     DALI_ENFORCE(!spec.HasArgument("dtype") || dtype_ >= 0, name_, ": invalid dtype ", dtype_);
     ddof_ = spec.HasArgument("ddof") ? spec.GetArgument<int>("ddof") : 0;
   }
-  ~ReduceGPU() override { dalib200ReducePlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
@@ -2539,14 +2440,9 @@ class ReduceGPU : public Operator<GPUBackend> {
       for (int i = 0; i < n; i++)
         ReduceCheckMean(name_.c_str(), i, m.tensor_shape_span(i), m.shape().sample_dim(), is.data() + (size_t)i * nd, nd, a.mask);
     }
-    if (n > cap_) {
-      dalib200ReducePlanDestroy(plan_);
-      plan_ = nullptr;
-      cap_ = std::max(n, max_batch_size_);
-      CheckStatus(dalib200ReducePlanCreate(&plan_, cap_), name_.c_str());
-    }
+    plan_.Ensure(n, name_.c_str());
     int32_t out_type = dtype_;
-    if (dalib200ReduceSetup(plan_, op_, static_cast<int>(in.type()), &out_type, n, nd, is.data(), a.mask, a.keep_dims, ddof_, os.data()))
+    if (dalib200ReduceSetup(plan_.get(), op_, static_cast<int>(in.type()), &out_type, n, nd, is.data(), a.mask, a.keep_dims, ddof_, os.data()))
       throw DALIException(dalib200GetLastError());
     int ond = 0;
     for (int k = 0; k < nd; k++) ond += a.keep_dims || !((a.mask >> k) & 1);
@@ -2568,10 +2464,10 @@ class ReduceGPU : public Operator<GPUBackend> {
       mp[i] = ws.NumInput() > 1 ? ws.Input<GPUBackend>(1).raw_tensor(i) : nullptr;
       op[i] = out.raw_mutable_tensor(i);
     }
-    CheckStatus(dalib200ReduceLaunch(plan_, ip.data(), ws.NumInput() > 1 ? mp.data() : nullptr, op.data(), ws.stream()), name_.c_str());
+    CheckStatus(dalib200ReduceLaunch(plan_.get(), ip.data(), ws.NumInput() > 1 ? mp.data() : nullptr, op.data(), ws.stream()), name_.c_str());
   }
-  dalib200ReducePlan *plan_ = nullptr;
-  int cap_ = 0, op_, dtype_ = -1, ddof_ = 0;
+  DALIB200_PLAN(Reduce) plan_{max_batch_size_};
+  int op_, dtype_ = -1, ddof_ = 0;
   std::string name_;
   TensorLayout layout_;
 };
@@ -2594,7 +2490,6 @@ DALI_SCHEMA(experimental__Equalize)
 class EqualizeGPU : public Operator<GPUBackend> {
  public:
   explicit EqualizeGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
-  ~EqualizeGPU() override { dalib200EqualizePlanDestroy(plan_); }
 
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
@@ -2602,13 +2497,8 @@ class EqualizeGPU : public Operator<GPUBackend> {
     const int n = in.num_samples(), nd = in.shape().sample_dim();
     std::vector<int64_t> is((size_t)n * nd);
     for (int i = 0; i < n; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
-    if (n > cap_) {
-      dalib200EqualizePlanDestroy(plan_);
-      plan_ = nullptr;
-      cap_ = std::max(n, max_batch_size_);
-      CheckStatus(dalib200EqualizePlanCreate(&plan_, cap_), "experimental.Equalize");
-    }
-    if (dalib200EqualizeSetup(plan_, static_cast<int>(in.type()), n, nd, is.data(), in.GetLayout().str().c_str()))
+    plan_.Ensure(n, "experimental.Equalize");
+    if (dalib200EqualizeSetup(plan_.get(), static_cast<int>(in.type()), n, nd, is.data(), in.GetLayout().str().c_str()))
       throw DALIException(dalib200GetLastError());
     out.resize(1);
     out[0].type = DALI_UINT8;
@@ -2619,17 +2509,9 @@ class EqualizeGPU : public Operator<GPUBackend> {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(in.GetLayout());
-    const int n = out.num_samples();
-    std::vector<const void *> ip(n);
-    std::vector<void *> op(n);
-    for (int i = 0; i < n; i++) {
-      ip[i] = in.raw_tensor(i);
-      op[i] = out.raw_mutable_tensor(i);
-    }
-    CheckStatus(dalib200EqualizeLaunch(plan_, ip.data(), op.data(), ws.stream()), "experimental.Equalize");
+    CheckStatus(dalib200EqualizeLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), "experimental.Equalize");
   }
-  dalib200EqualizePlan *plan_ = nullptr;
-  int cap_ = 0;
+  DALIB200_PLAN(Equalize) plan_{max_batch_size_};
 };
 DALI_REGISTER_OPERATOR(experimental__Equalize, EqualizeGPU, GPU);
 
@@ -2706,10 +2588,8 @@ class RotateGPU : public Operator<GPUBackend> {
     DALI_ENFORCE(!spec.ArgumentDefined("axis"), "Rotate: `axis` (3-D rotation) is not supported by the GPU path");
     use_fill_ = spec.ArgumentDefined("fill_value");
     if (use_fill_) fill_ = spec.GetArgument<float>("fill_value");
-    CheckStatus(dalib200WarpPlanCreate(&plan_, max_batch_size_ * 64), "Rotate");
-    plan_cap_ = max_batch_size_ * 64;
+    plan_.Ensure(max_batch_size_ * 64, "Rotate");
   }
-  ~RotateGPU() override { dalib200WarpPlanDestroy(plan_); }
  protected:
   bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
@@ -2717,11 +2597,10 @@ class RotateGPU : public Operator<GPUBackend> {
     out_type_ = spec_.ArgumentDefined("dtype") ? spec_.GetArgument<DALIDataType>("dtype") : DALI_UINT8;
     DALI_ENFORCE(out_type_ == DALI_UINT8 || out_type_ == DALI_FLOAT, "Rotate: output type must be UINT8 or FLOAT");
     const int n = in.num_samples();
-    frames_ = ExpandFrames(in.shape(), in.GetLayout(), "Rotate");
+    ExpandFrames(frames_, in.shape(), in.GetLayout(), "Rotate", true);
     const int nf = frames_.num_frames();
-    if (nf > plan_cap_) { dalib200WarpPlanDestroy(plan_); plan_ = nullptr; plan_cap_ = nf; CheckStatus(dalib200WarpPlanCreate(&plan_, nf), "Rotate"); }
+    plan_.Ensure(nf, "Rotate");
     samples_.assign(nf, dalib200WarpSample());
-    out_hw_.assign(n, {0, 0});
     int fk = 0;
     for (int i = 0; i < n; i++) {
       const int64_t *s = in.shape().tensor_shape_span(i);
@@ -2736,7 +2615,7 @@ class RotateGPU : public Operator<GPUBackend> {
       }
       int oh, ow; float M[6];
       rotate_detail::Params(angle, H, W, keep_size_, sz.empty() ? nullptr : sz.data(), oh, ow, M);
-      out_hw_[i] = { oh, ow };
+      frames_.out_hw[i] = { oh, ow };
       const int64_t frames = fs ? s[0] : 1;
       for (int64_t k = 0; k < frames; k++, fk++) {
         auto &w = samples_[fk];
@@ -2745,40 +2624,27 @@ class RotateGPU : public Operator<GPUBackend> {
         std::copy(M, M + 6, w.matrix);
       }
     }
-    CheckStatus(dalib200WarpPlanSetup(plan_, nf, samples_.data(), interp_, use_fill_, fill_, out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Rotate");
+    CheckStatus(dalib200WarpPlanSetup(plan_.get(), nf, samples_.data(), interp_, use_fill_, fill_, out_type_ == DALI_UINT8 ? DALIB200_UINT8 : DALIB200_FLOAT), "Rotate");
     out.resize(1);
     out[0].type = out_type_;
-    out[0].shape.resize(n, in.shape().sample_dim());
-    for (int i = 0; i < n; i++) {
-      TensorShape sh = in.shape().tensor_shape(i);
-      sh[frames_.first_spatial] = out_hw_[i].first; sh[frames_.first_spatial + 1] = out_hw_[i].second;
-      out[0].shape.set_tensor_shape(i, sh);
-    }
+    out[0].shape = frames_.OutputShape(in.shape());
     return true;
   }
   void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
-    out.SetLayout(in.GetLayout().empty() ? TensorLayout(frames_.first_spatial ? "FHWC" : "HWC") : in.GetLayout());
-    auto ip = FramePtrs(in, frames_, 1);
-    std::vector<void *> op(frames_.num_frames());
-    std::vector<int64_t> next(out.num_samples(), 0);
-    for (int k = 0; k < frames_.num_frames(); k++) {
-      const int s = frames_.sample_of_frame[k];
-      op[k] = static_cast<uint8_t *>(out.raw_mutable_tensor(s)) + next[s];
-      next[s] += static_cast<int64_t>(out_hw_[s].first) * out_hw_[s].second * frames_.c[k] * TypeSize(out_type_);
-    }
-    CheckStatus(dalib200WarpLaunch(plan_, ip.data(), op.data(), ws.stream()), "Rotate");
+    out.SetLayout(frames_.OutputLayout(in.GetLayout()));
+    const auto ip = frames_.InputPtrs(in);
+    const auto op = frames_.OutputPtrs(out, TypeSize(out_type_));
+    CheckStatus(dalib200WarpLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), "Rotate");
   }
  private:
-  dalib200WarpPlan *plan_ = nullptr;
-  int plan_cap_ = 0;
+  DALIB200_PLAN(Warp) plan_{max_batch_size_};
   bool interp_ = true, keep_size_ = false, use_fill_ = false;
   float fill_ = 0;
   DALIDataType out_type_ = DALI_UINT8;
   FrameList frames_;
   std::vector<dalib200WarpSample> samples_;
-  std::vector<std::pair<int, int>> out_hw_;
 };
 DALI_REGISTER_OPERATOR(Rotate, RotateGPU, GPU);
 
@@ -2786,20 +2652,16 @@ DALI_REGISTER_OPERATOR(Rotate, RotateGPU, GPU);
 class SignalOpBase : public Operator<GPUBackend> {
  public:
   explicit SignalOpBase(const OpSpec &spec, const char *name) : Operator<GPUBackend>(spec), name_(name) {
-    CheckStatus(dalib200SignalPlanCreate(&plan_, max_batch_size_), name_);
+    plan_.Ensure(max_batch_size_, name_);
   }
-  ~SignalOpBase() override { dalib200SignalPlanDestroy(plan_); }
  protected:
   void RunImpl(Workspace &ws) override {
     const auto &in = ws.Input<GPUBackend>(0);
     auto &out = ws.Output<GPUBackend>(0);
     out.SetLayout(in.GetLayout());
-    std::vector<const void *> ip(in.num_samples());
-    std::vector<void *> op(in.num_samples());
-    for (int i = 0; i < in.num_samples(); i++) { ip[i] = in.raw_tensor(i); op[i] = out.raw_mutable_tensor(i); }
-    CheckStatus(dalib200SignalLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
+    CheckStatus(dalib200SignalLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), name_);
   }
-  dalib200SignalPlan *plan_ = nullptr;
+  DALIB200_PLAN(Signal) plan_{max_batch_size_};
   const char *name_;
 };
 
@@ -2865,7 +2727,7 @@ class AudioResampleGPU : public SignalOpBase {
       if (nd == 2) out[0].shape.set_tensor_shape(i, { s[i].out_length, sh[1] });
       else out[0].shape.set_tensor_shape(i, { s[i].out_length });
     }
-    CheckStatus(dalib200AudioResampleSetup(plan_, n, s.data(), quality_), name_);
+    CheckStatus(dalib200AudioResampleSetup(plan_.get(), n, s.data(), quality_), name_);
     return true;
   }
   bool has_rates_ = false, has_scale_ = false, has_len_ = false;
@@ -2903,7 +2765,7 @@ class NonsilentRegionGPU : public SignalOpBase {
       args[i].reference_power = has_ref_ ? spec_.GetArgument<float>("reference_power", &ws, i) : 0.0f;
       DALI_ENFORCE(!has_ref_ || args[i].reference_power > 0, "`reference_power` has to be positive. Got: ", args[i].reference_power);
     }
-    CheckStatus(dalib200NonsilentSetup(plan_, n, len.data(), args.data(), window_, reset_), name_);
+    CheckStatus(dalib200NonsilentSetup(plan_.get(), n, len.data(), args.data(), window_, reset_), name_);
     out.resize(2);
     for (int o = 0; o < 2; o++) {
       out[o].type = DALI_INT32;
@@ -2919,7 +2781,7 @@ class NonsilentRegionGPU : public SignalOpBase {
     std::vector<const void *> ip(n);
     std::vector<void *> bp(n), lp(n);
     for (int i = 0; i < n; i++) { ip[i] = in.raw_tensor(i); bp[i] = begin.raw_mutable_tensor(i); lp[i] = length.raw_mutable_tensor(i); }
-    CheckStatus(dalib200NonsilentLaunch(plan_, ip.data(), bp.data(), lp.data(), ws.stream()), name_);
+    CheckStatus(dalib200NonsilentLaunch(plan_.get(), ip.data(), bp.data(), lp.data(), ws.stream()), name_);
   }
   int window_ = 2048, reset_ = 8192;
   bool has_ref_ = false;
@@ -2966,7 +2828,7 @@ class PreemphasisFilterGPU : public SignalOpBase, public PreemphasisProducer {
       lens[i] = vol;
       coeffs_[i] = spec_.GetArgument<float>("preemph_coeff", &ws, i);
     }
-    CheckStatus(dalib200PreemphasisSetup(plan_, n, lens.data(), coeffs_.data(), border_, in.type() == DALI_INT16 ? DALIB200_INT16 : DALIB200_FLOAT),
+    CheckStatus(dalib200PreemphasisSetup(plan_.get(), n, lens.data(), coeffs_.data(), border_, in.type() == DALI_INT16 ? DALIB200_INT16 : DALIB200_FLOAT),
                 name_);
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = DALI_FLOAT;
@@ -2978,8 +2840,7 @@ class PreemphasisFilterGPU : public SignalOpBase, public PreemphasisProducer {
     deferred_now_ = fuse_ && in.type() == DALI_FLOAT;
     if (deferred_now_) {
       ws.Output<GPUBackend>(0).SetLayout(in.GetLayout());
-      deferred_in_.resize(in.num_samples());
-      for (int i = 0; i < in.num_samples(); i++) deferred_in_[i] = in.raw_tensor(i);
+      deferred_in_ = InPtrs(in);
       return;
     }
     SignalOpBase::RunImpl(ws);
@@ -3015,7 +2876,7 @@ class ToDecibelsGPU : public SignalOpBase {
     const int n = in.num_samples();
     std::vector<int64_t> vol(n);
     for (int i = 0; i < n; i++) vol[i] = in.shape().tensor_size(i);
-    CheckStatus(dalib200ToDecibelsSetup(plan_, &args_, n, vol.data()), name_);
+    CheckStatus(dalib200ToDecibelsSetup(plan_.get(), &args_, n, vol.data()), name_);
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = DALI_FLOAT;
     return true;
@@ -3056,11 +2917,11 @@ class MfccGPU : public SignalOpBase {
     const int n = in.num_samples();
     std::vector<int64_t> shp(2 * n);
     for (int i = 0; i < n; i++) { shp[2 * i] = in.shape().tensor_shape_span(i)[0]; shp[2 * i + 1] = in.shape().tensor_shape_span(i)[1]; }
-    CheckStatus(dalib200MfccSetup(plan_, &args_, n, shp.data()), name_);
+    CheckStatus(dalib200MfccSetup(plan_.get(), &args_, n, shp.data()), name_);
     out.resize(1);
     out[0].type = DALI_FLOAT;
     out[0].shape.resize(n, 2);
-    for (int i = 0; i < n; i++) out[0].shape.set_tensor_shape(i, { dalib200SignalOutputRows(plan_), shp[2 * i + 1] });
+    for (int i = 0; i < n; i++) out[0].shape.set_tensor_shape(i, { dalib200SignalOutputRows(plan_.get()), shp[2 * i + 1] });
     return true;
   }
   dalib200MfccArgs args_{};
@@ -3113,7 +2974,7 @@ class NormalizeGPU : public SignalOpBase {
       const int64_t *s = in.shape().tensor_shape_span(i);
       shp[2 * i] = nd == 1 ? 1 : s[0]; shp[2 * i + 1] = nd == 1 ? s[0] : s[1];
     }
-    CheckStatus(dalib200NormalizeSetup(plan_, &args_, n, shp.data()), name_);
+    CheckStatus(dalib200NormalizeSetup(plan_.get(), &args_, n, shp.data()), name_);
     out.resize(1);
     out[0].shape = in.shape(); out[0].type = DALI_FLOAT;
     return true;
@@ -3143,9 +3004,8 @@ DALI_SCHEMA(Cast)
 class ArithmeticGPU : public Operator<GPUBackend> {
  public:
   explicit ArithmeticGPU(const OpSpec &spec, const char *name) : Operator<GPUBackend>(spec), name_(name) {
-    CheckStatus(dalib200ArithPlanCreate(&plan_, max_batch_size_), name_);
+    plan_.Ensure(max_batch_size_, name_);
   }
-  ~ArithmeticGPU() override { dalib200ArithPlanDestroy(plan_); }
 
  protected:
   virtual std::string Description() const { return spec_.GetArgument<std::string>("expression_desc"); }
@@ -3187,7 +3047,7 @@ class ArithmeticGPU : public Operator<GPUBackend> {
     Constants(ints, reals);
     const std::string desc = Description();
     int32_t out_type = 0;
-    CheckStatus(dalib200ArithCompile(plan_, desc.c_str(), nin, types.data(), scalar.data(), ints.data(), static_cast<int>(ints.size()),
+    CheckStatus(dalib200ArithCompile(plan_.get(), desc.c_str(), nin, types.data(), scalar.data(), ints.data(), static_cast<int>(ints.size()),
                                      reals.data(), static_cast<int>(reals.size()), &out_type), name_);
     std::vector<int64_t> shapes(static_cast<size_t>(n) * nin * 6, 0), oshapes(static_cast<size_t>(n) * 6, 0);
     std::vector<const void *> scal(static_cast<size_t>(n) * nin, nullptr);
@@ -3198,7 +3058,7 @@ class ArithmeticGPU : public Operator<GPUBackend> {
         std::copy(s, s + ndims[k], shapes.begin() + ((size_t)i * nin + k) * 6);
       }
     int32_t ond = 0;
-    CheckStatus(dalib200ArithSetup(plan_, n, ndims.data(), shapes.data(), scal.data(), oshapes.data(), &ond), name_);
+    CheckStatus(dalib200ArithSetup(plan_.get(), n, ndims.data(), shapes.data(), scal.data(), oshapes.data(), &ond), name_);
     // the output's layout: that of the first input, among those of the most dimensions, whose shape is the output's in every sample
     layout_ = TensorLayout();
     for (int k = 0; k < nin && layout_.empty(); k++) {
@@ -3226,10 +3086,10 @@ class ArithmeticGPU : public Operator<GPUBackend> {
       if (ws.InputIsType(k, true))
         for (int i = 0; i < n; i++) ip[(size_t)i * nin + k] = ws.Input<GPUBackend>(k).raw_tensor(i);
     for (int i = 0; i < n; i++) op[i] = out.raw_mutable_tensor(i);
-    CheckStatus(dalib200ArithLaunch(plan_, ip.data(), op.data(), ws.stream()), name_);
+    CheckStatus(dalib200ArithLaunch(plan_.get(), ip.data(), op.data(), ws.stream()), name_);
   }
 
-  dalib200ArithPlan *plan_ = nullptr;
+  DALIB200_PLAN(Arith) plan_{max_batch_size_};
   const char *name_;
   TensorLayout layout_;
 };
