@@ -31,6 +31,7 @@
 #include "common.cuh"
 #include "jpeg_recon.h"
 #include "jpeg_idct_core.h"
+#include "jpeg_huff_core.h"
 #include <algorithm>
 #include <cstring>
 #include <map>
@@ -38,34 +39,17 @@
 
 namespace dalib200 {
 
-constexpr int kDcLutBits = 9, kAcLutBits = 11;   // first-level Huffman lookup widths (std DC codes are <= 9 bits)
-constexpr int kDcLutSize = 1 << kDcLutBits, kAcLutSize = 1 << kAcLutBits;
-constexpr int kLutWords = 2 * kDcLutSize + 2 * kAcLutSize;          // DC0 DC1 AC0 AC1 back to back: 20 KB
 constexpr int kSyncThreads = 256;            // subsequences per synchronisation block
 constexpr int kChunkBytes = 4096;            // un-stuffing chunk
 constexpr uint32_t kCleanPad = 32;           // zero bytes behind the clean stream of every unit (at least: units are 16-byte aligned)
 constexpr int kMaxLog2Sub = 10;              // largest subsequence: 2^10 bits = 128 bytes
 
-// Huffman tables as the device sees them.  The first-level LUTs (one 32-bit entry per 10-bit prefix, see make_entry) are
-// copied to shared memory by every sync block; the canonical tables for longer codes stay in global memory.
-constexpr int kLongLut = 512;
-struct HuffSlow {
-  int32_t maxcode[18];        // T.81 F.2.2.3: maxcode[l] left-aligned to 16 bits (+1)
-  int32_t valoff[18];         // valptr[l] - mincode[l]
-  uint8_t vals[256];
-  // canonical codes grow with their length, so the codes longer than the first-level LUT occupy the top [long_base, 65536) of the
-  // left-aligned 16-bit code space -- 192 values for the standard tables.  When that range fits, ONE lookup indexed by
-  // (window - long_base) replaces the length search (which ran on a single lane while the warp waited).  Entry = code length | symbol << 8, 0 = not a code.  long_n == 0: use the search.
-  int32_t long_base, long_n;
-  uint16_t long_lut[kLongLut];
-};
-
+// Huffman tables as the device sees them (jpeg_huff_core.h).  The first-level LUTs are copied to shared memory by every block; the
+// canonical tables for longer codes stay in global memory.
 struct TableSet {             // the 4 tables a baseline scan can reference: DC0, DC1, AC0, AC1
-  uint32_t lut[kLutWords];    // 32-bit entries (make_entry): synchronisation passes
-  uint16_t lut16[kLutWords];  // 16-bit entries (make_entry16): write pass (half the shared memory -> 3 x 8 warps more per SM)
+  uint32_t lut[kLutWords];    // at LutOffset(t)
   HuffSlow slow[4];
 };
-__host__ __device__ inline int LutOffset(int t) { return t < 2 ? t * kDcLutSize : 2 * kDcLutSize + (t - 2) * kAcLutSize; }
 
 // Post pass of one sample (decoders.image with output_type / dtype / orientation / unaligned ROI handling): gathers the
 // oriented region of interest from the decoded window and converts colour space and type
@@ -387,72 +371,49 @@ __device__ __forceinline__ uint64_t pack_state(uint32_t p, int c, int z, uint32_
 }
 __device__ __forceinline__ uint32_t state_count(uint64_t s) { return (uint32_t)(s >> 42) & 1023u; }
 
-// LUT entry (host: MakeLutEntry): [4:0] bits consumed (code + magnitude, <= 31), [11:8] magnitude size s, [16:12] code
-// length, [26:20] zig-zag advance (run + 1; 16 for ZRL; 64 for EOB; 1 for DC).  0 = code longer than the first-level width.
-// The funnel shifts of the bit window take the entry register itself as the shift amount (shf.wrap masks it to 5 bits),
-// which keeps the loop-carried dependency at LDS -> SHF -> SHF -> LEA -> LDS.
-__device__ __forceinline__ uint32_t make_entry(uint32_t len, uint32_t sym, bool is_dc) {
-  const uint32_t s = sym & 15u, r = sym >> 4;
-  const uint32_t adv = is_dc ? 1u : (s == 0 ? (r == 15u ? 16u : 64u) : r + 1u);
-  return (len + s) | (s << 8) | (len << 12) | (adv << 20);
-}
-
-// 16-bit entry of the write pass (host: MakeLutEntry16): [4:0] bits consumed, [8:5] magnitude size s, [15:9] zig-zag advance;
-// code length = consumed - s.  0 = code longer than the first-level width.
-__device__ __forceinline__ uint32_t make_entry16(uint32_t len, uint32_t sym, bool is_dc) {
-  const uint32_t s = sym & 15u, r = sym >> 4;
-  const uint32_t adv = is_dc ? 1u : (s == 0 ? (r == 15u ? 16u : 64u) : r + 1u);
-  return (len + s) | (s << 5) | (adv << 9);
-}
-
 // codes longer than the first-level LUT (std tables: AC codes of 12..16 bits, < 1 % of the symbols): canonical search,
-// T.81 F.2.2.3.  `toff` = LUT word offset of the table, which identifies it.  Returns code length | symbol << 8; a window that matches
-// no code gives 17 | 0, which the 5-bit length fields of make_entry / make_entry16 and the >= 32-bit window hold.  The sync, walk and
-// write passes all decode through here, so they stay in step on damaged data.
+// T.81 F.2.2.3.  `toff` = LUT word offset of the table, which identifies it.  Returns the entry of the code (a single step,
+// huff_entry); a window that matches no code gives 17 bits and symbol 0, which the 5-bit bit counts and the >= 32-bit window hold.
+// The sync, walk and write passes all decode through here, so they stay in step on damaged data.
 __device__ __noinline__ uint32_t slow_lookup(const HuffSlow *__restrict__ slow, uint32_t toff, uint32_t hi, bool is_dc) {
   const int tbl = toff < 2u * kDcLutSize ? (int)(toff / kDcLutSize) : 2 + (int)((toff - 2u * kDcLutSize) / kAcLutSize);
   const HuffSlow *sl = slow + tbl;
   const int32_t code16 = (int32_t)(hi >> 16);
+  uint32_t len, sym = 0;
   if (sl->long_n > 0) {
     const int idx = min(max(code16 - sl->long_base, 0), sl->long_n - 1);
     const uint32_t e = sl->long_lut[idx];
-    return e ? e : 17u;                                      // not a code: 17 bits, symbol 0 (libjpeg jpeg_huff_decode)
+    len = e ? (e & 0xFFu) : 17u;                             // not a code: 17 bits, symbol 0 (libjpeg jpeg_huff_decode)
+    sym = e >> 8;
+  } else {
+    len = (is_dc ? kDcLutBits : kAcLutBits) + 1;
+    while (len <= 16 && code16 >= sl->maxcode[len]) len++;
+    if (len > 16) len = 17;                                  // not a code: 17 bits, symbol 0, as libjpeg (jpeg_huff_decode)
+    else sym = sl->vals[(sl->valoff[len] + (code16 >> (16 - len))) & 0xFF];
   }
-  uint32_t len = (is_dc ? kDcLutBits : kAcLutBits) + 1;
-  while (len <= 16 && code16 >= sl->maxcode[len]) len++;
-  uint32_t sym = 0;
-  if (len > 16) len = 17;                                    // not a code: 17 bits, symbol 0, as libjpeg (jpeg_huff_decode)
-  else sym = sl->vals[(sl->valoff[len] + (code16 >> (16 - len))) & 0xFF];
-  return len | (sym << 8);
-}
-__device__ __forceinline__ uint32_t slow_symbol(const HuffSlow *__restrict__ slow, uint32_t toff, uint32_t hi, bool is_dc) {
-  const uint32_t ls = slow_lookup(slow, toff, hi, is_dc);
-  return make_entry(ls & 0xFFu, ls >> 8, is_dc);
-}
-__device__ __forceinline__ uint32_t slow_symbol16(const HuffSlow *__restrict__ slow, uint32_t toff, uint32_t hi, bool is_dc) {
-  const uint32_t ls = slow_lookup(slow, toff, hi, is_dc);
-  return make_entry16(ls & 0xFFu, ls >> 8, is_dc);
+  return huff_entry(len, sym, is_dc);
 }
 
 // Decodes the symbols that START before `end` (absolute bit positions inside the unit) without producing coefficients: the
 // synchronisation only needs the state (pos, c, z) and `nb`, the number of completed blocks.  Branch-free apart from the loop
-// and the rare long-code path.
+// and the rare long-code path.  A step decodes one symbol or two of one block (huff_step); a block ends at most once per step.
 template <class Win, class Lut, class Tbl>
 __device__ __forceinline__ void decode_span(Win &win, const Lut &lut, const HuffSlow *__restrict__ slow,
                                             const Tbl &tbl, int bpm, uint32_t &pos, uint32_t end, int &c, int &z, uint32_t &nb) {
   uint32_t tb12 = tbl.load(c);                                // dc table offset | ac table offset << 16 (in LUT words)
   while (pos < end) {
+    const uint32_t thr = pair_threshold(z, pos, end);
     // the AC entry is fetched before z is known (it is the common case and sits on the loop-carried path); the DC entry only
     // by the lanes that start a block, so that its random-bank lookup costs one shared-memory wavefront instead of three
     const uint32_t e_ac = lut.load((tb12 >> 16) + (win.hi >> (32 - kAcLutBits)));
     const bool is_dc = z == 0;
     uint32_t e = e_ac;
     if (is_dc) e = lut.load((tb12 & 0xFFFFu) + (win.hi >> (32 - kDcLutBits)));
-    if (__builtin_expect(e == 0, 0)) e = slow_symbol(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
-    const uint32_t tb = e & 31u, adv = e >> 20;
-    win.consume(e);
-    pos += tb;
-    z += (int)adv;
+    if (__builtin_expect(e == 0, 0)) e = slow_lookup(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
+    const uint32_t st = huff_step(e, thr);
+    win.consume(st);
+    pos += step_bits(st);
+    z += (int)step_adv(st);
     const bool endb = z >= 64;                                // block finished (EOB, 64th coefficient, or garbage overrun)
     const int c1 = c + 1 == bpm ? 0 : c + 1;
     nb += endb ? 1u : 0u;
@@ -774,18 +735,18 @@ __global__ void __launch_bounds__(1024) huff_scan_kernel(HuffCtx cx) {
 //
 // The loop is a chain of dependent fixed-latency instructions (its stalls are fixed-latency waits and short scoreboards):
 // throughput scales with resident warps.  The pass therefore runs its own block shape -- kWriteThreads subsequences per CTA,
-// 16-bit LUT entries (10 KB instead of 20) and the stream read from global memory (StreamWindow), so that shared memory holds
-// only the tables and the block buffers: 10.1 KB + 128 B per thread.
+// and the stream read from global memory (StreamWindow), so that shared memory holds only the tables and the block buffers:
+// 20.1 KB + 128 B per thread.
 constexpr int kWriteThreads = 384;
-constexpr int kWriteCtasPerSm = 3;       // 3 x (58.1 KB + 1 KB reserved) of the 228 KB per SM
+constexpr int kWriteCtasPerSm = 3;       // 3 x (68.1 KB + 1 KB reserved) of the 228 KB per SM
 struct WriteSmem {
-  uint16_t *lut; uint32_t *tbl, *blkbuf; uint8_t *zig;
+  uint32_t *lut, *tbl, *blkbuf; uint8_t *zig;
 };
-__host__ __device__ inline size_t write_smem_bytes() { return kLutWords * 2 + 16 * 4 /*tbl*/ + 64 /*zig*/ + (size_t)kWriteThreads * 128; }
+__host__ __device__ inline size_t write_smem_bytes() { return kLutWords * 4 + 16 * 4 /*tbl*/ + 64 /*zig*/ + (size_t)kWriteThreads * 128; }
 __device__ __forceinline__ WriteSmem carve_write_smem(uint32_t *base) {
   WriteSmem s;
-  s.lut = reinterpret_cast<uint16_t *>(base);
-  s.tbl = base + kLutWords / 2;
+  s.lut = base;
+  s.tbl = base + kLutWords;
   s.zig = reinterpret_cast<uint8_t *>(s.tbl + 16);
   s.blkbuf = reinterpret_cast<uint32_t *>(s.zig + 64);                       // 16-byte aligned: every size above is a multiple of 16
   return s;
@@ -797,9 +758,9 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
   const JpegImage &im = cx.images[cx.wblock_image[blockIdx.x]];
   // ---- prologue: tables, per-thread subsequence geometry
   {
-    const uint4 *src = reinterpret_cast<const uint4 *>(cx.tables[im.table_set].lut16);
+    const uint4 *src = reinterpret_cast<const uint4 *>(cx.tables[im.table_set].lut);
     uint4 *dst = reinterpret_cast<uint4 *>(sm.lut);
-    for (int i = threadIdx.x; i < kLutWords * 2 / 16; i += blockDim.x) dst[i] = __ldg(src + i);
+    for (int i = threadIdx.x; i < kLutWords / 4; i += blockDim.x) dst[i] = __ldg(src + i);
     if (threadIdx.x < kMaxBlocksPerMcu) sm.tbl[threadIdx.x] = tbl_word(im, threadIdx.x);
     if (threadIdx.x < 64) sm.zig[threadIdx.x] = c_zigzag[threadIdx.x];
   }
@@ -859,28 +820,36 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
     const uint32_t blk = blk0 + nb;
     if (it & 1u) win.top_up();                                // warp-uniform, see StreamWindow
     if (active) {
-      const uint32_t e_ac = lds_u16(a_lut + 2u * ((tb12 >> 16) + (win.hi >> (32 - kAcLutBits))));
+      const uint32_t thr = pair_threshold(z, pos, hard_end);
+      const uint32_t e_ac = lds_u32(a_lut + 4u * ((tb12 >> 16) + (win.hi >> (32 - kAcLutBits))));
       const bool is_dc = z == 0;
       uint32_t e = e_ac;
-      if (is_dc) e = lds_u16(a_lut + 2u * ((tb12 & 0xFFFFu) + (win.hi >> (32 - kDcLutBits))));
-      if (__builtin_expect(e == 0, 0)) e = slow_symbol16(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
-      const uint32_t tb = e & 31u, adv = e >> 9, s = (e >> 5) & 15u;
+      if (is_dc) e = lds_u32(a_lut + 4u * ((tb12 & 0xFFFFu) + (win.hi >> (32 - kDcLutBits))));
+      if (__builtin_expect(e == 0, 0)) e = slow_lookup(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
+      // a pair needs the block open after its first symbol (z + adv1 < 64): nb, own and blk_limit are the same for both symbols.
+      // Its second symbol starts before hard_end, so `active` would have held for it.
+      const uint32_t st = huff_step(e, thr), one = e >> 16;
+      const uint32_t tb = step_bits(st), adv = step_adv(st), s = step_size(st);
       {
-        // magnitude bits (EXTEND, T.81 F.2.2.1), computed by every lane: s == 0 gives v == 0
-        const uint32_t len = tb - s;
-        const uint32_t bits = (uint32_t)(((uint64_t)(win.hi << len)) >> (32u - s));      // 64-bit shift: s == 0 -> 0
-        // (measured: a funnel-shift + sign-mask formulation of EXTEND is 3 instructions shorter but made this kernel slower)
-        const int v = (int)bits - ((s == 0 || ((bits >> (s - 1u)) & 1u)) ? 0 : (int)((1u << s) - 1u));
+        // magnitude bits of the step's last symbol, and of the first one of a pair, computed by every lane: s == 0 gives v == 0
+        const int v = huff_extend(win.hi, tb, s);
         if (own) {
           if (is_dc) {
             dcv[blk] = (int16_t)v;                            // every block has a DC term: the compact array needs no memset
-          } else if (s) {
-            const uint32_t nat = lds_u8(a_zig + min((uint32_t)z + adv - 1u, 63u));
-            sts_u16(a_mybuf + 4u * ((nat >> 1) ^ lane) + 2u * (nat & 1u), (uint32_t)v);
+          } else {
+            const uint32_t tb1 = step_bits(one), s1 = step_size(one);
+            if (tb != tb1 && s1) {                            // a pair whose first symbol has a value: it lands before coefficient 63
+              const uint32_t nat = lds_u8(a_zig + (uint32_t)z + step_adv(one) - 1u);
+              sts_u16(a_mybuf + 4u * ((nat >> 1) ^ lane) + 2u * (nat & 1u), (uint32_t)huff_extend(win.hi, tb1, s1));
+            }
+            if (s) {                                          // runs past coefficient 63 land on 63
+              const uint32_t nat = lds_u8(a_zig + min((uint32_t)z + adv - 1u, 63u));
+              sts_u16(a_mybuf + 4u * ((nat >> 1) ^ lane) + 2u * (nat & 1u), (uint32_t)v);
+            }
           }
         }
       }
-      win.consume(e);
+      win.consume(st);
       pos += tb;
       z += (int)adv;
       const bool endb = z >= 64;                              // block finished (EOB, 64th coefficient, or garbage overrun)
@@ -1703,63 +1672,6 @@ void FillInfo(const ParsedJpeg &j, dalib200JpegInfo *info) {
   info->orientation = j.orientation;
 }
 
-uint32_t MakeLutEntry(int len, int sym, bool is_dc) {       // keep in sync with make_entry (device)
-  const uint32_t s = sym & 15, r = (uint32_t)sym >> 4;
-  const uint32_t adv = is_dc ? 1u : (s == 0 ? (r == 15u ? 16u : 64u) : r + 1u);
-  return ((uint32_t)len + s) | (s << 8) | ((uint32_t)len << 12) | (adv << 20);
-}
-
-uint16_t MakeLutEntry16(int len, int sym, bool is_dc) {     // keep in sync with make_entry16 (device)
-  const uint32_t s = sym & 15, r = (uint32_t)sym >> 4;
-  const uint32_t adv = is_dc ? 1u : (s == 0 ? (r == 15u ? 16u : 64u) : r + 1u);
-  return (uint16_t)(((uint32_t)len + s) | (s << 5) | (adv << 9));
-}
-
-void BuildDeviceTable(const HostHuff &h, uint32_t *lut, uint16_t *lut16, HuffSlow &t, bool is_dc) {
-  const int kLutBits = is_dc ? kDcLutBits : kAcLutBits, kLutSize = 1 << kLutBits;
-  memset(&t, 0, sizeof(t));
-  memset(lut, 0, sizeof(uint32_t) * kLutSize);
-  memset(lut16, 0, sizeof(uint16_t) * kLutSize);
-  int code = 0, k = 0;
-  for (int l = 1; l <= 16; l++) {
-    const int mincode = code;
-    t.valoff[l] = k - mincode;
-    for (int i = 0; i < h.bits[l]; i++, k++, code++) {
-      if (l <= kLutBits) {
-        const int lo = code << (kLutBits - l), cnt = 1 << (kLutBits - l);
-        for (int e = 0; e < cnt && lo + e < kLutSize; e++) {
-          lut[lo + e] = MakeLutEntry(l, h.vals[k & 255], is_dc);
-          lut16[lo + e] = MakeLutEntry16(l, h.vals[k & 255], is_dc);
-        }
-      }
-    }
-    // a 16-bit window belongs to length l iff it is < maxcode[l] (exclusive bound, left-aligned) and matched
-    // no shorter length; for an empty length the bound equals the previous one, so nothing matches
-    t.maxcode[l] = code << (16 - l);
-    code <<= 1;
-  }
-  t.maxcode[17] = 0x7fffffff;
-  memcpy(t.vals, h.vals, 256);
-  // direct table for the codes behind the first level (see HuffSlow)
-  t.long_base = t.maxcode[kLutBits];
-  const int range = 65536 - t.long_base;
-  t.long_n = 0;
-  if (range > 0 && range <= kLongLut) {
-    t.long_n = range;
-    int c2 = 0, k2 = 0;
-    for (int l = 1; l <= 16; l++) {
-      for (int i = 0; i < h.bits[l]; i++, k2++, c2++) {
-        if (l > kLutBits) {
-          const int lo = (c2 << (16 - l)) - t.long_base, cnt = 1 << (16 - l);
-          for (int e = 0; e < cnt; e++)
-            if (lo + e >= 0 && lo + e < range) t.long_lut[lo + e] = (uint16_t)(l | (h.vals[k2 & 255] << 8));
-        }
-      }
-      c2 <<= 1;
-    }
-  }
-}
-
 }  // namespace
 
 // A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP, BMP / PNM), for samples whose decode is a serial
@@ -2355,8 +2267,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
         if (prog) memset(&ts, 0, sizeof(ts));
         else
         for (int t = 0; t < 2; t++) {
-          BuildDeviceTable(j.dc[t], ts.lut + LutOffset(t), ts.lut16 + LutOffset(t), ts.slow[t], true);
-          BuildDeviceTable(j.ac[t], ts.lut + LutOffset(2 + t), ts.lut16 + LutOffset(2 + t), ts.slow[2 + t], false);
+          BuildDeviceTable(j.dc[t].bits, j.dc[t].vals, ts.lut + LutOffset(t), ts.slow[t], true);
+          BuildDeviceTable(j.ac[t].bits, j.ac[t].vals, ts.lut + LutOffset(2 + t), ts.slow[2 + t], false);
         }
         p->tables.push_back(ts);
         it = table_cache.emplace(key, (int)p->tables.size() - 1).first;
