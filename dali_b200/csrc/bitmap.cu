@@ -31,27 +31,37 @@ __global__ void __launch_bounds__(256) bitmap_color_kernel(const BitmapImage *__
   }
 }
 
-int64_t BitmapGroups(std::vector<BitmapImage> &images) {
-  int64_t g = 0;
-  for (BitmapImage &d : images) {
-    d.first_grp = g;
-    g += ((int64_t)d.win_w * d.win_h + kBitmapGroup - 1) / kBitmapGroup;
-  }
-  return g;
+int BitmapStage::Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) {
+  BitmapImage im;
+  int64_t bytes = 0;
+  if (int rc = PlanBitmap(data, len, &im, scratch_bytes, &bytes, info, err)) return rc;
+  scratch_bytes += bytes;
+  if (im.unpack != kBitmapDirect) unpack.push_back((int32_t)images.size());
+  im.sample = sample; im.raw_off = raw_off;
+  images.push_back(im);
+  return DALIB200_SUCCESS;
 }
 
-int LaunchBitmap(const BitmapLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
-  if (a.nunpack > 0) {
-    const SerialLanes g = SerialLaneGeometry(a.nunpack, 1 << 30);
+int BitmapStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  FillWindows(images, in.images);
+  int64_t groups = 0;                        // each image's first_grp: the prefix of the 16-pixel groups of the windows
+  for (BitmapImage &d : images) {
+    d.first_grp = groups;
+    groups += ((int64_t)d.win_w * d.win_h + kBitmapGroup - 1) / kBitmapGroup;
+  }
+  const BitmapImage *d_images; const int32_t *d_unpack;
+  if (int rc = arena.Pack(s, std::tie(d_images, d_unpack), images, unpack)) return rc;
+  const int nunpack = (int)unpack.size();
+  if (nunpack > 0) {
+    const SerialLanes g = SerialLaneGeometry(nunpack, 1 << 30);
     ProfScope ps_("bitmap_unpack", s);
-    bitmap_unpack_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.d_unpack, a.nunpack, g.lanes, a.d_raw, a.d_scratch, a.d_status);
+    bitmap_unpack_kernel<<<g.warps, 32, 0, s>>>(d_images, d_unpack, nunpack, g.lanes, in.d_raw, d_scratch, in.d_status);
     CountLaunch();
   }
-  if (a.total_groups > 0) {
-    const int grid = (int)std::min<int64_t>((a.total_groups + 255) / 256, (int64_t)NumSMs() * 16);
+  if (groups > 0) {
+    const int grid = (int)std::min<int64_t>((groups + 255) / 256, (int64_t)NumSMs() * 16);
     ProfScope ps_("bitmap_color", s);
-    bitmap_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_groups, a.d_raw, a.d_scratch);
+    bitmap_color_kernel<<<grid, 256, 0, s>>>(d_images, (int)images.size(), groups, in.d_raw, d_scratch);
     CountLaunch();
   }
   DB_CUDA(cudaGetLastError());

@@ -1,25 +1,28 @@
-// dali_b200/csrc/bitmap.h -- launch interface of the BMP / PNM stage (bitmap.cu), called by dalib200JpegLaunch for the BMP and PNM
-// samples of a batch.
+// dali_b200/csrc/bitmap.h -- the BMP / PNM stage of decoders.image (bitmap.cu), planned and run by the image decoder plan (jpeg.cu).
 #ifndef DALI_B200_CSRC_BITMAP_H_
 #define DALI_B200_CSRC_BITMAP_H_
-#include <cuda_runtime.h>
 #include <vector>
-#include "bitmap_core.h"
+#include "decode_stage.h"
+#include "bitmap_plan.h"
 
 namespace dalib200 {
 
-struct BitmapLaunch {
-  const BitmapImage *d_images; int nimages;
-  const int32_t *d_unpack; int nunpack;      // the images (indices into d_images) that bitmap_unpack expands first
-  int64_t total_groups;                      // pixel groups of all windows (BitmapImage::first_grp is their prefix)
-  const uint8_t *d_raw;                      // the plan's staged bytes
-  uint8_t *d_scratch;                        // the unpacked planes (BitmapImage::plane_off)
-  int32_t *d_status;
+struct BitmapStage : StreamStage {
+  bool Empty() const override { return images.empty(); }
+  void Clear() override { images.clear(); unpack.clear(); scratch_bytes = 0; }
+  void Destroy() override { SideStage::Destroy(); cudaFree(d_scratch); }
+  int Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) override;
+
+  std::vector<BitmapImage> images;
+  std::vector<int32_t> unpack;               // the RLE / ASCII images among them (indices into images)
+  int64_t scratch_bytes = 0;
+  uint8_t *d_scratch = nullptr; size_t d_scratch_cap = 0;   // unpacked planes (BitmapImage::plane_off; grow only)
+
+ protected:
+  int Reserve() override { return GrowDevice(d_scratch, d_scratch_cap, (size_t)scratch_bytes + 16); }
+  // RLE / ASCII unpack (one lane per image, only when some image needs it), conversion of the decode windows
+  int Enqueue(const StageInputs &in, cudaStream_t s) override;
 };
-// Sets each image's first_grp from its window (after FillWindows) and returns the group total.
-int64_t BitmapGroups(std::vector<BitmapImage> &images);
-// RLE / ASCII unpack (one lane per image, only when nunpack > 0), conversion of the decode windows.  Returns a DALIB200 status.
-int LaunchBitmap(const BitmapLaunch &a, cudaStream_t s);
 
 }  // namespace dalib200
 #endif  // DALI_B200_CSRC_BITMAP_H_

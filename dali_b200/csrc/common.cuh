@@ -201,9 +201,13 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const void *tmap, int c0,
 
 // Host-only declarations: kept at the end of the header so that the line tables of the device code above do not move.
 #include <algorithm>
+#include <cstring>
 #include <exception>
 #include <new>
+#include <tuple>
 namespace dalib200 {
+inline size_t Align(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
 // Grow-only pinned host memory that per-batch data is staged in for asynchronous copies to the device.  It keeps the one rule that
 // makes reusing it safe: the host side is not rewritten while a copy may still be reading it.  Stage() hands the host side out only
 // after the copies covered by the last Record() have finished.  The event behind that is created at the first Record().
@@ -241,6 +245,20 @@ class DescArena : public PinnedStage {
   }
   int Upload(size_t bytes, cudaStream_t s);   // async H2D of the first `bytes`, then Record(s)
   void Free();
+  // Stages the vectors back to back, each at a 16-byte boundary, uploads them on s and points each of `dev` at its vector's copy:
+  //   arena.Pack(s, std::tie(d_images, d_chunks), images, chunks)
+  template <typename... T> int Pack(cudaStream_t s, std::tuple<const T *&...> out, const std::vector<T> &...v) {
+    size_t off[sizeof...(T)], bytes = 0, k = 0;
+    ((off[k++] = bytes, bytes = Align(bytes + sizeof(T) * v.size(), 16)), ...);
+    uint8_t *h;
+    if (int rc = Stage(bytes, &h)) return rc;
+    k = 0;
+    (memcpy(h + off[k++], v.data(), sizeof(T) * v.size()), ...);
+    if (int rc = Upload(bytes, s)) return rc;
+    k = 0;
+    std::apply([&](auto &...d) { ((d = reinterpret_cast<std::remove_reference_t<decltype(d)>>(dev + off[k++])), ...); }, out);
+    return DALIB200_SUCCESS;
+  }
 };
 
 // A grow-only device buffer of `cap` elements: when `need` exceeds it, it is replaced (contents not kept) by one of need + need / 4,

@@ -23,16 +23,17 @@
 //
 // Algorithmic bytes per unit (SURVEY.md 8d): J (encoded bytes) + H*W*3 (decoded image).
 //
-// The plan also takes PNG, TIFF, lossy WebP, BMP and PNM streams (detected by their signatures): png_plan.h, tiff_plan.h, webp_plan.h
-// and bitmap_plan.h read their headers at set-up, png.cu, tiff.cu, webp.cu and bitmap.cu decode them into the same decode windows on
-// streams of their own, and the post pass below serves every format.  Such a sample has no units, subsequences or MCUs, so every kernel
-// of this file skips it.  A lossless JPEG (SOF3) sample is parsed here and planned by ljpeg_plan.h: its restart intervals join U1 - U3 as
-// units of no JPEG image, and ljpeg.cu decodes their clean streams on a stream forked behind U3.
+// The plan also takes PNG, TIFF, lossy WebP, BMP and PNM streams (detected by their signatures): the stage of each format (png.h,
+// tiff.h, webp.h, bitmap.h; decode_stage.h) plans them at set-up and decodes them into the same decode windows on a stream of its own,
+// and the post pass below serves every format.  Such a sample has no units, subsequences or MCUs, so every kernel of this file skips it.
+// A lossless JPEG (SOF3) sample is parsed here and planned by the lossless stage (ljpeg.h): its restart intervals join U1 - U3 as units
+// of no JPEG image, and the stage decodes their clean streams on a stream forked behind U3.
 #include "common.cuh"
 #include "jpeg_recon.h"
 #include "jpeg_idct_core.h"
 #include "jpeg_huff_core.h"
 #include <algorithm>
+#include <array>
 #include <cstring>
 #include <map>
 #include <thread>
@@ -40,8 +41,6 @@
 namespace dalib200 {
 
 constexpr int kSyncThreads = 256;            // subsequences per synchronisation block
-constexpr int kChunkBytes = 4096;            // un-stuffing chunk
-constexpr uint32_t kCleanPad = 32;           // zero bytes behind the clean stream of every unit (at least: units are 16-byte aligned)
 constexpr int kMaxLog2Sub = 10;              // largest subsequence: 2^10 bits = 128 bytes
 
 // Huffman tables as the device sees them (jpeg_huff_core.h).  The first-level LUTs are copied to shared memory by every block; the
@@ -1521,29 +1520,20 @@ namespace {
 
 struct HostHuff { uint8_t bits[17]; uint8_t vals[256]; bool present = false; };
 }  // namespace
-// progressive streams: planner + launch interface of jpeg_prog.cu (included here, behind the kernels, so that their line tables stay put)
+// the decode stages of jpeg_prog.cu, png.cu, tiff.cu, webp.cu, bitmap.cu and ljpeg.cu (included here, behind the kernels, so that their
+// line tables stay put); EXIF orientation
 #include "jpeg_prog.h"
-#include "jpeg_prog_plan.h"
-// EXIF orientation (shared with the PNG and WebP planners); PNG, TIFF and WebP streams: planners + launch interfaces of png.cu, tiff.cu
-// and webp.cu
-#include "exif.h"
 #include "png.h"
-#include "png_plan.h"
 #include "tiff.h"
-#include "tiff_plan.h"
 #include "webp.h"
-#include "webp_plan.h"
-// BMP and PNM streams: planner + launch interface of bitmap.cu
 #include "bitmap.h"
-#include "bitmap_plan.h"
-// lossless JPEG (SOF3): planner + launch interface of ljpeg.cu
 #include "ljpeg.h"
-#include "ljpeg_plan.h"
+#include "exif.h"
 namespace {
 
-// The formats the plan takes, told apart by their signatures.  PNG, TIFF, WebP and BMP / PNM samples are planned by png_plan.h,
-// tiff_plan.h, webp_plan.h and bitmap_plan.h and decoded by png.cu, tiff.cu, webp.cu and bitmap.cu; everything else is parsed as JPEG.
-// A JPEG whose frame header is SOF3 becomes kLossless once parsed: ljpeg_plan.h plans it, ljpeg.cu decodes it.
+// The formats the plan takes, told apart by their signatures.  PNG, TIFF, WebP and BMP / PNM samples are planned and decoded by the
+// stage of their format; everything else is parsed as JPEG.  A JPEG whose frame header is SOF3 becomes kLossless once parsed: the
+// lossless stage plans and decodes it.
 enum class Format { kJpeg, kPng, kTiff, kWebp, kBitmap, kLossless };
 
 Format DetectFormat(const uint8_t *p, size_t n) {
@@ -1674,41 +1664,6 @@ void FillInfo(const ParsedJpeg &j, dalib200JpegInfo *info) {
 
 }  // namespace
 
-// A decode stage beside the baseline JPEG kernels (progressive JPEG, PNG, TIFF, WebP, BMP / PNM), for samples whose decode is a serial
-// chain per image or needs no JPEG kernel: it runs on a stream of its own, so that its work overlaps the JPEG kernels.  Its order on the
-// caller's stream s:
-//   Begin(s)   after the status clear: fork (s -> stage stream);
-//   the caller stages the arena and uploads it on the stage stream, then launches the stage's kernels there;
-//   End()      join event, which s waits on in front of the first kernel that reads the stage's result (dc_scan for the progressive
-//              stage, jpeg_post for the others).
-// A stage with no sample in the batch is not touched: no stream is created, no event recorded.
-struct SideStage {
-  dalib200::DescArena arena;
-  cudaStream_t stream = nullptr;            // created at the first launch that has samples for the stage
-  cudaEvent_t fork = nullptr, join = nullptr;
-
-  bool Create() {
-    return cudaEventCreateWithFlags(&fork, cudaEventDisableTiming) == cudaSuccess &&
-           cudaEventCreateWithFlags(&join, cudaEventDisableTiming) == cudaSuccess;
-  }
-  void Destroy() {
-    if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
-    if (fork) cudaEventDestroy(fork);
-    if (join) cudaEventDestroy(join);
-    arena.Free();
-  }
-  int Begin(cudaStream_t s) {
-    if (!stream) DB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    DB_CUDA(cudaEventRecord(fork, s));
-    DB_CUDA(cudaStreamWaitEvent(stream, fork, 0));
-    return DALIB200_SUCCESS;
-  }
-  int End() {
-    DB_CUDA(cudaEventRecord(join, stream));
-    return DALIB200_SUCCESS;
-  }
-};
-
 struct JpegGeo { int orient = 1, rx0 = 0, ry0 = 0, rx1 = 0, ry1 = 0, out_c = 3; bool direct = true, planar_ok = false; };
 
 struct dalib200JpegPlan {
@@ -1763,56 +1718,25 @@ struct dalib200JpegPlan {
   int32_t *h_status = nullptr; size_t h_status_cap = 0;        // pinned copy of d_status (JpegStatusAsync / JpegStatusFetch)
   dalib200::PinnedStage h_images;           // this launch's JpegImage and JpegPost descriptors (they carry the output pointers)
   bool staged = false, smem_opted = false;
-  // progressive (SOF2) samples: their entropy stage runs in jpeg_prog.cu, everything behind it is shared
-  std::vector<dalib200::ProgImage> prog_images;
-  std::vector<dalib200::ProgScan> prog_scans;     // sorted by wave
-  std::vector<dalib200::ProgHuff> prog_huff;
-  std::vector<int> prog_wave_begin;
-  std::vector<int64_t> prog_first_blk;
-  int64_t prog_total_blocks = 0;
-  SideStage prog;                           // the scans are serial chains on one warp each: they run beside the baseline entropy stage
-  // PNG samples: decoded by png.cu into the same decode windows; the post pass is shared
-  std::vector<dalib200::PngImage> png_images;
-  std::vector<dalib200::PngChunk> png_chunks;
-  int64_t png_scan_bytes = 0;
-  uint8_t *d_png_scan = nullptr; size_t d_png_scan_cap = 0;   // filtered scanlines (grow only)
-  SideStage png;
-  // TIFF samples: decoded by tiff.cu, like the PNG samples
-  std::vector<dalib200::TiffImage> tiff_images;
-  std::vector<dalib200::TiffSeg> tiff_segs;
-  int64_t tiff_dec_bytes = 0;
-  uint8_t *d_tiff_dec = nullptr; size_t d_tiff_dec_cap = 0;    // decoded segments (grow only)
-  uint8_t *d_tiff_slots = nullptr; size_t d_tiff_slots_cap = 0; // segment working memory (grow only)
-  SideStage tiff;
-  // WebP samples: decoded by webp.cu, like the PNG and TIFF samples
-  std::vector<dalib200::WebpImage> webp_images;
-  int64_t webp_scratch_bytes = 0;
-  uint8_t *d_webp_scratch = nullptr; size_t d_webp_scratch_cap = 0;   // coefficients, macroblocks, planes (grow only)
-  SideStage webp;
-  // BMP and PNM samples: decoded by bitmap.cu, like the PNG, TIFF and WebP samples
-  std::vector<dalib200::BitmapImage> bitmap_images;
-  std::vector<int32_t> bitmap_unpack;       // the RLE / ASCII images among them
-  int64_t bitmap_scratch_bytes = 0;
-  uint8_t *d_bitmap_scratch = nullptr; size_t d_bitmap_scratch_cap = 0;   // unpacked planes (grow only)
-  SideStage bitmap;
-  // lossless JPEG samples: their units join U1 - U3 (in `units`, skipped by every DCT kernel); ljpeg.cu decodes the clean streams on a
-  // stage forked behind U3
-  std::vector<dalib200::LjpegImage> ljpeg_images;
-  std::vector<dalib200::LjpegUnit> ljpeg_units;
-  std::vector<dalib200::LjpegTable> ljpeg_tables;
-  std::vector<dalib200::LjpegBand> ljpeg_bands;
-  int64_t ljpeg_total_sub = 0, ljpeg_diff_elems = 0;
-  int16_t *d_ljpeg_diff = nullptr; size_t d_ljpeg_diff_cap = 0;          // differences, reconstructed in place (grow only)
-  uint64_t *d_ljpeg_rec = nullptr; size_t d_ljpeg_rec_cap = 0;           // subsequence records (grow only)
-  uint32_t *d_ljpeg_first = nullptr; size_t d_ljpeg_first_cap = 0;      // first symbol of each subsequence (grow only)
-  SideStage ljpeg;
+  // the stages beside the baseline kernels (decode_stage.h).  The progressive stage writes coefficients for everything behind the entropy
+  // stage; the PNG, TIFF, WebP and BMP / PNM stages decode whole streams into the same decode windows; the lossless samples' units join
+  // U1 - U3 (in `units`, skipped by every DCT kernel) and their stage decodes the clean streams behind U3.  The post pass is shared.
+  ProgStage prog;
+  PngStage png;
+  TiffStage tiff;
+  WebpStage webp;
+  BitmapStage bitmap;
+  LjpegStage ljpeg;
+  std::array<SideStage *, 6> stages() { return { &prog, &png, &tiff, &webp, &bitmap, &ljpeg }; }   // in launch order
+  StreamStage &stage_of(Format f) {
+    switch (f) {
+      case Format::kPng: return png;
+      case Format::kTiff: return tiff;
+      case Format::kWebp: return webp;
+      default: return bitmap;
+    }
+  }
 };
-
-namespace {
-
-inline size_t Align(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-}  // namespace
 
 namespace {
 // Work lists that depend on the per-sample colour decision: post pass descriptors, colour work items, IDCT block ranges.  Run by
@@ -1853,45 +1777,12 @@ void BuildWorkLists(dalib200JpegPlan *p) {
   p->total_items = t.items;
 }
 
-// PNG, TIFF, WebP, BMP or PNM sample `sample` (format f): its planner appends its descriptors to the plan's stage and advances the
-// stage's scratch, its staged bytes go to `raw_off` of the raw staging area, and `j` receives the fields the plan reads for every sample.
-// Returns a DALIB200 status.
-int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t len, int sample, int64_t raw_off, ParsedJpeg &j) {
+// PNG, TIFF, WebP, BMP or PNM sample `sample` (format f): the stage of its format appends its descriptors, its staged bytes go to
+// `raw_off` of the raw staging area, and `j` receives the fields the plan reads for every sample.  Returns a DALIB200 status.
+int PlanSideSample(StreamStage &st, Format f, const uint8_t *data, size_t len, int sample, int64_t raw_off, ParsedJpeg &j) {
   StreamInfo info;
   std::string err;
-  int rc;
-  auto add = [&](auto &images, auto &im) { im.sample = sample; im.raw_off = raw_off; images.push_back(im); };
-  if (f == Format::kPng) {
-    PngImage im;
-    if (!(rc = PlanPng(data, len, (int)p->png_images.size(), &im, p->png_chunks, &info, &err))) {
-      im.scan_off = p->png_scan_bytes;
-      p->png_scan_bytes += (int64_t)Align((size_t)im.scan_bytes, 16);
-      add(p->png_images, im);
-    }
-  } else if (f == Format::kTiff) {
-    TiffImage im;
-    int64_t bytes = 0;
-    if (!(rc = PlanTiff(data, len, (int)p->tiff_images.size(), &im, p->tiff_segs, p->tiff_dec_bytes, &bytes, &info, &err))) {
-      p->tiff_dec_bytes += bytes;
-      add(p->tiff_images, im);
-    }
-  } else if (f == Format::kWebp) {
-    WebpImage im;
-    int64_t bytes = 0;
-    if (!(rc = PlanWebp(data, len, (int)p->webp_images.size(), &im, p->webp_scratch_bytes, &bytes, &info, &err))) {
-      p->webp_scratch_bytes += bytes;
-      add(p->webp_images, im);
-    }
-  } else {
-    BitmapImage im;
-    int64_t bytes = 0;
-    if (!(rc = PlanBitmap(data, len, &im, p->bitmap_scratch_bytes, &bytes, &info, &err))) {
-      p->bitmap_scratch_bytes += bytes;
-      if (im.unpack != kBitmapDirect) p->bitmap_unpack.push_back((int32_t)p->bitmap_images.size());
-      add(p->bitmap_images, im);
-    }
-  }
-  if (rc) { SetLastError("%s", err.c_str()); return rc; }
+  if (int rc = st.Plan(data, len, sample, raw_off, &info, &err)) { SetLastError("%s", err.c_str()); return rc; }
   j.format = f;
   j.width = info.width; j.height = info.height; j.ncomp = info.components; j.orientation = info.orientation;
   j.hs[0] = j.vs[0] = f == Format::kWebp ? 2 : 1;      // reported subsampling: WebP is 4:2:0 (VP8's only layout)
@@ -1899,10 +1790,8 @@ int PlanSideSample(dalib200JpegPlan *p, Format f, const uint8_t *data, size_t le
   return DALIB200_SUCCESS;
 }
 
-// Lossless JPEG sample `sample` (ParseHeaders found SOF3): checks the frame (ljpeg_plan.h), appends its image record, tables and
-// reconstruction bands, and one JpegUnit + LjpegUnit per restart interval, whose bytes sit at `raw` + their offset behind the scan start
-// in the raw staging area; `clean` and `chunks` advance as for a baseline unit.  Returns a DALIB200 status.
-int PlanLossless(dalib200JpegPlan *p, int sample, const uint8_t *d, size_t len, size_t raw, size_t &clean, uint32_t &chunks, ParsedJpeg &j) {
+// The frame of a lossless JPEG (SOF3) sample as the lossless stage's planner (ljpeg_plan.h) reads it.
+LjpegFrame LosslessFrame(const ParsedJpeg &j) {
   LjpegFrame f;
   f.width = j.width; f.height = j.height; f.ncomp = j.ncomp; f.precision = j.precision;
   for (int c = 0; c < 4; c++) { f.hs[c] = j.hs[c]; f.vs[c] = j.vs[c]; }
@@ -1912,69 +1801,7 @@ int PlanLossless(dalib200JpegPlan *p, int sample, const uint8_t *d, size_t len, 
   f.pred = j.ss; f.se = j.se; f.ah = j.ah; f.pt = j.al;
   f.restart_interval = j.restart_interval; f.jfif = j.jfif; f.adobe_transform = j.adobe_transform;
   for (int t = 0; t < 4; t++) if (j.dc[t].present) { f.bits[t] = j.dc[t].bits; f.vals[t] = j.dc[t].vals; }
-  LjpegImage im;
-  std::string err;
-  if (int rc = PlanLjpegFrame(f, &im, p->ljpeg_tables, &err)) { SetLastError("%s", err.c_str()); return rc; }
-  if ((int64_t)j.width * j.height >= (1ll << 31)) { SetLastError("images of 2^31 pixels or more are not supported"); return DALIB200_ERROR_UNSUPPORTED; }
-  const size_t sb = j.scan_begin;
-  size_t se = len;
-  if (se >= sb + 2 && d[se - 2] == 0xFF && d[se - 1] == 0xD9) se -= 2;
-  j.scan_end = se;
-  const int W = j.width, H = j.height, C = j.ncomp;
-  const int lines = j.restart_interval ? j.restart_interval / W : H;
-  const int nunits = (H + lines - 1) / lines;
-  std::vector<std::pair<size_t, size_t>> segs;
-  im.bad_rst = SplitLjpegUnits(d, sb, se, nunits, segs);
-  for (const auto &sg : segs)
-    if (sg.second - sg.first > kLjpegMaxUnitBytes) {
-      SetLastError("lossless JPEG: an entropy-coded segment above %zu bytes is not supported (use restart intervals)", kLjpegMaxUnitBytes);
-      return DALIB200_ERROR_UNSUPPORTED;
-    }
-  im.sample = sample;
-  im.diff_off = p->ljpeg_diff_elems;
-  p->ljpeg_diff_elems += (int64_t)Align((size_t)W * H * C, 8);
-  const int li = (int)p->ljpeg_images.size();
-  for (int k = 0; k < nunits; k++) {
-    JpegUnit u;
-    memset(&u, 0, sizeof(u));
-    u.raw_off = (uint32_t)(raw + (segs[k].first - sb));
-    u.raw_len = (uint32_t)(segs[k].second - segs[k].first);
-    u.clean_off = (uint32_t)clean;
-    u.first_chunk = chunks;
-    u.image = sample;
-    LjpegUnit lu;
-    lu.junit = (int32_t)p->units.size(); lu.image = li;
-    lu.first_sub = p->ljpeg_total_sub;
-    lu.nsub = (int32_t)((u.raw_len + (1u << (kLjpegLog2Sub - 3)) - 1) >> (kLjpegLog2Sub - 3));
-    lu.clean_off = u.clean_off;
-    const int y0 = k * lines, y1 = std::min(H, y0 + lines);
-    lu.nsym = (int64_t)(y1 - y0) * W * C;
-    lu.sym_off = im.diff_off + (int64_t)y0 * W * C;
-    for (int c = 0; c < C; c++) p->ljpeg_bands.push_back(LjpegBand{ li, c, y0, y1 });
-    p->ljpeg_total_sub += lu.nsub;
-    clean += Align(u.raw_len + kCleanPad, 16);
-    chunks += (u.raw_len + kChunkBytes - 1) / kChunkBytes;
-    p->units.push_back(u);
-    p->ljpeg_units.push_back(lu);
-  }
-  p->ljpeg_images.push_back(im);
-  j.format = Format::kLossless;
-  return DALIB200_SUCCESS;
-}
-
-// The decode window and output pointer of every PNG, TIFF, WebP, BMP or PNM image, from its sample's JpegImage as patched for this
-// launch (`hi`).  Returns the pixel total; each image's first_px is its prefix, by which the colour kernel finds the image of a pixel.
-template <typename Image>
-int64_t FillWindows(std::vector<Image> &images, const JpegImage *hi) {
-  int64_t px = 0;
-  for (Image &d : images) {
-    const JpegImage &im = hi[d.sample];
-    d.out = im.out; d.out_type = im.out_type;
-    d.win_x0 = im.win_x0; d.win_y0 = im.win_y0; d.win_w = im.win_w; d.win_h = im.win_h;
-    d.first_px = px;
-    px += (int64_t)im.win_w * im.win_h;
-  }
-  return px;
+  return f;
 }
 
 // Output geometry of sample i: orientation, region of interest, decode window, post pass.  Returns a DALIB200 status.
@@ -2041,8 +1868,13 @@ int dalib200JpegGetInfo(const uint8_t *data, size_t len, dalib200JpegInfo *info)
   DB_CHECK_ARG(data && info, "JpegGetInfo: null argument");
   ParsedJpeg j;
   const Format f = DetectFormat(data, len);
-  dalib200JpegPlan descs;                   // receives the descriptors of a PNG, TIFF, WebP, BMP or PNM stream; no device resources
-  int rc = f == Format::kJpeg ? ParseHeaders(data, len, j, false) : PlanSideSample(&descs, f, data, len, 0, 0, j);
+  // a PNG, TIFF, WebP, BMP or PNM stream is planned into a stage of its format of its own: no device resources
+  auto plan_into = [&](auto &&st) { return PlanSideSample(st, f, data, len, 0, 0, j); };
+  int rc = f == Format::kJpeg ? ParseHeaders(data, len, j, false)
+         : f == Format::kPng  ? plan_into(PngStage())
+         : f == Format::kTiff ? plan_into(TiffStage())
+         : f == Format::kWebp ? plan_into(WebpStage())
+                              : plan_into(BitmapStage());
   if (rc) return rc;
   FillInfo(j, info);
   return DALIB200_SUCCESS;
@@ -2052,22 +1884,20 @@ int dalib200JpegPlanCreate(dalib200JpegPlan **plan, int max_batch) try {
   DB_CHECK_ARG(plan && max_batch > 0, "JpegPlanCreate: bad arguments");
   auto *p = new dalib200JpegPlan();
   p->max_batch = max_batch;
-  if (!p->prog.Create() || !p->png.Create() || !p->tiff.Create() || !p->webp.Create() || !p->bitmap.Create() || !p->ljpeg.Create()) {
-    SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA;
-  }
+  for (SideStage *st : p->stages())
+    if (!st->Create()) { SetLastError("JpegPlanCreate: cudaEventCreate failed"); delete p; return DALIB200_ERROR_CUDA; }
   *plan = p;
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 
 int dalib200JpegPlanDestroy(dalib200JpegPlan *p) try {
   if (!p) return DALIB200_SUCCESS;
-  for (SideStage *st : { &p->prog, &p->png, &p->tiff, &p->webp, &p->bitmap, &p->ljpeg }) st->Destroy();
+  for (SideStage *st : p->stages()) st->Destroy();
   p->h_stage.Free();
   p->h_images.Free();
   if (p->h_status) cudaFreeHost(p->h_status);
   void *bufs[] = { p->d_stage, p->d_clean, p->d_chunk, p->d_unit_len, p->d_state, p->d_n, p->d_coef, p->d_dc, p->d_planes, p->d_status,
-                   p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk, p->d_png_scan,
-                   p->d_tiff_dec, p->d_tiff_slots, p->d_webp_scratch, p->d_bitmap_scratch, p->d_ljpeg_diff, p->d_ljpeg_rec, p->d_ljpeg_first };
+                   p->d_chain1, p->d_chain2, p->d_chain3, p->d_chain_count, p->d_post, p->d_posts, p->d_unit_nblk };
   for (void *b : bufs) if (b) cudaFree(b);
   delete p;
   return DALIB200_SUCCESS;
@@ -2141,15 +1971,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
   p->units.clear(); p->tables.clear(); p->quants.clear(); p->src_ptr.clear(); p->block_image.clear(); p->wblock_image.clear();
   p->first_quad.assign(n, 0);
   p->first_item.assign(n, 0);
-  p->prog_images.clear(); p->prog_scans.clear(); p->prog_huff.clear(); p->prog_wave_begin.clear(); p->prog_first_blk.clear();
-  p->prog_total_blocks = 0;
-  p->png_images.clear(); p->png_chunks.clear(); p->png_scan_bytes = 0;
-  p->tiff_images.clear(); p->tiff_segs.clear(); p->tiff_dec_bytes = 0;
-  p->webp_images.clear(); p->webp_scratch_bytes = 0;
-  p->bitmap_images.clear(); p->bitmap_unpack.clear(); p->bitmap_scratch_bytes = 0;
-  p->ljpeg_images.clear(); p->ljpeg_units.clear(); p->ljpeg_tables.clear(); p->ljpeg_bands.clear();
-  p->ljpeg_total_sub = 0; p->ljpeg_diff_elems = 0;
-  std::map<std::string, int> table_cache, quant_cache, prog_table_cache;
+  for (SideStage *st : p->stages()) st->Clear();
+  std::map<std::string, int> table_cache, quant_cache;
   size_t raw = 0, clean = 0;
   uint32_t chunks = 0;
   int64_t subseq = 0, coefs = 0, planes = 0;
@@ -2173,32 +1996,25 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     DB_CHECK_ARG(streams[i] && lengths[i] > 0, "decoders.image: sample %d is empty", i);
     auto sample_error = [&](int rc, const std::string &what) { SetLastError("decoders.image: sample %d: %s", i, what.c_str()); return rc; };
     const Format f = DetectFormat(streams[i], lengths[i]);
-    if (f != Format::kJpeg) {
-      // PNG, TIFF, WebP, BMP, PNM: no units, subsequences or MCUs, so every JPEG kernel skips the sample; png.cu / tiff.cu / webp.cu /
-      // bitmap.cu decode its staged range (the IDAT run, the span of the segments, the VP8 payload, the pixel array or raster) into the
-      // decode window, and the post pass behind it is shared
-      int rc = PlanSideSample(p, f, streams[i], lengths[i], i, (int64_t)raw, j);
-      if (rc) return sample_error(rc, dalib200GetLastError());
-      JpegImage &im = p->images[i];
-      memset(&im, 0, sizeof(im));
-      im.width = j.width; im.height = j.height; im.out_type = output_type;
-      im.unit_begin = im.unit_end = (int)p->units.size();
-      im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
-      if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
-      p->src_ptr.push_back(streams[i] + j.scan_begin);
-      raw += Align(j.scan_end - j.scan_begin, 16);
-      continue;
-    }
-    int rc = ParseHeaders(streams[i], lengths[i], j, true);
+    int rc = f != Format::kJpeg ? PlanSideSample(p->stage_of(f), f, streams[i], lengths[i], i, (int64_t)raw, j)
+                                : ParseHeaders(streams[i], lengths[i], j, true);
     if (rc) return sample_error(rc, dalib200GetLastError());
-    if (j.lossless) {
-      // lossless JPEG: units for U1 - U3 only (the DCT kernels see no unit, subsequence or MCU of the sample); ljpeg.cu decodes them
+    if (f != Format::kJpeg || j.lossless) {
+      // PNG, TIFF, WebP, BMP, PNM: no units, subsequences or MCUs, so every JPEG kernel skips the sample; the stage of its format decodes
+      // its staged range (the IDAT run, the span of the segments, the VP8 payload, the pixel array or raster) into the decode window.
+      // Lossless JPEG: units for U1 - U3 only (the DCT kernels see no unit, subsequence or MCU of the sample); the lossless stage decodes
+      // them.  The post pass behind is shared.
       JpegImage &im = p->images[i];
       memset(&im, 0, sizeof(im));
       im.width = j.width; im.height = j.height; im.out_type = output_type;
       im.unit_begin = im.unit_end = (int)p->units.size();
       im.subseq_begin = (int)subseq; im.block_begin = sync_blocks; im.wblock_begin = write_blocks; im.coef_off = coefs;
-      if ((rc = PlanLossless(p, i, streams[i], lengths[i], raw, clean, chunks, j))) return sample_error(rc, dalib200GetLastError());
+      if (j.lossless) {
+        std::string err;
+        rc = p->ljpeg.Plan(LosslessFrame(j), i, streams[i], lengths[i], j.scan_begin, raw, p->units, clean, chunks, &j.scan_end, &err);
+        if (rc) return sample_error(rc, err);
+        j.format = Format::kLossless;
+      }
       if ((rc = PlanGeometry(p, i, rois, j, im))) return rc;
       p->src_ptr.push_back(streams[i] + j.scan_begin);
       raw += Align(j.scan_end - j.scan_begin, 16);
@@ -2315,27 +2131,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     if (prog) {
       // no units: the scans are planned from the whole stream; their bytes are the staged range [scan_begin, scan_end) like a baseline
       // sample's, so JpegUpload needs no special case
-      dalib200::ProgImage pim;
-      memset(&pim, 0, sizeof(pim));
-      std::string perr;
-      const size_t first_new = p->prog_scans.size();
-      rc = dalib200::PlanProgressive(d, lengths[i], sb, (int)p->prog_images.size(), &pim, p->prog_scans, p->prog_huff, prog_table_cache, &perr);
-      if (rc) return sample_error(rc, perr);
-      for (size_t k = first_new; k < p->prog_scans.size(); k++)
-        if ((size_t)p->prog_scans[k].data_off + p->prog_scans[k].data_len > se - sb) {
-          // a scan that runs into the trimmed end-of-image marker ends in front of it
-          auto &sc = p->prog_scans[k];
-          sc.data_len = sc.data_off >= se - sb ? 0 : (uint32_t)(se - sb - sc.data_off);
-        }
-      if (pim.ncomp != im.ncomp || pim.mcux != im.mcux || pim.mcuy != im.mcuy || pim.bpm != bpm) {
-        SetLastError("decoders.image: sample %d: internal error (progressive frame layout)", i); return DALIB200_ERROR_INTERNAL;
-      }
-      pim.sample = i;
-      pim.raw_off = (int64_t)raw;
-      pim.coef_off = coefs;
-      p->prog_first_blk.push_back(p->prog_total_blocks);
-      p->prog_total_blocks += nmcu * bpm;
-      p->prog_images.push_back(pim);
+      std::string err;
+      if ((rc = p->prog.Plan(d, lengths[i], sb, se, i, (int64_t)raw, coefs, im, &err))) return sample_error(rc, err);
     } else if (j.restart_interval == 0) {
       add_unit(sb, se, 0, nmcu);
     } else {
@@ -2383,16 +2180,10 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     }
   }
   BuildWorkLists(p);
-  if (!p->prog_scans.empty()) {
-    std::stable_sort(p->prog_scans.begin(), p->prog_scans.end(), [](const dalib200::ProgScan &a, const dalib200::ProgScan &b) { return a.wave < b.wave; });
-    const int nw = p->prog_scans.back().wave + 1;
-    p->prog_wave_begin.assign(nw + 1, 0);
-    for (const auto &sc : p->prog_scans) p->prog_wave_begin[sc.wave + 1]++;
-    for (int w = 0; w < nw; w++) p->prog_wave_begin[w + 1] += p->prog_wave_begin[w];
-  }
+  p->prog.SortWaves();
   DB_CHECK_ARG(raw < (1ull << 32) && clean < (1ull << 32), "decoders.image: batch of encoded data exceeds 4 GiB");
   p->raw_bytes = raw; p->clean_bytes = clean; p->nchunks = chunks;
-  DB_CHECK_ARG(p->tiff_segs.size() < (1ull << 31), "decoders.image: batch of more than 2^31 TIFF segments");
+  DB_CHECK_ARG(p->tiff.segs.size() < (1ull << 31), "decoders.image: batch of more than 2^31 TIFF segments");
   p->clean_alloc = clean + (clean_read_behind(p->log2_sub) - kCleanPad);
   for (const JpegUnit &u : p->units)       // the clean length is at most raw_len: every load of the Huffman passes stays inside
     if ((size_t)u.clean_off + u.raw_len + clean_read_behind(p->log2_sub) > p->clean_alloc) {
@@ -2656,118 +2447,10 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   // (the clean stream is zero-padded behind every unit by the scatter kernel itself: no memset of the 129 MB buffer)
   DB_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(int32_t) * p->n, s));
   DB_CUDA(cudaMemsetAsync(p->d_chain_count, 0, sizeof(uint32_t) * 8, s));
-  if (!p->prog_images.empty()) {
-    // progressive samples: scans wave by wave into the same coefficient arena, DC left as differences for dc_scan (jpeg_prog.cu).
-    // A scan is a serial chain on ONE warp (milliseconds for a large image) that leaves the GPU empty: the stage runs beside the
-    // baseline samples' entropy kernels and is joined in front of dc_scan.  It touches only the progressive samples' ranges of the
-    // coefficient / DC arenas and their status words.
-    SideStage &st = p->prog;
-    if ((rc = st.Begin(s))) return rc;
-    const size_t npi = p->prog_images.size(), nsc = p->prog_scans.size(), nh = p->prog_huff.size();
-    const size_t o_img = 0, o_scan = Align(o_img + sizeof(ProgImage) * npi, 16), o_huff = Align(o_scan + sizeof(ProgScan) * nsc, 16),
-                 o_blk = Align(o_huff + sizeof(ProgHuff) * nh, 16), pbytes = Align(o_blk + sizeof(int64_t) * npi, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(pbytes, &h))) return rc;
-    memcpy(h + o_img, p->prog_images.data(), sizeof(ProgImage) * npi);
-    memcpy(h + o_scan, p->prog_scans.data(), sizeof(ProgScan) * nsc);
-    memcpy(h + o_huff, p->prog_huff.data(), sizeof(ProgHuff) * nh);
-    memcpy(h + o_blk, p->prog_first_blk.data(), sizeof(int64_t) * npi);
-    if ((rc = st.arena.Upload(pbytes, st.stream))) return rc;
-    ProgLaunch a;
-    a.d_images = reinterpret_cast<const ProgImage *>(st.arena.dev + o_img); a.nimages = (int)npi;
-    a.d_scans = reinterpret_cast<const ProgScan *>(st.arena.dev + o_scan);
-    a.d_huff = reinterpret_cast<const ProgHuff *>(st.arena.dev + o_huff);
-    a.d_first_blk = reinterpret_cast<const int64_t *>(st.arena.dev + o_blk);
-    a.total_blocks = p->prog_total_blocks;
-    a.wave_begin = &p->prog_wave_begin; a.h_images = &p->prog_images;
-    a.d_raw = d_raw; a.d_coef = p->d_coef; a.d_dc = p->d_dc; a.d_status = p->d_status;
-    if ((rc = LaunchProgressive(a, st.stream)) || (rc = st.End())) return rc;
-  }
-  if (!p->png_images.empty()) {
-    // PNG samples (png.cu): the inflate is a serial chain per image.  The stage writes only the PNG samples' decode windows, its
-    // scanline scratch and their status words.
-    SideStage &st = p->png;
-    if ((rc = GrowDevice(p->d_png_scan, p->d_png_scan_cap, (size_t)p->png_scan_bytes + 16))) return rc;
-    if ((rc = st.Begin(s))) return rc;
-    const int64_t px = FillWindows(p->png_images, hi);
-    const size_t npi = p->png_images.size(), nch = p->png_chunks.size();
-    const size_t o_chunk = Align(sizeof(PngImage) * npi, 16), pbytes = Align(o_chunk + sizeof(PngChunk) * nch, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(pbytes, &h))) return rc;
-    memcpy(h, p->png_images.data(), sizeof(PngImage) * npi);
-    memcpy(h + o_chunk, p->png_chunks.data(), sizeof(PngChunk) * nch);
-    if ((rc = st.arena.Upload(pbytes, st.stream))) return rc;
-    PngLaunch a;
-    a.d_images = reinterpret_cast<const PngImage *>(st.arena.dev); a.nimages = (int)npi;
-    a.d_chunks = reinterpret_cast<const PngChunk *>(st.arena.dev + o_chunk); a.nchunks = (int)nch;
-    a.total_px = px;
-    a.d_raw = d_raw; a.d_scan = p->d_png_scan; a.d_status = p->d_status;
-    if ((rc = LaunchPng(a, st.stream)) || (rc = st.End())) return rc;
-  }
-  if (!p->tiff_images.empty()) {
-    // TIFF samples (tiff.cu): a TIFF written as one big strip is a serial chain.  The stage writes only the TIFF samples' decode
-    // windows, its scratch and their status words.
-    SideStage &st = p->tiff;
-    const int nseg = (int)p->tiff_segs.size();
-    if ((rc = GrowDevice(p->d_tiff_dec, p->d_tiff_dec_cap, (size_t)p->tiff_dec_bytes + 16))) return rc;
-    if ((rc = GrowDevice(p->d_tiff_slots, p->d_tiff_slots_cap, (size_t)TiffSlotCount(nseg) * kTiffSlotBytes))) return rc;
-    if ((rc = st.Begin(s))) return rc;
-    const int64_t px = FillWindows(p->tiff_images, hi);
-    const size_t nti = p->tiff_images.size();
-    const size_t o_seg = Align(sizeof(TiffImage) * nti, 16), tbytes = Align(o_seg + sizeof(TiffSeg) * nseg, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(tbytes, &h))) return rc;
-    memcpy(h, p->tiff_images.data(), sizeof(TiffImage) * nti);
-    memcpy(h + o_seg, p->tiff_segs.data(), sizeof(TiffSeg) * nseg);
-    if ((rc = st.arena.Upload(tbytes, st.stream))) return rc;
-    TiffLaunch a;
-    a.d_images = reinterpret_cast<const TiffImage *>(st.arena.dev); a.nimages = (int)nti;
-    a.d_segs = reinterpret_cast<const TiffSeg *>(st.arena.dev + o_seg); a.nsegs = nseg;
-    a.total_px = px;
-    a.d_raw = d_raw; a.d_dec = p->d_tiff_dec; a.d_slots = p->d_tiff_slots; a.d_status = p->d_status;
-    if ((rc = LaunchTiff(a, st.stream)) || (rc = st.End())) return rc;
-  }
-  if (!p->webp_images.empty()) {
-    // WebP samples (webp.cu): the entropy decode of an image is a serial chain.  The stage writes only the WebP samples' decode
-    // windows, its scratch and their status words.
-    SideStage &st = p->webp;
-    if ((rc = GrowDevice(p->d_webp_scratch, p->d_webp_scratch_cap, (size_t)p->webp_scratch_bytes + 16))) return rc;
-    if ((rc = st.Begin(s))) return rc;
-    const int64_t px = FillWindows(p->webp_images, hi);
-    const size_t nwi = p->webp_images.size(), wbytes = Align(sizeof(WebpImage) * nwi, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(wbytes, &h))) return rc;
-    memcpy(h, p->webp_images.data(), sizeof(WebpImage) * nwi);
-    if ((rc = st.arena.Upload(wbytes, st.stream))) return rc;
-    WebpLaunch a;
-    a.d_images = reinterpret_cast<const WebpImage *>(st.arena.dev); a.nimages = (int)nwi;
-    a.total_px = px;
-    a.d_raw = d_raw; a.d_scratch = p->d_webp_scratch; a.d_status = p->d_status;
-    if ((rc = LaunchWebp(a, st.stream)) || (rc = st.End())) return rc;
-  }
-  if (!p->bitmap_images.empty()) {
-    // BMP and PNM samples (bitmap.cu): mostly uncompressed rasters read straight from the staged bytes; RLE and ASCII images are
-    // unpacked first, one serial lane each.  The stage writes only the BMP / PNM samples' decode windows, its scratch and their status
-    // words.
-    SideStage &st = p->bitmap;
-    if ((rc = GrowDevice(p->d_bitmap_scratch, p->d_bitmap_scratch_cap, (size_t)p->bitmap_scratch_bytes + 16))) return rc;
-    if ((rc = st.Begin(s))) return rc;
-    FillWindows(p->bitmap_images, hi);
-    const int64_t groups = BitmapGroups(p->bitmap_images);
-    const size_t nbi = p->bitmap_images.size(), nun = p->bitmap_unpack.size();
-    const size_t o_un = Align(sizeof(BitmapImage) * nbi, 16), bbytes = Align(o_un + sizeof(int32_t) * nun, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(bbytes, &h))) return rc;
-    memcpy(h, p->bitmap_images.data(), sizeof(BitmapImage) * nbi);
-    memcpy(h + o_un, p->bitmap_unpack.data(), sizeof(int32_t) * nun);
-    if ((rc = st.arena.Upload(bbytes, st.stream))) return rc;
-    BitmapLaunch a;
-    a.d_images = reinterpret_cast<const BitmapImage *>(st.arena.dev); a.nimages = (int)nbi;
-    a.d_unpack = reinterpret_cast<const int32_t *>(st.arena.dev + o_un); a.nunpack = (int)nun;
-    a.total_groups = groups;
-    a.d_raw = d_raw; a.d_scratch = p->d_bitmap_scratch; a.d_status = p->d_status;
-    if ((rc = LaunchBitmap(a, st.stream)) || (rc = st.End())) return rc;
-  }
+  const StageInputs in{ hi, d_raw, p->d_status, p->d_coef, p->d_dc, p->d_clean, p->d_unit_len };
+  if ((rc = p->prog.Run(in, s)) || (rc = p->png.Run(in, s)) || (rc = p->tiff.Run(in, s)) || (rc = p->webp.Run(in, s)) ||
+      (rc = p->bitmap.Run(in, s)))
+    return rc;
   // any_units: the batch has a baseline sample; lossless samples have units for U1 - U3 but nothing for the baseline entropy kernels
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;
   if (nunits > 0 && p->nchunks > 0) {
@@ -2777,35 +2460,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     { ProfScope ps_("jpeg_unstuff_scatter", s); unstuff_scatter_kernel<<<grid, 256, 0, s>>>(d_raw, d_units, nunits, p->nchunks, p->d_chunk, p->d_clean); }
     CountLaunch(3);
   }
-  if (!p->ljpeg_images.empty()) {
-    // lossless JPEG samples (ljpeg.cu): forked behind U3, whose clean streams they read.  The stage writes only the lossless samples'
-    // decode windows, its scratch and their status words.
-    SideStage &st = p->ljpeg;
-    if ((rc = GrowDevice(p->d_ljpeg_diff, p->d_ljpeg_diff_cap, (size_t)p->ljpeg_diff_elems + 8))) return rc;
-    if ((rc = GrowDevice(p->d_ljpeg_rec, p->d_ljpeg_rec_cap, (size_t)p->ljpeg_total_sub + 1))) return rc;
-    if ((rc = GrowDevice(p->d_ljpeg_first, p->d_ljpeg_first_cap, (size_t)p->ljpeg_total_sub + 1))) return rc;
-    if ((rc = st.Begin(s))) return rc;
-    const int64_t px = FillWindows(p->ljpeg_images, hi);
-    const size_t nli = p->ljpeg_images.size(), nlu = p->ljpeg_units.size(), nlt = p->ljpeg_tables.size(), nlb = p->ljpeg_bands.size();
-    const size_t o_unit = Align(sizeof(LjpegImage) * nli, 16), o_tab = Align(o_unit + sizeof(LjpegUnit) * nlu, 16),
-                 o_band = Align(o_tab + sizeof(LjpegTable) * nlt, 16), lbytes = Align(o_band + sizeof(LjpegBand) * nlb, 16);
-    uint8_t *h;
-    if ((rc = st.arena.Stage(lbytes, &h))) return rc;
-    memcpy(h, p->ljpeg_images.data(), sizeof(LjpegImage) * nli);
-    memcpy(h + o_unit, p->ljpeg_units.data(), sizeof(LjpegUnit) * nlu);
-    memcpy(h + o_tab, p->ljpeg_tables.data(), sizeof(LjpegTable) * nlt);
-    memcpy(h + o_band, p->ljpeg_bands.data(), sizeof(LjpegBand) * nlb);
-    if ((rc = st.arena.Upload(lbytes, st.stream))) return rc;
-    LjpegLaunch a;
-    a.d_images = reinterpret_cast<const LjpegImage *>(st.arena.dev); a.nimages = (int)nli;
-    a.d_units = reinterpret_cast<const LjpegUnit *>(st.arena.dev + o_unit); a.nunits = (int)nlu;
-    a.d_tables = reinterpret_cast<const LjpegTable *>(st.arena.dev + o_tab);
-    a.d_bands = reinterpret_cast<const LjpegBand *>(st.arena.dev + o_band); a.nbands = (int)nlb;
-    a.total_sub = p->ljpeg_total_sub; a.total_px = px;
-    a.d_clean = p->d_clean; a.d_unit_clean_len = p->d_unit_len;
-    a.d_rec = p->d_ljpeg_rec; a.d_first = p->d_ljpeg_first; a.d_diff = p->d_ljpeg_diff; a.d_status = p->d_status;
-    if ((rc = LaunchLjpeg(a, st.stream)) || (rc = st.End())) return rc;
-  }
+  if ((rc = p->ljpeg.Run(in, s))) return rc;            // forked behind U3, whose clean streams it reads
   HuffCtx cx;
   cx.images = d_images; cx.nimages = p->n; cx.block_image = reinterpret_cast<const int32_t *>(p->d_stage + p->off_blkimg);
   cx.wblock_image = reinterpret_cast<const int32_t *>(p->d_stage + p->off_wblkimg);
@@ -2840,7 +2495,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   { ProfScope ps_("jpeg_huff_scan", s); huff_scan_kernel<<<p->n, 1024, 0, s>>>(cx); }
   CountLaunch();
   if (any_units && p->total_blocks_write > 0) { ProfScope ps_("jpeg_huff_write", s); huff_write_kernel<<<p->total_blocks_write, kWriteThreads, wsmem, s>>>(cx); }
-  if (!p->prog_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->prog.join, 0));      // the progressive samples' coefficients and DC differences are in place
+  if ((rc = p->prog.Join(s))) return rc;                // the progressive samples' coefficients and DC differences are in place
   { ProfScope ps_("jpeg_dc_scan", s); dc_scan_kernel<<<p->n, 1024, 0, s>>>(d_images, p->d_dc); }
   { ProfScope ps_("jpeg_truncation_fixup", s); truncation_fixup_kernel<<<p->n, 256, 0, s>>>(cx); }
   CountLaunch();
@@ -2854,11 +2509,9 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     ra.d_coef = p->d_coef; ra.d_dc = p->d_dc; ra.d_quants = d_quants; ra.d_planes = p->d_planes;
     if ((rc = LaunchReconstruct(ra, s))) return rc;
   }
-  if (!p->png_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->png.join, 0));       // the PNG samples' windows and status are in place
-  if (!p->tiff_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->tiff.join, 0));     // the TIFF samples' windows and status are in place
-  if (!p->webp_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->webp.join, 0));     // the WebP samples' windows and status are in place
-  if (!p->bitmap_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->bitmap.join, 0)); // the BMP / PNM samples' windows and status are in place
-  if (!p->ljpeg_images.empty()) DB_CUDA(cudaStreamWaitEvent(s, p->ljpeg.join, 0));   // the lossless samples' windows and status are in place
+  // the other stages' decode windows and status words are in place
+  if ((rc = p->png.Join(s)) || (rc = p->tiff.Join(s)) || (rc = p->webp.Join(s)) || (rc = p->bitmap.Join(s)) || (rc = p->ljpeg.Join(s)))
+    return rc;
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
     ProfScope ps_("jpeg_post", s);

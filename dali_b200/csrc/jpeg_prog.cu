@@ -10,6 +10,7 @@
 // This is a correctness path, not a fast one: ~0.1 us per symbol on the critical path (a 500 kB stream: tens of ms).
 #include "common.cuh"
 #include "jpeg_prog.h"
+#include "jpeg_prog_plan.h"
 #include <algorithm>
 
 namespace dalib200 {
@@ -34,22 +35,61 @@ __global__ void __launch_bounds__(256) prog_dc_kernel(const ProgImage *__restric
   }
 }
 
-int LaunchProgressive(const ProgLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
-  for (const ProgImage &im : *a.h_images)
-    DB_CUDA(cudaMemsetAsync(a.d_coef + im.coef_off, 0, sizeof(int16_t) * 64 * (size_t)im.mcux * im.mcuy * im.bpm, s));
-  const std::vector<int> &wb = *a.wave_begin;
-  for (size_t w = 0; w + 1 < wb.size(); w++) {
-    const int cnt = wb[w + 1] - wb[w];
+void ProgStage::Clear() {
+  images.clear(); scans.clear(); huff.clear(); wave_begin.clear(); first_blk.clear(); table_cache.clear();
+  total_blocks = 0;
+}
+
+int ProgStage::Plan(const uint8_t *d, size_t len, size_t sb, size_t se, int sample, int64_t raw_off, int64_t coef_off, const JpegImage &im,
+                    std::string *err) {
+  ProgImage pim;
+  memset(&pim, 0, sizeof(pim));
+  const size_t first_new = scans.size();
+  if (int rc = PlanProgressive(d, len, sb, (int)images.size(), &pim, scans, huff, table_cache, err)) return rc;
+  for (size_t k = first_new; k < scans.size(); k++)
+    if ((size_t)scans[k].data_off + scans[k].data_len > se - sb) {
+      // a scan that runs into the trimmed end-of-image marker ends in front of it
+      auto &sc = scans[k];
+      sc.data_len = sc.data_off >= se - sb ? 0 : (uint32_t)(se - sb - sc.data_off);
+    }
+  if (pim.ncomp != im.ncomp || pim.mcux != im.mcux || pim.mcuy != im.mcuy || pim.bpm != im.bpm) {
+    *err = "internal error (progressive frame layout)";
+    return DALIB200_ERROR_INTERNAL;
+  }
+  pim.sample = sample;
+  pim.raw_off = raw_off;
+  pim.coef_off = coef_off;
+  first_blk.push_back(total_blocks);
+  total_blocks += (int64_t)im.mcux * im.mcuy * im.bpm;
+  images.push_back(pim);
+  return DALIB200_SUCCESS;
+}
+
+void ProgStage::SortWaves() {
+  if (scans.empty()) return;
+  std::stable_sort(scans.begin(), scans.end(), [](const ProgScan &a, const ProgScan &b) { return a.wave < b.wave; });
+  const int nw = scans.back().wave + 1;
+  wave_begin.assign(nw + 1, 0);
+  for (const auto &sc : scans) wave_begin[sc.wave + 1]++;
+  for (int w = 0; w < nw; w++) wave_begin[w + 1] += wave_begin[w];
+}
+
+int ProgStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  const ProgImage *d_images; const ProgScan *d_scans; const ProgHuff *d_huff; const int64_t *d_first_blk;
+  if (int rc = arena.Pack(s, std::tie(d_images, d_scans, d_huff, d_first_blk), images, scans, huff, first_blk)) return rc;
+  for (const ProgImage &im : images)
+    DB_CUDA(cudaMemsetAsync(in.d_coef + im.coef_off, 0, sizeof(int16_t) * 64 * (size_t)im.mcux * im.mcuy * im.bpm, s));
+  for (size_t w = 0; w + 1 < wave_begin.size(); w++) {
+    const int cnt = wave_begin[w + 1] - wave_begin[w];
     if (cnt <= 0) continue;
     ProfScope ps_("jpeg_prog_scan", s);
-    prog_scan_kernel<<<cnt, 32, 0, s>>>(a.d_scans, wb[w], a.d_images, a.d_huff, a.d_raw, a.d_coef, a.d_status);
+    prog_scan_kernel<<<cnt, 32, 0, s>>>(d_scans, wave_begin[w], d_images, d_huff, in.d_raw, in.d_coef, in.d_status);
     CountLaunch();
   }
-  if (a.total_blocks > 0) {
-    const int grid = (int)std::min<int64_t>((a.total_blocks + 255) / 256, (int64_t)NumSMs() * 8);
+  if (total_blocks > 0) {
+    const int grid = (int)std::min<int64_t>((total_blocks + 255) / 256, (int64_t)NumSMs() * 8);
     ProfScope ps_("jpeg_prog_dc", s);
-    prog_dc_kernel<<<grid, 256, 0, s>>>(a.d_images, a.d_first_blk, a.nimages, a.total_blocks, a.d_coef, a.d_dc, a.d_status);
+    prog_dc_kernel<<<grid, 256, 0, s>>>(d_images, d_first_blk, (int)images.size(), total_blocks, in.d_coef, in.d_dc, in.d_status);
     CountLaunch();
   }
   DB_CUDA(cudaGetLastError());

@@ -72,6 +72,8 @@ struct JpegUnit {
   int64_t slot_base;                       // first coefficient slot of this unit (image-local)
   int64_t nslots;                          // expected number of slots (= MCUs * bpm * 64)
 };
+constexpr int kChunkBytes = 4096;            // un-stuffing chunk
+constexpr uint32_t kCleanPad = 32;           // zero bytes behind the clean stream of every unit (at least: units are 16-byte aligned)
 
 // idct_color_420 (jpeg.cu): work item = a strip of kFusedMcus MCU columns of one image's window, walked down one MCU row ("band") at a
 // time over a segment of at most kFusedMaxBands bands.

@@ -109,8 +109,74 @@ __global__ void __launch_bounds__(256) ljpeg_color_kernel(const LjpegImage *__re
   }
 }
 
-int LaunchLjpeg(const LjpegLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
+int LjpegStage::Plan(const LjpegFrame &f, int sample, const uint8_t *d, size_t len, size_t sb, size_t raw, std::vector<JpegUnit> &junits,
+                     size_t &clean, uint32_t &chunks, size_t *scan_end, std::string *err) {
+  LjpegImage im;
+  if (int rc = PlanLjpegFrame(f, &im, tables, err)) return rc;
+  if ((int64_t)f.width * f.height >= (1ll << 31)) {
+    *err = "images of 2^31 pixels or more are not supported";
+    return DALIB200_ERROR_UNSUPPORTED;
+  }
+  size_t se = len;
+  if (se >= sb + 2 && d[se - 2] == 0xFF && d[se - 1] == 0xD9) se -= 2;
+  *scan_end = se;
+  const int W = f.width, H = f.height, C = f.ncomp;
+  const int lines = f.restart_interval ? f.restart_interval / W : H;
+  const int nunits = (H + lines - 1) / lines;
+  std::vector<std::pair<size_t, size_t>> segs;
+  im.bad_rst = SplitLjpegUnits(d, sb, se, nunits, segs);
+  for (const auto &sg : segs)
+    if (sg.second - sg.first > kLjpegMaxUnitBytes) {
+      *err = "lossless JPEG: an entropy-coded segment above " + std::to_string(kLjpegMaxUnitBytes) +
+             " bytes is not supported (use restart intervals)";
+      return DALIB200_ERROR_UNSUPPORTED;
+    }
+  im.sample = sample;
+  im.diff_off = diff_elems;
+  diff_elems += (int64_t)Align((size_t)W * H * C, 8);
+  const int li = (int)images.size();
+  for (int k = 0; k < nunits; k++) {
+    JpegUnit u;
+    memset(&u, 0, sizeof(u));
+    u.raw_off = (uint32_t)(raw + (segs[k].first - sb));
+    u.raw_len = (uint32_t)(segs[k].second - segs[k].first);
+    u.clean_off = (uint32_t)clean;
+    u.first_chunk = chunks;
+    u.image = sample;
+    LjpegUnit lu;
+    lu.junit = (int32_t)junits.size(); lu.image = li;
+    lu.first_sub = total_sub;
+    lu.nsub = (int32_t)((u.raw_len + (1u << (kLjpegLog2Sub - 3)) - 1) >> (kLjpegLog2Sub - 3));
+    lu.clean_off = u.clean_off;
+    const int y0 = k * lines, y1 = std::min(H, y0 + lines);
+    lu.nsym = (int64_t)(y1 - y0) * W * C;
+    lu.sym_off = im.diff_off + (int64_t)y0 * W * C;
+    for (int c = 0; c < C; c++) bands.push_back(LjpegBand{ li, c, y0, y1 });
+    total_sub += lu.nsub;
+    clean += Align(u.raw_len + kCleanPad, 16);
+    chunks += (u.raw_len + kChunkBytes - 1) / kChunkBytes;
+    junits.push_back(u);
+    units.push_back(lu);
+  }
+  images.push_back(im);
+  return DALIB200_SUCCESS;
+}
+
+int LjpegStage::Reserve() {
+  int rc;
+  if ((rc = GrowDevice(d_diff, d_diff_cap, (size_t)diff_elems + 8))) return rc;
+  if ((rc = GrowDevice(d_rec, d_rec_cap, (size_t)total_sub + 1))) return rc;
+  return GrowDevice(d_first, d_first_cap, (size_t)total_sub + 1);
+}
+
+int LjpegStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  LjpegLaunch a;
+  a.total_px = FillWindows(images, in.images);
+  if (int rc = arena.Pack(s, std::tie(a.d_images, a.d_units, a.d_tables, a.d_bands), images, units, tables, bands)) return rc;
+  a.nimages = (int)images.size(); a.nunits = (int)units.size(); a.nbands = (int)bands.size();
+  a.total_sub = total_sub;
+  a.d_clean = in.d_clean; a.d_unit_clean_len = in.d_unit_clean_len;
+  a.d_rec = d_rec; a.d_first = d_first; a.d_diff = d_diff; a.d_status = in.d_status;
   const int sms = NumSMs();
   auto grid_of = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sms * 16)); };
   if (a.total_sub > 0) {

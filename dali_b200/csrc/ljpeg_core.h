@@ -54,7 +54,7 @@ struct LjpegUnit {
 // Reconstruction work: the samples of one component of the lines [y0, y1) of an image (a restart band, or the whole image).
 struct LjpegBand { int32_t image, comp, y0, y1; };
 
-// What the kernels of ljpeg.cu read (LaunchLjpeg, ljpeg.h).
+// What the kernels of ljpeg.cu read (LjpegStage::Enqueue, ljpeg.h).
 struct LjpegLaunch {
   const LjpegImage *d_images; int nimages;
   const LjpegUnit *d_units; int nunits;

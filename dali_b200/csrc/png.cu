@@ -45,22 +45,35 @@ __global__ void __launch_bounds__(256) png_color_kernel(const PngImage *__restri
   }
 }
 
-int LaunchPng(const PngLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
-  if (a.nchunks > 0) {
+int PngStage::Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) {
+  PngImage im;
+  if (int rc = PlanPng(data, len, (int)images.size(), &im, chunks, info, err)) return rc;
+  im.scan_off = scan_bytes;
+  scan_bytes += (int64_t)Align((size_t)im.scan_bytes, 16);
+  im.sample = sample; im.raw_off = raw_off;
+  images.push_back(im);
+  return DALIB200_SUCCESS;
+}
+
+int PngStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  const int64_t total_px = FillWindows(images, in.images);
+  const PngImage *d_images; const PngChunk *d_chunks;
+  if (int rc = arena.Pack(s, std::tie(d_images, d_chunks), images, chunks)) return rc;
+  const int nimages = (int)images.size(), nchunks = (int)chunks.size();
+  if (nchunks > 0) {
     ProfScope ps_("png_crc", s);
-    png_crc_kernel<<<(a.nchunks + 127) / 128, 128, 0, s>>>(a.d_chunks, a.nchunks, a.d_images, a.d_raw, a.d_status);
+    png_crc_kernel<<<(nchunks + 127) / 128, 128, 0, s>>>(d_chunks, nchunks, d_images, in.d_raw, in.d_status);
     CountLaunch();
   }
   {
     ProfScope ps_("png_inflate", s);
-    png_inflate_kernel<<<a.nimages, 32, 0, s>>>(a.d_images, a.d_chunks, a.d_raw, a.d_scan, a.d_status);
+    png_inflate_kernel<<<nimages, 32, 0, s>>>(d_images, d_chunks, in.d_raw, d_scan, in.d_status);
     CountLaunch();
   }
-  if (a.total_px > 0) {
-    const int grid = (int)std::min<int64_t>((a.total_px + 255) / 256, (int64_t)NumSMs() * 16);
+  if (total_px > 0) {
+    const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
     ProfScope ps_("png_color", s);
-    png_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_scan);
+    png_color_kernel<<<grid, 256, 0, s>>>(d_images, nimages, total_px, d_scan);
     CountLaunch();
   }
   DB_CUDA(cudaGetLastError());

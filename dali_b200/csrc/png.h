@@ -1,21 +1,28 @@
-// dali_b200/csrc/png.h -- launch interface of the PNG stage (png.cu), called by dalib200JpegLaunch for the PNG samples of a batch.
+// dali_b200/csrc/png.h -- the PNG stage of decoders.image (png.cu), planned and run by the image decoder plan (jpeg.cu).
 #ifndef DALI_B200_CSRC_PNG_H_
 #define DALI_B200_CSRC_PNG_H_
-#include <cuda_runtime.h>
-#include "png_core.h"
+#include <vector>
+#include "decode_stage.h"
+#include "png_plan.h"
 
 namespace dalib200 {
 
-struct PngLaunch {
-  const PngImage *d_images; int nimages;
-  const PngChunk *d_chunks; int nchunks;
-  int64_t total_px;                          // window pixels of all PNG images (PngImage::first_px is their prefix)
-  const uint8_t *d_raw;                      // the plan's staged bytes
-  uint8_t *d_scan;                           // scratch for the filtered scanlines (PngImage::scan_off)
-  int32_t *d_status;
+struct PngStage : StreamStage {
+  bool Empty() const override { return images.empty(); }
+  void Clear() override { images.clear(); chunks.clear(); scan_bytes = 0; }
+  void Destroy() override { SideStage::Destroy(); cudaFree(d_scan); }
+  int Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) override;
+
+  std::vector<PngImage> images;
+  std::vector<PngChunk> chunks;
+  int64_t scan_bytes = 0;
+  uint8_t *d_scan = nullptr; size_t d_scan_cap = 0;   // filtered scanlines (PngImage::scan_off; grow only)
+
+ protected:
+  int Reserve() override { return GrowDevice(d_scan, d_scan_cap, (size_t)scan_bytes + 16); }
+  // IDAT CRCs, inflate + unfilter (one thread per image), conversion of the decode windows
+  int Enqueue(const StageInputs &in, cudaStream_t s) override;
 };
-// IDAT CRCs, inflate + unfilter (one thread per image), conversion of the decode windows.  Returns a DALIB200 status.
-int LaunchPng(const PngLaunch &a, cudaStream_t s);
 
 }  // namespace dalib200
 #endif  // DALI_B200_CSRC_PNG_H_

@@ -42,23 +42,38 @@ __global__ void __launch_bounds__(256) tiff_color_kernel(const TiffImage *__rest
   }
 }
 
-int TiffSlotCount(int nsegs) {
-  const SerialLanes g = SerialLaneGeometry(nsegs, kTiffMaxWorkers);
-  return g.warps * g.lanes;
+int TiffStage::Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) {
+  TiffImage im;
+  int64_t bytes = 0;
+  if (int rc = PlanTiff(data, len, (int)images.size(), &im, segs, dec_bytes, &bytes, info, err)) return rc;
+  dec_bytes += bytes;
+  im.sample = sample; im.raw_off = raw_off;
+  images.push_back(im);
+  return DALIB200_SUCCESS;
 }
 
-int LaunchTiff(const TiffLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
-  if (a.nsegs > 0) {
+int TiffStage::Reserve() {
+  const SerialLanes g = SerialLaneGeometry((int)segs.size(), kTiffMaxWorkers);     // a slot per tiff_segment thread
+  int rc;
+  if ((rc = GrowDevice(d_dec, d_dec_cap, (size_t)dec_bytes + 16))) return rc;
+  return GrowDevice(d_slots, d_slots_cap, (size_t)(g.warps * g.lanes) * kTiffSlotBytes);
+}
+
+int TiffStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  const int64_t total_px = FillWindows(images, in.images);
+  const TiffImage *d_images; const TiffSeg *d_segs;
+  if (int rc = arena.Pack(s, std::tie(d_images, d_segs), images, segs)) return rc;
+  const int nsegs = (int)segs.size();
+  if (nsegs > 0) {
     ProfScope ps_("tiff_segment", s);
-    const SerialLanes g = SerialLaneGeometry(a.nsegs, kTiffMaxWorkers);
-    tiff_segment_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.d_segs, a.nsegs, g.lanes, a.d_raw, a.d_dec, a.d_slots, a.d_status);
+    const SerialLanes g = SerialLaneGeometry(nsegs, kTiffMaxWorkers);
+    tiff_segment_kernel<<<g.warps, 32, 0, s>>>(d_images, d_segs, nsegs, g.lanes, in.d_raw, d_dec, d_slots, in.d_status);
     CountLaunch();
   }
-  if (a.total_px > 0) {
-    const int grid = (int)std::min<int64_t>((a.total_px + 255) / 256, (int64_t)NumSMs() * 16);
+  if (total_px > 0) {
+    const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
     ProfScope ps_("tiff_color", s);
-    tiff_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_segs, a.d_dec);
+    tiff_color_kernel<<<grid, 256, 0, s>>>(d_images, (int)images.size(), total_px, d_segs, d_dec);
     CountLaunch();
   }
   DB_CUDA(cudaGetLastError());

@@ -1,24 +1,29 @@
-// dali_b200/csrc/tiff.h -- launch interface of the TIFF stage (tiff.cu), called by dalib200JpegLaunch for the TIFF samples of a batch.
+// dali_b200/csrc/tiff.h -- the TIFF stage of decoders.image (tiff.cu), planned and run by the image decoder plan (jpeg.cu).
 #ifndef DALI_B200_CSRC_TIFF_H_
 #define DALI_B200_CSRC_TIFF_H_
-#include <cuda_runtime.h>
-#include "tiff_core.h"
+#include <vector>
+#include "decode_stage.h"
+#include "tiff_plan.h"
 
 namespace dalib200 {
 
-struct TiffLaunch {
-  const TiffImage *d_images; int nimages;
-  const TiffSeg *d_segs; int nsegs;
-  int64_t total_px;                          // window pixels of all TIFF images (TiffImage::first_px is their prefix)
-  const uint8_t *d_raw;                      // the plan's staged bytes
-  uint8_t *d_dec;                            // scratch for the decoded segments (TiffSeg::dec_off)
-  uint8_t *d_slots;                          // TiffSlotCount(nsegs) x kTiffSlotBytes of segment working memory
-  int32_t *d_status;
+struct TiffStage : StreamStage {
+  bool Empty() const override { return images.empty(); }
+  void Clear() override { images.clear(); segs.clear(); dec_bytes = 0; }
+  void Destroy() override { SideStage::Destroy(); cudaFree(d_dec); cudaFree(d_slots); }
+  int Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) override;
+
+  std::vector<TiffImage> images;
+  std::vector<TiffSeg> segs;
+  int64_t dec_bytes = 0;
+  uint8_t *d_dec = nullptr; size_t d_dec_cap = 0;       // decoded segments (TiffSeg::dec_off; grow only)
+  uint8_t *d_slots = nullptr; size_t d_slots_cap = 0;   // segment working memory, kTiffSlotBytes per tiff_segment thread (grow only)
+
+ protected:
+  int Reserve() override;
+  // segment decode (one lane per segment), conversion of the decode windows
+  int Enqueue(const StageInputs &in, cudaStream_t s) override;
 };
-// threads of tiff_segment, and so working-memory slots, for `nsegs` segments
-int TiffSlotCount(int nsegs);
-// segment decode (one lane per segment), conversion of the decode windows.  Returns a DALIB200 status.
-int LaunchTiff(const TiffLaunch &a, cudaStream_t s);
 
 }  // namespace dalib200
 #endif  // DALI_B200_CSRC_TIFF_H_

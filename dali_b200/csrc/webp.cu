@@ -63,20 +63,33 @@ __global__ void __launch_bounds__(256) webp_color_kernel(const WebpImage *__rest
   }
 }
 
-int LaunchWebp(const WebpLaunch &a, cudaStream_t s) {
-  if (a.nimages == 0) return DALIB200_SUCCESS;
+int WebpStage::Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) {
+  WebpImage im;
+  int64_t bytes = 0;
+  if (int rc = PlanWebp(data, len, (int)images.size(), &im, scratch_bytes, &bytes, info, err)) return rc;
+  scratch_bytes += bytes;
+  im.sample = sample; im.raw_off = raw_off;
+  images.push_back(im);
+  return DALIB200_SUCCESS;
+}
+
+int WebpStage::Enqueue(const StageInputs &in, cudaStream_t s) {
+  const int64_t total_px = FillWindows(images, in.images);
+  const WebpImage *d_images;
+  if (int rc = arena.Pack(s, std::tie(d_images), images)) return rc;
+  const int nimages = (int)images.size();
   {
-    const SerialLanes g = SerialLaneGeometry(a.nimages, 1 << 30);
+    const SerialLanes g = SerialLaneGeometry(nimages, 1 << 30);
     ProfScope ps_("webp_entropy", s);
-    webp_entropy_kernel<<<g.warps, 32, 0, s>>>(a.d_images, a.nimages, g.lanes, a.d_raw, a.d_scratch, a.d_status);
+    webp_entropy_kernel<<<g.warps, 32, 0, s>>>(d_images, nimages, g.lanes, in.d_raw, d_scratch, in.d_status);
   }
-  { ProfScope ps_("webp_recon", s); webp_wave_kernel<false><<<a.nimages, kWebpWaveThreads, 0, s>>>(a.d_images, a.d_scratch, a.d_status); }
-  { ProfScope ps_("webp_filter", s); webp_wave_kernel<true><<<a.nimages, kWebpWaveThreads, 0, s>>>(a.d_images, a.d_scratch, a.d_status); }
+  { ProfScope ps_("webp_recon", s); webp_wave_kernel<false><<<nimages, kWebpWaveThreads, 0, s>>>(d_images, d_scratch, in.d_status); }
+  { ProfScope ps_("webp_filter", s); webp_wave_kernel<true><<<nimages, kWebpWaveThreads, 0, s>>>(d_images, d_scratch, in.d_status); }
   CountLaunch(3);
-  if (a.total_px > 0) {
-    const int grid = (int)std::min<int64_t>((a.total_px + 255) / 256, (int64_t)NumSMs() * 16);
+  if (total_px > 0) {
+    const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
     ProfScope ps_("webp_color", s);
-    webp_color_kernel<<<grid, 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_scratch);
+    webp_color_kernel<<<grid, 256, 0, s>>>(d_images, nimages, total_px, d_scratch);
     CountLaunch();
   }
   DB_CUDA(cudaGetLastError());

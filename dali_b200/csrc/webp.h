@@ -1,21 +1,28 @@
-// dali_b200/csrc/webp.h -- launch interface of the WebP stage (webp.cu), called by dalib200JpegLaunch for the WebP samples of a batch.
+// dali_b200/csrc/webp.h -- the WebP stage of decoders.image (webp.cu), planned and run by the image decoder plan (jpeg.cu).
 #ifndef DALI_B200_CSRC_WEBP_H_
 #define DALI_B200_CSRC_WEBP_H_
-#include <cuda_runtime.h>
-#include "webp_core.h"
+#include <vector>
+#include "decode_stage.h"
+#include "webp_plan.h"
 
 namespace dalib200 {
 
-struct WebpLaunch {
-  const WebpImage *d_images; int nimages;
-  int64_t total_px;                          // window pixels of all WebP images (WebpImage::first_px is their prefix)
-  const uint8_t *d_raw;                      // the plan's staged bytes
-  uint8_t *d_scratch;                        // coefficients, macroblock records, planes, column contexts (WebpImage::*_off)
-  int32_t *d_status;
+struct WebpStage : StreamStage {
+  bool Empty() const override { return images.empty(); }
+  void Clear() override { images.clear(); scratch_bytes = 0; }
+  void Destroy() override { SideStage::Destroy(); cudaFree(d_scratch); }
+  int Plan(const uint8_t *data, size_t len, int sample, int64_t raw_off, StreamInfo *info, std::string *err) override;
+
+  std::vector<WebpImage> images;
+  int64_t scratch_bytes = 0;
+  uint8_t *d_scratch = nullptr; size_t d_scratch_cap = 0;   // coefficients, macroblock records, planes, column contexts (grow only)
+
+ protected:
+  int Reserve() override { return GrowDevice(d_scratch, d_scratch_cap, (size_t)scratch_bytes + 16); }
+  // entropy decode (one lane per image), reconstruction and loop filter (one CTA per image, macroblock wavefront), conversion of the
+  // decode windows
+  int Enqueue(const StageInputs &in, cudaStream_t s) override;
 };
-// entropy decode (one lane per image), reconstruction and loop filter (one CTA per image, macroblock wavefront), conversion of the
-// decode windows.  Returns a DALIB200 status.
-int LaunchWebp(const WebpLaunch &a, cudaStream_t s);
 
 }  // namespace dalib200
 #endif  // DALI_B200_CSRC_WEBP_H_

@@ -1,12 +1,13 @@
-"""Stream ordering of the image decoder's side stages, checked WITHOUT a GPU.  Progressive JPEG, PNG, TIFF and WebP samples are decoded
-on side streams of their own, forked from the caller's stream and joined back into it; a missing fork, join or upload wait is a race
-that a GPU shows only as an intermittent wrong image, and the emulated launches (which run synchronously) never show.  So this test
-reads the call trace of tools/emul/cuda_emul_stub.cc (DALIB200_EMUL_TRACE) of a batch holding every sample kind, launched twice on one
-plan with float output, then a JPEG-only batch on the same plan, and a WebP-only batch with YCbCr output on a plan of its own (float and
-YCbCr output make the post pass run):
+"""Stream ordering of the image decoder's side stages, checked WITHOUT a GPU.  Progressive JPEG, PNG, TIFF, WebP, BMP / PNM and lossless
+JPEG samples are decoded on side streams of their own, forked from the caller's stream and joined back into it; a missing fork, join or
+upload wait is a race that a GPU shows only as an intermittent wrong image, and the emulated launches (which run synchronously) never
+show.  So this test reads the call trace of tools/emul/cuda_emul_stub.cc (DALIB200_EMUL_TRACE) of a batch holding every sample kind,
+launched twice on one plan with float output, then a JPEG-only batch on the same plan, and a WebP-only batch with YCbCr output on a plan
+of its own (float and YCbCr output make the post pass run):
   1. every side-stage kernel runs on its stage's stream, one stream per stage, none of them the caller's;
   2. before a stage's first upload, memset or launch, its stream waits on an event the caller's stream recorded behind the status clear;
-  3. the caller's stream waits on the progressive stage's join in front of dc_scan, on the PNG / TIFF / WebP joins in front of jpeg_post;
+     the lossless stage's event is recorded behind unstuff_scatter, whose clean streams it reads;
+  3. the caller's stream waits on the progressive stage's join in front of dc_scan, on the other stages' joins in front of jpeg_post;
   4. on the second launch, each stage's upload event is synchronised before its descriptor arena is uploaded again;
   5. a batch without a side stage makes no stream or event call for it."""
 import os
@@ -42,6 +43,8 @@ from dali_b200 import capi
 import png_streams as ps
 import tiff_streams as ts
 import webp_streams as ws
+import bitmap_streams as bs
+import ljpeg_streams as ls
 
 lib = capi.lib()
 stub = C.CDLL(os.environ["EMUL_STUB"])
@@ -70,8 +73,10 @@ prog = cv2.imencode(".jpg", g.synth_image(64, 80, 2), [cv2.IMWRITE_JPEG_PROGRESS
 png = ps.encode(ps.samples(30, 41, 2, 8, 5), 2, 8, filters="mixed")
 tif = ts.encode(ts.samples(20, 30, 3, 8, 6), 2, 8, 5, 2, rows_per_strip=3)
 webp = ws.cv2_webp(ws.image(40, 56, 7), 70)
-mixed = [jpg, prog, png, tif, webp]
-plan = capi.Plan("Jpeg", 6)
+bmp = bs.bmp(31, 17, 24, bs.rows(bs.image(17, 31, 1), 24))
+ljp = ls.encode(ls.image(33, 17, 1, 6, 71), P=6, Pt=2, restart=17 * 4)
+mixed = [jpg, prog, png, tif, webp, bmp, ljp]
+plan = capi.Plan("Jpeg", 7)
 for k in range(2):
     mark("mixed %%d" %% k)
     decode(plan, mixed, capi.RGB, capi.FLOAT)
@@ -87,7 +92,7 @@ del plan
 print("trace-ok")
 """
 
-STAGES = ("prog", "png", "tiff", "webp")
+STAGES = ("prog", "png", "tiff", "webp", "bitmap", "ljpeg")
 
 
 def run_trace(stub, trace):
@@ -141,6 +146,9 @@ def check_launch(ops, n, want_stages):
         forks = [ops[i][2] for i in range(first) if ops[i][0] == "wait" and ops[i][1] == s]
         recorded = {ops[i][1]: i for i in range(status + 1, first) if ops[i][0] == "record" and ops[i][2] == main}
         assert any(e in recorded for e in forks), (stage, forks, recorded)
+        if stage == "ljpeg":
+            scatter = next(i for i, o in enumerate(ops) if o[0] == "launch" and o[1] == "dalib200::unstuff_scatter_kernel")
+            assert any(recorded[e] > scatter for e in forks if e in recorded), (stage, forks, recorded, scatter)
         # 3. joined in front of the kernel that reads the stage's result
         last = launches[-1]
         joins = [ops[i][1] for i in range(last + 1, len(ops)) if ops[i][0] == "record" and ops[i][2] == s]
@@ -158,8 +166,8 @@ def test_side_stages_fork_join_and_reuse_their_arenas_in_order(stub, tmp_path):
     sections = run_trace(stub, str(tmp_path / "trace.txt"))
     names = [" ".join(t) for t, _ in sections]
     assert names == ["mixed 0", "mixed 1", "jpeg-only 3", "destroy", "webp-only 2", "destroy"], names
-    first = check_launch(sections[0][1], 5, STAGES)
-    second = check_launch(sections[1][1], 5, STAGES)
+    first = check_launch(sections[0][1], 7, STAGES)
+    second = check_launch(sections[1][1], 7, STAGES)
     ops = sections[1][1]
     assert not any(o[0] == "stream_create" for o in ops), "a stage stream was created twice"
     for stage, (s, upload, h2d) in second.items():

@@ -18,7 +18,7 @@
 using namespace dalib200;
 
 namespace {
-constexpr uint32_t kPad = 32;                      // jpeg.cu kCleanPad: zero bytes behind every clean stream
+constexpr uint32_t kPad = 32;                      // jpeg_recon.h kCleanPad: zero bytes behind every clean stream
 inline int rd16(const uint8_t *p) { return (p[0] << 8) | p[1]; }
 
 // the marker walk of ParseHeaders, reduced to what a lossless frame needs.  Returns a DALIB200 status.
