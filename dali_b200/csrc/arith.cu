@@ -105,10 +105,7 @@ int dalib200ArithLaunch(dalib200ArithPlan *p, const void *const *in_ptrs, void *
   if ((rc = p->arena.Upload(sizeof(ArithSample) * p->n, stream))) return rc;
   const ArithSample *d = reinterpret_cast<const ArithSample *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 8);
-  ProfScope ps_("arith", stream);
-  if (p->c.prog.wide) arith_kernel<true><<<grid, kArithThreads, 0, stream>>>(p->c.prog, d, p->n, p->total_items);
-  else arith_kernel<false><<<grid, kArithThreads, 0, stream>>>(p->c.prog, d, p->n, p->total_items);
-  CountLaunch();
+  Launch("arith", p->c.prog.wide ? arith_kernel<true> : arith_kernel<false>, grid, kArithThreads, 0, stream, p->c.prog, d, p->n, p->total_items);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -795,17 +795,14 @@ static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *
       mt.w_up = reinterpret_cast<const float *>(mel->tables.dev + o_up);
       mt.w_down = reinterpret_cast<const float *>(mel->tables.dev + o_down);
       mt.nfilter = mel->nfilter;
-      ProfScope ps_(pre ? "preemph_spectrogram_mel_fused" : "spectrogram_mel_fused", stream);
-      auto *k = pre ? spectrogram1024_kernel<true, true> : spectrogram1024_kernel<true, false>;
-      k<<<grid, kF1024Warps * 32, kF1024Smem, stream>>>(reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window,
-                                                        p->d_twiddle, mt, reinterpret_cast<const MelDesc *>(mel->arena.dev), out_ptrs ? 1 : 0);
+      Launch(pre ? "preemph_spectrogram_mel_fused" : "spectrogram_mel_fused", pre ? spectrogram1024_kernel<true, true> : spectrogram1024_kernel<true, false>,
+             grid, kF1024Warps * 32, kF1024Smem, stream, reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window,
+             p->d_twiddle, mt, reinterpret_cast<const MelDesc *>(mel->arena.dev), out_ptrs ? 1 : 0);
     } else {
-      ProfScope ps_(pre ? "preemph_spectrogram_stft" : "spectrogram_stft", stream);
-      auto *k = pre ? spectrogram1024_kernel<false, true> : spectrogram1024_kernel<false, false>;
-      k<<<grid, kF1024Warps * 32, kF1024Smem, stream>>>(reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window,
-                                                        p->d_twiddle, mt, nullptr, 1);
+      Launch(pre ? "preemph_spectrogram_stft" : "spectrogram_stft", pre ? spectrogram1024_kernel<false, true> : spectrogram1024_kernel<false, false>,
+             grid, kF1024Warps * 32, kF1024Smem, stream, reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window,
+             p->d_twiddle, mt, nullptr, 1);
     }
-    CountLaunch();
     DB_CUDA(cudaGetLastError());
     return DALIB200_SUCCESS;
   }
@@ -813,18 +810,16 @@ static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *
     auto *k = pre ? spectrogram_dft_kernel<true> : spectrogram_dft_kernel<false>;
     DB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(p->smem, 48 * 1024)));
     const int gridd = (int)std::min<int64_t>(p->total_groups, (int64_t)NumSMs() * 4);
-    ProfScope ps_(pre ? "preemph_spectrogram_dft" : "spectrogram_dft", stream);
-    k<<<gridd, 256, p->smem, stream>>>(reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window, p->d_twiddle);
-    CountLaunch();
+    Launch(pre ? "preemph_spectrogram_dft" : "spectrogram_dft", k, gridd, 256, p->smem, stream, reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n,
+           p->total_groups, P, p->d_window, p->d_twiddle);
     DB_CUDA(cudaGetLastError());
     return DALIB200_SUCCESS;
   }
   auto *k = pre ? spectrogram_kernel<true> : spectrogram_kernel<false>;
   DB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(p->smem, 96 * 1024)));
   const int grid = (int)std::min<int64_t>(p->total_groups, (int64_t)NumSMs() * 8);
-  ProfScope ps_(pre ? "preemph_spectrogram_stft_radix2" : "spectrogram_stft_radix2", stream);
-  k<<<grid, 256, p->smem, stream>>>(reinterpret_cast<const SpecDesc *>(p->arena.dev), p->n, p->total_groups, P, p->d_window, p->d_twiddle);
-  CountLaunch();
+  Launch(pre ? "preemph_spectrogram_stft_radix2" : "spectrogram_stft_radix2", k, grid, 256, p->smem, stream, reinterpret_cast<const SpecDesc *>(p->arena.dev),
+         p->n, p->total_groups, P, p->d_window, p->d_twiddle);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 }
@@ -960,21 +955,16 @@ int dalib200MelLaunch(dalib200MelPlan *p, const void *const *in_ptrs, void *cons
       p->dense_dirty = false;
     }
     const int grid = (int)std::min<int64_t>(p->total_items_mma, (int64_t)NumSMs() * 8);
-    ProfScope ps_("mel_filter_bank_mma", stream);
-    mel_mma_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items_mma, p->nfilter, p->nbin,
-                                             p->kpad, reinterpret_cast<const float *>(p->dense.dev),
-                                             reinterpret_cast<const int2 *>(p->dense.dev + (size_t)p->mpad * p->kpad * 4));
-    CountLaunch();
+    Launch("mel_filter_bank_mma", mel_mma_kernel, grid, 256, 0, stream, reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items_mma,
+           p->nfilter, p->nbin, p->kpad, reinterpret_cast<const float *>(p->dense.dev),
+           reinterpret_cast<const int2 *>(p->dense.dev + (size_t)p->mpad * p->kpad * 4));
     DB_CUDA(cudaGetLastError());
     return DALIB200_SUCCESS;
   }
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 32);
-  ProfScope ps_("mel_filter_bank", stream);
-  mel_kernel<<<grid, 128, 0, stream>>>(reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items, p->nfilter,
-                                       reinterpret_cast<const int32_t *>(p->tables.dev),
-                                       reinterpret_cast<const float *>(p->tables.dev + o_up),
-                                       reinterpret_cast<const float *>(p->tables.dev + o_down));
-  CountLaunch();
+  Launch("mel_filter_bank", mel_kernel, grid, 128, 0, stream, reinterpret_cast<const MelDesc *>(p->arena.dev), p->n, p->total_items, p->nfilter,
+         reinterpret_cast<const int32_t *>(p->tables.dev), reinterpret_cast<const float *>(p->tables.dev + o_up),
+         reinterpret_cast<const float *>(p->tables.dev + o_down));
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -267,22 +267,16 @@ int dalib200AudioLaunch(dalib200AudioPlan *p, void *const *out_ptrs, void *const
   const int sms = NumSMs();
   auto grid_of = [&](int64_t m) { return (int)std::max<int64_t>(1, std::min<int64_t>((m + 255) / 256, (int64_t)sms * 16)); };
   if (nf && p->flac_bytes > 0) {
-    { ProfScope ps_("flac_sync", stream); flac_sync_kernel<<<grid_of(p->flac_bytes), 256, 0, stream>>>(a); }
-    {
-      const SerialLanes g = SerialLaneGeometry((int)std::min<int64_t>(p->cand_slots, INT32_MAX), INT32_MAX);
-      ProfScope ps_("flac_frame", stream);
-      flac_frame_kernel<<<g.warps, 32, 0, stream>>>(a, g.lanes);
-    }
-    CountLaunch(2);
+    Launch("flac_sync", flac_sync_kernel, grid_of(p->flac_bytes), 256, 0, stream, a);
+    const SerialLanes g = SerialLaneGeometry((int)std::min<int64_t>(p->cand_slots, INT32_MAX), INT32_MAX);
+    Launch("flac_frame", flac_frame_kernel, g.warps, 32, 0, stream, a, g.lanes);
   }
   if (nf) {
-    { ProfScope ps_("flac_chain", stream); flac_chain_kernel<<<(nf + 127) / 128, 128, 0, stream>>>(a); }
+    Launch("flac_chain", flac_chain_kernel, (nf + 127) / 128, 128, 0, stream, a);
     const SerialLanes g = SerialLaneGeometry((int)std::min<int64_t>(p->frame_slots, INT32_MAX), INT32_MAX);
-    { ProfScope ps_("flac_decode", stream); flac_decode_kernel<<<g.warps, 32, 0, stream>>>(a, g.lanes); }
-    CountLaunch(2);
+    Launch("flac_decode", flac_decode_kernel, g.warps, 32, 0, stream, a, g.lanes);
   }
-  { ProfScope ps_("audio_convert", stream); audio_convert_kernel<<<grid_of(std::max<int64_t>(p->total_elems, n)), 256, 0, stream>>>(a); }
-  CountLaunch();
+  Launch("audio_convert", audio_convert_kernel, grid_of(std::max<int64_t>(p->total_elems, n)), 256, 0, stream, a);
   DB_CUDA(cudaGetLastError());
   if (!p->resampled.empty()) {
     std::vector<const void *> in(p->resampled.size());

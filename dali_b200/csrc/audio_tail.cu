@@ -594,10 +594,8 @@ static int PreemphasisLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, 
   if ((rc = p->arena.Upload(sizeof(PeDesc) * p->n, stream))) return rc;
   const PeDesc *d = reinterpret_cast<const PeDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
-  ProfScope ps_("preemphasis_filter", stream);
-  if (p->pe_dtype == DALIB200_INT16) preemphasis_kernel<int16_t><<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->pe_border);
-  else preemphasis_kernel<float><<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->pe_border);
-  CountLaunch();
+  Launch("preemphasis_filter", p->pe_dtype == DALIB200_INT16 ? preemphasis_kernel<int16_t> : preemphasis_kernel<float>, grid, 256, 0, stream, d, p->n,
+         p->total_items, p->pe_border);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 }
@@ -619,10 +617,8 @@ int dalib200NonsilentLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, v
   }
   if ((rc = p->arena.Upload(sizeof(NsDesc) * p->n, stream))) return rc;
   const NsDesc *d = reinterpret_cast<const NsDesc *>(p->arena.dev);
-  { ProfScope ps_("nonsilent_mms", stream); nonsilent_mms_kernel<<<(unsigned)((p->total_items + 127) / 128), 128, 0, stream>>>(d, p->n, p->total_items); }
-  CountLaunch();
-  { ProfScope ps_("nonsilent_region", stream); nonsilent_region_kernel<<<p->n, 256, 0, stream>>>(d); }
-  CountLaunch();
+  Launch("nonsilent_mms", nonsilent_mms_kernel, (unsigned)((p->total_items + 127) / 128), 128, 0, stream, d, p->n, p->total_items);
+  Launch("nonsilent_region", nonsilent_region_kernel, p->n, 256, 0, stream, d);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH
@@ -640,9 +636,7 @@ static int AudioResampleLaunch(dalib200SignalPlan *p, const void *const *in_ptrs
   if ((rc = p->arena.Upload(sizeof(ArDesc) * p->n, stream))) return rc;
   ArWindow w{ p->ar_scale, p->ar_center, p->ar_lobes, p->d_lookup };
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 8);
-  ProfScope ps_("audio_resample", stream);
-  audio_resample_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const ArDesc *>(p->arena.dev), p->n, p->total_items, w);
-  CountLaunch();
+  Launch("audio_resample", audio_resample_kernel, grid, 256, 0, stream, reinterpret_cast<const ArDesc *>(p->arena.dev), p->n, p->total_items, w);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 }
@@ -670,12 +664,10 @@ int dalib200SignalLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void
         p->d_max_cap = p->max_batch;
       }
       DB_CUDA(cudaMemsetAsync(p->d_max, 0, sizeof(uint32_t) * p->n, stream));
-      { ProfScope ps_("to_decibels_max", stream); todb_max_kernel<<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->d_max); }
-      CountLaunch();
+      Launch("to_decibels_max", todb_max_kernel, grid, 256, 0, stream, d, p->n, p->total_items, p->d_max);
       smax = p->d_max;
     }
-    { ProfScope ps_("to_decibels", stream); todb_kernel<<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->mul_log2, p->s_ref, p->min_ratio, smax); }
-    CountLaunch();
+    Launch("to_decibels", todb_kernel, grid, 256, 0, stream, d, p->n, p->total_items, p->mul_log2, p->s_ref, p->min_ratio, smax);
   } else if (p->kind == SIG_MFCC) {
     if ((rc = GrowDevice(p->d_table, p->d_table_cap, p->h_table.size()))) return rc;
     if (p->table_dirty) {
@@ -686,14 +678,10 @@ int dalib200SignalLaunch(dalib200SignalPlan *p, const void *const *in_ptrs, void
     const size_t smem = (size_t)p->ndct * p->nfeat * sizeof(float);
     DB_CHECK_ARG(smem <= 200 * 1024, "MFCC: the cosine table (%d x %d) does not fit shared memory", p->ndct, p->nfeat);
     if (smem > 48 * 1024) DB_CUDA(cudaFuncSetAttribute(mfcc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ProfScope ps_("mfcc_dct", stream);
-    mfcc_kernel<<<grid, 128, smem, stream>>>(d, p->n, p->total_items, p->nfeat, p->ndct, p->d_table,
-                                             p->has_lifter ? p->d_table + (size_t)p->ndct * p->nfeat : nullptr);
-    CountLaunch();
+    Launch("mfcc_dct", mfcc_kernel, grid, 128, smem, stream, d, p->n, p->total_items, p->nfeat, p->ndct, p->d_table,
+           p->has_lifter ? p->d_table + (size_t)p->ndct * p->nfeat : nullptr);
   } else {
-    ProfScope ps_("normalize", stream);
-    normalize_kernel<<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->mode, p->scale, p->shift, p->eps, p->ddof);
-    CountLaunch();
+    Launch("normalize", normalize_kernel, grid, 256, 0, stream, d, p->n, p->total_items, p->mode, p->scale, p->shift, p->eps, p->ddof);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

@@ -54,15 +54,11 @@ int BitmapStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   const int nunpack = (int)unpack.size();
   if (nunpack > 0) {
     const SerialLanes g = SerialLaneGeometry(nunpack, 1 << 30);
-    ProfScope ps_("bitmap_unpack", s);
-    bitmap_unpack_kernel<<<g.warps, 32, 0, s>>>(d_images, d_unpack, nunpack, g.lanes, in.d_raw, d_scratch, in.d_status);
-    CountLaunch();
+    Launch("bitmap_unpack", bitmap_unpack_kernel, g.warps, 32, 0, s, d_images, d_unpack, nunpack, g.lanes, in.d_raw, d_scratch, in.d_status);
   }
   if (groups > 0) {
     const int grid = (int)std::min<int64_t>((groups + 255) / 256, (int64_t)NumSMs() * 16);
-    ProfScope ps_("bitmap_color", s);
-    bitmap_color_kernel<<<grid, 256, 0, s>>>(d_images, (int)images.size(), groups, in.d_raw, d_scratch);
-    CountLaunch();
+    Launch("bitmap_color", bitmap_color_kernel, grid, 256, 0, s, d_images, (int)images.size(), groups, in.d_raw, d_scratch);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

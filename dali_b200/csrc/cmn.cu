@@ -300,23 +300,15 @@ int dalib200CmnLaunch(dalib200CmnPlan *p, const void *const *in_ptrs, void *cons
   if (p->total_units > 0) {
     int64_t blocks = (p->total_units + 7) / 8;
     int grid = (int)std::min<int64_t>(blocks, (int64_t)sms * 8);
-    ProfScope ps_("cmn_hwc2chw", stream);
-    if (p->out_dtype == DALIB200_FLOAT)
-      cmn_hwc2chw_kernel<float><<<grid, 256, 0, stream>>>(dd, p->n, p->total_units, p->out_c);
-    else
-      cmn_hwc2chw_kernel<uint16_t><<<grid, 256, 0, stream>>>(dd, p->n, p->total_units, p->out_c);
-    CountLaunch();
+    Launch("cmn_hwc2chw", p->out_dtype == DALIB200_FLOAT ? cmn_hwc2chw_kernel<float> : cmn_hwc2chw_kernel<uint16_t>, grid, 256, 0, stream, dd, p->n,
+           p->total_units, p->out_c);
   }
   if (p->total_elems > 0) {
     int64_t blocks = (p->total_elems + 255) / 256;
     int grid = (int)std::min<int64_t>(blocks, (int64_t)sms * 16);
     const int chw = p->out_layout == DALIB200_LAYOUT_CHW;
-    ProfScope ps_("cmn_generic", stream);
-    if (p->out_dtype == DALIB200_FLOAT)
-      cmn_generic_kernel<float><<<grid, 256, 0, stream>>>(dd, p->n, p->total_elems, p->out_c, chw);
-    else
-      cmn_generic_kernel<uint16_t><<<grid, 256, 0, stream>>>(dd, p->n, p->total_elems, p->out_c, chw);
-    CountLaunch();
+    Launch("cmn_generic", p->out_dtype == DALIB200_FLOAT ? cmn_generic_kernel<float> : cmn_generic_kernel<uint16_t>, grid, 256, 0, stream, dd, p->n,
+           p->total_elems, p->out_c, chw);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

@@ -142,7 +142,7 @@ int dalib200DebugCheckHalfConversion(uint64_t *mismatches) try {
   unsigned long long *d = nullptr;
   DB_CUDA(cudaMalloc(reinterpret_cast<void **>(&d), 8));
   DB_CUDA(cudaMemset(d, 0, 8));
-  dalib200::half_cvt_check_kernel<<<dalib200::NumSMs() * 8, 256>>>(d);
+  dalib200::Launch("half_cvt_check", dalib200::half_cvt_check_kernel, dalib200::NumSMs() * 8, 256, 0, nullptr, d);
   unsigned long long h = 0;
   const cudaError_t e = cudaMemcpy(&h, d, 8, cudaMemcpyDeviceToHost);
   cudaFree(d);

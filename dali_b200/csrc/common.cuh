@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdarg>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../../include/dali_b200.h"
 #include "host_device.h"
@@ -18,8 +19,7 @@ namespace dalib200 {
 // ---------------------------------------------------------------------------------------------
 // error plumbing (thread-local message, as the reference C API does: dali/c_api_2/error_handling.cc)
 void SetLastError(const char *fmt, ...);
-extern std::atomic<uint64_t> g_launch_count;
-inline void CountLaunch(int n = 1) { g_launch_count.fetch_add(n, std::memory_order_relaxed); }
+extern std::atomic<uint64_t> g_launch_count;   // dalib200GetLaunchCount
 
 #define DB_CHECK_ARG(cond, ...)                                   \
   do { if (!(cond)) { ::dalib200::SetLastError(__VA_ARGS__); return DALIB200_ERROR_INVALID_ARGUMENT; } } while (0)
@@ -40,14 +40,9 @@ struct SerialLanes { int warps, lanes; };
 SerialLanes SerialLaneGeometry(int nchains, int max_workers);
 
 // Optional per-launch timing (CUDA events on the launching stream), switched on by dalib200ProfilingEnable.
-// bench.py uses it to time the dominant kernel live inside the timed region.
+// bench.py uses it to time the dominant kernel live inside the timed region.  Launch (below) brackets every launch with them.
 void ProfBegin(const char *name, cudaStream_t s);
 void ProfEnd(cudaStream_t s);
-struct ProfScope {
-  cudaStream_t s;
-  ProfScope(const char *name, cudaStream_t st) : s(st) { ProfBegin(name, s); }
-  ~ProfScope() { ProfEnd(s); }
-};
 
 // ---------------------------------------------------------------------------------------------
 // numerics shared by the kernels -- these restate the reference HOST (CPU backend) conventions,
@@ -193,6 +188,16 @@ __device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t by
 __device__ __forceinline__ void tma_load_3d(void *dst, const void *tmap, int c0, int c1, int c2, uint64_t *bar) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
                :: "r"(smem_u32(dst)), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
+}
+
+// Every kernel launch of the library goes through here: an NVTX range and, with profiling on, one timing record under `name`
+// around the launch, and one count in dalib200GetLaunchCount.  So the count and the records are the launches, one each.
+template <typename... P, typename... A>
+inline void Launch(const char *name, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, A &&...args) {
+  ProfBegin(name, s);
+  kernel<<<grid, block, smem, s>>>(std::forward<A>(args)...);
+  ProfEnd(s);
+  g_launch_count.fetch_add(1, std::memory_order_relaxed);
 }
 
 #endif  // __CUDACC__

@@ -126,20 +126,12 @@ int dalib200EqualizeLaunch(dalib200EqualizePlan *p, const void *const *in_ptrs, 
   if ((rc = p->arena.Upload(bytes, stream))) return rc;
   const EqSample *d = reinterpret_cast<const EqSample *>(p->arena.dev);
   DB_CUDA(cudaMemsetAsync(p->hist, 0, (size_t)pd.hist_words * sizeof(uint32_t), stream));
-  {
-    ProfScope ps_("equalize_hist", stream);
-    const int grid = (int)std::min<int64_t>(pd.items, (int64_t)NumSMs() * p->hist_ctas);
-    equalize_hist_kernel<<<grid, kEqThreads, 0, stream>>>(d, n, pd.items, p->hist);
-    CountLaunch();
-    DB_CUDA(cudaGetLastError());
-  }
-  {
-    ProfScope ps_("equalize_apply", stream);
-    const int grid = (int)std::min<int64_t>(pd.items, (int64_t)NumSMs() * p->apply_ctas);
-    equalize_apply_kernel<<<grid, kEqThreads, 0, stream>>>(d, n, pd.items, p->hist);
-    CountLaunch();
-    DB_CUDA(cudaGetLastError());
-  }
+  Launch("equalize_hist", equalize_hist_kernel, (int)std::min<int64_t>(pd.items, (int64_t)NumSMs() * p->hist_ctas), kEqThreads, 0, stream, d, n,
+         pd.items, p->hist);
+  DB_CUDA(cudaGetLastError());
+  Launch("equalize_apply", equalize_apply_kernel, (int)std::min<int64_t>(pd.items, (int64_t)NumSMs() * p->apply_ctas), kEqThreads, 0, stream, d, n,
+         pd.items, p->hist);
+  DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH
 

@@ -247,11 +247,9 @@ static int PadLaunch(dalib200GenericPlan *p, const void *const *in_ptrs, void *c
   if ((rc = p->arena.Upload(sizeof(PadDesc) * p->n, stream))) return rc;
   const PadDesc *d = reinterpret_cast<const PadDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
-  ProfScope ps_("pad", stream);
-  if (p->pad_elem == 1) pad_kernel<uint8_t><<<grid, 256, 0, stream>>>(d, p->n, p->total_items, (uint8_t)p->pad_fill);
-  else if (p->pad_elem == 2) pad_kernel<uint16_t><<<grid, 256, 0, stream>>>(d, p->n, p->total_items, (uint16_t)p->pad_fill);
-  else pad_kernel<uint32_t><<<grid, 256, 0, stream>>>(d, p->n, p->total_items, p->pad_fill);
-  CountLaunch();
+  if (p->pad_elem == 1) Launch("pad", pad_kernel<uint8_t>, grid, 256, 0, stream, d, p->n, p->total_items, (uint8_t)p->pad_fill);
+  else if (p->pad_elem == 2) Launch("pad", pad_kernel<uint16_t>, grid, 256, 0, stream, d, p->n, p->total_items, (uint16_t)p->pad_fill);
+  else Launch("pad", pad_kernel<uint32_t>, grid, 256, 0, stream, d, p->n, p->total_items, p->pad_fill);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 }
@@ -267,15 +265,11 @@ int dalib200GenericLaunch(dalib200GenericPlan *p, const void *const *in_ptrs, vo
   if ((rc = p->arena.Upload(sizeof(GenDesc) * p->n, stream))) return rc;
   const GenDesc *d = reinterpret_cast<const GenDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 16);
-  if (p->kind == 1) {
-    ProfScope ps_("multiply_add", stream);
-    if (p->out_dtype == DALIB200_UINT8) multiply_add_kernel<uint8_t><<<grid, 256, 0, stream>>>(d, p->n, p->total_items);
-    else multiply_add_kernel<float><<<grid, 256, 0, stream>>>(d, p->n, p->total_items);
-  } else {
-    ProfScope ps_("window_copy", stream);
-    window_copy_kernel<<<grid, 256, 0, stream>>>(d, p->n, p->total_items);
-  }
-  CountLaunch();
+  if (p->kind == 1)
+    Launch("multiply_add", p->out_dtype == DALIB200_UINT8 ? multiply_add_kernel<uint8_t> : multiply_add_kernel<float>, grid, 256, 0, stream, d, p->n,
+           p->total_items);
+  else
+    Launch("window_copy", window_copy_kernel, grid, 256, 0, stream, d, p->n, p->total_items);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -1489,23 +1489,17 @@ int LaunchReconstruct(const ReconLaunch &a, cudaStream_t s) {
   const int sms = NumSMs();
   const int64_t total_blocks = a.totals.work;
   const int grid = (int)std::min<int64_t>((total_blocks + 127) / 128, (int64_t)sms * 32);
-  if (total_blocks > 0) {
-    ProfScope ps_("jpeg_idct", s);
-    idct_kernel<<<grid, 128, 0, s>>>(a.d_images, a.d_first_work, a.nimages, total_blocks, a.d_coef, a.d_dc, a.d_quants, a.d_planes);
-  }
-  if (a.totals.fused > 0) {
-    { ProfScope ps_("jpeg_idct_color", s); idct_color_420<<<(int)a.totals.fused, kFusedThreads, 0, s>>>(a.d_images, a.d_first_fused, a.nimages, a.d_coef, a.d_dc, a.d_quants); }
-    CountLaunch();
-  }
+  if (total_blocks > 0)
+    Launch("jpeg_idct", idct_kernel, grid, 128, 0, s, a.d_images, a.d_first_work, a.nimages, total_blocks, a.d_coef, a.d_dc, a.d_quants, a.d_planes);
+  if (a.totals.fused > 0)
+    Launch("jpeg_idct_color", idct_color_420, (int)a.totals.fused, kFusedThreads, 0, s, a.d_images, a.d_first_fused, a.nimages, a.d_coef, a.d_dc, a.d_quants);
   if (a.totals.quads > 0) {
     const int grid2 = (int)std::min<int64_t>((a.totals.quads + 255) / 256, (int64_t)sms * 32);
-    { ProfScope ps_("jpeg_upsample_color_generic", s); color_kernel<<<grid2, 256, 0, s>>>(a.d_images, a.d_first_quad, a.nimages, a.totals.quads, a.d_planes); }
-    CountLaunch();
+    Launch("jpeg_upsample_color_generic", color_kernel, grid2, 256, 0, s, a.d_images, a.d_first_quad, a.nimages, a.totals.quads, a.d_planes);
   }
   if (a.totals.items > 0) {
     const int grid3 = (int)std::min<int64_t>(a.totals.items, (int64_t)sms * 64);
-    { ProfScope ps_("jpeg_upsample_color", s); color_fast_kernel<<<grid3, 128, 0, s>>>(a.d_images, a.d_first_item, a.nimages, a.totals.items, a.d_planes); }
-    CountLaunch();
+    Launch("jpeg_upsample_color", color_fast_kernel, grid3, 128, 0, s, a.d_images, a.d_first_item, a.nimages, a.totals.items, a.d_planes);
   }
   return DALIB200_SUCCESS;
 }
@@ -2455,10 +2449,9 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   const bool any_units = nunits > 0 && p->nchunks > 0 && p->total_blocks_sync > 0;
   if (nunits > 0 && p->nchunks > 0) {
     const int grid = (int)std::min<uint32_t>(p->nchunks, (uint32_t)sms * 16);
-    { ProfScope ps_("jpeg_unstuff_count", s); unstuff_count_kernel<<<grid, 256, 0, s>>>(d_raw, d_units, nunits, p->nchunks, p->d_chunk); }
-    { ProfScope ps_("jpeg_unstuff_scan", s); unstuff_scan_kernel<<<(nunits + 7) / 8, 256, 0, s>>>(d_units, nunits, p->d_chunk, p->d_unit_len); }
-    { ProfScope ps_("jpeg_unstuff_scatter", s); unstuff_scatter_kernel<<<grid, 256, 0, s>>>(d_raw, d_units, nunits, p->nchunks, p->d_chunk, p->d_clean); }
-    CountLaunch(3);
+    Launch("jpeg_unstuff_count", unstuff_count_kernel, grid, 256, 0, s, d_raw, d_units, nunits, p->nchunks, p->d_chunk);
+    Launch("jpeg_unstuff_scan", unstuff_scan_kernel, (nunits + 7) / 8, 256, 0, s, d_units, nunits, p->d_chunk, p->d_unit_len);
+    Launch("jpeg_unstuff_scatter", unstuff_scatter_kernel, grid, 256, 0, s, d_raw, d_units, nunits, p->nchunks, p->d_chunk, p->d_clean);
   }
   if ((rc = p->ljpeg.Run(in, s))) return rc;            // forked behind U3, whose clean streams it reads
   HuffCtx cx;
@@ -2479,26 +2472,23 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     p->walk_max_grid = std::max(1, per_sm) * sms * 4;
     p->smem_opted = true;
   }
-  if (any_units) { ProfScope ps_("jpeg_huff_sync_intra", s); huff_sync_intra_kernel<<<p->total_blocks_sync, kSyncThreads, hsmem, s>>>(cx); }
   if (any_units) {
+    Launch("jpeg_huff_sync_intra", huff_sync_intra_kernel, p->total_blocks_sync, kSyncThreads, hsmem, s, cx);
     // chain walk: grids sized for the expected list lengths (about 30 % / 8 % / 2.5 % of the subsequences carry a live chain
     // after 1 / 2 / 3 visits); CTAs beyond the actual length return at once, grid-stride loops cover longer lists
     auto walk_grid = [&](double frac) {
       const int64_t want = (int64_t)(p->total_subseq * frac) / kTailThreads + p->total_blocks_sync / kTailThreads + 1;
       return (int)std::max<int64_t>(1, std::min<int64_t>(p->walk_max_grid, want));
     };
-    { ProfScope ps_("jpeg_huff_sync_walk1", s); huff_sync_walk_kernel<<<walk_grid(0.40), kTailThreads, walk_smem, s>>>(cx, 0, 1, 1); }
-    { ProfScope ps_("jpeg_huff_sync_walk2", s); huff_sync_walk_kernel<<<walk_grid(0.14), kTailThreads, walk_smem, s>>>(cx, 1, 2, 1); }
-    { ProfScope ps_("jpeg_huff_sync_walk3", s); huff_sync_walk_kernel<<<walk_grid(0.06), kTailThreads, walk_smem, s>>>(cx, 2, 0, 1 << 30); }
-    CountLaunch(2);
+    Launch("jpeg_huff_sync_walk1", huff_sync_walk_kernel, walk_grid(0.40), kTailThreads, walk_smem, s, cx, 0, 1, 1);
+    Launch("jpeg_huff_sync_walk2", huff_sync_walk_kernel, walk_grid(0.14), kTailThreads, walk_smem, s, cx, 1, 2, 1);
+    Launch("jpeg_huff_sync_walk3", huff_sync_walk_kernel, walk_grid(0.06), kTailThreads, walk_smem, s, cx, 2, 0, 1 << 30);
   }
-  { ProfScope ps_("jpeg_huff_scan", s); huff_scan_kernel<<<p->n, 1024, 0, s>>>(cx); }
-  CountLaunch();
-  if (any_units && p->total_blocks_write > 0) { ProfScope ps_("jpeg_huff_write", s); huff_write_kernel<<<p->total_blocks_write, kWriteThreads, wsmem, s>>>(cx); }
+  Launch("jpeg_huff_scan", huff_scan_kernel, p->n, 1024, 0, s, cx);
+  if (any_units && p->total_blocks_write > 0) Launch("jpeg_huff_write", huff_write_kernel, p->total_blocks_write, kWriteThreads, wsmem, s, cx);
   if ((rc = p->prog.Join(s))) return rc;                // the progressive samples' coefficients and DC differences are in place
-  { ProfScope ps_("jpeg_dc_scan", s); dc_scan_kernel<<<p->n, 1024, 0, s>>>(d_images, p->d_dc); }
-  { ProfScope ps_("jpeg_truncation_fixup", s); truncation_fixup_kernel<<<p->n, 256, 0, s>>>(cx); }
-  CountLaunch();
+  Launch("jpeg_dc_scan", dc_scan_kernel, p->n, 1024, 0, s, d_images, p->d_dc);
+  Launch("jpeg_truncation_fixup", truncation_fixup_kernel, p->n, 256, 0, s, cx);
   {
     ReconLaunch ra;
     ra.d_images = d_images; ra.nimages = p->n;
@@ -2514,12 +2504,9 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
     return rc;
   if (!p->posts.empty()) {
     const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((p->total_post_px + 255) / 256, (int64_t)sms * 16));
-    ProfScope ps_("jpeg_post", s);
-    if (p->dtype == DALIB200_FLOAT) jpeg_post_kernel<float><<<grid, 256, 0, s>>>(p->d_posts, (int)p->posts.size(), p->total_post_px);
-    else jpeg_post_kernel<uint8_t><<<grid, 256, 0, s>>>(p->d_posts, (int)p->posts.size(), p->total_post_px);
-    CountLaunch();
+    Launch("jpeg_post", p->dtype == DALIB200_FLOAT ? jpeg_post_kernel<float> : jpeg_post_kernel<uint8_t>, grid, 256, 0, s, p->d_posts, (int)p->posts.size(),
+           p->total_post_px);
   }
-  CountLaunch(5);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -146,13 +146,8 @@ int dalib200JpegDistortLaunch(dalib200JpegDistortPlan *p, const void *const *in_
   if ((rc = p->arena.Upload(bytes, s))) return rc;
   const uint8_t *dv = p->arena.dev;
   const auto *d_quants = reinterpret_cast<const QuantSet *>(dv + o_q);
-  {
-    ProfScope ps_("jpeg_distort_fdct", s);
-    jpeg_distort_fdct_kernel<<<(unsigned)p->total_strips, kJdThreads, 0, s>>>(reinterpret_cast<const JdImage *>(dv),
-                                                                             reinterpret_cast<const int64_t *>(dv + o_pre), n, d_quants,
-                                                                             p->d_coef, p->d_dc);
-  }
-  CountLaunch();
+  Launch("jpeg_distort_fdct", jpeg_distort_fdct_kernel, (unsigned)p->total_strips, kJdThreads, 0, s, reinterpret_cast<const JdImage *>(dv),
+         reinterpret_cast<const int64_t *>(dv + o_pre), n, d_quants, p->d_coef, p->d_dc);
   ReconLaunch ra;
   ra.d_images = reinterpret_cast<const JpegImage *>(dv + o_img); ra.nimages = n;
   ra.totals = p->totals;
@@ -162,7 +157,6 @@ int dalib200JpegDistortLaunch(dalib200JpegDistortPlan *p, const void *const *in_
   ra.d_first_item = reinterpret_cast<const int64_t *>(dv + o_pre + 4 * pre);
   ra.d_coef = p->d_coef; ra.d_dc = p->d_dc; ra.d_quants = d_quants; ra.d_planes = p->d_planes;
   if ((rc = LaunchReconstruct(ra, s))) return rc;
-  if (p->totals.work > 0) CountLaunch();     // idct_kernel (LaunchReconstruct counts the colour launches)
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

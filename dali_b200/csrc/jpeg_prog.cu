@@ -82,15 +82,11 @@ int ProgStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   for (size_t w = 0; w + 1 < wave_begin.size(); w++) {
     const int cnt = wave_begin[w + 1] - wave_begin[w];
     if (cnt <= 0) continue;
-    ProfScope ps_("jpeg_prog_scan", s);
-    prog_scan_kernel<<<cnt, 32, 0, s>>>(d_scans, wave_begin[w], d_images, d_huff, in.d_raw, in.d_coef, in.d_status);
-    CountLaunch();
+    Launch("jpeg_prog_scan", prog_scan_kernel, cnt, 32, 0, s, d_scans, wave_begin[w], d_images, d_huff, in.d_raw, in.d_coef, in.d_status);
   }
   if (total_blocks > 0) {
     const int grid = (int)std::min<int64_t>((total_blocks + 255) / 256, (int64_t)NumSMs() * 8);
-    ProfScope ps_("jpeg_prog_dc", s);
-    prog_dc_kernel<<<grid, 256, 0, s>>>(d_images, d_first_blk, (int)images.size(), total_blocks, in.d_coef, in.d_dc, in.d_status);
-    CountLaunch();
+    Launch("jpeg_prog_dc", prog_dc_kernel, grid, 256, 0, s, d_images, d_first_blk, (int)images.size(), total_blocks, in.d_coef, in.d_dc, in.d_status);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

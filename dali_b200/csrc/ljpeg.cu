@@ -181,13 +181,12 @@ int LjpegStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   auto grid_of = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sms * 16)); };
   if (a.total_sub > 0) {
     DB_CUDA(cudaMemsetAsync(a.d_rec, 0, sizeof(uint64_t) * a.total_sub, s));
-    { ProfScope ps_("ljpeg_sync", s); ljpeg_sync_kernel<<<grid_of(a.total_sub), 256, 0, s>>>(a); }
+    Launch("ljpeg_sync", ljpeg_sync_kernel, grid_of(a.total_sub), 256, 0, s, a);
   }
-  { ProfScope ps_("ljpeg_scan", s); ljpeg_scan_kernel<<<a.nunits, 256, 0, s>>>(a); }
-  if (a.total_sub > 0) { ProfScope ps_("ljpeg_write", s); ljpeg_write_kernel<<<grid_of(a.total_sub), 256, 0, s>>>(a); }
-  { ProfScope ps_("ljpeg_recon", s); ljpeg_recon_kernel<<<a.nbands, kLjpegRecThreads, 0, s>>>(a.d_images, a.d_bands, a.d_diff); }
-  { ProfScope ps_("ljpeg_color", s); ljpeg_color_kernel<<<grid_of(a.total_px), 256, 0, s>>>(a.d_images, a.nimages, a.total_px, a.d_diff); }
-  CountLaunch(a.total_sub > 0 ? 5 : 3);
+  Launch("ljpeg_scan", ljpeg_scan_kernel, a.nunits, 256, 0, s, a);
+  if (a.total_sub > 0) Launch("ljpeg_write", ljpeg_write_kernel, grid_of(a.total_sub), 256, 0, s, a);
+  Launch("ljpeg_recon", ljpeg_recon_kernel, a.nbands, kLjpegRecThreads, 0, s, a.d_images, a.d_bands, a.d_diff);
+  Launch("ljpeg_color", ljpeg_color_kernel, grid_of(a.total_px), 256, 0, s, a.d_images, a.nimages, a.total_px, a.d_diff);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 }

@@ -109,9 +109,7 @@ int dalib200PermuteLaunch(dalib200PermutePlan *p, const void *const *in_ptrs, vo
   const int grid = (int)std::min<int64_t>(p->total_items, (int64_t)NumSMs() * 8);
   const char *name = kinds == 1 << kPermKindRows ? "permute_rows" : kinds == 1 << kPermKindTiled ? "permute_tiled"
                    : kinds == 1 << kPermKindSmall ? "permute_small" : "permute_mixed";
-  ProfScope ps_(name, stream);
-  permute_kernel<<<grid, kPermThreads, 0, stream>>>(d, live, p->total_items);
-  CountLaunch();
+  Launch(name, permute_kernel, grid, kPermThreads, 0, stream, d, live, p->total_items);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -60,21 +60,11 @@ int PngStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   const PngImage *d_images; const PngChunk *d_chunks;
   if (int rc = arena.Pack(s, std::tie(d_images, d_chunks), images, chunks)) return rc;
   const int nimages = (int)images.size(), nchunks = (int)chunks.size();
-  if (nchunks > 0) {
-    ProfScope ps_("png_crc", s);
-    png_crc_kernel<<<(nchunks + 127) / 128, 128, 0, s>>>(d_chunks, nchunks, d_images, in.d_raw, in.d_status);
-    CountLaunch();
-  }
-  {
-    ProfScope ps_("png_inflate", s);
-    png_inflate_kernel<<<nimages, 32, 0, s>>>(d_images, d_chunks, in.d_raw, d_scan, in.d_status);
-    CountLaunch();
-  }
+  if (nchunks > 0) Launch("png_crc", png_crc_kernel, (nchunks + 127) / 128, 128, 0, s, d_chunks, nchunks, d_images, in.d_raw, in.d_status);
+  Launch("png_inflate", png_inflate_kernel, nimages, 32, 0, s, d_images, d_chunks, in.d_raw, d_scan, in.d_status);
   if (total_px > 0) {
     const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
-    ProfScope ps_("png_color", s);
-    png_color_kernel<<<grid, 256, 0, s>>>(d_images, nimages, total_px, d_scan);
-    CountLaunch();
+    Launch("png_color", png_color_kernel, grid, 256, 0, s, d_images, nimages, total_px, d_scan);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

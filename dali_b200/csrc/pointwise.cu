@@ -340,14 +340,11 @@ int dalib200PointwiseLaunch(dalib200PointwisePlan *p, const void *const *in_ptrs
   if (rc) return rc;
   const auto *dd = reinterpret_cast<const PwDesc *>(p->arena.dev);
   const int grid = (int)std::min<int64_t>((p->total_quads + 255) / 256, (int64_t)NumSMs() * 32);
-  ProfScope ps_(p->mode == PW_LINEAR ? "linear_transform" : "color_space_conversion", stream);
-  if (p->mode == PW_LINEAR) {
-    if (p->out_dtype == DALIB200_UINT8) linear_transform_kernel<uint8_t><<<grid, 256, 0, stream>>>(dd, p->n, p->total_quads);
-    else linear_transform_kernel<float><<<grid, 256, 0, stream>>>(dd, p->n, p->total_quads);
-  } else {
-    csc_kernel<<<grid, 256, 0, stream>>>(dd, p->n, p->total_quads, p->in_type, p->out_type);
-  }
-  CountLaunch();
+  if (p->mode == PW_LINEAR)
+    Launch("linear_transform", p->out_dtype == DALIB200_UINT8 ? linear_transform_kernel<uint8_t> : linear_transform_kernel<float>, grid, 256, 0, stream,
+           dd, p->n, p->total_quads);
+  else
+    Launch("color_space_conversion", csc_kernel, grid, 256, 0, stream, dd, p->n, p->total_quads, p->in_type, p->out_type);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

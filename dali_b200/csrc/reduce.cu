@@ -129,25 +129,21 @@ int dalib200ReduceLaunch(dalib200ReducePlan *p, const void *const *in_ptrs, cons
       for (int i = 0; i < n; i++) if (pd.kinds[(size_t)i * kRedMaxPasses + q] >= 0) kinds |= 1 << pd.kinds[(size_t)i * kRedMaxPasses + q];
       const char *name = kinds == 1 ? names[0] : kinds == 2 ? names[1] : kinds == 4 ? names[2] : "reduce_mixed";
       const int grid = (int)std::min<int64_t>(pd.items[q], cap);
-      ProfScope ps_(name, stream);
       const auto launch = [&](auto t, auto a, auto e) {
-        reduce_pass_kernel<decltype(t), decltype(a), decltype(e)::value><<<grid, kRedThreads, 0, stream>>>(d, n, pd.items[q], f);
+        Launch(name, reduce_pass_kernel<decltype(t), decltype(a), decltype(e)::value>, grid, kRedThreads, 0, stream, d, n, pd.items[q], f);
       };
       if (q == 0) red_dispatch(pd.in_type, pd.acc, pd.elem, launch);
       else red_dispatch(pd.acc == kAccI64 ? kRedI64 : pd.acc == kAccU64 ? kRedU64 : pd.acc == kAccF32 ? kRedF32 : kRedF64, pd.acc,
                         RedCombineElem(pd.elem), launch);
-      CountLaunch();
       DB_CUDA(cudaGetLastError());
     }
     if (pd.citems[q] > 0) {
       const int grid = (int)std::min<int64_t>(pd.citems[q], cap);
-      ProfScope ps_("reduce_combine", stream);
       const auto launch = [&](auto, auto a, auto e) {
-        reduce_combine_kernel<decltype(a), decltype(e)::value><<<grid, kRedThreads, 0, stream>>>(d, n, pd.citems[q], f);
+        Launch("reduce_combine", reduce_combine_kernel<decltype(a), decltype(e)::value>, grid, kRedThreads, 0, stream, d, n, pd.citems[q], f);
       };
       red_dispatch(pd.acc == kAccI64 ? kRedI64 : pd.acc == kAccU64 ? kRedU64 : pd.acc == kAccF32 ? kRedF32 : kRedF64, pd.acc,
                    RedCombineElem(pd.elem), launch);
-      CountLaunch();
       DB_CUDA(cudaGetLastError());
     }
   }

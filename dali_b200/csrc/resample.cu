@@ -1258,14 +1258,13 @@ int dalib200ResampleLaunchPlanar(dalib200ResamplePlan *p, const dalib200PlanarIm
       DB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kPlSmemBytes));
       p->smem_opted[slot] = true;
     }
-    { ProfScope ps_("resample_planar", stream); kern<<<sgrid, kStThreads, kPlSmemBytes, stream>>>(dd, tb, di, nitems); }
+    Launch("resample_planar", kern, sgrid, kStThreads, kPlSmemBytes, stream, dd, tb, di, nitems);
     return DALIB200_SUCCESS;
   };
   if (wmax <= 2)      rc = slaunch(resample_planar_kernel<2>, 10);
   else if (wmax == 3) rc = slaunch(resample_planar_kernel<3>, 11);
   else                rc = slaunch(resample_planar_kernel<4>, 12);
   if (rc) return rc;
-  CountLaunch();
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH
@@ -1299,7 +1298,7 @@ int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, 
         DB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kStSmemBytes));
         p->smem_opted[slot] = true;
       }
-      { ProfScope ps_("resample_stream", stream); kern<<<sgrid, kStThreads, kStSmemBytes, stream>>>(dd, tb, di, nitems); }
+      Launch("resample_stream", kern, sgrid, kStThreads, kStSmemBytes, stream, dd, tb, di, nitems);
       return DALIB200_SUCCESS;
     };
     int wmax = 1;
@@ -1309,7 +1308,6 @@ int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, 
     else if (wmax == 3) rc = u8o ? slaunch(resample_stream_kernel<uint8_t, 3>, 6) : slaunch(resample_stream_kernel<float, 3>, 7);
     else                rc = u8o ? slaunch(resample_stream_kernel<uint8_t, 4>, 8) : slaunch(resample_stream_kernel<float, 4>, 9);
     if (rc) return rc;
-    CountLaunch();
     DB_CUDA(cudaGetLastError());
     if (nstream == p->n) return DALIB200_SUCCESS;
   }
@@ -1320,14 +1318,13 @@ int dalib200ResampleLaunch(dalib200ResamplePlan *p, const void *const *in_ptrs, 
       DB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
       p->smem_opted[slot] = true;
     }
-    { ProfScope ps_("resample_fused", stream); kern<<<grid, 256, smem, stream>>>(dd, tb, p->n, p->total_tiles); }
+    Launch("resample_fused", kern, grid, 256, smem, stream, dd, tb, p->n, p->total_tiles);
     return DALIB200_SUCCESS;
   };
   if (p->in_dtype == DALIB200_UINT8 && p->out_dtype == DALIB200_UINT8) rc = launch(resample_fused_kernel<uint8_t, uint8_t>, 0);
   else if (p->in_dtype == DALIB200_UINT8) rc = launch(resample_fused_kernel<uint8_t, float>, 1);
   else rc = launch(resample_fused_kernel<float, float>, 2);
   if (rc) return rc;
-  CountLaunch();
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

@@ -122,9 +122,7 @@ int dalib200Resample3DLaunch(dalib200Resample3DPlan *p, const void *const *in_pt
     if (stage_max[k] == 0) continue;
     const int64_t chunks = (stage_max[k] + kR3Threads - 1) / kR3Threads;
     const int gx = (int)std::min<int64_t>(chunks, std::max<int64_t>(1, (int64_t)NumSMs() * 8 / n) * 4);
-    ProfScope ps_("resample3d_pass", stream);
-    resample3d_pass_kernel<<<dim3(gx, n), kR3Threads, 0, stream>>>(dp + k, dt, 3);
-    CountLaunch();
+    Launch("resample3d_pass", resample3d_pass_kernel, dim3(gx, n), kR3Threads, 0, stream, dp + k, dt, 3);
     DB_CUDA(cudaGetLastError());
   }
   return DALIB200_SUCCESS;

@@ -65,16 +65,12 @@ int TiffStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   if (int rc = arena.Pack(s, std::tie(d_images, d_segs), images, segs)) return rc;
   const int nsegs = (int)segs.size();
   if (nsegs > 0) {
-    ProfScope ps_("tiff_segment", s);
     const SerialLanes g = SerialLaneGeometry(nsegs, kTiffMaxWorkers);
-    tiff_segment_kernel<<<g.warps, 32, 0, s>>>(d_images, d_segs, nsegs, g.lanes, in.d_raw, d_dec, d_slots, in.d_status);
-    CountLaunch();
+    Launch("tiff_segment", tiff_segment_kernel, g.warps, 32, 0, s, d_images, d_segs, nsegs, g.lanes, in.d_raw, d_dec, d_slots, in.d_status);
   }
   if (total_px > 0) {
     const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
-    ProfScope ps_("tiff_color", s);
-    tiff_color_kernel<<<grid, 256, 0, s>>>(d_images, (int)images.size(), total_px, d_segs, d_dec);
-    CountLaunch();
+    Launch("tiff_color", tiff_color_kernel, grid, 256, 0, s, d_images, (int)images.size(), total_px, d_segs, d_dec);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

@@ -527,25 +527,17 @@ int dalib200WarpLaunch(dalib200WarpPlan *p, const void *const *in_ptrs, void *co
       attr_set = true;
     }
     const int grid = (int)std::min<int64_t>(total_tiles, (int64_t)NumSMs() * 2);
-    ProfScope ps_(tma ? "warp_affine_tma" : "warp_affine_band", stream);
-    if (clampb) warp_affine_band_kernel<true><<<grid, 256, kBandSmem, stream>>>(dd, p->n, total_tiles, p->border, p->tmap, tma ? 1 : 0);
-    else warp_affine_band_kernel<false><<<grid, 256, kBandSmem, stream>>>(dd, p->n, total_tiles, p->border, p->tmap, tma ? 1 : 0);
-    CountLaunch();
+    Launch(tma ? "warp_affine_tma" : "warp_affine_band", clampb ? warp_affine_band_kernel<true> : warp_affine_band_kernel<false>, grid, 256, kBandSmem,
+           stream, dd, p->n, total_tiles, p->border, p->tmap, tma ? 1 : 0);
     DB_CUDA(cudaGetLastError());
     return DALIB200_SUCCESS;
   }
   const int grid = (int)std::min<int64_t>(total_tiles, (int64_t)NumSMs() * 16);
-  ProfScope ps_("warp_affine", stream);
-#define LAUNCH(O, L, Cc) warp_affine_kernel<O, L, Cc><<<grid, 256, 0, stream>>>(dd, p->n, total_tiles, p->border)
-  if (u8) {
-    if (lin) { if (clampb) LAUNCH(uint8_t, true, true); else LAUNCH(uint8_t, true, false); }
-    else     { if (clampb) LAUNCH(uint8_t, false, true); else LAUNCH(uint8_t, false, false); }
-  } else {
-    if (lin) { if (clampb) LAUNCH(float, true, true); else LAUNCH(float, true, false); }
-    else     { if (clampb) LAUNCH(float, false, true); else LAUNCH(float, false, false); }
-  }
-#undef LAUNCH
-  CountLaunch();
+  const auto kernel = u8 ? (lin ? (clampb ? warp_affine_kernel<uint8_t, true, true> : warp_affine_kernel<uint8_t, true, false>)
+                                : (clampb ? warp_affine_kernel<uint8_t, false, true> : warp_affine_kernel<uint8_t, false, false>))
+                         : (lin ? (clampb ? warp_affine_kernel<float, true, true> : warp_affine_kernel<float, true, false>)
+                                : (clampb ? warp_affine_kernel<float, false, true> : warp_affine_kernel<float, false, false>));
+  Launch("warp_affine", kernel, grid, 256, 0, stream, dd, p->n, total_tiles, p->border);
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;
 } DB_API_CATCH

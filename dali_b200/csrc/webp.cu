@@ -78,19 +78,13 @@ int WebpStage::Enqueue(const StageInputs &in, cudaStream_t s) {
   const WebpImage *d_images;
   if (int rc = arena.Pack(s, std::tie(d_images), images)) return rc;
   const int nimages = (int)images.size();
-  {
-    const SerialLanes g = SerialLaneGeometry(nimages, 1 << 30);
-    ProfScope ps_("webp_entropy", s);
-    webp_entropy_kernel<<<g.warps, 32, 0, s>>>(d_images, nimages, g.lanes, in.d_raw, d_scratch, in.d_status);
-  }
-  { ProfScope ps_("webp_recon", s); webp_wave_kernel<false><<<nimages, kWebpWaveThreads, 0, s>>>(d_images, d_scratch, in.d_status); }
-  { ProfScope ps_("webp_filter", s); webp_wave_kernel<true><<<nimages, kWebpWaveThreads, 0, s>>>(d_images, d_scratch, in.d_status); }
-  CountLaunch(3);
+  const SerialLanes g = SerialLaneGeometry(nimages, 1 << 30);
+  Launch("webp_entropy", webp_entropy_kernel, g.warps, 32, 0, s, d_images, nimages, g.lanes, in.d_raw, d_scratch, in.d_status);
+  Launch("webp_recon", webp_wave_kernel<false>, nimages, kWebpWaveThreads, 0, s, d_images, d_scratch, in.d_status);
+  Launch("webp_filter", webp_wave_kernel<true>, nimages, kWebpWaveThreads, 0, s, d_images, d_scratch, in.d_status);
   if (total_px > 0) {
     const int grid = (int)std::min<int64_t>((total_px + 255) / 256, (int64_t)NumSMs() * 16);
-    ProfScope ps_("webp_color", s);
-    webp_color_kernel<<<grid, 256, 0, s>>>(d_images, nimages, total_px, d_scratch);
-    CountLaunch();
+    Launch("webp_color", webp_color_kernel, grid, 256, 0, s, d_images, nimages, total_px, d_scratch);
   }
   DB_CUDA(cudaGetLastError());
   return DALIB200_SUCCESS;

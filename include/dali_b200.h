@@ -44,7 +44,7 @@ enum {
 
 const char *dalib200GetLastError(void);
 int dalib200GetVersion(void);
-/* number of kernels this library has launched from the calling process (bench.py's gpu_launches) */
+/* number of kernels this library has launched from the calling process, one per launch (bench.py's gpu_launches) */
 uint64_t dalib200GetLaunchCount(void);
 /* Per-launch device timing with CUDA events on the launching stream (off by default).  Collect synchronises,
  * returns the records in launch order and clears the log. */
