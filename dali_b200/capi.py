@@ -53,6 +53,7 @@ EXPORTS = [
     "dalib200PermutePlanGetPaths",
     "dalib200ReducePlanCreate", "dalib200ReducePlanDestroy", "dalib200ReduceSetup", "dalib200ReduceLaunch", "dalib200ReducePlanGetPaths",
     "dalib200EqualizePlanCreate", "dalib200EqualizePlanDestroy", "dalib200EqualizeSetup", "dalib200EqualizeLaunch",
+    "dalib200FilterPlanCreate", "dalib200FilterPlanDestroy", "dalib200FilterSetup", "dalib200FilterLaunch",
 ]
 
 

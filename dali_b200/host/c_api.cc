@@ -262,4 +262,25 @@ int dalihTestEqualize(int in_type, int n, int ndim, const int64_t *in_shapes, co
   API_END
 }
 
+// Test hook (CPU): fn.experimental.filter's argument, type, layout and shape rules without a device -- the argument resolution and the
+// plan set-up the operator makes.  anchors: n x nanchor values of `anchor` per sample; dtype -1: none; fill_type -1: no input 2.
+// out_shapes: n x ndim.
+int dalihTestFilter(int in_type, int dtype, int n, int ndim, const int64_t *in_shapes, const char *layout, int filter_type, int filter_ndim,
+                    const int64_t *filter_shapes, const int32_t *anchors, int nanchor, const char *border, const char *mode, int fill_type,
+                    const int64_t *fill_counts, int64_t *out_shapes) {
+  API_BEGIN
+  OpSpec spec("experimental__Filter");
+  spec.AddArg("border", MakeArg(std::string(border))).AddArg("mode", MakeArg(std::string(mode)));
+  const FilterArgs a = FilterResolveArgs(spec);
+  std::vector<int32_t> rc2((size_t)n * 2);
+  for (int i = 0; i < n; i++) FilterAnchor(i, std::vector<int>(anchors + (size_t)i * nanchor, anchors + (size_t)(i + 1) * nanchor), rc2.data() + 2 * i);
+  dalib200FilterPlan *plan = nullptr;
+  PermuteSetupOrThrow(dalib200FilterPlanCreate(&plan, std::max(n, 1)));
+  const int rc = dalib200FilterSetup(plan, in_type, dtype, n, ndim, in_shapes, layout, filter_type, filter_ndim, filter_shapes, rc2.data(),
+                                     a.border, a.mode, fill_type, fill_counts, out_shapes);
+  dalib200FilterPlanDestroy(plan);
+  PermuteSetupOrThrow(rc);
+  API_END
+}
+
 }  // extern "C"

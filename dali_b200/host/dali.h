@@ -462,6 +462,14 @@ int ReduceOpOf(const std::string &schema);
 // StdDev / Variance: the mean of sample i must have the output's shape, with or without the reduced axes as unit axes
 void ReduceCheckMean(const char *name, int i, const int64_t *mean_shape, int mean_ndim, const int64_t *in_shape, int ndim, uint32_t mask);
 
+// fn.experimental.filter: `border` and `mode` as DALIB200_FILTER_* codes; FilterAnchor: the (row, column) anchor of sample i from
+// the values of `anchor` (one per filter axis, or [-1]).  Throw on bad arguments.
+struct FilterArgs {
+  int border = 0, mode = 0;
+};
+FilterArgs FilterResolveArgs(const OpSpec &spec);
+void FilterAnchor(int i, const std::vector<int> &vals, int32_t *row_col);
+
 template <typename Backend>
 class Operator : public OperatorBase {
  public:

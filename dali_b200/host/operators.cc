@@ -2515,6 +2515,108 @@ class EqualizeGPU : public Operator<GPUBackend> {
 };
 DALI_REGISTER_OPERATOR(experimental__Equalize, EqualizeGPU, GPU);
 
+// =============================================================================================== experimental.Filter
+// dali/operators/image/convolution/filter (the reference's documented behaviour, DESIGN.md section 2): every frame of every sample is
+// correlated with its sample's 2-D float filter, channels independently, by the batched kernel of csrc/filter.cu.  Input 1 holds the
+// filters, optional input 2 the fill values of border="constant"; both may be CPU or GPU inputs.
+DALI_SCHEMA(experimental__Filter)
+    .DocStr("Correlates each image (HW, HWC and their sequences FHW, FHWC) with its sample's 2-D float filter (input 1); "
+            "input 2, optional, is the fill value of border=\"constant\" (one per sample, or one per frame of a sequence).")
+    .NumInput(2, 3).NumOutput(1).AllowSequences()
+    .AddOptionalArg("anchor", "Position of the filter over the output point: one value per filter axis (row, column), or [-1] for "
+                    "the centre (extent // 2).  Ignored in \"valid\" mode.", std::vector<int>{-1}, true)
+    .AddOptionalArg("border", "Values beyond the edges: reflect_101, reflect_1001, wrap, clamp or constant.", std::string("reflect_101"))
+    .AddOptionalArg("mode", "same (the output has the input's shape) or valid (each spatial extent becomes n - f + 1).", std::string("same"))
+    .AddOptionalArgNoDefault("dtype", "The output type: the input's type (default) or FLOAT.");
+
+FilterArgs FilterResolveArgs(const OpSpec &spec) {
+  static const char *const borders[] = { "reflect_101", "reflect_1001", "wrap", "clamp", "constant" };
+  FilterArgs a;
+  const std::string b = spec.GetArgument<std::string>("border"), m = spec.GetArgument<std::string>("mode");
+  a.border = -1;
+  for (int k = 0; k < 5; k++)
+    if (b == borders[k]) a.border = k;
+  DALI_ENFORCE(a.border >= 0, "experimental.Filter: unknown border \"", b, "\"; expected reflect_101, reflect_1001, wrap, clamp or constant");
+  DALI_ENFORCE(m == "same" || m == "valid", "experimental.Filter: unknown mode \"", m, "\"; expected same or valid");
+  a.mode = m == "same" ? DALIB200_FILTER_SAME : DALIB200_FILTER_VALID;
+  return a;
+}
+
+void FilterAnchor(int i, const std::vector<int> &vals, int32_t *row_col) {
+  DALI_ENFORCE(vals.size() == 2 || (vals.size() == 1 && vals[0] == -1), "experimental.Filter: sample ", i, ": anchor must have one "
+               "value per filter axis (2), or be [-1]; got ", vals.size(), " values");
+  row_col[0] = vals[0];
+  row_col[1] = vals.size() == 2 ? vals[1] : -1;
+}
+
+class FilterGPU : public Operator<GPUBackend> {
+ public:
+  explicit FilterGPU(const OpSpec &spec) : Operator<GPUBackend>(spec), args_(FilterResolveArgs(spec)) {
+    dtype_ = spec.HasArgument("dtype") ? spec.GetArgument<int>("dtype") : -1;
+    DALI_ENFORCE(!spec.HasArgument("dtype") || dtype_ >= 0, "experimental.Filter: invalid dtype ", dtype_);
+  }
+
+ protected:
+  // the type, sample count and per-sample shapes of input k, which may be a CPU or a GPU input
+  template <typename F> void ForInput(const Workspace &ws, int k, F &&f) const {
+    if (ws.InputIsType(k, true)) f(ws.Input<GPUBackend>(k));
+    else f(ws.Input<CPUBackend>(k));
+  }
+
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    const int n = in.num_samples(), nd = in.shape().sample_dim();
+    std::vector<int64_t> is((size_t)n * nd), os((size_t)n * nd), fs, counts(n, 0);
+    for (int i = 0; i < n; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
+    int ftype = 0, fnd = 0, vtype = -1;
+    ForInput(ws, 1, [&](const auto &f) {
+      DALI_ENFORCE(f.num_samples() == n, "experimental.Filter: input 1 (the filter) has ", f.num_samples(), " samples, input 0 has ", n);
+      ftype = static_cast<int>(f.type());
+      fnd = f.sample_dim();
+      fs.assign((size_t)n * 2, 0);
+      for (int i = 0; i < n && fnd == 2; i++) std::copy(f.tensor_shape_span(i), f.tensor_shape_span(i) + 2, fs.begin() + (size_t)i * 2);
+    });
+    if (ws.NumInput() > 2)
+      ForInput(ws, 2, [&](const auto &v) {
+        DALI_ENFORCE(v.num_samples() == n, "experimental.Filter: input 2 (fill_value) has ", v.num_samples(), " samples, input 0 has ", n);
+        vtype = static_cast<int>(v.type());
+        for (int i = 0; i < n; i++) counts[i] = v.shape().tensor_size(i);
+      });
+    std::vector<int32_t> anchors((size_t)n * 2);
+    for (int i = 0; i < n; i++) {
+      std::vector<int> vals;
+      for (float v : spec_.GetFloatVecArgument("anchor", &ws, i)) vals.push_back(static_cast<int>(v));
+      FilterAnchor(i, vals, anchors.data() + (size_t)i * 2);
+    }
+    plan_.Ensure(n, "experimental.Filter");
+    if (dalib200FilterSetup(plan_.get(), static_cast<int>(in.type()), dtype_, n, nd, is.data(), in.GetLayout().str().c_str(), ftype, fnd,
+                            fs.data(), anchors.data(), args_.border, args_.mode, vtype, counts.data(), os.data()))
+      throw DALIException(dalib200GetLastError());
+    out.resize(1);
+    out[0].type = static_cast<DALIDataType>(dtype_ < 0 ? static_cast<int>(in.type()) : dtype_);
+    out[0].shape.resize(n, nd);
+    for (int i = 0; i < n; i++) out[0].shape.set_tensor_shape(i, TensorShape(os.begin() + (size_t)i * nd, os.begin() + (size_t)(i + 1) * nd));
+    return true;
+  }
+
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(in.GetLayout());
+    std::vector<const void *> filters, fills;
+    ForInput(ws, 1, [&](const auto &f) { filters = InPtrs(f); });
+    if (ws.NumInput() > 2) ForInput(ws, 2, [&](const auto &v) { fills = InPtrs(v); });
+    CheckStatus(dalib200FilterLaunch(plan_.get(), InPtrs(in).data(), filters.data(), ws.InputIsType(1, true), fills.empty() ? nullptr : fills.data(),
+                                     ws.NumInput() > 2 && ws.InputIsType(2, true), OutPtrs(out).data(), ws.stream()),
+                "experimental.Filter");
+  }
+
+  DALIB200_PLAN(Filter) plan_{max_batch_size_};
+  FilterArgs args_;
+  int dtype_ = -1;
+};
+DALI_REGISTER_OPERATOR(experimental__Filter, FilterGPU, GPU);
+
 // =============================================================================================== Rotate
 // dali/operators/image/remap/rotate.cc + rotate_params.h: a WarpAffine whose matrix is
 // translation(in / 2) * rotation2D(-a) * translation(-out / 2) with a = deg2rad(-angle) (counter-clockwise for a top-left origin)

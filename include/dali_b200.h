@@ -546,6 +546,36 @@ int dalib200EqualizeSetup(dalib200EqualizePlan *plan, int in_type, int n, int nd
 int dalib200EqualizeLaunch(dalib200EqualizePlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * fn.experimental.filter (the reference's experimental.Filter): 2-D correlation of images and sequences with one float32 filter per
+ * sample, out[y][x][c] = sum_r sum_s f[r][s] in[y + r - a_r][x + s - a_s][c], channels independent, every frame of a sequence with its
+ * sample's filter (DESIGN.md section 2).  One launch per batch (DESIGN.md section 5).  Each output is one float32 fmaf chain in a fixed
+ * order (filter rows outer), so it is the same alone or in any batch.
+ *   in_type         DALIDataType code of the data: UINT8, INT8, UINT16, INT16, FLOAT16 or FLOAT
+ *   out_type        the input's type or FLOAT; -1: the input's type.  ConvertSat: half away from zero, saturating, NaN -> 0
+ *   in_shapes       n x ndim; out_shapes (n x ndim) receives the output shapes
+ *   layout          HW, HWC, FHW or FHWC; "" or NULL: HW, HWC or FHWC by rank (2, 3, 4)
+ *   filter_type / filter_ndim / filter_shapes   FLOAT, 2, n x 2: each extent 1 to 255
+ *   anchors         NULL or n x 2 (row, column): -1 for extent / 2, else in [0, extent - 1]; ignored in DALIB200_FILTER_VALID
+ *   border, mode    DALIB200_FILTER_BORDER_*, DALIB200_FILTER_SAME / VALID (each spatial extent n - f + 1)
+ *   fill_type       -1 without fill values, else the input's type; fill_counts: n, 1 value or (sequences) one per frame; the fill
+ *                   value is read only with DALIB200_FILTER_BORDER_CONSTANT (0 without fill values)
+ * 1 to 64 channels, at most 2^31 - 1 elements in one frame.  A type, layout, shape or argument that does not fit fails with
+ * DALIB200_ERROR_INVALID_ARGUMENT and a message naming the sample.  Launch: in_ptrs, out_ptrs: n device buffers aligned to their
+ * element size (else DALIB200_ERROR_INVALID_ARGUMENT); filters, fills: n pointers, in device memory (read in place) when *_on_device, else in host memory (uploaded with the
+ * descriptors); fills may be NULL when the set-up had no fill values. */
+enum { DALIB200_FILTER_BORDER_REFLECT_101 = 0, DALIB200_FILTER_BORDER_REFLECT_1001 = 1, DALIB200_FILTER_BORDER_WRAP = 2,
+       DALIB200_FILTER_BORDER_CLAMP = 3, DALIB200_FILTER_BORDER_CONSTANT = 4 };
+enum { DALIB200_FILTER_SAME = 0, DALIB200_FILTER_VALID = 1 };
+typedef struct dalib200FilterPlan dalib200FilterPlan;
+int dalib200FilterPlanCreate(dalib200FilterPlan **plan, int max_samples);
+int dalib200FilterPlanDestroy(dalib200FilterPlan *plan);
+int dalib200FilterSetup(dalib200FilterPlan *plan, int in_type, int out_type, int n, int ndim, const int64_t *in_shapes, const char *layout,
+                        int filter_type, int filter_ndim, const int64_t *filter_shapes, const int32_t *anchors, int border, int mode,
+                        int fill_type, const int64_t *fill_counts, int64_t *out_shapes);
+int dalib200FilterLaunch(dalib200FilterPlan *plan, const void *const *in_ptrs, const void *const *filters, int filters_on_device,
+                         const void *const *fills, int fills_on_device, void *const *out_ptrs, dalib200Stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Audio decode (fn.decoders.audio).  WAV (PCM 8 / 16 / 24 / 32-bit, IEEE float 32, WAVE_FORMAT_EXTENSIBLE with either) and native FLAC
  * (8 / 16 / 24 bits per sample, optional ID3v2 tag in front), detected from the bytes.  The host parses the container and STREAMINFO
  * only; the FLAC frames are found, checked (CRC-8, CRC-16, frame chain) and decoded on the device.  Samples read as libsndfile's

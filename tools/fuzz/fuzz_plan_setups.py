@@ -16,6 +16,7 @@ jd_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 1]
 pe_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 2])
 red_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 3])
 eq_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 4])
+flt_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 5])
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
 L = capi.lib()
 MILD = float(os.environ.get("FUZZ_BAD_SCALE", "1"))      # < 1: fewer adversarial values per call -> more set-ups reach their deep paths
@@ -70,6 +71,8 @@ red_plan = C.c_void_p()
 capi.check(L.dalib200ReducePlanCreate(C.byref(red_plan), 8))
 eq_plan = C.c_void_p()
 capi.check(L.dalib200EqualizePlanCreate(C.byref(eq_plan), 8))
+flt_plan = C.c_void_p()
+capi.check(L.dalib200FilterPlanCreate(C.byref(flt_plan), 8))
 for it in range(N):
     n = int(rng.integers(0, 9)) if rng.random() < 0.9 else int(rng.choice([9, 100, -1]))
     m = max(n, 1) if n < 64 else 8
@@ -305,5 +308,32 @@ for it in range(N):
     note("equalize", rc)
     if rc == 0 and all(0 <= e < 2 ** 20 for e in ext) and np.prod([max(e, 1) for e in ext], dtype=np.float64) < 2 ** 26:
         launch("equalize", L.dalib200EqualizeLaunch, eq_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
+    rng = main_rng
+    # ---- filter: a generator of its own.  Zero, negative and 2^31-sized extents, filter extents of 0 and above 255, anchors outside the
+    # filter, more channels than the limit, layouts of the wrong rank, channel-first or unknown, invalid type, border and mode codes,
+    # fill values of the wrong count; the launch takes host filters and fill values (they are copied) or fake device ones
+    rng, main_rng = flt_rng, rng
+    lay = [b"", b"HW", b"HWC", b"FHW", b"FHWC", b"CHW", b"DHWC", b"HWCC"][int(rng.integers(0, 8))]
+    nd = small(0, 6) if rng.random() < 0.1 * MILD or not lay else len(lay)
+    nd_alloc = nd if 0 < nd <= 8 else 1
+    ext = [int(rng.choice([0, 1, -1, 65, 2 ** 31, 2 ** 31 - 1, 2 ** 40])) if rng.random() < 0.08 * MILD else int(rng.integers(1, 40))
+           for _ in range(m * nd_alloc)]
+    fext = [int(rng.choice([0, -1, 256, 2 ** 31])) if rng.random() < 0.05 * MILD else int(rng.integers(1, 9)) for _ in range(2 * m)]
+    anc = [int(rng.choice([-2, 9, 2 ** 31 - 1])) if rng.random() < 0.05 * MILD else int(rng.integers(-1, 3)) for _ in range(2 * m)]
+    cnt = [int(rng.choice([0, 2, -1, 2 ** 40])) if rng.random() < 0.05 * MILD else 1 for _ in range(m)]
+    ft = code([-1, -1, 0, 1, 9])
+    osh = (C.c_int64 * (m * nd_alloc))()
+    rc = L.dalib200FilterSetup(flt_plan, code([0, 4, 1, 5, 8, 9, 2, 11]), code([-1, -1, 9, 0, 5]), n, nd, (C.c_int64 * len(ext))(*ext), lay,
+                               code([9, 9, 10]), code([2, 2, 3]), (C.c_int64 * len(fext))(*fext), (C.c_int32 * len(anc))(*anc),
+                               code(range(5)), code([0, 1]), ft, (C.c_int64 * len(cnt))(*cnt), osh)
+    note("filter", rc)
+    if rc == 0 and all(0 <= e < 2 ** 20 for e in ext) and np.prod([max(e, 1) for e in ext], dtype=np.float64) < 2 ** 26:
+        taps = [np.zeros(max(1, fext[2 * i] * fext[2 * i + 1]), np.float32) for i in range(m)]
+        fills = [np.zeros(64, np.uint8) for _ in range(m)]
+        host = rng.random() < 0.5
+        fptrs = (C.c_void_p * m)(*[t.ctypes.data for t in taps]) if host else fake_ptrs(m, 0x9000000000)
+        vptrs = (C.c_void_p * m)(*[v.ctypes.data for v in fills]) if host else fake_ptrs(m, 0xA000000000)
+        launch("filter", L.dalib200FilterLaunch, flt_plan, fake_ptrs(m, 0x10000000), fptrs, int(not host), vptrs if ft >= 0 else None,
+               int(not host), fake_ptrs(m, 0x7000000000), None)
     rng = main_rng
 print("seed", sys.argv[1] if len(sys.argv) > 1 else 0, "iterations", N, "- no sanitizer report;", {f"{k[0]}:{k[1]}": v for k, v in sorted(hist.items())})
