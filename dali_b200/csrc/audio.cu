@@ -774,13 +774,14 @@ static int SpectrogramLaunchImpl(dalib200SpectrogramPlan *p, const void *const *
   static const bool radix2_only = getenv("DALIB200_STFT_RADIX2") != nullptr;
   if (P.nfft == 1024 && (!radix2_only || mel)) {
     // register-resident 32 x 32 FFT, one warp per pair of frames (16 frames per CTA = the grouping the descriptors were built with)
-    static bool attr_set = false;
-    if (!attr_set) {
+    // the shared-memory attribute belongs to the kernel on the current device, so it is set once per PLAN, not once per process: a
+    // plan's descriptor arena lives on the device it was created on, and a process running on two devices has a plan on each
+    if (!p->smem_set) {
       DB_CUDA(cudaFuncSetAttribute(spectrogram1024_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF1024Smem));
       DB_CUDA(cudaFuncSetAttribute(spectrogram1024_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF1024Smem));
       DB_CUDA(cudaFuncSetAttribute(spectrogram1024_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF1024Smem));
       DB_CUDA(cudaFuncSetAttribute(spectrogram1024_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kF1024Smem));
-      attr_set = true;
+      p->smem_set = true;
     }
     const int grid = (int)std::min<int64_t>(p->total_groups, (int64_t)NumSMs() * 2);
     MelTables mt{};

@@ -380,6 +380,7 @@ struct dalib200WarpPlan {
   CUtensorMap tmap;
   const void *tmap_base = nullptr; size_t tmap_stride = 0; int tmap_h = 0, tmap_w = 0, tmap_n = 0;
   int path = 0;                  // last launch: 0 generic kernel, 1 band kernel with tensor-map TMA boxes, 2 band kernel without
+  bool smem_set = false;         // the band kernel's dynamic shared-memory attribute is set (on this plan's device)
 };
 
 namespace {
@@ -520,11 +521,12 @@ int dalib200WarpLaunch(dalib200WarpPlan *p, const void *const *in_ptrs, void *co
   const auto *dd = reinterpret_cast<const WarpDesc *>(p->arena.dev);
   const bool lin = p->interp == 1, clampb = !p->use_fill, u8 = p->out_dtype == DALIB200_UINT8;
   if (band) {
-    static bool attr_set = false;
-    if (!attr_set) {
+    // the shared-memory attribute belongs to the kernel on the current device, so it is set once per PLAN, not once per process: a
+    // plan's descriptor arena lives on the device it was created on, and a process warping on two devices has a plan on each
+    if (!p->smem_set) {
       DB_CUDA(cudaFuncSetAttribute(warp_affine_band_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBandSmem));
       DB_CUDA(cudaFuncSetAttribute(warp_affine_band_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBandSmem));
-      attr_set = true;
+      p->smem_set = true;
     }
     const int grid = (int)std::min<int64_t>(total_tiles, (int64_t)NumSMs() * 2);
     Launch(tma ? "warp_affine_tma" : "warp_affine_band", clampb ? warp_affine_band_kernel<true> : warp_affine_band_kernel<false>, grid, 256, kBandSmem,
