@@ -54,6 +54,7 @@ EXPORTS = [
     "dalib200ReducePlanCreate", "dalib200ReducePlanDestroy", "dalib200ReduceSetup", "dalib200ReduceLaunch", "dalib200ReducePlanGetPaths",
     "dalib200EqualizePlanCreate", "dalib200EqualizePlanDestroy", "dalib200EqualizeSetup", "dalib200EqualizeLaunch",
     "dalib200FilterPlanCreate", "dalib200FilterPlanDestroy", "dalib200FilterSetup", "dalib200FilterLaunch",
+    "dalib200ErasePlanCreate", "dalib200ErasePlanDestroy", "dalib200EraseSetup", "dalib200EraseLaunch",
 ]
 
 

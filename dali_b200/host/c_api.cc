@@ -283,4 +283,30 @@ int dalihTestFilter(int in_type, int dtype, int n, int ndim, const int64_t *in_s
   API_END
 }
 
+// Test hook (CPU): fn.erase's argument, type, layout, region and fill rules without a device -- the argument resolution and the plan
+// set-up the operator makes.  Arguments left unset: axis_names NULL, naxes -1, normalized* -1, nfill -1.  anchors / region_shapes:
+// every sample's values back to back, anchor_counts / shape_counts per sample.
+int dalihTestErase(int type, int n, int ndim, const int64_t *shapes, const char *layout, const char *axis_names, const int32_t *axes, int naxes,
+                   const float *anchors, const int64_t *anchor_counts, const float *region_shapes, const int64_t *shape_counts, int normalized,
+                   int normalized_anchor, int normalized_shape, int centered_anchor, const float *fill, int nfill) {
+  API_BEGIN
+  OpSpec spec("Erase");
+  if (axis_names) spec.AddArg("axis_names", MakeArg(std::string(axis_names)));
+  if (naxes >= 0) spec.AddArg("axes", MakeArg(std::vector<int>(axes, axes + naxes)));
+  if (normalized >= 0) spec.AddArg("normalized", MakeArg(normalized != 0));
+  if (normalized_anchor >= 0) spec.AddArg("normalized_anchor", MakeArg(normalized_anchor != 0));
+  if (normalized_shape >= 0) spec.AddArg("normalized_shape", MakeArg(normalized_shape != 0));
+  spec.AddArg("centered_anchor", MakeArg(centered_anchor != 0));
+  if (nfill >= 0) spec.AddArg("fill_value", MakeArg(std::vector<float>(fill, fill + nfill)));
+  const EraseArgs a = EraseResolveArgs(spec, layout ? layout : "");
+  dalib200ErasePlan *plan = nullptr;
+  PermuteSetupOrThrow(dalib200ErasePlanCreate(&plan, std::max(n, 1)));
+  const int rc = dalib200EraseSetup(plan, type, n, ndim, shapes, layout, a.by_name ? a.axis_names.c_str() : nullptr, a.axes.data(),
+                                    (int)a.axes.size(), anchors, anchor_counts, region_shapes, shape_counts, a.norm_anchor, a.norm_shape,
+                                    a.centered, a.fill.data(), (int)a.fill.size());
+  dalib200ErasePlanDestroy(plan);
+  PermuteSetupOrThrow(rc);
+  API_END
+}
+
 }  // extern "C"

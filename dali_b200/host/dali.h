@@ -470,6 +470,17 @@ struct FilterArgs {
 FilterArgs FilterResolveArgs(const OpSpec &spec);
 void FilterAnchor(int i, const std::vector<int> &vals, int32_t *row_col);
 
+// fn.erase: the erased axes -- axis_names when given, else axes when given, else "HW" for an input with a layout and axes' default
+// [1, 0] for one without -- the coordinate flags (normalized_anchor / normalized_shape override normalized) and the fill values.
+struct EraseArgs {
+  bool by_name = false;
+  std::string axis_names;
+  std::vector<int32_t> axes;
+  int norm_anchor = 0, norm_shape = 0, centered = 0;
+  std::vector<float> fill;
+};
+EraseArgs EraseResolveArgs(const OpSpec &spec, const std::string &layout);
+
 template <typename Backend>
 class Operator : public OperatorBase {
  public:

@@ -2617,6 +2617,79 @@ class FilterGPU : public Operator<GPUBackend> {
 };
 DALI_REGISTER_OPERATOR(experimental__Filter, FilterGPU, GPU);
 
+// =============================================================================================== Erase
+// dali/operators/erase (the reference's documented arguments, DESIGN.md section 2): the regions given by anchor and shape along the
+// erased axes are filled with fill_value and every other element is copied, by the batched kernel of csrc/erase.cu.
+DALI_SCHEMA(Erase)
+    .DocStr("Erases one or more rectangular regions of each sample: the elements inside them take fill_value, the others are copied. "
+            "Any layout of rank 1 to 6 and any type; the output has the input's shape, type and layout.")
+    .NumInput(1).NumOutput(1).AllowSequences()
+    .AddOptionalArg("anchor", "Region starts along the erased axes; several regions back to back, e.g. (y0, x0, y1, x1, ...) for "
+                    "axis_names=\"HW\".", std::vector<float>{}, true)
+    .AddOptionalArg("shape", "Region extents, laid out as anchor.", std::vector<float>{}, true)
+    .AddOptionalArg("axis_names", "The erased axes as layout characters; wins over axes when given.", std::string("HW"))
+    .AddOptionalArg("axes", "The erased axes as dimension indices.", std::vector<int>{1, 0})
+    .AddOptionalArg("normalized", "anchor and shape are fractions of each axis's extent.", false)
+    .AddOptionalArgNoDefault("normalized_anchor", "anchor is a fraction of each axis's extent (overrides normalized).")
+    .AddOptionalArgNoDefault("normalized_shape", "shape is a fraction of each axis's extent (overrides normalized).")
+    .AddOptionalArg("centered_anchor", "The anchor is the centre of the region, not its start.", false)
+    .AddOptionalArg("fill_value", "One value, or one per channel of a C axis that is not erased.", std::vector<float>{0.0f});
+
+EraseArgs EraseResolveArgs(const OpSpec &spec, const std::string &layout) {
+  EraseArgs a;
+  a.by_name = spec.HasArgument("axis_names") || (!spec.HasArgument("axes") && !layout.empty());
+  if (a.by_name) a.axis_names = spec.GetArgument<std::string>("axis_names");
+  else for (int v : spec.GetRepeatedArgument<int>("axes")) a.axes.push_back(v);
+  const bool norm = spec.GetArgument<bool>("normalized");
+  a.norm_anchor = spec.HasArgument("normalized_anchor") ? spec.GetArgument<bool>("normalized_anchor") : norm;
+  a.norm_shape = spec.HasArgument("normalized_shape") ? spec.GetArgument<bool>("normalized_shape") : norm;
+  a.centered = spec.GetArgument<bool>("centered_anchor");
+  a.fill = spec.GetRepeatedArgument<float>("fill_value");
+  return a;
+}
+
+class EraseGPU : public Operator<GPUBackend> {
+ public:
+  explicit EraseGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
+
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    const int n = in.num_samples(), nd = in.shape().sample_dim();
+    const std::string layout = in.GetLayout().str();
+    const EraseArgs a = EraseResolveArgs(spec_, layout);
+    std::vector<int64_t> is((size_t)n * nd), na(n), ns(n);
+    std::vector<float> anchors, shapes;
+    for (int i = 0; i < n; i++) {
+      std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + nd, is.begin() + (size_t)i * nd);
+      const std::vector<float> av = spec_.GetFloatVecArgument("anchor", &ws, i), sv = spec_.GetFloatVecArgument("shape", &ws, i);
+      na[i] = (int64_t)av.size();
+      ns[i] = (int64_t)sv.size();
+      anchors.insert(anchors.end(), av.begin(), av.end());
+      shapes.insert(shapes.end(), sv.begin(), sv.end());
+    }
+    plan_.Ensure(n, "erase");
+    if (dalib200EraseSetup(plan_.get(), static_cast<int>(in.type()), n, nd, is.data(), layout.c_str(),
+                           a.by_name ? a.axis_names.c_str() : nullptr, a.axes.data(), (int)a.axes.size(), anchors.data(), na.data(),
+                           shapes.data(), ns.data(), a.norm_anchor, a.norm_shape, a.centered, a.fill.data(), (int)a.fill.size()))
+      throw DALIException(dalib200GetLastError());
+    out.resize(1);
+    out[0].type = in.type();
+    out[0].shape = in.shape();
+    return true;
+  }
+
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(in.GetLayout());
+    CheckStatus(dalib200EraseLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), "erase");
+  }
+
+  DALIB200_PLAN(Erase) plan_{max_batch_size_};
+};
+DALI_REGISTER_OPERATOR(Erase, EraseGPU, GPU);
+
 // =============================================================================================== Rotate
 // dali/operators/image/remap/rotate.cc + rotate_params.h: a WarpAffine whose matrix is
 // translation(in / 2) * rotation2D(-a) * translation(-out / 2) with a = deg2rad(-angle) (counter-clockwise for a top-left origin)

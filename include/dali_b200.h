@@ -576,6 +576,30 @@ int dalib200FilterLaunch(dalib200FilterPlan *plan, const void *const *in_ptrs, c
                          const void *const *fills, int fills_on_device, void *const *out_ptrs, dalib200Stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * fn.erase: rectangular regions of each sample filled with a value (or one value per channel), every other element copied bit for
+ * bit; the output has the input's shape, type and layout (DESIGN.md section 2).  One launch per batch (DESIGN.md section 5).
+ *   type            any of the 12 DALIDataType codes
+ *   shapes          n x ndim, ndim 1 to 6; layout: ndim distinct characters, or "" / NULL
+ *   axis_names      the erased axes as layout characters (needs a layout), or NULL to take axes: naxes dimension indices
+ *   anchors, region_shapes   the region values of all samples back to back, anchor_counts / shape_counts of them per sample; a
+ *                   sample's two counts are equal and a multiple of the number of erased axes (0: no region), laid out region by
+ *                   region in the order of the erased axes
+ *   normalized_anchor, normalized_shape   values are fractions of each axis's extent; centered_anchor: the anchor is the centre
+ *   fill, nfill     one value, or one per channel of a C axis that is not erased; converted with ConvertSat
+ * Per axis, in double precision: a, s scaled if normalised; a -= s / 2 if centred; [llround(a), llround(a + s)) clipped to the
+ * extent.  A type, layout, axis, region or fill that does not fit fails with DALIB200_ERROR_INVALID_ARGUMENT and a message naming the
+ * sample and the argument.  Launch: in_ptrs, out_ptrs: n device buffers aligned to their element size (else
+ * DALIB200_ERROR_INVALID_ARGUMENT); no launch when the batch has no elements. */
+typedef struct dalib200ErasePlan dalib200ErasePlan;
+int dalib200ErasePlanCreate(dalib200ErasePlan **plan, int max_samples);
+int dalib200ErasePlanDestroy(dalib200ErasePlan *plan);
+int dalib200EraseSetup(dalib200ErasePlan *plan, int type, int n, int ndim, const int64_t *shapes, const char *layout, const char *axis_names,
+                       const int32_t *axes, int naxes, const float *anchors, const int64_t *anchor_counts, const float *region_shapes,
+                       const int64_t *shape_counts, int normalized_anchor, int normalized_shape, int centered_anchor, const float *fill,
+                       int nfill);
+int dalib200EraseLaunch(dalib200ErasePlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Audio decode (fn.decoders.audio).  WAV (PCM 8 / 16 / 24 / 32-bit, IEEE float 32, WAVE_FORMAT_EXTENSIBLE with either) and native FLAC
  * (8 / 16 / 24 bits per sample, optional ID3v2 tag in front), detected from the bytes.  The host parses the container and STREAMINFO
  * only; the FLAC frames are found, checked (CRC-8, CRC-16, frame chain) and decoded on the device.  Samples read as libsndfile's

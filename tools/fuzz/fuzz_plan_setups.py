@@ -17,6 +17,7 @@ pe_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 2]
 red_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 3])
 eq_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 4])
 flt_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 5])
+er_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 6])
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
 L = capi.lib()
 MILD = float(os.environ.get("FUZZ_BAD_SCALE", "1"))      # < 1: fewer adversarial values per call -> more set-ups reach their deep paths
@@ -73,6 +74,8 @@ eq_plan = C.c_void_p()
 capi.check(L.dalib200EqualizePlanCreate(C.byref(eq_plan), 8))
 flt_plan = C.c_void_p()
 capi.check(L.dalib200FilterPlanCreate(C.byref(flt_plan), 8))
+er_plan = C.c_void_p()
+capi.check(L.dalib200ErasePlanCreate(C.byref(er_plan), 8))
 for it in range(N):
     n = int(rng.integers(0, 9)) if rng.random() < 0.9 else int(rng.choice([9, 100, -1]))
     m = max(n, 1) if n < 64 else 8
@@ -335,5 +338,28 @@ for it in range(N):
         vptrs = (C.c_void_p * m)(*[v.ctypes.data for v in fills]) if host else fake_ptrs(m, 0xA000000000)
         launch("filter", L.dalib200FilterLaunch, flt_plan, fake_ptrs(m, 0x10000000), fptrs, int(not host), vptrs if ft >= 0 else None,
                int(not host), fake_ptrs(m, 0x7000000000), None)
+    rng = main_rng
+    # ---- erase: a generator of its own.  Zero, negative and 2^31-sized extents, ranks 0-7, layouts of the wrong rank or with repeated
+    # axes, unknown or repeated axis names and indices, anchor / shape counts that differ or do not divide, non-finite, negative and
+    # huge region values, many regions, fill counts that do not match the channels; the launch runs the descriptor build
+    rng, main_rng = er_rng, rng
+    lay = [b"", b"HW", b"HWC", b"CHW", b"FHWC", b"ft", b"T", b"HWW", b"DHWC"][int(rng.integers(0, 9))]
+    nd = small(0, 8) if rng.random() < 0.1 * MILD or not lay else len(lay)
+    nd_alloc = nd if 0 < nd <= 8 else 1
+    ext = [int(rng.choice([0, -1, 2 ** 31, 2 ** 40])) if rng.random() < 0.05 * MILD else int(rng.integers(1, 40)) for _ in range(m * nd_alloc)]
+    names = [None, b"HW", b"WH", b"C", b"HWC", b"HX", b"HH", b"", b"ft", b"t"][int(rng.integers(0, 10))]
+    axes = [int(rng.choice([-1, 7, 0])) if rng.random() < 0.05 * MILD else int(rng.integers(0, max(nd, 1))) for _ in range(int(rng.integers(0, 4)))]
+    nax = max(1, len(names) if names is not None else len(axes))
+    counts = [nax * int(rng.choice([0, 1, 2, 64])) for _ in range(m)]
+    scounts = [c if rng.random() > 0.05 * MILD else c + 1 for c in counts]
+    vals = [flt(-5.0, 45.0) for _ in range(max(1, sum(max(a, b) for a, b in zip(counts, scounts))))]
+    fill = [flt() for _ in range(int(rng.choice([1, 1, 3, 0, 4])))]
+    rc = L.dalib200EraseSetup(er_plan, code(range(12)), n, nd, (C.c_int64 * len(ext))(*ext), lay, names, (C.c_int32 * max(1, len(axes)))(*axes),
+                              len(axes), (C.c_float * len(vals))(*vals), (C.c_int64 * m)(*counts), (C.c_float * len(vals))(*vals),
+                              (C.c_int64 * m)(*scounts), int(rng.integers(0, 2)), int(rng.integers(0, 2)), int(rng.integers(0, 2)),
+                              (C.c_float * max(1, len(fill)))(*fill), len(fill))
+    note("erase", rc)
+    if rc == 0:
+        launch("erase", L.dalib200EraseLaunch, er_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
     rng = main_rng
 print("seed", sys.argv[1] if len(sys.argv) > 1 else 0, "iterations", N, "- no sanitizer report;", {f"{k[0]}:{k[1]}": v for k, v in sorted(hist.items())})
