@@ -55,6 +55,7 @@ EXPORTS = [
     "dalib200EqualizePlanCreate", "dalib200EqualizePlanDestroy", "dalib200EqualizeSetup", "dalib200EqualizeLaunch",
     "dalib200FilterPlanCreate", "dalib200FilterPlanDestroy", "dalib200FilterSetup", "dalib200FilterLaunch",
     "dalib200ErasePlanCreate", "dalib200ErasePlanDestroy", "dalib200EraseSetup", "dalib200EraseLaunch",
+    "dalib200PastePlanCreate", "dalib200PastePlanDestroy", "dalib200PasteSetup", "dalib200PasteCanvasSetup", "dalib200PasteLaunch",
 ]
 
 

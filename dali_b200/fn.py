@@ -32,7 +32,7 @@ _INPUT_DEVICE = {"mixed": "cpu", "cpu": "cpu", "gpu": "gpu"}
 _SEEDED_SCHEMAS = ("decoders__ImageRandomCrop", "RandomResizedCrop")
 # operators all of whose inputs are data: any GPU input selects the GPU operator, and a CPU input is then moved with .gpu() wherever
 # it stands, not only as input 0
-_GPU_DATA_SCHEMAS = ("Cat", "Stack")
+_GPU_DATA_SCHEMAS = ("Cat", "Stack", "MultiPaste")
 
 
 def _make_wrapper(schema):

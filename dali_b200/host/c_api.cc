@@ -309,4 +309,32 @@ int dalihTestErase(int type, int n, int ndim, const int64_t *shapes, const char 
   API_END
 }
 
+// Test hook (CPU): fn.multi_paste's argument reading, type, layout, shape and region rules without a device -- the argument resolution
+// and the plan set-up the operator makes, every argument given as a list (the same for every sample).  NULL in_ids, region_args[a]
+// or output_size: not given; dtype -1: not given.  out_shapes: n x 3, written.
+int dalihTestMultiPaste(int in_type, int dtype, int ninputs, int n, const int *ndims, const char *const *layouts, const int64_t *in_shapes,
+                        const int64_t *in_ids, int nids, const double *const *region_args, const int *region_nvals, const int64_t *output_size,
+                        int64_t *out_shapes) {
+  API_BEGIN
+  static const char *const names[kMultiPasteRegionArgs] = { "in_anchors", "in_anchors_rel", "shapes", "shapes_rel", "out_anchors",
+                                                            "out_anchors_rel" };
+  OpSpec spec("MultiPaste");
+  if (dtype >= 0) spec.AddArg("dtype", MakeArg(dtype));
+  if (in_ids) spec.AddArg("in_ids", MakeArg(std::vector<int64_t>(in_ids, in_ids + nids)));
+  for (int r = 0; r < kMultiPasteRegionArgs; r++) {
+    if (!region_args[r]) continue;
+    ArgValue a = MakeArg(std::vector<float>(region_args[r], region_args[r] + region_nvals[r]));
+    a.dv.assign(region_args[r], region_args[r] + region_nvals[r]);
+    spec.AddArg(names[r], a);
+  }
+  if (output_size) spec.AddArg("output_size", MakeArg(std::vector<int64_t>(output_size, output_size + 2)));
+  const MultiPasteArgs a = MultiPasteResolveArgs(spec, nullptr, n);
+  dalib200PastePlan *plan = nullptr;
+  PermuteSetupOrThrow(dalib200PastePlanCreate(&plan, std::max(n, 1)));
+  const int rc = MultiPasteSetup(plan, a, in_type, ninputs, n, ndims, layouts, in_shapes, out_shapes);
+  dalib200PastePlanDestroy(plan);
+  PermuteSetupOrThrow(rc);
+  API_END
+}
+
 }  // extern "C"

@@ -26,6 +26,8 @@
 #include <utility>
 #include <vector>
 
+struct dalib200PastePlan;   // include/dali_b200.h
+
 namespace dali {
 
 // ---------------------------------------------------------------------------------------------- errors
@@ -480,6 +482,24 @@ struct EraseArgs {
   std::vector<float> fill;
 };
 EraseArgs EraseResolveArgs(const OpSpec &spec, const std::string &layout);
+
+// fn.multi_paste: in_ids and the six region arguments (in_anchors, in_anchors_rel, shapes, shapes_rel, out_anchors, out_anchors_rel)
+// of every sample back to back with their per-sample counts -- a per-sample CPU tensor input read with its shape ([K] for in_ids,
+// [K, 2] for the others), or a list used for every sample -- output_size per sample, and dtype (-1: the input's type).
+constexpr int kMultiPasteRegionArgs = 6;
+struct MultiPasteArgs {
+  bool has_ids = false, has_size = false;
+  bool has[kMultiPasteRegionArgs] = {};
+  std::vector<int32_t> ids;
+  std::vector<int64_t> id_counts, sizes;
+  std::vector<double> vals[kMultiPasteRegionArgs];
+  std::vector<int64_t> counts[kMultiPasteRegionArgs];
+  int dtype = -1;
+};
+MultiPasteArgs MultiPasteResolveArgs(const OpSpec &spec, const Workspace *ws, int n);
+// dalib200PasteSetup with the resolved arguments (fill 0); returns its status.
+int MultiPasteSetup(::dalib200PastePlan *plan, const MultiPasteArgs &a, int in_type, int ninputs, int n, const int *ndims,
+                    const char *const *layouts, const int64_t *in_shapes, int64_t *out_shapes);
 
 template <typename Backend>
 class Operator : public OperatorBase {

@@ -2690,6 +2690,221 @@ class EraseGPU : public Operator<GPUBackend> {
 };
 DALI_REGISTER_OPERATOR(Erase, EraseGPU, GPU);
 
+// =============================================================================================== MultiPaste, Paste
+// dali/operators/image/paste (the reference's documented arguments, DESIGN.md section 2): each output is built from rectangles of
+// input samples, later rectangles on top, the rest a fill (0 for MultiPaste, fill_value for Paste), by the batched kernel of
+// csrc/paste.cu.  Paste is one rectangle per output on a larger canvas.
+DALI_SCHEMA(MultiPaste)
+    .DocStr("Builds each output from rectangles of input samples (HWC): with in_ids, region k of output i comes from sample in_ids[i][k] "
+            "of the one input; without, from sample i of input k.  Later regions are pasted on top of earlier ones; elements no region "
+            "covers are 0.  Region arguments are per-sample [K, 2] CPU tensors of (y, x) pairs, or flat lists used for every sample.")
+    .NumInput(1, 64).NumOutput(1)
+    .AddOptionalArgNoDefault("in_ids", "Per output, the batch index of each region's source sample ([K] tensor).", true)
+    .AddOptionalArgNoDefault("in_anchors", "Region starts in the source, (y, x) in pixels.  Default 0.", true)
+    .AddOptionalArgNoDefault("in_anchors_rel", "Region starts in the source as fractions of its extent.", true)
+    .AddOptionalArgNoDefault("shapes", "Region extents (h, w) in pixels.  Default: the source extent minus the in-anchor.", true)
+    .AddOptionalArgNoDefault("shapes_rel", "Region extents as fractions of the source extent.", true)
+    .AddOptionalArgNoDefault("out_anchors", "Region starts in the output, (y, x) in pixels.  Default 0.", true)
+    .AddOptionalArgNoDefault("out_anchors_rel", "Region starts in the output as fractions of its extent.", true)
+    .AddOptionalArgNoDefault("output_size", "(H, W) of the output.  Default: the common shape of the input samples.", true)
+    .AddOptionalArgNoDefault("dtype", "The output type; default the input's.  Converted with ConvertSat.");
+
+DALI_SCHEMA(Paste)
+    .DocStr("Puts each uint8 HWC image on a larger canvas filled with fill_value (SSD's zoom-out): the canvas is "
+            "max(int(ratio * H), int(min_canvas_size)) by max(int(ratio * W), int(min_canvas_size)), the image at "
+            "(int(paste_y * (H' - H)), int(paste_x * (W' - W))).")
+    .NumInput(1).NumOutput(1)
+    .AddArg("ratio", "Canvas size over image size, >= 1.", true)
+    .AddOptionalArg("paste_x", "Horizontal position of the image in [0, 1].", 0.5f, true)
+    .AddOptionalArg("paste_y", "Vertical position of the image in [0, 1].", 0.5f, true)
+    .AddOptionalArg("min_canvas_size", "Smallest canvas extent.", 0.0f, true)
+    .AddOptionalArg("fill_value", "The canvas colour: one value per channel, or one for all.", std::vector<float>{0.0f})
+    .AddOptionalArg("n_channels", "Channels of the image.", 3);
+
+// One argument of sample i: a CPU tensor input read in its own type with its shape ([K, 2] for the region arguments, [K] for in_ids,
+// [2] for output_size), or a list, the same for every sample.  False when the argument is not given.
+static bool PasteArgValues(const OpSpec &spec, const Workspace *ws, const std::string &name, int i, std::vector<double> *v) {
+  v->clear();
+  if (ws && spec.HasTensorArgument(name)) {
+    const auto &tl = ws->ArgumentInput(name);
+    DALI_ENFORCE(i < tl.num_samples(), "multi_paste: argument input '", name, "' has ", tl.num_samples(), " samples, sample ", i, " requested");
+    const int nd = tl.sample_dim();
+    const int64_t *sh = tl.tensor_shape_span(i);
+    const bool ok = name == "in_ids" ? nd == 1 : name == "output_size" ? nd == 1 && sh[0] == 2 : nd == 2 && sh[1] == 2;
+    std::string shs = "[";
+    for (int d = 0; d < nd; d++) shs += (d ? ", " : "") + std::to_string(sh[d]);
+    DALI_ENFORCE(ok, "multi_paste: sample ", i, ": ", name, " has the shape ", shs, "]; expected ",
+                 name == "in_ids" ? "[K]" : name == "output_size" ? "[2]" : "[K, 2]");
+    const int64_t cnt = tl.shape().tensor_size(i);
+    const void *p = tl.raw_tensor(i);
+    for (int64_t k = 0; k < cnt; k++) {
+      switch (tl.type()) {
+        case DALI_INT32: v->push_back(static_cast<const int32_t *>(p)[k]); break;
+        case DALI_INT64: v->push_back(static_cast<double>(static_cast<const int64_t *>(p)[k])); break;
+        case DALI_FLOAT: v->push_back(static_cast<const float *>(p)[k]); break;
+        case DALI_FLOAT64: v->push_back(static_cast<const double *>(p)[k]); break;
+        default: DALI_FAIL(make_string("multi_paste: argument input '", name, "' has an unsupported type ", static_cast<int>(tl.type()),
+                                       "; INT32, INT64, FLOAT or FLOAT64 is expected"));
+      }
+    }
+    return true;
+  }
+  if (!spec.HasArgument(name)) return false;
+  const ArgValue *a = spec.FindArg(name);
+  switch (a->kind) {
+    case ArgValue::FLOAT_VEC:
+      if (a->dv.size() == a->fv.size()) v->assign(a->dv.begin(), a->dv.end());
+      else v->assign(a->fv.begin(), a->fv.end());
+      break;
+    case ArgValue::INT_VEC: for (int64_t x : a->iv) v->push_back(static_cast<double>(x)); break;
+    case ArgValue::FLOAT: v->push_back(a->f); break;
+    case ArgValue::INT: v->push_back(static_cast<double>(a->i)); break;
+    default: DALI_FAIL(make_string("multi_paste: argument '", name, "' is not a list of numbers"));
+  }
+  return true;
+}
+
+MultiPasteArgs MultiPasteResolveArgs(const OpSpec &spec, const Workspace *ws, int n) {
+  static const char *const names[kMultiPasteRegionArgs] = { "in_anchors", "in_anchors_rel", "shapes", "shapes_rel", "out_anchors",
+                                                            "out_anchors_rel" };
+  MultiPasteArgs a;
+  a.dtype = spec.HasArgument("dtype") ? spec.GetArgument<int>("dtype") : -1;
+  DALI_ENFORCE(!spec.HasArgument("dtype") || (a.dtype >= 0 && a.dtype <= 11), "multi_paste: invalid dtype ", a.dtype);
+  std::vector<double> v;
+  a.has_ids = spec.ArgumentDefined("in_ids");
+  a.id_counts.assign(n, 0);
+  for (int i = 0; i < n && a.has_ids; i++) {
+    PasteArgValues(spec, ws, "in_ids", i, &v);
+    for (double x : v) {
+      DALI_ENFORCE(x == std::floor(x) && std::fabs(x) < 2147483648.0, "multi_paste: sample ", i, ": in_ids value ", x, " is not an index");
+      a.ids.push_back(static_cast<int32_t>(x));
+    }
+    a.id_counts[i] = static_cast<int64_t>(v.size());
+  }
+  for (int r = 0; r < kMultiPasteRegionArgs; r++) {
+    a.has[r] = spec.ArgumentDefined(names[r]);
+    a.counts[r].assign(n, 0);
+    for (int i = 0; i < n && a.has[r]; i++) {
+      PasteArgValues(spec, ws, names[r], i, &v);
+      a.vals[r].insert(a.vals[r].end(), v.begin(), v.end());
+      a.counts[r][i] = static_cast<int64_t>(v.size());
+    }
+    if (a.vals[r].empty()) a.vals[r].push_back(0.0);                   // a valid pointer for samples without regions
+  }
+  a.has_size = spec.ArgumentDefined("output_size");
+  for (int i = 0; i < n && a.has_size; i++) {
+    PasteArgValues(spec, ws, "output_size", i, &v);
+    DALI_ENFORCE(v.size() == 2, "multi_paste: sample ", i, ": output_size has ", v.size(), " values; (H, W) is expected");
+    for (double x : v) {
+      DALI_ENFORCE(x == std::floor(x) && std::fabs(x) < 9.0e15, "multi_paste: sample ", i, ": output_size value ", x, " is not an integer");
+      a.sizes.push_back(static_cast<int64_t>(x));
+    }
+  }
+  return a;
+}
+
+int MultiPasteSetup(dalib200PastePlan *plan, const MultiPasteArgs &a, int in_type, int ninputs, int n, const int *ndims,
+                    const char *const *layouts, const int64_t *in_shapes, int64_t *out_shapes) {
+  const double *args[kMultiPasteRegionArgs];
+  const int64_t *counts[kMultiPasteRegionArgs];
+  for (int r = 0; r < kMultiPasteRegionArgs; r++) {
+    args[r] = a.has[r] ? a.vals[r].data() : nullptr;
+    counts[r] = a.has[r] ? a.counts[r].data() : nullptr;
+  }
+  const int32_t zero_id = 0;
+  const float zero = 0.0f;
+  return dalib200PasteSetup(plan, in_type, a.dtype, ninputs, n, ndims, layouts, in_shapes, a.has_ids ? (a.ids.empty() ? &zero_id : a.ids.data()) : nullptr,
+                            a.has_ids ? a.id_counts.data() : nullptr, args, counts, a.has_size ? a.sizes.data() : nullptr, &zero, 1, out_shapes);
+}
+
+class MultiPasteGPU : public Operator<GPUBackend> {
+ public:
+  explicit MultiPasteGPU(const OpSpec &spec) : Operator<GPUBackend>(spec) {}
+
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const int ninputs = ws.NumInput(), n = ws.Input<GPUBackend>(0).num_samples();
+    std::vector<int> ndims(ninputs);
+    std::vector<std::string> lay(ninputs);
+    std::vector<const char *> lp(ninputs);
+    std::vector<int64_t> is((size_t)ninputs * n * 3, 0), os((size_t)n * 3, 0);
+    for (int k = 0; k < ninputs; k++) {
+      const auto &in = ws.Input<GPUBackend>(k);
+      DALI_ENFORCE(in.num_samples() == n, "multi_paste: input ", k, " has ", in.num_samples(), " samples, input 0 has ", n);
+      DALI_ENFORCE(in.type() == ws.Input<GPUBackend>(0).type(), "multi_paste: input ", k, " has type code ", static_cast<int>(in.type()),
+                   ", input 0 has ", static_cast<int>(ws.Input<GPUBackend>(0).type()), "; all inputs must have one type");
+      ndims[k] = in.sample_dim();
+      lay[k] = in.GetLayout().str();
+      for (int i = 0; i < n && ndims[k] == 3; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + 3, is.begin() + ((size_t)k * n + i) * 3);
+    }
+    for (int k = 0; k < ninputs; k++) lp[k] = lay[k].c_str();
+    const MultiPasteArgs a = MultiPasteResolveArgs(spec_, &ws, n);
+    plan_.Ensure(n, "multi_paste");
+    if (MultiPasteSetup(plan_.get(), a, static_cast<int>(ws.Input<GPUBackend>(0).type()), ninputs, n, ndims.data(), lp.data(), is.data(), os.data()))
+      throw DALIException(dalib200GetLastError());
+    out.resize(1);
+    out[0].type = static_cast<DALIDataType>(a.dtype < 0 ? static_cast<int>(ws.Input<GPUBackend>(0).type()) : a.dtype);
+    out[0].shape.resize(n, 3);
+    for (int i = 0; i < n; i++) out[0].shape.set_tensor_shape(i, TensorShape(os.begin() + (size_t)i * 3, os.begin() + (size_t)(i + 1) * 3));
+    return true;
+  }
+
+  void RunImpl(Workspace &ws) override {
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(TensorLayout("HWC"));
+    std::vector<const void *> ip;
+    for (int k = 0; k < ws.NumInput(); k++) {
+      const auto p = InPtrs(ws.Input<GPUBackend>(k));
+      ip.insert(ip.end(), p.begin(), p.end());
+    }
+    CheckStatus(dalib200PasteLaunch(plan_.get(), ip.data(), OutPtrs(out).data(), ws.stream()), "multi_paste");
+  }
+
+  DALIB200_PLAN(Paste) plan_{max_batch_size_};
+};
+DALI_REGISTER_OPERATOR(MultiPaste, MultiPasteGPU, GPU);
+
+class PasteGPU : public Operator<GPUBackend> {
+ public:
+  explicit PasteGPU(const OpSpec &spec) : Operator<GPUBackend>(spec), fill_(spec.GetRepeatedArgument<float>("fill_value")) {}
+
+ protected:
+  bool SetupImpl(std::vector<OutputDesc> &out, const Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    const int n = in.num_samples(), nd = in.sample_dim();
+    std::vector<int64_t> is((size_t)n * 3, 0), os((size_t)n * 3, 0);
+    for (int i = 0; i < n && nd == 3; i++) std::copy(in.tensor_shape_span(i), in.tensor_shape_span(i) + 3, is.begin() + (size_t)i * 3);
+    std::vector<float> ratio(n), px(n), py(n), mc(n);
+    for (int i = 0; i < n; i++) {
+      ratio[i] = spec_.GetArgument<float>("ratio", &ws, i);
+      px[i] = spec_.GetArgument<float>("paste_x", &ws, i);
+      py[i] = spec_.GetArgument<float>("paste_y", &ws, i);
+      mc[i] = spec_.GetArgument<float>("min_canvas_size", &ws, i);
+    }
+    plan_.Ensure(n, "paste");
+    if (dalib200PasteCanvasSetup(plan_.get(), static_cast<int>(in.type()), n, nd, in.GetLayout().str().c_str(), is.data(),
+                                 spec_.GetArgument<int>("n_channels"), ratio.data(), px.data(), py.data(), mc.data(), fill_.data(),
+                                 (int)fill_.size(), os.data()))
+      throw DALIException(dalib200GetLastError());
+    out.resize(1);
+    out[0].type = in.type();
+    out[0].shape.resize(n, 3);
+    for (int i = 0; i < n; i++) out[0].shape.set_tensor_shape(i, TensorShape(os.begin() + (size_t)i * 3, os.begin() + (size_t)(i + 1) * 3));
+    return true;
+  }
+
+  void RunImpl(Workspace &ws) override {
+    const auto &in = ws.Input<GPUBackend>(0);
+    auto &out = ws.Output<GPUBackend>(0);
+    out.SetLayout(TensorLayout("HWC"));
+    CheckStatus(dalib200PasteLaunch(plan_.get(), InPtrs(in).data(), OutPtrs(out).data(), ws.stream()), "paste");
+  }
+
+  DALIB200_PLAN(Paste) plan_{max_batch_size_};
+  std::vector<float> fill_;
+};
+DALI_REGISTER_OPERATOR(Paste, PasteGPU, GPU);
+
 // =============================================================================================== Rotate
 // dali/operators/image/remap/rotate.cc + rotate_params.h: a WarpAffine whose matrix is
 // translation(in / 2) * rotation2D(-a) * translation(-out / 2) with a = deg2rad(-angle) (counter-clockwise for a top-left origin)

@@ -600,6 +600,40 @@ int dalib200EraseSetup(dalib200ErasePlan *plan, int type, int n, int ndim, const
 int dalib200EraseLaunch(dalib200ErasePlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * fn.multi_paste and fn.paste: each output built from rectangles of input samples, later rectangles on top of earlier ones, every
+ * element no rectangle covers a fill (DESIGN.md section 2).  HWC images only.  One launch per batch (DESIGN.md section 5).
+ * Setup (multi_paste):
+ *   in_type, out_type   DALIDataType codes; out_type -1: the input's type.  A converting paste applies ConvertSat.
+ *   ninputs, n          1 to 64 inputs of n samples each (exactly 1 with in_ids); n outputs
+ *   ndims, layouts      per input: the rank (3) and the layout ("HWC", "" or NULL); layouts may be NULL
+ *   in_shapes           ninputs x n x (H, W, C), input-major; one channel count across all of them
+ *   in_ids, in_id_counts  NULL for the multi-input form (region k of output i is sample i of input k), else in_id_counts[i] sample
+ *                       indices per output, back to back
+ *   region_args[6], region_counts[6]   in_anchors, in_anchors_rel, shapes, shapes_rel, out_anchors, out_anchors_rel: NULL when not
+ *                       given, else region_counts[a][i] values per output ((y, x) per region, 2 K values for K regions), back to back.
+ *                       Absolute values are integers; relative ones are llround(value * extent) in double.  Defaults: anchors 0,
+ *                       shapes the source extent minus the in-anchor.
+ *   output_sizes        NULL (every input sample has one shape, which the outputs take) or n x (H, W)
+ *   fill, nfill         the value of uncovered elements: one, or one per channel (multi_paste passes 0)
+ *   out_shapes          n x (H, W, C), written
+ * CanvasSetup (paste): UINT8 input of n_channels channels; per sample ratio >= 1, paste_x, paste_y in [0, 1], min_canvas_size >= 0;
+ *   H' = max(int(ratio * H), int(min_canvas_size)) (float product, truncated), W' the same way; the image at
+ *   (int(paste_y * (H' - H)), int(paste_x * (W' - W))); fill: one value per channel, or one for all.
+ * A type, layout, shape, region or fill that does not fit fails with DALIB200_ERROR_INVALID_ARGUMENT and a message naming the sample,
+ * the region and the argument.  Launch: in_ptrs: ninputs x n device buffers, input-major (only those a region reads must be set),
+ * out_ptrs: n; each aligned to its element size (else DALIB200_ERROR_INVALID_ARGUMENT); no launch when the batch has no elements. */
+typedef struct dalib200PastePlan dalib200PastePlan;
+int dalib200PastePlanCreate(dalib200PastePlan **plan, int max_samples);
+int dalib200PastePlanDestroy(dalib200PastePlan *plan);
+int dalib200PasteSetup(dalib200PastePlan *plan, int in_type, int out_type, int ninputs, int n, const int *ndims, const char *const *layouts,
+                       const int64_t *in_shapes, const int32_t *in_ids, const int64_t *in_id_counts, const double *const *region_args,
+                       const int64_t *const *region_counts, const int64_t *output_sizes, const float *fill, int nfill, int64_t *out_shapes);
+int dalib200PasteCanvasSetup(dalib200PastePlan *plan, int in_type, int n, int ndim, const char *layout, const int64_t *in_shapes, int n_channels,
+                             const float *ratio, const float *paste_x, const float *paste_y, const float *min_canvas_size, const float *fill,
+                             int nfill, int64_t *out_shapes);
+int dalib200PasteLaunch(dalib200PastePlan *plan, const void *const *in_ptrs, void *const *out_ptrs, dalib200Stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Audio decode (fn.decoders.audio).  WAV (PCM 8 / 16 / 24 / 32-bit, IEEE float 32, WAVE_FORMAT_EXTENSIBLE with either) and native FLAC
  * (8 / 16 / 24 bits per sample, optional ID3v2 tag in front), detected from the bytes.  The host parses the container and STREAMINFO
  * only; the FLAC frames are found, checked (CRC-8, CRC-16, frame chain) and decoded on the device.  Samples read as libsndfile's

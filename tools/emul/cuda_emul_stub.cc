@@ -1,6 +1,6 @@
 // tools/emul/cuda_emul_stub.cc -- TEST INFRASTRUCTURE.  LD_PRELOAD replacement of the CUDA runtime calls the library makes, like
 // tools/fuzz/cuda_stub.c, with two differences: "device" memory is host memory whose copies and memsets really happen, and the launches
-// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM, lossless JPEG, audio decode, arithmetic-expression, reduction, equalize, filter and erase kernels (and U2 / U3, which feed the
+// of the 3-D resize, progressive JPEG, PNG, TIFF, WebP, BMP / PNM, lossless JPEG, audio decode, arithmetic-expression, reduction, equalize, filter, erase and paste kernels (and U2 / U3, which feed the
 // lossless JPEG stage) are
 // EXECUTED on the host -- their bodies are single
 // host/device functions (dali_b200/csrc/resample3d_core.h, jpeg_prog_core.h, png_core.h, tiff_core.h, webp_core.h, bitmap_core.h, arith_core.h ...), so a
@@ -46,6 +46,7 @@
 #include "../../dali_b200/csrc/equalize_core.h"
 #include "../../dali_b200/csrc/filter_plan.h"
 #include "../../dali_b200/csrc/erase_plan.h"
+#include "../../dali_b200/csrc/paste_plan.h"
 
 using namespace dalib200;
 typedef int cudaError_t;
@@ -153,7 +154,7 @@ cudaError_t cudaFuncSetAttribute(const void *, int, int) { return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, const void *, int, size_t) { *n = 2; return 0; }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *, int, size_t, unsigned) { *n = 2; return 0; }
 
-static long g_emulated[34];
+static long g_emulated[35];
 long emul_launch_count(int which) { return g_emulated[which]; }
 void emul_trace_mark(const char *text) { TRACE("# %s", text); }    // a section header in the trace, written by the test
 
@@ -661,6 +662,7 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
   const bool is_eq_apply = !strcmp(name, "_ZN8dalib20021equalize_apply_kernelEPKNS_8EqSampleEilPKj");
   const bool is_filter = !kname.compare(0, 24, "dalib200::filter_kernel<");
   const bool is_erase = !kname.compare(0, 23, "dalib200::erase_kernel<");
+  const bool is_paste = !kname.compare(0, 23, "dalib200::paste_kernel<");
   if (grid.x == 0 || grid.y == 0 || grid.z == 0 || block.x == 0 || grid.y > 65535 || block.x > 1024) {
     g_last_error = 9;                              // cudaErrorInvalidConfiguration
     return 9;
@@ -707,6 +709,11 @@ cudaError_t cudaLaunchKernel(const void *func, Dim3 grid, Dim3 block, void **arg
     ErRunOnHost(*static_cast<const ErSample **>(args[0]), *static_cast<int *>(args[1]), *static_cast<int64_t *>(args[2]),
                 *static_cast<const uint8_t **>(args[3]), *static_cast<int *>(args[4]));
     g_emulated[33]++;
+  }
+  else if (is_paste) {                             // paste.cu: PsRunOnHost, the element size and conversion from the batch
+    PsRunOnHost(*static_cast<const PsSample **>(args[0]), *static_cast<int *>(args[1]), *static_cast<int64_t *>(args[2]),
+                *static_cast<const PsBatch *>(args[3]));
+    g_emulated[34]++;
   }
   return 0;
 }

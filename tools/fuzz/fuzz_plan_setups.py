@@ -18,6 +18,7 @@ red_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 3
 eq_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 4])
 flt_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 5])
 er_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 6])
+ps_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 7])
 N = int(sys.argv[2]) if len(sys.argv) > 2 else 2000
 L = capi.lib()
 MILD = float(os.environ.get("FUZZ_BAD_SCALE", "1"))      # < 1: fewer adversarial values per call -> more set-ups reach their deep paths
@@ -76,6 +77,8 @@ flt_plan = C.c_void_p()
 capi.check(L.dalib200FilterPlanCreate(C.byref(flt_plan), 8))
 er_plan = C.c_void_p()
 capi.check(L.dalib200ErasePlanCreate(C.byref(er_plan), 8))
+ps_plan = C.c_void_p()
+capi.check(L.dalib200PastePlanCreate(C.byref(ps_plan), 8))
 for it in range(N):
     n = int(rng.integers(0, 9)) if rng.random() < 0.9 else int(rng.choice([9, 100, -1]))
     m = max(n, 1) if n < 64 else 8
@@ -361,5 +364,45 @@ for it in range(N):
     note("erase", rc)
     if rc == 0:
         launch("erase", L.dalib200EraseLaunch, er_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
+    rng = main_rng
+    # ---- multi_paste / paste: a generator of its own.  Zero, negative and 2^31-sized extents, ranks other than 3, wrong layouts, mixed
+    # channel counts, 1-3 inputs (and 0 / 65), in_ids out of range, region counts that do not match, both forms of one argument,
+    # non-integer, non-finite and huge coordinates, regions outside their source or the output, output sizes and fills that do not
+    # fit; paste ratios, positions and canvas sizes out of range; the launch runs the descriptor build
+    rng, main_rng = ps_rng, rng
+    ninputs = int(rng.choice([0, 65])) if rng.random() < 0.03 * MILD else int(rng.integers(1, 4))
+    ni = min(max(ninputs, 1), 3)
+    ext = [int(rng.choice([0, -1, 2 ** 31, 2 ** 40])) if rng.random() < 0.03 * MILD else int(rng.integers(1, 40)) for _ in range(ni * m * 3)]
+    chans = int(rng.integers(1, 5))
+    for s_ in range(ni * m):
+        if rng.random() > 0.05 * MILD:
+            ext[s_ * 3 + 2] = chans
+    use_ids = rng.random() < 0.6
+    kk = [int(rng.choice([0, 1, 2, 4, 64])) for _ in range(m)]
+    ids = [int(rng.choice([-1, m, 2 ** 31 - 1])) if rng.random() < 0.03 * MILD else int(rng.integers(0, m)) for _ in range(max(1, sum(kk)))]
+    av, ac, keep = (C.POINTER(C.c_double) * 6)(), (C.POINTER(C.c_int64) * 6)(), []
+    for a in range(6):
+        if rng.random() < 0.4:
+            cnt = np.array([2 * (kk[i] if use_ids else ni) + (1 if rng.random() < 0.03 * MILD else 0) for i in range(m)], np.int64)
+            vals = np.array([flt(-2.0, 2.0) if a % 2 else float(small(0, 40)) for _ in range(int(cnt.sum()) + 1)], np.float64)
+            keep += [cnt, vals]
+            av[a], ac[a] = vals.ctypes.data_as(C.POINTER(C.c_double)), cnt.ctypes.data_as(C.POINTER(C.c_int64))
+    osz = (C.c_int64 * (2 * m))(*[small(0, 60) for _ in range(2 * m)]) if rng.random() < 0.7 else None
+    lays = (C.c_char_p * ni)(*[[b"HWC", b"", b"CHW", b"HW", None][int(rng.integers(0, 5))] if rng.random() < 0.1 * MILD else b"HWC" for _ in range(ni)])
+    nds = (C.c_int * ni)(*[small(2, 4) if rng.random() < 0.1 * MILD else 3 for _ in range(ni)])
+    fill = [flt() for _ in range(int(rng.choice([1, 1, chans, 0, 7])))]
+    oshapes = (C.c_int64 * (3 * m))()
+    rc = L.dalib200PasteSetup(ps_plan, code(range(12)), code(list(range(12)) + [-1]), ninputs, n, nds, lays, (C.c_int64 * len(ext))(*ext),
+                              (C.c_int32 * len(ids))(*ids) if use_ids else None, (C.c_int64 * m)(*kk) if use_ids else None, av, ac, osz,
+                              (C.c_float * max(1, len(fill)))(*fill), len(fill), oshapes)
+    note("paste", rc)
+    if rc == 0:
+        launch("paste", L.dalib200PasteLaunch, ps_plan, fake_ptrs(ni * m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
+    f = lambda lo, hi: (C.c_float * m)(*[flt(lo, hi) for _ in range(m)])  # noqa: E731
+    rc = L.dalib200PasteCanvasSetup(ps_plan, code([0]), n, nds[0], lays[0], (C.c_int64 * len(ext))(*ext), small(1, 5), f(0.5, 5.0), f(-0.2, 1.2),
+                                    f(-0.2, 1.2), f(-5.0, 80.0), (C.c_float * max(1, len(fill)))(*fill), len(fill), oshapes)
+    note("paste_canvas", rc)
+    if rc == 0:
+        launch("paste_canvas", L.dalib200PasteLaunch, ps_plan, fake_ptrs(m, 0x10000000), fake_ptrs(m, 0x7000000000), None)
     rng = main_rng
 print("seed", sys.argv[1] if len(sys.argv) > 1 else 0, "iterations", N, "- no sanitizer report;", {f"{k[0]}:{k[1]}": v for k, v in sorted(hist.items())})
