@@ -2052,7 +2052,8 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
     for (int si = 0; si < j.scan_ncomp; si++) {
       const int c = j.scan_comp[si];
       im.hs[c] = j.hs[c]; im.vs[c] = j.vs[c]; im.tq[c] = j.tq[c];
-      if (!j.qt_present[j.tq[c]]) { SetLastError("decoders.image: sample %d: missing quantisation table", i); return DALIB200_ERROR_BAD_DATA; }
+      // multi-scan: each component's table is the one defined when its first scan starts (the planner checks it below)
+      if (!prog && !j.qt_present[j.tq[c]]) { SetLastError("decoders.image: sample %d: missing quantisation table", i); return DALIB200_ERROR_BAD_DATA; }
       if (j.td[si] > 1 || j.ta[si] > 1) return unsupported("Huffman table ids above 1 are not supported (baseline allows 0..1)");
       if (!prog && (!j.dc[j.td[si]].present || !j.ac[j.ta[si]].present)) { SetLastError("decoders.image: sample %d: missing Huffman table", i); return DALIB200_ERROR_BAD_DATA; }
       for (int v = 0; v < j.vs[c]; v++)
@@ -2084,15 +2085,18 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
         it = table_cache.emplace(key, (int)p->tables.size() - 1).first;
       }
       im.table_set = it->second;
-      std::string qk(reinterpret_cast<const char *>(j.qt), sizeof(j.qt));
+    }
+    auto set_quant = [&](const uint16_t (*qt)[64]) {         // quantisation tables, deduplicated by content
+      std::string qk(reinterpret_cast<const char *>(qt), sizeof(QuantSet::q));
       auto qi = quant_cache.find(qk);
       if (qi == quant_cache.end()) {
-        QuantSet qs; memcpy(qs.q, j.qt, sizeof(j.qt));
+        QuantSet qs; memcpy(qs.q, qt, sizeof(qs.q));
         p->quants.push_back(qs);
         qi = quant_cache.emplace(qk, (int)p->quants.size() - 1).first;
       }
       im.quant_set = qi->second;
-    }
+    };
+    if (!prog) set_quant(j.qt);                              // multi-scan samples: the tables the planner latches, below
     // entropy-coded segment(s)
     const uint8_t *d = streams[i];
     size_t sb = j.scan_begin, se = lengths[i];
@@ -2126,7 +2130,10 @@ int dalib200JpegPlanSetupEx(dalib200JpegPlan *p, int n, const uint8_t *const *st
       // no units: the scans are planned from the whole stream; their bytes are the staged range [scan_begin, scan_end) like a baseline
       // sample's, so JpegUpload needs no special case
       std::string err;
-      if ((rc = p->prog.Plan(d, lengths[i], sb, se, i, (int64_t)raw, coefs, im, &err))) return sample_error(rc, err);
+      uint16_t quant[4][64];
+      if ((rc = p->prog.Plan(d, lengths[i], sb, se, i, (int64_t)raw, coefs, im, quant, &err))) return sample_error(rc, err);
+      set_quant(quant);                                      // slot c of the set: the table component c latched
+      for (int c = 0; c < j.ncomp; c++) im.tq[c] = c;
     } else if (j.restart_interval == 0) {
       add_unit(sb, se, 0, nmcu);
     } else {

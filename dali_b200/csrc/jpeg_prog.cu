@@ -41,11 +41,11 @@ void ProgStage::Clear() {
 }
 
 int ProgStage::Plan(const uint8_t *d, size_t len, size_t sb, size_t se, int sample, int64_t raw_off, int64_t coef_off, const JpegImage &im,
-                    std::string *err) {
+                    uint16_t quant[4][64], std::string *err) {
   ProgImage pim;
   memset(&pim, 0, sizeof(pim));
   const size_t first_new = scans.size();
-  if (int rc = PlanProgressive(d, len, sb, (int)images.size(), &pim, scans, huff, table_cache, err)) return rc;
+  if (int rc = PlanProgressive(d, len, sb, (int)images.size(), &pim, scans, huff, table_cache, quant, err)) return rc;
   for (size_t k = first_new; k < scans.size(); k++)
     if ((size_t)scans[k].data_off + scans[k].data_len > se - sb) {
       // a scan that runs into the trimmed end-of-image marker ends in front of it

@@ -17,10 +17,10 @@ struct ProgStage : SideStage {
   bool Empty() const override { return images.empty(); }
   void Clear() override;
   // Plans the scans of sample `sample` of stream d[0, len), whose first scan's data starts at `sb` and whose last ends at `se`; `im` is
-  // the frame layout the baseline plan derived, the coefficients start at `coef_off`, the staged bytes at `raw_off`.  Returns a DALIB200
-  // status; *err says why on failure.
+  // the frame layout the baseline plan derived, the coefficients start at `coef_off`, the staged bytes at `raw_off`.  quant[c]: the
+  // quantisation table component c latched at its first scan (PlanProgressive).  Returns a DALIB200 status; *err says why on failure.
   int Plan(const uint8_t *d, size_t len, size_t sb, size_t se, int sample, int64_t raw_off, int64_t coef_off, const JpegImage &im,
-           std::string *err);
+           uint16_t quant[4][64], std::string *err);
   void SortWaves();                          // after the batch's last sample
 
   std::vector<ProgImage> images;

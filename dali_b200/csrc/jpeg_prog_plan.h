@@ -51,15 +51,21 @@ inline int Rd16(const uint8_t *p) { return (p[0] << 8) | p[1]; }
 // Walks stream[0, n).  `base`: file offset the scans' data_off are relative to (the first scan's data = what the decoder stages).
 // Fills im's geometry (not coef_off / raw_off / sample), appends the scans (image index = `image`) and the derived tables (deduplicated
 // through `table_cache`).  Returns 0, or DALIB200_ERROR_BAD_DATA / _UNSUPPORTED with *err.
+// quant[c]: the quantisation table of component c (natural order) as it stood when the component's first scan started -- a DQT may come
+// between scans, and like libjpeg (jdinput.c latch_quant_tables) a later redefinition does not change a component already scanned;
+// zeros for a component no scan codes (its coefficients are all zero).
 inline int PlanProgressive(const uint8_t *d, size_t n, size_t base, int image, ProgImage *im, std::vector<ProgScan> &scans,
-                           std::vector<ProgHuff> &huff, std::map<std::string, int> &table_cache, std::string *err) {
+                           std::vector<ProgHuff> &huff, std::map<std::string, int> &table_cache, uint16_t quant[4][64], std::string *err) {
   using namespace progdetail;
   auto bad = [&](const char *m) { if (err) *err = m; return DALIB200_ERROR_BAD_DATA; };
   auto unsup = [&](const char *m) { if (err) *err = m; return DALIB200_ERROR_UNSUPPORTED; };
   if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return bad("not a JPEG stream (missing SOI)");
   RawHuff dc[4], ac[4];
-  int width = 0, height = 0, ncomp = 0, cid[4] = { 0 }, hs[4] = { 0 }, vs[4] = { 0 }, hmax = 1, vmax = 1;
+  int width = 0, height = 0, ncomp = 0, cid[4] = { 0 }, hs[4] = { 0 }, vs[4] = { 0 }, tq[4] = { 0 }, hmax = 1, vmax = 1;
   bool got_sof = false, sequential = false;
+  uint16_t qt[4][64];
+  bool qt_present[4] = { false, false, false, false }, latched[4] = { false, false, false, false };
+  memset(quant, 0, sizeof(uint16_t) * 4 * 64);
   int dri = 0;
   const size_t first_scan = scans.size();
   int coef_bits[4][64];                              // libjpeg's coef_bits: the Al each coefficient has reached, -1 = never sent
@@ -94,7 +100,15 @@ inline int PlanProgressive(const uint8_t *d, size_t n, size_t base, int image, P
     }
     const uint8_t *s = d + pos + 2;
     const int sl = L - 2;
-    if (m == 0xC4) {
+    if (m == 0xDB) {
+      int o = 0;
+      while (o < sl) {
+        const int wide = s[o] >> 4 ? 2 : 1, t = s[o] & 15; o++;
+        if (t > 3 || o + 64 * wide > sl) return bad("JPEG: bad DQT");
+        for (int i = 0; i < 64; i++, o += wide) qt[t][h_prog_natural[i]] = (uint16_t)(wide == 2 ? Rd16(s + o) : s[o]);
+        qt_present[t] = true;
+      }
+    } else if (m == 0xC4) {
       int o = 0;
       while (o < sl) {
         if (o + 17 > sl) return bad("JPEG: bad DHT");
@@ -116,8 +130,8 @@ inline int PlanProgressive(const uint8_t *d, size_t n, size_t base, int image, P
       if (s[0] != 8) return unsup("only 8-bit JPEG is supported");
       if ((ncomp != 1 && ncomp != 3 && ncomp != 4) || sl < 6 + 3 * ncomp) return unsup("only 1-, 3- or 4-component JPEG is supported");
       for (int c = 0; c < ncomp; c++) {
-        cid[c] = s[6 + 3 * c]; hs[c] = s[7 + 3 * c] >> 4; vs[c] = s[7 + 3 * c] & 15;
-        if (hs[c] < 1 || hs[c] > 4 || vs[c] < 1 || vs[c] > 4) return bad("JPEG: bad sampling factors");
+        cid[c] = s[6 + 3 * c]; hs[c] = s[7 + 3 * c] >> 4; vs[c] = s[7 + 3 * c] & 15; tq[c] = s[8 + 3 * c];
+        if (hs[c] < 1 || hs[c] > 4 || vs[c] < 1 || vs[c] > 4 || tq[c] > 3) return bad("JPEG: bad sampling factors");
       }
       if (ncomp == 1) hs[0] = vs[0] = 1;                     // a single component is never interleaved
       for (int c = 0; c < ncomp; c++) { hmax = std::max(hmax, hs[c]); vmax = std::max(vmax, vs[c]); }
@@ -153,7 +167,13 @@ inline int PlanProgressive(const uint8_t *d, size_t n, size_t base, int image, P
         if (sc.ss == 0 ? sc.se != 0 : sc.ncomp != 1) return bad("JPEG: bad progression parameters");
         if (sc.ah != 0 && sc.ah != sc.al + 1) return bad("JPEG: bad successive approximation");
       }
-      if (sc.ncomp != 1 && sc.ncomp != ncomp) return unsup("scans that interleave a subset of the components are not supported");
+      for (int i = 0; i < sc.ncomp; i++) {
+        const int c = sc.comp[i];
+        if (latched[c]) continue;
+        if (!qt_present[tq[c]]) return bad("JPEG: missing quantisation table");
+        memcpy(quant[c], qt[tq[c]], sizeof(qt[0]));
+        latched[c] = true;
+      }
       for (int i = 0; i < sc.ncomp; i++) {
         if (sc.seq) { if (!table_index(dc[td[i]], &sc.dc_tbl[i]) || !table_index(ac[ta[i]], &sc.seq_ac_tbl[i])) return bad("JPEG: missing or invalid Huffman table"); }
         else if (sc.ss == 0) { if (sc.ah == 0 && !table_index(dc[td[i]], &sc.dc_tbl[i])) return bad("JPEG: missing or invalid Huffman table"); }

@@ -3,10 +3,14 @@
 Natural streams keep every IDCT value in range; these do not.  baseline() codes coefficient planes as one interleaved scan (SOF0 with
 8-bit DQT, or SOF1 with 16-bit DQT), with the standard Huffman tables (DC categories <= 11, AC sizes <= 10) or wide built tables
 (every DC category 0..15, every AC run / size up to 15, codes of up to 16 bits), optionally with a restart interval and an Adobe APP14
-marker for 4-component frames.  progressive() codes the same planes as a spectral-selection script (one DC scan, two AC bands per
-component); jpeg_cmyk_streams.one_scan_per_component() re-codes a baseline one as one scan per component.  extreme_corpus() and
+marker for 4-component frames.  progressive() codes the same planes under any scan script (T.81 G.1.2: successive approximation,
+EOB runs, refinement, restart intervals, tables and DQT placed between scans), expected() and waves() state what the decoder's arena
+holds after any prefix of a script and how many launches its planner makes, and the catalogue below names the scripts encoders
+write; jpeg_cmyk_streams.one_scan_per_component() re-codes a baseline stream as one scan per component.  extreme_corpus() and
 mutated() are the corpora of tests/test_jpeg_extreme_cpu.py and tests/test_gpu_jpeg_extreme.py, which compare them with
 cv2.imdecode."""
+from collections import Counter, namedtuple
+
 import numpy as np
 
 from jpeg_cmyk_streams import _ZZ, _BitWriter, _huff_codes, _seg, _segments
@@ -55,8 +59,9 @@ def wide_tables():
 
 
 def _dqt(tables, dqt16):
+    """tables: a list (ids 0, 1, ...) or {id: values}, natural order"""
     out = b""
-    for t, q in enumerate(tables):
+    for t, q in (tables.items() if isinstance(tables, dict) else enumerate(tables)):
         zz = [int(q[_ZZ[k]]) for k in range(64)]
         out += bytes([(16 if dqt16 else 0) | t]) + (b"".join(v.to_bytes(2, "big") for v in zz) if dqt16 else bytes(zz))
     return _seg(0xDB, out)
@@ -104,73 +109,425 @@ def baseline(h, w, sampling, planes, qtabs, dqt16=False, wide=False, rst=0, adob
     return bytes(out + bw.finish() + b"\xff\xd9")
 
 
-def _ac_band(bw, blk, ss, se, ac_t):
-    """AC first scan of one block, Al = 0, every block ends with its own EOB (no EOB runs)"""
-    run = 0
-    for k in range(ss, se + 1):
-        val = int(blk[_ZZ[k]])
-        if val == 0:
-            run += 1
-            continue
-        while run > 15:
-            bw.put(*ac_t[0xF0])
-            run -= 16
-        s, bits = _BitWriter._val(val)
-        bw.put(*ac_t[(run << 4) | s])
-        bw.put(bits, s)
-        run = 0
-    if run:
-        bw.put(*ac_t[0])
+# ---- progressive scripts (T.81 G.1.2; the coding decisions follow libjpeg's jcphuff.c) --------------------------------------------
+Scan = namedtuple("Scan", "comps ss se ah al rst slot dqt", defaults=(None, 0, None))
+Scan.__doc__ = """One SOS of a script: the component indices it codes, the band Ss..Se and the successive approximation Ah / Al.  rst: a DRI
+segment in front of the scan (0 switches restarts off; None keeps the interval in force).  slot: the Huffman table slot of the scan's
+tables (component i of a DC scan takes slot + i, mod 4).  dqt: {table id: 64 values, natural order}, a DQT segment in front of the scan."""
+
+_EOB_FLUSH_BITS = 1000 - 64 + 1        # jcphuff.c MAX_CORR_BITS - DCTSIZE2 + 1: more buffered correction bits end the EOB run
 
 
-def progressive(h, w, sampling, planes, qtabs, dqt16=False, wide=False, rst=0, adobe=None, bands=((1, 5), (6, 63))):
-    """SOF2: one DC scan over all components (interleaved when there are several), then one scan per component and band.  The image
-    size must be a whole number of MCUs, so that the non-interleaved scans code every block of the planes."""
-    tables = wide_tables() if wide else std_tables()
-    out = _header(h, w, sampling, qtabs, dqt16, tables, rst, adobe, 0xC2)
-    codes = _huff_codes(b"".join(tables))
+def _geometry(h, w, sampling):
+    """(mcux, mcuy, [(blocks per column, blocks per row)] of each component in a non-interleaved scan: ceil(component extent / 8))"""
     hmax, vmax = max(s[0] for s in sampling), max(s[1] for s in sampling)
-    assert h % (8 * vmax) == 0 and w % (8 * hmax) == 0
-    mcux, mcuy = w // (8 * hmax), h // (8 * vmax)
-    ncomp = len(sampling)
-    out += _seg(0xDA, bytes([ncomp]) + b"".join(bytes([c + 1, _tsel(c) & 0xF0]) for c in range(ncomp)) + bytes([0, 0, 0]))
-    bw, pred = _BitWriter(), [0] * ncomp
-    nmcu = mcux * mcuy if ncomp > 1 else planes[0].shape[0] * planes[0].shape[1]
-    for m in range(nmcu):
-        if rst and m and m % rst == 0:
-            bw.restart(m // rst - 1)
-            pred = [0] * ncomp
-        if ncomp == 1:
-            by, bx = divmod(m, planes[0].shape[1])
-            blk = planes[0][by, bx]
-            s, bits = _BitWriter._val(int(blk[0]) - pred[0])
-            bw.put(*codes[0x00][s])
-            bw.put(bits, s)
-            pred[0] = int(blk[0])
-            continue
-        my, mx = divmod(m, mcux)
-        for c, (hs, vs) in enumerate(sampling):
-            dct = codes[_tsel(c) >> 4]
-            for v in range(vs):
-                for hh in range(hs):
-                    blk = planes[c][my * vs + v, mx * hs + hh]
-                    s, bits = _BitWriter._val(int(blk[0]) - pred[c])
-                    bw.put(*dct[s])
-                    bw.put(bits, s)
-                    pred[c] = int(blk[0])
-    out += bw.finish()
-    for c in range(ncomp):
-        act = codes[0x10 | (_tsel(c) & 15)]
-        for ss, se in bands:
-            out += _seg(0xDA, bytes([1, c + 1, _tsel(c) & 0x0F, ss, se, 0]))
-            bw, (bh, bwid) = _BitWriter(), planes[c].shape[:2]
-            for n in range(bh * bwid):
-                if rst and n and n % rst == 0:
-                    bw.restart(n // rst - 1)
-                by, bx = divmod(n, bwid)
-                _ac_band(bw, planes[c][by, bx], ss, se, act)
-            out += bw.finish()
+    blk = [((-(-h * vs // vmax) + 7) // 8, (-(-w * hs // hmax) + 7) // 8) for hs, vs in sampling]
+    return -(-w // (8 * hmax)), -(-h // (8 * vmax)), blk
+
+
+def _optimal_dht(tc_th, counts, skew=False):
+    """DHT payload of a table built from symbol counts by jchuff.c jpeg_gen_optimal_table (a reserved all-ones code, then no code longer
+    than 16 bits).  skew: the counts are replaced by weights that halve with each rank, so that the rarer symbols get 9..16-bit codes."""
+    freq = [0] * 257
+    ranked = sorted(counts, key=lambda s: (-counts[s], s))
+    for rank, s in enumerate(ranked):
+        freq[s] = 1 << max(0, 40 - rank) if skew else counts[s]
+    freq[256] = 1
+    codesize, others = [0] * 257, [-1] * 257
+    active = [i for i in range(257) if freq[i]]
+    while len(active) > 1:
+        c1 = min(active, key=lambda i: (freq[i], -i))             # the smallest count, on a tie the largest symbol (jchuff.c)
+        c2 = min((i for i in active if i != c1), key=lambda i: (freq[i], -i))
+        freq[c1] += freq[c2]
+        active.remove(c2)
+        codesize[c1] += 1
+        while others[c1] >= 0:
+            c1 = others[c1]
+            codesize[c1] += 1
+        others[c1] = c2
+        codesize[c2] += 1
+        while others[c2] >= 0:
+            c2 = others[c2]
+            codesize[c2] += 1
+    maxl = max(codesize)
+    bits = [0] * (max(maxl, 16) + 1)
+    for i in range(257):
+        if codesize[i]:
+            bits[codesize[i]] += 1
+    for i in range(maxl, 16, -1):
+        while bits[i] > 0:
+            j = i - 2
+            while bits[j] == 0:
+                j -= 1
+            bits[i] -= 2
+            bits[i - 1] += 1
+            bits[j + 1] += 2
+            bits[j] -= 1
+    i = 16
+    while bits[i] == 0:
+        i -= 1
+    bits[i] -= 1                                                  # drop the reserved code
+    vals = [s for l in range(1, maxl + 1) for s in range(256) if codesize[s] == l]
+    return bytes([tc_th] + bits[1:17] + vals)
+
+
+class _ScanCoder:
+    """The symbols, raw bits and restart markers of one scan in stream order; the tables are built from the symbols afterwards."""
+
+    def __init__(self, overlong):
+        self.ev, self.eobrun, self.pend, self.overlong = [], 0, [], overlong
+
+    def sym(self, key, s):
+        self.ev.append((0, key, s))
+
+    def bits(self, v, n):
+        if n:
+            self.ev.append((1, v, n))
+
+    def flush_eobrun(self, key):                                  # jcphuff.c emit_eobrun: the run, then the bits buffered behind it
+        if self.eobrun:
+            n = self.eobrun.bit_length() - 1
+            self.sym(key, n << 4)
+            self.bits(self.eobrun, n)
+            for b in self.pend:
+                self.bits(b, 1)
+            self.eobrun, self.pend = 0, []
+
+    def end_block(self, key, pend):
+        self.eobrun += 1
+        self.pend += pend
+        if self.eobrun == 0x7FFF or len(self.pend) > _EOB_FLUSH_BITS:
+            self.flush_eobrun(key)
+
+    def ac_first(self, key, a, sgn, al):                           # encode_mcu_AC_first; a: |coefficients| >> Al of the band
+        nk, prev = len(a), -1
+        for p in np.flatnonzero(a):
+            r = p - prev - 1
+            prev = p
+            self.flush_eobrun(key)
+            while r > 15:
+                self.sym(key, 0xF0)
+                r -= 16
+            v = int(a[p])
+            s = v.bit_length()
+            self.sym(key, (r << 4) | s)
+            self.bits(v if sgn[p] else ~v, s)
+        if prev < nk - 1:
+            self.end_block(key, [])
+
+    def ac_refine(self, key, a, sgn):                              # encode_mcu_AC_refine
+        nz = np.flatnonzero(a)
+        eob = max((p for p in nz if a[p] == 1), default=-1)       # the last coefficient that becomes nonzero in this pass
+        r, br, prev = 0, [], -1
+        for p in nz:
+            r += p - prev - 1
+            prev = p
+            while r > 15 and p <= eob:
+                self.flush_eobrun(key)
+                self.sym(key, 0xF0)
+                r -= 16
+                for b in br:
+                    self.bits(b, 1)
+                br = []
+            if a[p] > 1:
+                br.append(int(a[p]) & 1)                          # a correction bit of an already nonzero coefficient
+                continue
+            self.flush_eobrun(key)
+            self.sym(key, (r << 4) | 1)
+            self.bits(int(sgn[p]), 1)
+            for b in br:
+                self.bits(b, 1)
+            br, r = [], 0
+        r += len(a) - 1 - prev
+        if r > 0 or br:
+            self.end_block(key, br)
+
+    def block(self, dkey, akey, blk, pred):                       # one block of a sequential scan
+        s, b = _BitWriter._val(int(blk[0]) - pred)
+        self.sym(dkey, s)
+        self.bits(b, s)
+        z = np.asarray(blk, np.int64)[_ZZ]
+        prev = 0
+        for p in np.flatnonzero(z[1:]) + 1:
+            r = p - prev - 1
+            prev = p
+            while r > 15:
+                self.sym(akey, 0xF0)
+                r -= 16
+            s, b = _BitWriter._val(int(z[p]))
+            self.sym(akey, (r << 4) | s)
+            self.bits(b, s)
+        if prev < 63:
+            self.sym(akey, 0)
+        return int(blk[0])
+
+    def code(self, skew):
+        """(DHT payload, entropy-coded bytes)"""
+        counts = {}
+        for e in self.ev:
+            if e[0] == 0:
+                counts.setdefault(e[1], Counter())[e[2]] += 1
+        dht = b"".join(_optimal_dht((tc << 4) | th, counts[(tc, th)], skew) for tc, th in sorted(counts))
+        codes = _huff_codes(dht)
+        bw = _BitWriter()
+        for kind, x, y in self.ev:
+            if kind == 0:
+                bw.put(*codes[(x[0] << 4) | x[1]][y])
+            elif kind == 1:
+                bw.put(x, y)
+            else:
+                bw.restart(x)
+        return dht, bw.finish()
+
+
+def _scan_data(sc, planes, sampling, geo, dri, sequential, skew, overlong):
+    """(SOS payload, DHT payload, entropy-coded bytes) of one scan"""
+    mcux, mcuy, blk = geo
+    comps, single = sc.comps, len(sc.comps) == 1
+    if single:
+        c = comps[0]
+        units = [[(0, c, by, bx)] for by in range(blk[c][0]) for bx in range(blk[c][1])]
+    else:
+        units = [[(i, c, my * sampling[c][1] + v, mx * sampling[c][0] + hh) for i, c in enumerate(comps)
+                  for v in range(sampling[c][1]) for hh in range(sampling[c][0])] for my in range(mcuy) for mx in range(mcux)]
+    dc_slot = [(sc.slot + i) % 4 for i in range(len(comps))]
+    akey = (1, sc.slot)
+    if sequential:
+        sel = [(t << 4) | t for t in dc_slot]
+    elif sc.ss == 0:
+        sel = [t << 4 if sc.ah == 0 else 0 for t in dc_slot]
+    else:
+        sel = [sc.slot]
+    sos = bytes([len(comps)]) + b"".join(bytes([c + 1, t]) for c, t in zip(comps, sel)) + bytes([sc.ss, sc.se, (sc.ah << 4) | sc.al])
+    e = _ScanCoder(overlong)
+    if sc.ss > 0:                                                 # the band of every block, |v| >> Al, and the signs
+        c = comps[0]
+        band = planes[c][:blk[c][0], :blk[c][1]].reshape(-1, 64)[:, [_ZZ[k] for k in range(sc.ss, sc.se + 1)]].astype(np.int64)
+        mag, pos = np.abs(band) >> sc.al, band >= 0
+        any_ = mag.any(1)
+    pred = [0] * 4
+    for u, unit in enumerate(units):
+        if dri and u and u % dri == 0:
+            if e.eobrun and e.overlong:
+                e.eobrun = min(e.eobrun + 5, 0x7FFF)              # a run that claims blocks past the marker
+            e.flush_eobrun(akey)
+            e.ev.append((2, (u // dri - 1) & 7, None))
+            pred = [0] * 4
+        if sequential:
+            for i, c, by, bx in unit:
+                t = dc_slot[i]
+                pred[i] = e.block((0, t), (1, t), planes[c][by, bx], pred[i])
+        elif sc.ss == 0:
+            for i, c, by, bx in unit:
+                v = int(planes[c][by, bx, 0]) >> sc.al
+                if sc.ah:
+                    e.bits(v & 1, 1)                              # encode_mcu_DC_refine
+                else:
+                    s, b = _BitWriter._val(v - pred[i])           # encode_mcu_DC_first: the point transform is an arithmetic shift
+                    pred[i] = v
+                    e.sym((0, dc_slot[i]), s)
+                    e.bits(b, s)
+        elif not any_[u]:
+            e.end_block(akey, [])                                 # nothing in the band at this bit position: the block joins the run
+        elif sc.ah == 0:
+            e.ac_first(akey, mag[u], pos[u], sc.al)
+        else:
+            e.ac_refine(akey, mag[u], pos[u])
+    e.flush_eobrun(akey)
+    return sos, *e.code(skew)
+
+
+def progressive(h, w, sampling, planes, qtabs, dqt16=False, wide=False, rst=0, adobe=None, script=None, sof=0xC2, qhead=None,
+                overlong_runs=False):
+    """Codes planes[c] ([mcuy * vs, mcux * hs, 64] coefficients, natural order, absolute DC) as the scans of `script` (a list of Scan;
+    default spectral(): one DC scan, then the bands 1..5 and 6..63 of each component).  Non-interleaved scans code ceil(component
+    extent / 8) blocks per axis, interleaved ones whole MCUs, so any image size works.  Each scan gets Huffman tables built from its own
+    symbol counts, defined in front of it; wide=True skews them so that the rarer symbols sit on 9..16-bit codes.  Component c uses
+    quantisation table c, qtabs[c]; the frame header defines the tables of qhead ({id: values}, default all of them), the script's dqt
+    the others.  rst: the restart interval in force from the start.  sof 0xC0 / 0xC1: a sequential frame, every scan 0..63, Ah = Al = 0,
+    coding whole blocks of its components.  overlong_runs: an EOB run in front of a restart marker claims 5 more blocks than the interval
+    has left; a decoder must end every run at a marker (jdphuff.c process_restart), as libjpeg does."""
+    script = spectral(len(sampling)) if script is None else script
+    out = _header(h, w, sampling, dict(enumerate(qtabs)) if qhead is None else qhead, dqt16, [], rst, adobe, sof)
+    geo = _geometry(h, w, sampling)
+    dri = rst
+    for sc in script:
+        if sc.dqt:
+            out += _dqt(sc.dqt, dqt16)
+        if sc.rst is not None:
+            dri = sc.rst
+            out += _seg(0xDD, bytes([dri >> 8, dri & 255]))
+        sos, dht, data = _scan_data(sc, planes, sampling, geo, dri, sof != 0xC2, wide, overlong_runs)
+        if dht:
+            out += _seg(0xC4, dht)
+        out += _seg(0xDA, sos) + data
     return bytes(out + b"\xff\xd9")
+
+
+def segments(stream):
+    """(offset, marker, payload) of every marker segment of a stream, in order: a marker walk that skips entropy-coded data"""
+    b, pos, out = bytes(stream), 2, []
+    while pos + 4 <= len(b) and b[pos + 1] != 0xD9:
+        m, L = b[pos + 1], (b[pos + 2] << 8) | b[pos + 3]
+        out.append((pos, m, b[pos + 4:pos + 2 + L]))
+        pos += 2 + L
+        while m == 0xDA and not (b[pos] == 0xFF and b[pos + 1] != 0 and not 0xD0 <= b[pos + 1] <= 0xD7):
+            pos += 1
+    return out
+
+
+def scan_starts(stream):
+    return [pos for pos, m, _ in segments(stream) if m == 0xDA]
+
+
+def prefix(stream, k):
+    """the stream cut in front of its scan k (k scans kept), with EOI appended"""
+    starts = scan_starts(stream)
+    return stream if k >= len(starts) else bytes(stream[:starts[k]]) + b"\xff\xd9"
+
+
+def arena(planes, sampling):
+    """per-component planes -> the decoder's coefficient arena: MCU by MCU, in each the blocks of every component, v-major"""
+    parts = []
+    for p, (hs, vs) in zip(planes, sampling):
+        my, mx = p.shape[0] // vs, p.shape[1] // hs
+        parts.append(p.reshape(my, vs, mx, hs, 64).transpose(0, 2, 1, 3, 4).reshape(my, mx, vs * hs, 64))
+    return np.concatenate(parts, 2).reshape(-1, 64)
+
+
+def expected(h, w, sampling, planes, script, upto=None):
+    """The decoder's arena after the first `upto` scans of script (all by default), absolute DC in slot 0.  A DC first scan leaves the
+    value shifted right by Al ARITHMETICALLY (toward -inf) and back, a refinement ORs in the next bit; an AC coefficient last sent with
+    point transform Al holds sign * (|v| >> Al << Al), its MAGNITUDE shifted (toward 0).  A coefficient no scan sent is 0: an
+    interleaved scan codes whole MCUs, a non-interleaved one ceil(component extent / 8) blocks per axis."""
+    _, _, blk = _geometry(h, w, sampling)
+    out = []
+    for c, p in enumerate(planes):
+        v = p.astype(np.int64)
+        al = np.full(p.shape[:2] + (64,), -1, np.int64)
+        dc = np.zeros(p.shape[:2], np.int64)
+        for sc in script[:upto]:
+            if c not in sc.comps:
+                continue
+            bh, bw = p.shape[:2] if len(sc.comps) > 1 else blk[c]
+            al[:bh, :bw, [_ZZ[k] for k in range(sc.ss, sc.se + 1)]] = sc.al
+            if sc.ss == 0:
+                dc[:bh, :bw] = ((v[:bh, :bw, 0] >> sc.al) << sc.al) if sc.ah == 0 else dc[:bh, :bw] | ((v[:bh, :bw, 0] >> sc.al & 1) << sc.al)
+        a = np.maximum(al, 0)
+        q = np.where(al >= 0, np.sign(v) * ((np.abs(v) >> a) << a), 0)
+        q[..., 0] = dc
+        out.append(q.astype(np.int16))
+    return arena(out, sampling)
+
+
+def waves(script):
+    """the planner's launch count: a scan runs one wave after the latest earlier scan that shares a component AND a coefficient"""
+    w = []
+    for i, b in enumerate(script):
+        w.append(max((w[k] + 1 for k, a in enumerate(script[:i]) if not (a.se < b.ss or b.se < a.ss) and set(a.comps) & set(b.comps)),
+                     default=0))
+    return max(w) + 1
+
+
+def complete(script, ncomp, upto=None):
+    """every coefficient of every component has received its last bit (Al = 0) within the first `upto` scans"""
+    al = np.full((ncomp, 64), -1)
+    for sc in script[:upto]:
+        for c in sc.comps:
+            al[c, sc.ss:sc.se + 1] = sc.al
+    return bool((al == 0).all())
+
+
+# The catalogue.  Each function returns the script for `n` components (frame order 0..n-1).
+def spectral(n):
+    """spectral selection only: one DC scan, then the bands 1..5 and 6..63 of each component"""
+    return [Scan(tuple(range(n)), 0, 0, 0, 0)] + [Scan((c,), ss, se, 0, 0) for c in range(n) for ss, se in ((1, 5), (6, 63))]
+
+
+def simple(n):
+    """libjpeg's jpeg_simple_progression (jcparam.c), the script cv2 writes"""
+    a = tuple(range(n))
+    if n == 3:
+        return [Scan(a, 0, 0, 0, 1), Scan((0,), 1, 5, 0, 2), Scan((2,), 1, 63, 0, 1), Scan((1,), 1, 63, 0, 1), Scan((0,), 6, 63, 0, 2),
+                Scan((0,), 1, 63, 2, 1), Scan(a, 0, 0, 1, 0), Scan((2,), 1, 63, 1, 0), Scan((1,), 1, 63, 1, 0), Scan((0,), 1, 63, 1, 0)]
+    return ([Scan(a, 0, 0, 0, 1)] + [Scan((c,), ss, se, 0, 2) for c in a for ss, se in ((1, 5), (6, 63))]
+            + [Scan((c,), 1, 63, 2, 1) for c in a] + [Scan(a, 0, 0, 1, 0)] + [Scan((c,), 1, 63, 1, 0) for c in a])
+
+
+def deep(n, al=3):
+    """full bands at point transform al, then al refinements of every one: DC interleaved, AC per component"""
+    a = tuple(range(n))
+    out = [Scan(a, 0, 0, 0, al)] + [Scan((c,), 1, 63, 0, al) for c in a]
+    for t in range(al, 0, -1):
+        out += [Scan(a, 0, 0, t, t - 1)] + [Scan((c,), 1, 63, t, t - 1) for c in a]
+    return out
+
+
+def per_component_dc(n):
+    """one DC scan per component with its own refinements (mozjpeg's shape)"""
+    a = range(n)
+    return ([Scan((c,), 0, 0, 0, 2) for c in a] + [Scan((c,), 1, 63, 0, 1) for c in a] + [Scan((c,), 0, 0, 2, 1) for c in a]
+            + [Scan((c,), 0, 0, 1, 0) for c in a] + [Scan((c,), 1, 63, 1, 0) for c in a])
+
+
+def subset_dc(n):
+    """DC scans that interleave some of the components: Y alone then the chroma together, refined as Y + Cb, then the rest (n >= 3)"""
+    return ([Scan((0,), 0, 0, 0, 1), Scan(tuple(range(1, n)), 0, 0, 0, 1)] + [Scan((c,), 1, 63, 0, 1) for c in range(n)]
+            + [Scan((0, 1), 0, 0, 1, 0), Scan(tuple(range(2, n)), 0, 0, 1, 0)] + [Scan((c,), 1, 63, 1, 0) for c in range(n)])
+
+
+def sequential_subset(n):
+    """a SEQUENTIAL frame (progressive(..., sof=0xC0)) coded as Y + Cb in one scan and the rest in another (n >= 3)"""
+    return [Scan((0, 1), 0, 63, 0, 0), Scan(tuple(range(2, n)), 0, 63, 0, 0)]
+
+
+def single_coefficient(n):
+    """Ss = Se = k for every k from 1 to 63: after the DC scan, one wide wave"""
+    return [Scan(tuple(range(n)), 0, 0, 0, 0)] + [Scan((c,), k, k, 0, 0) for c in range(n) for k in range(1, 64)]
+
+
+def reordered(n):
+    """the last component first, bands high to low, the last component's refinement between the first component's first scans, the
+    DC refinement last"""
+    last, out = n - 1, [Scan((c,), 0, 0, 0, 1) for c in reversed(range(n))]
+    for c in reversed(range(n)):
+        for i, (ss, se) in enumerate(((33, 63), (6, 32), (1, 5))):
+            out.append(Scan((c,), ss, se, 0, 1))
+            if c == 0 and i == 0 and n > 1:
+                out.append(Scan((last,), 1, 63, 1, 0))
+    out += [Scan((c,), 1, 63, 1, 0) for c in reversed(range(n)) if c != last or n == 1]
+    return out + [Scan(tuple(range(n)), 0, 0, 1, 0)]
+
+
+def restarts(n):
+    """simple() with restart intervals of 1, 2 and 7 blocks / MCUs, changed between scans and switched off (DRI 0) in the middle"""
+    pattern = [1, 2, None, 7, 0, 3, None, 1, 0, 2]
+    return [sc._replace(rst=pattern[i % len(pattern)]) for i, sc in enumerate(simple(n))]
+
+
+def repeated_dc_refinement(n):
+    """simple() with its DC refinement sent twice: libjpeg warns of a bogus progression and ORs the same bit in again"""
+    sc = simple(n)
+    k = next(i for i, x in enumerate(sc) if x.ss == 0 and x.ah)
+    return sc[:k + 1] + sc[k:]
+
+
+def table_slots(n):
+    """simple() with its tables in slots 2 and 3 (a DC scan's components take slot, slot + 1, ... mod 4)"""
+    return [sc._replace(slot=2 + i % 2) for i, sc in enumerate(simple(n))]
+
+
+def scan_limit(total, n=3):
+    """exactly `total` scans (up to 14 * n + 882 n / 3): each component's DC at Al = 13 with 13 refinements, then single-coefficient
+    bands, each sent at some Al and refined down to 0"""
+    out = [Scan((c,), 0, 0, 0, 13) for c in range(n)] + [Scan((c,), 0, 0, t, t - 1) for t in range(13, 0, -1) for c in range(n)]
+    pairs = [(c, k) for c in range(n) for k in range(1, 64)]
+    base, extra = divmod(total - len(out), len(pairs))
+    assert 1 <= base and base + (extra > 0) <= 14
+    for i, (c, k) in enumerate(pairs):
+        al = base + (i < extra) - 1
+        out += [Scan((c,), k, k, 0, al)] + [Scan((c,), k, k, t, t - 1) for t in range(al, 0, -1)]
+    return out
 
 
 # ---- random extreme content ------------------------------------------------------------------------------------------------------

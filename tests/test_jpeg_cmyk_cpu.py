@@ -83,9 +83,14 @@ def test_one_scan_per_component_cmyk(emul, cmyk):  # noqa: F811
             assert np.array_equal(got, multiscan_expected(s, hblk, wblk))
 
 
-def test_scan_interleaving_a_subset_of_four_components_is_rejected(emul, cmyk):  # noqa: F811
-    prog = bytearray(next(f["enc"] for f in cmyk if f["name"] == "cmyk_s0_prog_61x77"))
-    i = prog.find(b"\xff\xda")
-    assert prog[i + 4] == 4                                   # the first (DC) scan interleaves all four components
-    three = prog[:i + 2] + bytes([0, 12, 3]) + prog[i + 5:i + 11] + prog[i + 13:]
-    assert decode(emul, bytes(three))[0] == 2                 # DALIB200_ERROR_UNSUPPORTED
+def test_scan_interleaving_a_subset_of_four_components_decodes(emul, cmyk):  # noqa: F811
+    """DC scans of C + M + Y interleaved and K alone, then refined as C + M and Y + K (T.81 G.1.1.1): the twin's coefficients"""
+    import jpeg_extreme_streams as xs
+    base = next(f["enc"] for f in cmyk if f["name"] == "cmyk_s0_base_61x77")
+    planes = cmyk_oracle.coeffs(base)
+    script = ([xs.Scan((0, 1, 2), 0, 0, 0, 1), xs.Scan((3,), 0, 0, 0, 1)] + [xs.Scan((c,), 1, 63, 0, 0) for c in range(4)]
+              + [xs.Scan((0, 1), 0, 0, 1, 0), xs.Scan((2, 3), 0, 0, 1, 0)])
+    stream = xs.progressive(61, 77, xs.SAMPLINGS["cmyk"], planes, [np.ones(64, np.int64)] * 4, adobe=0, script=script)
+    rc, got, info = decode(emul, stream)
+    assert rc == 0 and info["truncated"] == 0 and info["nwaves"] == 2, (rc, info)
+    assert np.array_equal(got, cmyk_oracle.mcu_order(base))

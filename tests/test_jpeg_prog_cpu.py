@@ -101,7 +101,7 @@ def test_large_image_and_decoded_pixels_equal_libjpeg(emul):
     assert np.array_equal(po.jpeg_decode(base), want)
 
 
-def test_truncated_and_hostile_streams_return(emul):
+def test_truncated_and_malformed_streams_return_a_status(emul):
     import cv2
     base, prog = twins(synth(64, 80, 7), 90, cv2.IMWRITE_JPEG_SAMPLING_FACTOR_420)
     full = mcu_order(base)
@@ -116,11 +116,21 @@ def test_truncated_and_hostile_streams_return(emul):
     i = bad.find(b"\xff\xda")
     bad[i + 4 + 2 * bad[i + 4] + 1] = 70                                           # Ss = 70
     assert decode(emul, bytes(bad))[0] == 4
-    sub = bytearray(prog)
-    i = sub.find(b"\xff\xda")
-    assert sub[i + 4] == 3
-    two = sub[:i + 2] + bytes([0, 10, 2]) + sub[i + 5:i + 9] + sub[i + 11:]         # the first scan interleaves 2 of the 3 components
-    assert decode(emul, bytes(two))[0] == 2
+
+
+def test_dc_scan_interleaving_a_subset_of_the_components_decodes(emul):
+    """the DC scan split into Y + Cb interleaved and Cr alone (T.81 G.1.1.1 allows a scan to interleave a subset of the components):
+    the twin's coefficients"""
+    import cv2
+    import jpeg_extreme_streams as xs
+    base, _ = twins(synth(64, 80, 7), 90, cv2.IMWRITE_JPEG_SAMPLING_FACTOR_420)
+    full = mcu_order(base)
+    planes, info = po.jpeg_coeffs(base), po.jpeg_info(base)
+    sampling = [(info["hs"][c], info["vs"][c]) for c in range(3)]
+    script = [xs.Scan((0, 1), 0, 0, 0, 0), xs.Scan((2,), 0, 0, 0, 0)] + [xs.Scan((c,), 1, 63, 0, 0) for c in range(3)]
+    two = xs.progressive(64, 80, sampling, planes, [np.ones(64, np.int64)] * 3, script=script)
+    rc, got, info = decode(emul, two)
+    assert rc == 0 and info["truncated"] == 0 and np.array_equal(got, full)
 
 
 # ---- sequential frames coded in several scans (one per component) -----------------------------------------------------------------

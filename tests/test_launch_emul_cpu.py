@@ -101,6 +101,28 @@ for c in range(3):
     b0 += nb
 n_scan, n_dc = stub.emul_launch_count(1), stub.emul_launch_count(2)
 assert n_scan == 3 * 5 and n_dc == 5, (n_scan, n_dc)        # three waves per launch (the last batch: progressive + sequential), one DC pass
+# other encoders' scripts (jpeg_extreme_streams): reordered bands, subset-interleaved DC, ten refinements, restart changes; one launch
+# per wave of the batch, and the arena holds what the statement says
+import jpeg_extreme_streams as xs
+from test_jpeg_prog_scripts_cpu import encode, source
+batch, wants = [], []
+for layout, h, w, make in [("420", 33, 47, xs.reordered), ("ycck", 24, 17, xs.subset_dc), ("422", 17, 23, lambda n: xs.deep(n, 10)),
+                           ("gray", 29, 1, xs.restarts), ("411", 16, 40, xs.single_coefficient)]:
+    src = source(layout, h, w, 90, 40 + len(batch))
+    script = make(len(src["sampling"]))
+    batch.append(encode(src, h, w, script))
+    wants.append((xs.expected(h, w, src["sampling"], src["planes"], script), src["sampling"], xs.waves(script)))
+outs, status, plan3 = g.jpeg_decode(batch + [cases[0][0]], want_coefs=True)
+assert status == [0] * len(status), status
+for i, (want, sampling, _) in enumerate(wants):
+    got = g.jpeg_coefs(plan3, i, want.size).reshape(want.shape)
+    assert np.array_equal(got[:, 1:], want[:, 1:]), ("AC", i)
+    bpm, b0 = sum(h * v for h, v in sampling), 0
+    for h, v in sampling:
+        idx = (np.arange(len(want) // bpm)[:, None] * bpm + b0 + np.arange(h * v)[None, :]).reshape(-1)
+        assert np.array_equal(np.cumsum(got[idx, 0].astype(np.int64)), want[idx, 0].astype(np.int64)), ("DC", i)
+        b0 += h * v
+assert stub.emul_launch_count(1) - n_scan == max(w for *_, w in wants), (stub.emul_launch_count(1) - n_scan, [w for *_, w in wants])
 print("progressive-emul-ok")
 """
 

@@ -24,7 +24,8 @@ extern "C" int emul_jpeg_progressive(const uint8_t *data, size_t len, int16_t *c
   std::string err;
   ProgImage im;
   memset(&im, 0, sizeof(im));
-  int rc = PlanProgressive(data, len, 0, 0, &im, scans, huff, cache, &err);
+  uint16_t quant[4][64];
+  int rc = PlanProgressive(data, len, 0, 0, &im, scans, huff, cache, quant, &err);
   if (rc) return rc;
   int nwaves = 0;
   for (auto &s : scans) nwaves = std::max(nwaves, s.wave + 1);
@@ -45,4 +46,15 @@ extern "C" int emul_jpeg_progressive(const uint8_t *data, size_t len, int16_t *c
       for (int k = 0; k < nb; k++) { const int64_t b = m * im.bpm + im.blk0[c] + k; pred += dc[b]; coef[b * 64] = (int16_t)pred; }
   }
   return 0;
+}
+
+// qt: [4][64] uint16, the quantisation table each component latched at its first scan (natural order).  Returns the planner's status.
+extern "C" int emul_jpeg_prog_quant(const uint8_t *data, size_t len, uint16_t *qt) {
+  std::vector<ProgScan> scans;
+  std::vector<ProgHuff> huff;
+  std::map<std::string, int> cache;
+  std::string err;
+  ProgImage im;
+  memset(&im, 0, sizeof(im));
+  return PlanProgressive(data, len, 0, 0, &im, scans, huff, cache, reinterpret_cast<uint16_t (*)[64]>(qt), &err);
 }
