@@ -363,6 +363,10 @@ struct StreamWindow {
 //   [31:0] exit bit position  [35:32] block in MCU (c)  [41:36] zig-zag index (z)  [51:42] blocks completed in the subsequence
 //   [63:52] priority t = distance of the chain that wrote the record from its origin (x - origin): the larger, the further
 //   left the chain started, the better informed it is.  The state proper is the low 42 bits.
+// A chain stops when its priority is full (t = kMaxChainLen).  Valid data can get there: a segment in which no speculative decoder
+// meets the true one for 4095 subsequences (e.g. all-zero bits under tables whose all-zero codes are real codes, with an odd MCU
+// length above 4096 bits).  The records up to subsequence kMaxChainLen - 1 of a unit are then still right; H2b re-decodes the rest of
+// the unit sequentially from there (resync_unit).
 constexpr uint64_t kStateMask = (1ull << 42) - 1;
 constexpr uint32_t kMaxChainLen = 4095;
 __device__ __forceinline__ uint64_t pack_state(uint32_t p, int c, int z, uint32_t cnt = 0, uint32_t t = 0) {
@@ -440,6 +444,7 @@ struct HuffCtx {
   // live chains of the synchronisation: record = (bit position, c | z << 8 | t << 16, target subsequence, image)
   uint4 *chains[3];        // [0] filled by H1, [1] survivors of the first walk step, [2] survivors of the second
   uint32_t *chain_count;   // [3]
+  uint32_t *chain_cut;     // per image: nonzero when a chain of one of its units stopped at kMaxChainLen before the unit's end
 };
 
 __device__ __forceinline__ uint32_t tbl_word(const JpegImage &im, int b) {
@@ -659,7 +664,8 @@ __device__ __forceinline__ void walk_chain(const HuffCtx &cx, const uint4 rec, i
     const uint64_t old = atomicMax(reinterpret_cast<unsigned long long *>(cx.s_state + g), (unsigned long long)ns);
     if ((uint32_t)(old >> 52) >= t) break;                    // overtaken by a better informed chain
     if (((old ^ ns) & kStateMask) == 0) break;                // synchronised
-    if (jl + 1 >= nsub_eff || t >= kMaxChainLen) break;       // end of the unit (or an absurdly long chain: corrupt data)
+    if (jl + 1 >= nsub_eff) break;                            // end of the unit
+    if (t >= kMaxChainLen) { cx.chain_cut[img_i] = 1u; break; }   // the priority is full: H2b finishes the unit (resync_unit)
     g++; jl++; t++;
     if (++visit >= max_visits) { push_chain(cx, out_list, pos, c, z, t, g, img_i); break; }
   }
@@ -687,13 +693,53 @@ __global__ void __launch_bounds__(kTailThreads) huff_sync_walk_kernel(HuffCtx cx
   for (uint32_t i = gtid; i < n; i += gsize) walk_chain(cx, cx.chains[in_list][i], out_list, max_visits, s_lut, s_slow, s_table_set, col, tblcol);
 }
 
+// The per-block table offsets of an image, read from its descriptor (resync_unit: one thread, no shared copy).
+struct ImageTbl {
+  const JpegImage *im;
+  __device__ __forceinline__ uint32_t load(int c) const { return tbl_word(*im, c); }
+};
+
+// A unit whose true chain may have stopped at kMaxChainLen (walk_chain): its records up to subsequence kMaxChainLen - 1 are right (a
+// chain only stops at t >= kMaxChainLen, so no stop can reach further left); the records behind are re-decoded sequentially from there.
+// Not inlined, and given the few fields it reads by value (a reference to the kernel's HuffCtx would put the context on the stack):
+// the scan keeps its registers and no spill of this rare path reaches it.
+__device__ __noinline__ void resync_unit(const JpegImage *__restrict__ imp, const JpegUnit *__restrict__ units,
+                                         const uint32_t *__restrict__ unit_clean_len, const TableSet *__restrict__ tables,
+                                         const uint8_t *__restrict__ clean, uint64_t *__restrict__ s_state, int log2_sub, int ui) {
+  const JpegImage &im = *imp;
+  const JpegUnit &u = units[ui];
+  const uint32_t clean_bits = unit_clean_len[ui] * 8u;
+  const uint32_t nsub_eff = (clean_bits + (1u << log2_sub) - 1) >> log2_sub;
+  if (nsub_eff <= kMaxChainLen) return;
+  const int64_t g0 = (int64_t)im.subseq_begin + u.first_subseq;
+  const uint64_t st = s_state[g0 + kMaxChainLen - 1];
+  uint32_t pos = (uint32_t)st;
+  int c = (int)((st >> 32) & 15u), z = (int)((st >> 36) & 63u);
+  BitWindow<GlobalSrc> win;
+  win.init(GlobalSrc{reinterpret_cast<const uint32_t *>(clean + u.clean_off)}, pos >> 5, pos & 31u);
+  const TableSet &ts = tables[im.table_set];
+  for (uint32_t jl = kMaxChainLen; jl < nsub_eff; jl++) {
+    uint32_t nb = 0;
+    decode_span(win, GlobalLut{ts.lut}, ts.slow, ImageTbl{&im}, im.bpm, pos, min((jl + 1) << log2_sub, clean_bits), c, z, nb);
+    s_state[g0 + jl] = pack_state(pos, c, z, nb);
+  }
+}
+
 // H2b: one CTA per image: per-unit exclusive scan of the block counts (in place), status check.
-__global__ void __launch_bounds__(1024) huff_scan_kernel(HuffCtx cx) {
+// Two 1024-thread CTAs per SM (32 registers).  The bound binds resync_unit too: it spills in its own frame, and the scan saves a few
+// registers around the call, inside the flagged branch only; the scan loop itself has no local-memory access.
+__global__ void __launch_bounds__(1024, 2) huff_scan_kernel(HuffCtx cx) {
   __shared__ uint32_t warp_tot[32];
   __shared__ uint32_t carry;
   const JpegImage &im = cx.images[blockIdx.x];
   const uint32_t sub_bits = 1u << cx.log2_sub;
-  for (int ui = im.unit_begin; ui < im.unit_end; ui++) {
+  const int unit_begin = im.unit_begin, unit_end = im.unit_end;    // read first: these loads and the flag's are in flight together
+  if (cx.chain_cut[blockIdx.x]) {                            // rare: only streams built to defeat the synchronisation get here
+    for (int ui = unit_begin + (int)threadIdx.x; ui < unit_end; ui += blockDim.x) 
+      resync_unit(&im, cx.units, cx.unit_clean_len, cx.tables, cx.clean, cx.s_state, cx.log2_sub, ui);
+    __syncthreads();
+  }
+  for (int ui = unit_begin; ui < unit_end; ui++) {
     const JpegUnit &u = cx.units[ui];
     const uint32_t clean_bits = cx.unit_clean_len[ui] * 8u;
     const uint32_t nsub_eff = (clean_bits + sub_bits - 1) >> cx.log2_sub;
@@ -2404,7 +2450,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   if ((rc = GrowDevice(p->d_chain1, p->d_chain1_cap, (size_t)p->total_subseq + 1))) return rc;
   if ((rc = GrowDevice(p->d_chain2, p->d_chain2_cap, (size_t)p->total_subseq + 1))) return rc;
   if ((rc = GrowDevice(p->d_chain3, p->d_chain3_cap, (size_t)p->total_subseq + 1))) return rc;
-  if ((rc = GrowDevice(p->d_chain_count, p->d_chain_count_cap, (size_t)8))) return rc;
+  if ((rc = GrowDevice(p->d_chain_count, p->d_chain_count_cap, (size_t)8 + p->n))) return rc;     // chain counts, then chain_cut
   if ((rc = GrowDevice(p->d_coef, p->d_coef_cap, (size_t)p->total_coefs + 64))) return rc;
   if ((rc = GrowDevice(p->d_dc, p->d_dc_cap, (size_t)p->total_coefs / 64 + 64))) return rc;
   if ((rc = GrowDevice(p->d_planes, p->d_planes_cap, (size_t)p->total_plane_bytes + 64))) return rc;
@@ -2447,7 +2493,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   cudaStream_t s = stream;
   // (the clean stream is zero-padded behind every unit by the scatter kernel itself: no memset of the 129 MB buffer)
   DB_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(int32_t) * p->n, s));
-  DB_CUDA(cudaMemsetAsync(p->d_chain_count, 0, sizeof(uint32_t) * 8, s));
+  DB_CUDA(cudaMemsetAsync(p->d_chain_count, 0, sizeof(uint32_t) * (8 + p->n), s));
   const StageInputs in{ hi, d_raw, p->d_status, p->d_coef, p->d_dc, p->d_clean, p->d_unit_len };
   if ((rc = p->prog.Run(in, s)) || (rc = p->png.Run(in, s)) || (rc = p->tiff.Run(in, s)) || (rc = p->webp.Run(in, s)) ||
       (rc = p->bitmap.Run(in, s)))
@@ -2468,6 +2514,7 @@ int dalib200JpegLaunch(dalib200JpegPlan *p, void *const *out_ptrs, dalib200Strea
   cx.clean = p->d_clean; cx.s_state = p->d_state; cx.s_n = p->d_n; cx.coef = p->d_coef; cx.dc = p->d_dc; cx.log2_sub = p->log2_sub;
   cx.status = p->d_status; cx.unit_nblk = p->d_unit_nblk;
   cx.chains[0] = p->d_chain1; cx.chains[1] = p->d_chain2; cx.chains[2] = p->d_chain3; cx.chain_count = p->d_chain_count;
+  cx.chain_cut = p->d_chain_count + 8;
   const size_t hsmem = sync_smem_bytes(p->log2_sub, false), wsmem = write_smem_bytes();
   const size_t walk_smem = kLutWords * 4 + 4 * sizeof(HuffSlow) + (size_t)(kTailColWords + kMaxBlocksPerMcu) * kTailThreads * 4;
   if (!p->smem_opted) {

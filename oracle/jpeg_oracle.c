@@ -299,6 +299,9 @@ static int jo_entropy(jo_dec *d, int16_t *coef[4]) {
     if (in->restart_interval && rst_left == 0) {
       /* byte align, expect RSTn */
       b.acc = 0; b.nbits = 0; b.pad = 0;
+      /* 0xFF fill bytes in front of the marker (T.81 B.1.1.2), which libjpeg's next_marker skips */
+      if (b.marker == 0xFF)
+        while (b.pos + 1 < b.end && b.p[b.pos] == 0xFF && b.p[b.pos + 1] == 0xFF) b.pos++;
       if (!b.marker) {
         /* skip to next marker */
         while (b.pos + 1 < b.end && !(b.p[b.pos] == 0xFF && b.p[b.pos + 1] >= 0xD0 && b.p[b.pos + 1] <= 0xD7)) b.pos++;
