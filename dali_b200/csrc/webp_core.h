@@ -11,6 +11,11 @@
 //   * reconstruction reads the UNFILTERED neighbours (libwebp keeps its own copy of the top samples from before the loop filter), with
 //     127 above the first row, 129 left of the first column, and the top-right samples of a 4x4 block in column 3 taken from the
 //     above-right macroblock's bottom row (the replicated last pixel on the right edge);
+//   * out-of-range coefficients: the inverse DCT is libwebp's choice per block (frame_dec.c DoTransform / DoUVTransform).  A luma block
+//     with a token past zigzag index 2, and all four blocks of a chroma plane in which any block has an AC token, take the full
+//     transform, which cv2's x86 build runs in int16 SIMD lanes (dec_sse2.c Transform_SSE2): the vertical pass's outputs and the sums
+//     in front of the final >> 3 wrap to int16.  The other blocks take TransformAC3 / TransformDC in int.  The two agree until the
+//     dequantised coefficients near the int16 limit, i.e. at high quantizer indices (cv2 quality-100 streams re-quantised at 127);
 //   * the loop filter is a separate pass over the finished planes, in libwebp's order per macroblock: left edge, inner vertical edges,
 //     top edge, inner horizontal edges;
 //   * colour: libwebp's fancy upsampler (UpsampleRgbLinePair) and VP8YUVToR/G/B; GRAY is cv2's BGR2GRAY of the colour decode.
@@ -34,6 +39,7 @@ struct WebpBitState {          // a boolean decoder, as byte offsets into the im
 
 struct WebpMb {                // one macroblock, written by webp_entropy
   uint32_t nz;                 // bit n: block n has a residual (0-15: Y in raster order, 16-19: U, 20-23: V)
+  uint32_t wrap;               // bit n: block n takes libwebp's full inverse DCT, whose intermediate sums are int16 (webp_idct_add)
   uint8_t segment, i4, uvmode, inner;   // inner: the loop filter runs on the inner edges
   uint8_t modes[16];           // i4: the 4x4 modes in raster order; 16x16: modes[0]
 };
@@ -277,7 +283,7 @@ DB_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int
       mb.segment = (uint8_t)seg; mb.i4 = (uint8_t)i4;
       // ---- residuals (libwebp ParseResiduals)
       uint32_t tnz_all = (t >> 16) & 0xFF, tnz_dc = (t >> 24) & 1;
-      uint32_t nzmask = 0;
+      uint32_t nzmask = 0, wrap = 0;
       if (!skip) {
         int16_t *dst = coef + m * 384;
         for (int k = 0; k < 384; k++) dst[k] = 0;
@@ -312,6 +318,7 @@ DB_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int
             l = nz > first;
             tnz = (tnz >> 1) | ((uint32_t)l << 7);
             if (nz > 1 || blk[0] != 0) nzmask |= 1u << (4 * y + x);
+            if (nz > 3) wrap |= 1u << (4 * y + x);              // libwebp's DoTransform: full transform past zigzag index 2
           }
           tnz >>= 4;
           lnzy = (lnzy >> 1) | ((uint32_t)l << 7);
@@ -329,6 +336,7 @@ DB_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int
               l = nz > 0;
               tc = (tc >> 1) | ((uint32_t)l << 3);
               if (nz > 1 || blk[0] != 0) nzmask |= 1u << b;
+              if (nz > 1) wrap |= 0xFu << (16 + 2 * ch);   // libwebp's DoUVTransform: an AC coefficient sends all 4 blocks
             }
             tc >>= 2;
             lc = (lc >> 1) | ((uint32_t)l << 5);
@@ -343,6 +351,7 @@ DB_HD int webp_entropy(const WebpImage &im, const uint8_t *raw, WebpMb *mbs, int
         if (!i4) tnz_dc = lnz_dc = 0;
       }
       mb.nz = nzmask;
+      mb.wrap = wrap;
       mb.inner = (uint8_t)(i4 || nzmask != 0);
       mbs[m] = mb;
       top[mbx] = tmodes | (tnz_all << 16) | (tnz_dc << 24);
@@ -359,14 +368,19 @@ DB_HD uint8_t webp_clip8(int v) { return (uint8_t)(v < 0 ? 0 : v > 255 ? 255 : v
 DB_HD int webp_mul1(int a) { return ((a * 20091) >> 16) + a; }
 DB_HD int webp_mul2(int a) { return (a * 35468) >> 16; }
 
-// libwebp TransformOne: adds the inverse DCT of `in` to the 4x4 block at dst
-DB_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride) {
+// libwebp TransformOne / TransformAC3 / TransformDC: adds the inverse DCT of `in` to the 4x4 block at dst.  `wrap`: the block takes
+// libwebp's full transform (VP8Transform), which cv2's x86 build runs as Transform_SSE2 in int16 lanes: each output of the vertical
+// pass and each sum in front of the final >> 3 is truncated to int16.  Those wrap only for dequantised coefficients near the int16
+// limit (high quantizer indices); below it both forms agree.  TransformAC3 and TransformDC run in int.
+DB_HD int webp_wrap16(int v, bool wrap) { return wrap ? (int)(int16_t)v : v; }
+DB_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride, bool wrap) {
   int C[16];
   int *tmp = C;
   for (int i = 0; i < 4; ++i) {
     const int a = in[0] + in[8], b = in[0] - in[8];
     const int c = webp_mul2(in[4]) - webp_mul1(in[12]), d = webp_mul1(in[4]) + webp_mul2(in[12]);
-    tmp[0] = a + d; tmp[1] = b + c; tmp[2] = b - c; tmp[3] = a - d;
+    tmp[0] = webp_wrap16(a + d, wrap); tmp[1] = webp_wrap16(b + c, wrap);
+    tmp[2] = webp_wrap16(b - c, wrap); tmp[3] = webp_wrap16(a - d, wrap);
     tmp += 4; in++;
   }
   tmp = C;
@@ -374,10 +388,10 @@ DB_HD void webp_idct_add(const int16_t *in, uint8_t *dst, int stride) {
     const int dc = tmp[0] + 4;
     const int a = dc + tmp[8], b = dc - tmp[8];
     const int c = webp_mul2(tmp[4]) - webp_mul1(tmp[12]), d = webp_mul1(tmp[4]) + webp_mul2(tmp[12]);
-    dst[0] = webp_clip8(dst[0] + ((a + d) >> 3));
-    dst[1] = webp_clip8(dst[1] + ((b + c) >> 3));
-    dst[2] = webp_clip8(dst[2] + ((b - c) >> 3));
-    dst[3] = webp_clip8(dst[3] + ((a - d) >> 3));
+    dst[0] = webp_clip8(dst[0] + (webp_wrap16(a + d, wrap) >> 3));
+    dst[1] = webp_clip8(dst[1] + (webp_wrap16(b + c, wrap) >> 3));
+    dst[2] = webp_clip8(dst[2] + (webp_wrap16(b - c, wrap) >> 3));
+    dst[3] = webp_clip8(dst[3] + (webp_wrap16(a - d, wrap) >> 3));
     tmp++; dst += stride;
   }
 }
@@ -526,7 +540,7 @@ DB_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t *
     if (!mb.i4) {
       webp_pred_block(mb.modes[0], 16, mbx, mby, top, left, Y, ys);
       for (int n = 0; n < 16; n++)
-        if (mb.nz & (1u << n)) webp_idct_add(c + n * 16, Y + (int64_t)4 * (n >> 2) * ys + 4 * (n & 3), ys);
+        if (mb.nz & (1u << n)) webp_idct_add(c + n * 16, Y + (int64_t)4 * (n >> 2) * ys + 4 * (n & 3), ys, (mb.wrap >> n) & 1);
     } else {
       for (int n = 0; n < 16; n++) {
         const int bx = 4 * (n & 3), by = 4 * (n >> 2);
@@ -539,7 +553,7 @@ DB_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t *
         for (int j = 0; j < 4; j++) L[j] = bx == 0 ? left[by + j] : d[(int64_t)j * ys - 1];
         webp_pred4(mb.modes[n], T, L, P);
         for (int y = 0; y < 4; y++) for (int x = 0; x < 4; x++) d[(int64_t)y * ys + x] = P[4 * y + x];
-        if (mb.nz & (1u << n)) webp_idct_add(c + n * 16, d, ys);
+        if (mb.nz & (1u << n)) webp_idct_add(c + n * 16, d, ys, (mb.wrap >> n) & 1);
       }
     }
   }
@@ -555,7 +569,7 @@ DB_HD void webp_recon_mb(const WebpImage &im, const WebpMb *mbs, const int16_t *
     webp_pred_block(mb.uvmode, 8, mbx, mby, top, left, U, cs);
     for (int k = 0; k < 4; k++) {
       const int b = 16 + 4 * (ch - 1) + k;
-      if (mb.nz & (1u << b)) webp_idct_add(c + b * 16, U + (int64_t)4 * (k >> 1) * cs + 4 * (k & 1), cs);
+      if (mb.nz & (1u << b)) webp_idct_add(c + b * 16, U + (int64_t)4 * (k >> 1) * cs + 4 * (k & 1), cs, (mb.wrap >> b) & 1);
     }
   }
 }

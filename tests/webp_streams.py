@@ -139,6 +139,175 @@ def corpus(big=False):
     return out
 
 
+def simple_format(streams):
+    """the [(name, bytes)] whose VP8 chunk holds the whole frame (the edge_ streams run past it): what tests/vp8_rewrite.py rewrites"""
+    return [(n, s) for n, s in streams if s[8:16] == b"WEBPVP8 " and not n.startswith("edge_")]
+
+
+def _opt(rng, p, draw):
+    return draw() if rng.random() < p else None
+
+
+def _i(rng, lo, hi):
+    """an int in [lo, hi]"""
+    return int(rng.integers(lo, hi + 1))
+
+
+def _cycle_modes(f, v):
+    """every macroblock's modes from its position and v: across v = 0..9 each 4x4 block takes every 4x4 mode, and across v = 0..3
+    each macroblock every 16x16 and chroma mode"""
+    for i, m in enumerate(f["mbs"]):
+        y, x = divmod(i, f["mb_w"])
+        m["uvmode"] = (v + x + 2 * y) % 4
+        if m["i4"]:
+            m["bmodes"] = [(v + 4 * x + (k & 3) + 3 * (4 * y + (k >> 2))) % 10 for k in range(16)]
+        else:
+            m["ymode"] = (v + 3 * x + y) % 4
+
+
+def _random_modes(f, rng):
+    for m in f["mbs"]:
+        m["uvmode"] = _i(rng, 0, 3)
+        if m["i4"]:
+            m["bmodes"] = [_i(rng, 0, 9) for _ in range(16)]
+        else:
+            m["ymode"] = _i(rng, 0, 3)
+
+
+def _segments(f, rng, q=None, strength=None, absolute=1, update_map=1, update_data=1, seg_proba=None):
+    h = f["hdr"]
+    h.update(use_segment=1, update_map=update_map, update_data=update_data, absolute_delta=absolute)
+    h["quantizer"] = q if q is not None else [_opt(rng, 0.8, lambda: _i(rng, -127, 127)) for _ in range(4)]
+    h["filter_strength"] = strength if strength is not None else [_opt(rng, 0.8, lambda: _i(rng, -63, 63)) for _ in range(4)]
+    h["seg_proba"] = seg_proba if seg_proba is not None else [_opt(rng, 0.8, lambda: _i(rng, 1, 255)) for _ in range(3)]
+    for m in f["mbs"]:
+        m["segment"] = _i(rng, 0, 3) if update_map else 0
+
+
+def rewritten(seed=0):
+    """[(name, bytes, base)]: corpus streams (`base`) whose partition 0 tests/vp8_rewrite.py rewrote into header and mode values the
+    encoders never write.  The name's first word is the family: segrel (relative segment deltas past both quantizer ends and the
+    filter level's top), segnomap / segnodata (segmentation without a map or without data), segmap (random maps, each tree probability
+    absent, 1 or 254), lfdelta (ref and mode filter deltas of both signs, unused deltas set, or no update), level0 (frame level 0 with
+    segment strengths), level63 (every sharpness, both filters), quant (every quantizer delta at base index 0 and 127), q127 (cv2
+    quality 90 / 100 streams at index 127), colorspace, modes (every mode at every edge position), skip (skip_p, use_skip 0 -> 1),
+    scale (frame-tag scale bits, also inside VP8X) and mix (everything at random)."""
+    import vp8_rewrite as vr
+    rng = np.random.default_rng(seed)
+    bases = dict(simple_format(corpus()))
+    out = []
+
+    def emit(name, f, base):
+        out.append((name, vr.write(f), bases[base]))
+
+    def frame(base):
+        return vr.parse(bases[base])
+    # both 16x16 and 4x4 macroblocks, sizes not multiples of 16
+    mixed = ["cv2_63x80_q50", "cv2_97x131_q75", "cv2_128x200_q90", "pil_method4", "enc_segments4", "cv2_17x33_q100"]
+    for k, b in enumerate(mixed):
+        f = frame(b)
+        h = f["hdr"]
+        h["base_q0"], h["level"] = _i(rng, 20, 100), _i(rng, 20, 50)
+        q0, lv = h["base_q0"], h["level"]
+        _segments(f, rng, absolute=0,
+                  q=[-(q0 + _i(rng, 1, 20)), 127 - q0 + _i(rng, 1, 20), _i(rng, -20, -1), None],
+                  strength=[63 - lv + _i(rng, 1, 10), -(lv + _i(rng, 1, 10)), _i(rng, -10, -1), None])
+        h["simple"] = k & 1
+        emit(f"segrel_{b}", f, b)
+        f = frame(b)
+        _segments(f, rng, absolute=k & 1, update_map=0)
+        f["hdr"]["level"] = _i(rng, 10, 40)
+        emit(f"segnomap_{b}", f, b)
+        f = frame(b)
+        _segments(f, rng, update_data=0)
+        f["hdr"]["level"] = _i(rng, 10, 40)
+        f["hdr"].update(use_lf_delta=1, update_lf_delta=1, ref_lf_delta=[_i(rng, 5, 20), None, None, None],
+                        mode_lf_delta=[_i(rng, 5, 20), None, None, None])
+        emit(f"segnodata_{b}", f, b)
+        for v in range(3):
+            f = frame(b)
+            _segments(f, rng, absolute=v & 1, seg_proba=[[None, 1, 254][(v + i) % 3] for i in range(3)])
+            emit(f"segmap{v}_{b}", f, b)
+        for v, (rs, ms) in enumerate([(1, 1), (1, -1), (-1, 1), (-1, -1)]):
+            f = frame(b)
+            h = f["hdr"]
+            h.update(use_lf_delta=1, update_lf_delta=1, level=_i(rng, 15, 45), simple=(v + k) & 1, sharpness=_i(rng, 0, 7))
+            h["ref_lf_delta"] = [rs * _i(rng, 4, 25)] + [_i(rng, -63, 63) for _ in range(3)]
+            h["mode_lf_delta"] = [ms * _i(rng, 4, 25)] + [_i(rng, -63, 63) for _ in range(3)]
+            if v == 3:
+                _segments(f, rng)
+            emit(f"lfdelta{v}_{b}", f, b)
+        f = frame(b)
+        f["hdr"].update(use_lf_delta=1, update_lf_delta=0, level=_i(rng, 15, 45))
+        emit(f"lfdeltanoupdate_{b}", f, b)
+        f = frame(b)
+        _segments(f, rng, absolute=k & 1, strength=[_i(rng, 10, 63) for _ in range(4)])
+        f["hdr"]["level"] = 0
+        emit(f"level0_{b}", f, b)
+        for ct in range(3):
+            f = frame(b)
+            f["hdr"]["color_space"], f["hdr"]["clamp_type"] = (ct + 1) & 1, (ct + 1) >> 1
+            emit(f"colorspace{ct}_{b}", f, b)
+    for sharp in range(8):
+        for simple in (0, 1):
+            b = mixed[(sharp + simple) % len(mixed)]
+            f = frame(b)
+            f["hdr"].update(level=63, sharpness=sharp, simple=simple)
+            emit(f"level63_sharp{sharp}_simple{simple}_{b}", f, b)
+    for d in range(5):
+        for q0 in (0, 127):
+            for sign in (-1, 1):
+                b = mixed[(d + q0 + sign) % len(mixed)]
+                f = frame(b)
+                f["hdr"].update(use_segment=0, update_map=0, base_q0=q0)
+                f["hdr"]["dq"] = [sign * _i(rng, 8, 15) if j == d else None for j in range(5)]
+                emit(f"quant_dq{d}_q{q0}_{'neg' if sign < 0 else 'pos'}_{b}", f, b)
+    for b in bases:
+        if b.startswith("cv2_") and (b.endswith("_q90") or b.endswith("_q100")):
+            f = frame(b)
+            f["hdr"].update(use_segment=0, update_map=0, base_q0=127, dq=[None] * 5)
+            emit(f"q127_{b}", f, b)
+    for b in ("cv2_17x33_q100", "cv2_29x1_q90", "cv2_1x37_q90", "cv2_63x80_q10", "cv2_97x131_q100", "cv2_128x200_q50",
+              "pil_method0", "pil_flat_method2"):
+        for v in range(10):
+            f = frame(b)
+            _cycle_modes(f, v)
+            emit(f"modes{v}_{b}", f, b)
+    for b in bases:
+        f = frame(b)
+        h = f["hdr"]
+        if h["use_skip"]:
+            h["skip_p"] = [1, 254, _i(rng, 2, 253)][len(out) % 3]
+            emit(f"skip_p_{b}", f, b)
+        elif b.startswith("cv2_") or b.startswith("enc_"):
+            h["use_skip"], h["skip_p"] = 1, _i(rng, 1, 255)
+            emit(f"skip_on_{b}", f, b)
+    for k, b in enumerate(["cv2_63x80_q75", "cv2_97x131_q50", "cv2_1x1_q90", "pil_method6"]):
+        f = frame(b)
+        _random_modes(f, rng)
+        s = vr.set_scale_bits(vr.write(f), 1 + k % 3, 3 - k % 3)
+        out.append((f"scale_{b}", s, bases[b]))
+        out.append((f"scale_vp8x_{b}", vr.to_vp8x(s), bases[b]))
+    names = sorted(bases)
+    for k in range(40):
+        b = names[_i(rng, 0, len(names) - 1)]
+        f = frame(b)
+        h = f["hdr"]
+        if rng.random() < 0.6:
+            _segments(f, rng, absolute=_i(rng, 0, 1), update_map=_i(rng, 0, 1), update_data=int(rng.random() < 0.85))
+        if rng.random() < 0.6:
+            h.update(use_lf_delta=1, update_lf_delta=int(rng.random() < 0.9))
+            h["ref_lf_delta"] = [_opt(rng, 0.7, lambda: _i(rng, -63, 63)) for _ in range(4)]
+            h["mode_lf_delta"] = [_opt(rng, 0.7, lambda: _i(rng, -63, 63)) for _ in range(4)]
+        if rng.random() < 0.6:
+            h["base_q0"] = _i(rng, 0, 127)
+            h["dq"] = [_opt(rng, 0.7, lambda: _i(rng, -15, 15)) for _ in range(5)]
+        h.update(simple=_i(rng, 0, 1), level=_i(rng, 0, 63), sharpness=_i(rng, 0, 7))
+        _random_modes(f, rng)
+        emit(f"mix{k}_{b}", f, b)
+    return out
+
+
 def _chunks(s):
     """[(tag, payload)] of the chunks of a well-formed stream"""
     out, pos = [], 12
