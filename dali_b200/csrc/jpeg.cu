@@ -312,6 +312,19 @@ __device__ __forceinline__ void ldg_stream(bool pred, uint4 &v, const uint4 *p) 
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %5, 0;\n\t@q ld.global.nc.L2::128B.v4.u32 {%0, %1, %2, %3}, [%4];\n\t}"
                : "+r"(v.x), "+r"(v.y), "+r"(v.z), "+r"(v.w) : "l"(p), "r"((uint32_t)pred));
 }
+// plain (weak) global stores to a 64-bit global address
+__device__ __forceinline__ void stg_u16(uint64_t a, uint32_t v) { asm volatile("st.global.u16 [%0], %1;" :: "l"(a), "h"((unsigned short)v)); }
+__device__ __forceinline__ void stg_v4(uint64_t a, uint4 v) {
+  asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" :: "l"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
+}
+__device__ __forceinline__ uint4 lds_v4(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ void sts_v4(uint32_t a, uint4 v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
 struct StreamWindow {
   uint32_t hi, lo;
   int avail;
@@ -774,16 +787,25 @@ __global__ void __launch_bounds__(1024, 2) huff_scan_kernel(HuffCtx cx) {
 // A block belongs to the thread in whose subsequence it STARTS: a thread skips the tail of the block that is open at its
 // entry and runs past its own end until its last block is complete (its window simply reads on into the following
 // subsequences).  Every block therefore has exactly one writer, which assembles it in a private 128-byte shared-memory buffer
-// (word j of lane l at l * 32 + (j ^ l): conflict free for the per-symbol 16-bit scatter of all lanes to the same j and for the
-// flush) and the warp writes each finished block to HBM as ONE coalesced 128-byte line: no memset of the coefficient arena,
-// no 2-byte read-modify-write traffic, ~12x fewer store wavefronts than a per-symbol scatter.
+// (16-byte chunk k of lane l at l * 8 + (k ^ (l & 7))) and the warp writes each finished block to HBM as ONE coalesced 128-byte
+// line: no memset of the coefficient arena, no 2-byte read-modify-write traffic, ~12x fewer store wavefronts than a per-symbol
+// scatter.  A flush step moves four blocks, one per quarter-warp, each lane a 16-byte chunk: the swizzle puts the 8 chunks a
+// quarter reads in 8 different bank groups, and spreads the per-symbol 16-bit scatter of lanes at the same position over them.
 //
 // The loop is a chain of dependent fixed-latency instructions (its stalls are fixed-latency waits and short scoreboards):
 // throughput scales with resident warps.  The pass therefore runs its own block shape -- kWriteThreads subsequences per CTA,
 // and the stream read from global memory (StreamWindow), so that shared memory holds only the tables and the block buffers:
 // 20.1 KB + 128 B per thread.
+//
+// Every instruction of the symbol loop runs on every trip, so the loop holds no per-phase tests.  A thread passes through three
+// phases -- skip the tail of the block open at its entry, decode its own blocks while symbols start inside its subsequence, finish
+// the last one behind it -- and each is a value, not a branch: the block index carries kSkipBlock while the entry's open block is
+// decoded (its coefficients go to the lane's buffer like any others and the flush clears them without writing the line), and the
+// decode limit `lim` is hard_end inside a block and, where a block is about to start, the subsequence end or 0 (blk_limit reached).
+// The DC difference is stored into the buffer at natural position 0 like a coefficient, and the flush moves it to the DC array.
 constexpr int kWriteThreads = 384;
 constexpr int kWriteCtasPerSm = 3;       // 3 x (68.1 KB + 1 KB reserved) of the 228 KB per SM
+constexpr uint32_t kSkipBlock = 1u << 31;   // block indices stay below 2^31: the arena would hold 256 GB of coefficients
 struct WriteSmem {
   uint32_t *lut, *tbl, *blkbuf; uint8_t *zig;
 };
@@ -806,8 +828,14 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
     const uint4 *src = reinterpret_cast<const uint4 *>(cx.tables[im.table_set].lut);
     uint4 *dst = reinterpret_cast<uint4 *>(sm.lut);
     for (int i = threadIdx.x; i < kLutWords / 4; i += blockDim.x) dst[i] = __ldg(src + i);
-    if (threadIdx.x < kMaxBlocksPerMcu) sm.tbl[threadIdx.x] = tbl_word(im, threadIdx.x);
-    if (threadIdx.x < 64) sm.zig[threadIdx.x] = c_zigzag[threadIdx.x];
+    // table word of block b of the MCU, with the next block's index in the free bits [15:12] (DC offsets are < 1024): the loop
+    // follows the MCU through this word alone
+    if (threadIdx.x < kMaxBlocksPerMcu) {
+      const int b = threadIdx.x, next = b + 1 == im.bpm ? 0 : b + 1;
+      sm.tbl[b] = tbl_word(im, b) | ((uint32_t)next << 12);
+    }
+    // byte offset of each zig-zag position in a block buffer (2 x natural position), before the lane's swizzle
+    if (threadIdx.x < 64) sm.zig[threadIdx.x] = (uint8_t)(2 * c_zigzag[threadIdx.x]);
   }
   SubGeom sg;
   {
@@ -835,10 +863,9 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
 #pragma unroll
   for (int j = 0; j < 32; j++) sts_u32(a_mybuf + 4u * j, 0u);
   __syncwarp();
-  uint32_t pos = 0, nb = 0, end = 0, hard_end = 0, blk0 = 0, blk_limit = 0;
+  uint32_t pos = 0, end = 0, hard_end = 0, blk = 0, blk_limit = 0, lim = 0;
   int c = 0, z = 0;
-  bool active = sg.valid;
-  if (active) {
+  if (sg.valid) {
     const JpegUnit &u = cx.units[sg.ui];
     if (sg.jl > 0) {
       const uint64_t prev = cx.s_state[sg.g - 1];
@@ -847,78 +874,82 @@ __global__ void __launch_bounds__(kWriteThreads, kWriteCtasPerSm) huff_write_ker
     end = min((sg.jl + 1) << cx.log2_sub, sg.clean_bits);
     hard_end = sg.clean_bits;
     const uint32_t ublk = (uint32_t)(u.slot_base >> 6);
-    blk0 = ublk + cx.s_n[sg.g];
+    const uint32_t blk0 = ublk + cx.s_n[sg.g];
     blk_limit = ublk + (uint32_t)(u.nslots >> 6);
-    active = pos < end && blk0 < blk_limit;                  // pad bits behind the last block of a unit are not symbols
+    blk = blk0 | (z != 0 ? kSkipBlock : 0u);                  // z != 0: the entry is inside a block of the previous thread
+    lim = blk0 < blk_limit ? end : 0u;                        // pad bits behind the last block of a unit are not symbols
   }
-  bool own = z == 0;                                          // a block starts exactly at the entry: it is ours
   StreamWindow win;
   win.clear();
-  if (active) win.init(cx.clean + cx.units[sg.ui].clean_off, pos);
+  if (pos < lim) win.init(cx.clean + cx.units[sg.ui].clean_off, pos);
   __syncthreads();                                            // the tables; the window's first loads are in flight meanwhile
-  int16_t *coef = cx.coef + im.coef_off;
-  int16_t *dcv = cx.dc + im.coef_off / 64;
-  const int bpm = im.bpm;
+  // this lane's chunk of coefficient line 0, and DC 0, as plain 64-bit global addresses: the flush then forms each store address
+  // with one multiply-add (as pointers, the compiler rebuilt them from the context inside the flush loop)
+  const uint32_t chunk = lane & 7u, quarter = lane >> 3;
+  const uint64_t a_line = (uint64_t)__cvta_generic_to_global(cx.coef + im.coef_off) + 16u * chunk;
+  const uint64_t a_dc = (uint64_t)__cvta_generic_to_global(cx.dc + im.coef_off / 64);
+  const uint32_t swz = 16u * chunk;                           // the lane's buffer swizzle, applied to a byte offset
   uint32_t tb12 = lds_u32(a_tbl + 4u * c);
-  for (uint32_t it = 1; __any_sync(0xffffffffu, active); it++) {
-    bool flush = false;
-    const uint32_t blk = blk0 + nb;
+  for (uint32_t it = 1; __any_sync(0xffffffffu, pos < lim); it++) {
+    bool endb = false;
+    uint32_t next_blk = blk;
     if (it & 1u) win.top_up();                                // warp-uniform, see StreamWindow
-    if (active) {
+    if (pos < lim) {
       const uint32_t thr = pair_threshold(z, pos, hard_end);
       const uint32_t e_ac = lds_u32(a_lut + 4u * ((tb12 >> 16) + (win.hi >> (32 - kAcLutBits))));
       const bool is_dc = z == 0;
       uint32_t e = e_ac;
-      if (is_dc) e = lds_u32(a_lut + 4u * ((tb12 & 0xFFFFu) + (win.hi >> (32 - kDcLutBits))));
-      if (__builtin_expect(e == 0, 0)) e = slow_lookup(slow, is_dc ? (tb12 & 0xFFFFu) : (tb12 >> 16), win.hi, is_dc);
-      // a pair needs the block open after its first symbol (z + adv1 < 64): nb, own and blk_limit are the same for both symbols.
-      // Its second symbol starts before hard_end, so `active` would have held for it.
+      if (is_dc) e = lds_u32(a_lut + 4u * ((tb12 & 0xFFFu) + (win.hi >> (32 - kDcLutBits))));
+      if (__builtin_expect(e == 0, 0)) e = slow_lookup(slow, is_dc ? (tb12 & 0xFFFu) : (tb12 >> 16), win.hi, is_dc);
+      // a pair needs the block open after its first symbol (z + adv1 < 64): blk and blk_limit are the same for both symbols.
+      // Its second symbol starts before hard_end, so `lim` would have admitted it.
       const uint32_t st = huff_step(e, thr), one = e >> 16;
       const uint32_t tb = step_bits(st), adv = step_adv(st), s = step_size(st);
-      {
-        // magnitude bits of the step's last symbol, and of the first one of a pair, computed by every lane: s == 0 gives v == 0
-        const int v = huff_extend(win.hi, tb, s);
-        if (own) {
-          if (is_dc) {
-            dcv[blk] = (int16_t)v;                            // every block has a DC term: the compact array needs no memset
-          } else {
-            const uint32_t tb1 = step_bits(one), s1 = step_size(one);
-            if (tb != tb1 && s1) {                            // a pair whose first symbol has a value: it lands before coefficient 63
-              const uint32_t nat = lds_u8(a_zig + (uint32_t)z + step_adv(one) - 1u);
-              sts_u16(a_mybuf + 4u * ((nat >> 1) ^ lane) + 2u * (nat & 1u), (uint32_t)huff_extend(win.hi, tb1, s1));
-            }
-            if (s) {                                          // runs past coefficient 63 land on 63
-              const uint32_t nat = lds_u8(a_zig + min((uint32_t)z + adv - 1u, 63u));
-              sts_u16(a_mybuf + 4u * ((nat >> 1) ^ lane) + 2u * (nat & 1u), (uint32_t)v);
-            }
-          }
-        }
+      const uint32_t tb1 = step_bits(one), s1 = step_size(one);
+      if (tb != tb1 && s1) {                                  // a pair whose first symbol has a value: it lands before coefficient 63
+        const uint32_t off = lds_u8(a_zig + (uint32_t)z + step_adv(one) - 1u);
+        sts_u16(a_mybuf + (off ^ swz), (uint32_t)huff_extend(win.hi, tb1, s1));
+      }
+      if (s) {                                                // runs past coefficient 63 land on 63; a DC difference on 0
+        const uint32_t off = lds_u8(a_zig + min((uint32_t)z + adv - 1u, 63u));
+        sts_u16(a_mybuf + (off ^ swz), (uint32_t)huff_extend(win.hi, tb, s));
       }
       win.consume(st);
       pos += tb;
       z += (int)adv;
-      const bool endb = z >= 64;                              // block finished (EOB, 64th coefficient, or garbage overrun)
-      const int c1 = c + 1 == bpm ? 0 : c + 1;
-      flush = endb && own;
-      nb += endb ? 1u : 0u;
-      own = own || endb;                                      // the open block of the entry is over: what follows is ours
-      c = endb ? c1 : c;
-      z = endb ? 0 : z;
-      if (endb) tb12 = lds_u32(a_tbl + 4u * c);
-      // keep going while symbols start inside the subsequence, then until the last own block is complete
-      active = blk0 + nb < blk_limit && (pos < end || (z != 0 && pos < hard_end));
+      if (is_dc) lim = hard_end;                              // a block once begun is decoded to its end
+      endb = z >= 64;                                         // block finished (EOB, 64th coefficient, or garbage overrun)
+      if (endb) {
+        z = 0;
+        tb12 = lds_u32(a_tbl + ((tb12 >> 10) & 0x3Cu));
+        next_blk = (blk & ~kSkipBlock) + 1u;
+        // the next block is ours if it starts inside the subsequence and inside the unit
+        lim = next_blk < blk_limit ? end : 0u;
+      }
     }
-    // ---- flush the finished blocks of this warp, one coalesced line each
-    uint32_t m = __ballot_sync(0xffffffffu, flush);
+    // ---- flush the finished blocks of this warp, four per step: quarter q takes the q-th lowest one, one coalesced line each (the
+    // entry's open block only clears its buffer)
+    uint32_t m = __ballot_sync(0xffffffffu, endb);
     while (m) {
-      const uint32_t L = __ffs(m) - 1u;
-      m &= m - 1u;
+      const uint32_t m1 = m & (m - 1u), m2 = m1 & (m1 - 1u), m3 = m2 & (m2 - 1u);
+      const uint32_t mq = quarter == 0 ? m : quarter == 1 ? m1 : quarter == 2 ? m2 : m3;
+      m = m3 & (m3 - 1u);
+      const uint32_t L = (__ffs(mq) - 1u) & 31u;
       const uint32_t fb = __shfl_sync(0xffffffffu, blk, L);
-      const uint32_t a_src = a_wbuf + L * 128u + 4u * (lane ^ L);
-      const uint32_t w = lds_u32(a_src);
-      sts_u32(a_src, 0u);
-      reinterpret_cast<uint32_t *>(coef + (size_t)fb * 64)[lane] = w;
+      if (mq) {
+        const uint32_t a_src = a_wbuf + L * 128u + 16u * (chunk ^ (L & 7u));
+        uint4 w = lds_v4(a_src);
+        sts_v4(a_src, make_uint4(0u, 0u, 0u, 0u));
+        if (fb < kSkipBlock) {
+          if (chunk == 0) {                                   // natural position 0: the DC difference goes to the DC array
+            stg_u16(a_dc + 2ull * fb, w.x);                   // every block has a DC term: the array needs no memset
+            w.x &= 0xFFFF0000u;
+          }
+          stg_v4(a_line + 128ull * fb, w);
+        }
+      }
     }
+    blk = next_blk;
     __syncwarp();
   }
 }
